@@ -1,10 +1,10 @@
 #!/usr/bin/env python
-"""bench.py -- registration pairs/sec of the BUFFER-X hot path on B200 (BASELINE.json metric).
+"""bench.py -- registration pairs/sec of the BUFFER-X hot path on H100 (BASELINE.json metric).
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--workload C2|C3|C4|C5|C1]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--workload C2|C3|C4|C5|C1] [--dump-outputs DIR]
 
-A "step" is one pass of the hot path over one BATCH of synthetic pairs (``--pairs-per-step``, default 48 C2 pairs: a
-step is ~0.28 s of GPU work, the default 20 steps a 5-6 s timed region through 48 distinct pairs per rank).  Every pair
+A "step" is one pass of the hot path over one BATCH of synthetic pairs (``--pairs-per-step``, default 48 C2 pairs: on
+one H100 at 700 W a step is ~0.5 s of GPU work, the default 20 steps a ~10 s timed region through 48 distinct pairs per rank).  Every pair
 goes through the whole path (FPS -> radius estimation -> 6x [patch gathering, LRF, SPT, conv stack, pooling] -> 3x
 [matching, cost volume, hypotheses] -> consensus -> RANSAC -> refinement); the one collective of the path, the
 all-gather of the 32-float result records, is INSIDE the timed region.
@@ -19,6 +19,10 @@ all-gather of the 32-float result records, is INSIDE the timed region.
                  the other stages.
   cpu_baseline : the CPU oracle port (oracle/) timed on the host cores on whole pairs, thread count chosen by a measured sweep.
 ``--impl reference`` times that CPU path alone (rank 0 only): one whole pair per step.
+``--dump-outputs DIR`` writes, after the timed steps, what the timed path returned for every pair of its last step (rank 0's
+pairs): DIR/pose.npy [B,4,4] float64 and DIR/num_inliers.npy, mutual_matches.npy, inlier_ind.npy, success.npy [B] float64.
+The inputs (seeded synthetic pairs and permutations) are the same on every run with the same arguments, so two builds can be
+compared output for output.
 """
 import argparse
 import copy
@@ -44,19 +48,9 @@ def measured_peaks():
     p = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.exists(p):
         d = json.load(open(p))
-        return dict(hbm=float(d["hbm_gbs"]), tf=float(d.get("bf16_tflops_sustained", d["bf16_tflops"])), src="measured")
-    return dict(hbm=6650.0, tf=1400.0, src="fallback")
-
-
-def conv_traffic():
-    """dram__bytes_read.sum + dram__bytes_write.sum per conv_sd_kernel launch, averaged over the layers of one batched
-    descriptor pass, from the committed `ncu --set full` capture (profiles/r02_conv_traffic.json, else round 1's)."""
-    for name in ("r02_conv_traffic.json", "r01_conv_traffic.json"):
-        try:
-            return float(json.load(open(os.path.join(ROOT, "profiles", name)))["dram_bytes_per_launch"])
-        except Exception:
-            continue
-    return None
+        return dict(hbm=float(d["hbm_gbs"]), tf=float(d.get("bf16_tflops_sustained", d["bf16_tflops"])), src="measured",
+                    tf_kind="bf16 dense, sustained (measured)")
+    return dict(hbm=3350.0, tf=989.0, src="H100 SXM data sheet", tf_kind="bf16 dense, data-sheet peak at up to 700 W (not measured)")
 
 
 def workload_desc(name, cfg, ns, nt):
@@ -72,7 +66,7 @@ def static_config(name, cfg, ns, nt):
     """The part of `config` that identifies the workload: identical in the `ours` and `reference` arms."""
     return {"workload": workload_desc(name, cfg, ns, nt),
             "sharding": "pair i -> rank i mod world; one all_gather of 32-float records inside the timed region",
-            "l2": "every pair's working set (~1 GB of activations) exceeds the 126 MB L2 and a batch cycles through >= 32 distinct pairs; "
+            "l2": "every pair's working set (~1 GB of activations) exceeds the 50 MB L2 and a batch cycles through >= 32 distinct pairs; "
                   "the eager roofline pass flushes 256 MB between pairs"}
 
 
@@ -164,8 +158,8 @@ def cpu_thread_sweep(cfg, sd, data, perms, fixed=None):
         t0 = time.perf_counter()
         O.register_pair(sd, small, data, perms, 0)
         res[c] = round(time.perf_counter() - t0, 3)
-        if res[c] > 1.5 * min(res.values()):       # oversubscription only gets worse from here (measured on the 128-thread
-            break                                  # box: 8: 0.83 s, 16: 0.74 s, 32: 0.92 s, 64: 2.1 s, 128: 53.7 s)
+        if res[c] > 1.5 * min(res.values()):       # oversubscription only gets worse from here
+            break
     best = min(res, key=res.get)
     return best, res
 
@@ -221,6 +215,14 @@ def run_reference(args, rank, world):
     print(json.dumps(line), flush=True)
 
 
+def dump_outputs(out_dir, outs):
+    """The forward tuples (pose, times, num_inliers, mutual_matches, inlier_ind, success) of one step -> DIR/<name>.npy."""
+    os.makedirs(out_dir, exist_ok=True)
+    np.save(os.path.join(out_dir, "pose.npy"), np.stack([np.asarray(o[0], dtype=np.float64) for o in outs]))
+    for i, name in ((2, "num_inliers"), (3, "mutual_matches"), (4, "inlier_ind"), (5, "success")):
+        np.save(os.path.join(out_dir, name + ".npy"), np.array([float(o[i]) for o in outs], dtype=np.float64))
+
+
 # ------------------------------------------------------------------------------------------------
 def main():
     ap = argparse.ArgumentParser()
@@ -232,12 +234,12 @@ def main():
                     help="BASELINE.json configs; C4 = 512 C2 pairs split round-robin over the ranks (strong scaling, one step = the whole job)")
     ap.add_argument("--pairs-per-step", type=int, default=None, help="pairs per step and rank (default: C2 48, C3 16, C5 32, C1 128; C4: 512 / world)")
     ap.add_argument("--depth", type=int, default=6,
-                    help="pairs in flight per GPU (CUDA-graph slots on separate streams).  Measured on 1xB200 (round 1): "
-                         "2 -> 92.6, 3 -> 97.3, 4 -> 111.7, 6 -> 112.8, 8 -> 114.3 pairs/s")
+                    help="pairs in flight per GPU (CUDA-graph slots on separate streams)")
     ap.add_argument("--cpu-threads", type=int, default=None, help="skip the CPU thread sweep and use this many threads")
     ap.add_argument("--cpu-pairs", type=int, default=2, help="whole pairs of the cpu_baseline leg (N=1 only)")
     ap.add_argument("--no-cpu-baseline", action="store_true")
-    ap.add_argument("--short", action="store_true", help="profiling runs under ncu: allow < 3 warm-up steps, skip the e2e legs")
+    ap.add_argument("--short", action="store_true", help="profiling runs: allow < 3 warm-up steps, skip the e2e legs")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR", help="write the results of the last timed step as DIR/<name>.npy")
     args = ap.parse_args()
     if args.impl == "ours" and not args.short:
         args.warmup = max(args.warmup, 3)
@@ -296,7 +298,7 @@ def main():
     ns, nt = len(host[0][2]["src_fds_pcd"]), len(host[0][2]["tgt_fds_pcd"])
     h2d_pair = (ns + nt) * 12 + S * (ns + nt) * 4
     d2h_pair = (18 + S + 2 + 16) * 8
-    flush = torch.empty(256 * 1024 * 1024, dtype=torch.uint8, device=dev)   # > 126 MB L2
+    flush = torch.empty(256 * 1024 * 1024, dtype=torch.uint8, device=dev)   # > 50 MB L2
     rte_th, rre_th = cfg.test.rte_thresh, cfg.test.rre_thresh
 
     def barrier():
@@ -311,7 +313,7 @@ def main():
         """`steps` batches of this rank's B pairs, DEPTH pairs in flight, then (when timed) the all-gather of the records --
         everything between two CUDA events.  mode 'dev': inputs resident in HBM; 'e2e': pinned host tensors through the
         public forward_async()."""
-        recs, handles = [], []
+        recs, handles, last = [], [], {}
         a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
         torch.cuda.synchronize()
         a.record()
@@ -321,6 +323,8 @@ def main():
 
         def collect(h, s, j):
             out = h.result()
+            if s == steps - 1:
+                last[j] = out
             if timed:
                 gt = host[j][2]["relt_pose"]
                 rte, rre = compute_rte(out[0], gt), compute_rre(out[0], gt)
@@ -353,9 +357,12 @@ def main():
             allrec = gather_records(np.stack(recs), steps * total_pairs, device=dev)   # the one collective of the path
         b.record()
         b.synchronize()
+        if timed:
+            last_outputs[mode] = [last[j] for j in range(B)]
         return a.elapsed_time(b), allrec
 
     ransac_stats = []
+    last_outputs = {}
 
     def run_eager(steps, record=False):
         """Per-kernel event brackets (ops.Profiler) need eager launches: the roofline pass."""
@@ -435,12 +442,11 @@ def main():
         e2e = n_pairs_timed / (ms_e2e / 1e3)
         cd = prof.get("conv_desc", dict(launches=0, ms=0.0, work=0.0))
         ach_tf = cd["work"] / (cd["ms"] / 1e3) / 1e12 if cd["ms"] > 0 else 0.0
-        roof = {"bound": "tensor", "kernel": "conv_sd_kernel (Cylindrical_Net layers; shifted-descriptor implicit GEMM, tcgen05 kind::f16 on fp16 hi/lo split operands = 3 MMAs per fp32-grade product, fp32-equivalent FLOPs)",
+        roof = {"bound": "tensor", "kernel": "conv_sd_kernel (Cylindrical_Net layers; shifted-descriptor implicit GEMM, wgmma f16 on fp16 hi/lo split operands = 3 MMAs per fp32-grade product, fp32-equivalent FLOPs)",
                 "achieved": ach_tf, "peak": pk["tf"], "unit": "TFLOP/s", "frac": ach_tf / pk["tf"],
-                "peak_source": f"{pk['src']} bf16 dense (sustained); three fp16 MMAs per product over the 176-row padded raster put the ceiling of this formulation at 0.265 of it",
+                "peak_source": f"{pk['src']}: {pk['tf_kind']}; three fp16 MMAs per product over the 176-row padded raster put the ceiling of this formulation at 0.265 of it",
                 "launches": cd["launches"], "avg_launch_ms": cd["ms"] / max(cd["launches"], 1),
-                "share_of_step": cd["ms"] / ms_eager if ms_eager else None, "traffic": conv_traffic(),
-                "measured_in": "eager (non-graph) pass of this run: per-kernel CUDA-event brackets need individual launches"}
+                "share_of_step": cd["ms"] / ms_eager if ms_eager else None, "measured_in": "eager (non-graph) pass of this run: per-kernel CUDA-event brackets need individual launches"}
         kern = {}
         sp = prof.get("select_patches")
         if sp and sp["ms"] > 0:
@@ -481,7 +487,7 @@ def main():
             t0 = time.perf_counter()
             best, sweep = cpu_thread_sweep(cfg, sd_cpu, host[0][2], host[0][3], fixed=args.cpu_threads)
             secs, stages = [], {}
-            for h in host[:max(1, args.cpu_pairs)]:          # whole pairs: ~10 s of CPU work each on the box
+            for h in host[:max(1, args.cpu_pairs)]:          # whole pairs: seconds of CPU work each
                 sec, st = cpu_whole_pair(cfg, sd_cpu, h[2], h[3], best)
                 secs.append(sec)
                 for k, v in st.items():
@@ -493,6 +499,8 @@ def main():
                                     "stage_seconds_per_pair": {k: round(v, 4) for k, v in stages.items()},
                                     "wall_s": round(time.perf_counter() - t0, 2)}
         print(json.dumps(line), flush=True)
+        if args.dump_outputs:
+            dump_outputs(args.dump_outputs, last_outputs["dev"])
     if world > 1:
         dist.destroy_process_group()
 

@@ -1,4 +1,4 @@
-"""bufferx-b200: the BUFFER-X per-pair registration hot path, hand-written for B200 (sm_100a).
+"""bufferx-b200: the BUFFER-X per-pair registration hot path, hand-written for H100 (sm_90a).
 
 Package layout (only what the path needs):
     csrc/      CUDA kernels + the C-ABI shared library (include/bufferx_b200.h)

@@ -10,7 +10,7 @@ override list), which is all the hot path needs.
 
 When this package is used as a drop-in inside the reference checkout the
 reference's own ``config`` package is used instead (see INTEGRATION.md); this
-module exists so that the B200 path, its tests and ``bench.py`` run without the
+module exists so that the H100 path, its tests and ``bench.py`` run without the
 reference tree and without the ``easydict`` dependency.
 """
 from pathlib import Path

@@ -1,4 +1,4 @@
-"""Build libbufferx_b200.so (sm_100a only) with nvcc, in-tree.
+"""Build libbufferx_b200.so (sm_90a, H100) with nvcc, in-tree.
 
     python buffer-x_b200/csrc/build.py [--force]
 
@@ -7,8 +7,7 @@ Two groups of translation units:
          that must be bit-identical to the oracle (FPS, radius histogram, ball query, LRF, SPT,
          matching, consensus, RANSAC).
   FAST   compiled with FMA contraction: the convolution stacks (tolerance parity).
-The shared object lands next to the package (buffer-x_b200/libbufferx_b200.so): it is git-ignored
-but travels to the GPU box with the repository snapshot.
+The shared object lands next to the package (buffer-x_b200/libbufferx_b200.so); it is git-ignored.
 """
 import os
 import subprocess
@@ -23,12 +22,8 @@ OBJ = os.path.join(HERE, "_obj")
 EXACT = ["bx_api.cu", "bx_fps.cu", "bx_radius.cu", "bx_patches.cu", "bx_spt.cu", "bx_match.cu", "bx_ransac.cu", "bx_neighbors.cu",
          "bx_bootstrap.cu"]
 FAST = ["bx_conv.cu", "bx_conv_tc.cu", "bx_conv_sd.cu"]
-ARCH = ["-gencode", "arch=compute_100a,code=sm_100a"]
+ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 COMMON = ["-O3", "-lineinfo", "-std=c++17", "-Xcompiler", "-fPIC,-fvisibility=hidden", "--expt-relaxed-constexpr"]
-if os.environ.get("BX_SD_KPAD"):          # experiment: pad between the K halves of the conv_sd A images
-    COMMON = COMMON + ["-DSD_KPAD=" + os.environ["BX_SD_KPAD"]]
-if os.environ.get("BX_BUILD_TRACE"):      # debugging aid: clock64 stage timeline in the tensor-core convolution
-    COMMON = COMMON + ["-DBX_TC_TRACE"]
 
 
 def _nvcc():
@@ -47,7 +42,7 @@ def _stale(target, deps):
 
 def build(force=False, verbose=False):
     os.makedirs(OBJ, exist_ok=True)
-    # objects are only reusable for the flag set they were compiled with (a trace build must not leak into a normal one)
+    # objects are only reusable for the flag set they were compiled with
     stamp, flags = os.path.join(OBJ, "flags.txt"), " ".join(ARCH + COMMON)
     if not os.path.exists(stamp) or open(stamp).read() != flags:
         force = True

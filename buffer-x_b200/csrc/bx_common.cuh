@@ -1,4 +1,4 @@
-// bx_common.cuh -- shared helpers of the bufferx_b200 CUDA library (sm_100a only).
+// bx_common.cuh -- shared helpers of the bufferx_b200 CUDA library (sm_90a, H100).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -6,8 +6,8 @@
 
 #include "../../include/bufferx_b200.h"
 
-#if defined(__CUDA_ARCH__) && (__CUDA_ARCH__ < 1000)
-#error "bufferx_b200 is written for sm_100a (B200) only"
+#if defined(__CUDA_ARCH__) && (__CUDA_ARCH__ != 900)
+#error "bufferx_b200 is written for sm_90a (H100)"
 #endif
 
 #define BX_API extern "C" __attribute__((visibility("default")))

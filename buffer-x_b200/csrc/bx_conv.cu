@@ -444,7 +444,7 @@ BX_API int bx_costvol_ab(const float *equi_s, const float *equi_t, const int32_t
     if (bx_needs_attr(attr_done))
         BX_CUDA(cudaFuncSetAttribute(costvol_ab_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, AB_SMEM));
     int sms = bx_device_sm_count();
-    if (sms <= 0) sms = 148;
+    if (sms <= 0) sms = 132;
     const int grid = (maxM + 1) / 2 < sms ? (maxM + 1) / 2 : sms;
     costvol_ab_kernel<<<grid, AB_T, AB_SMEM, bx_stream(stream)>>>(equi_s, equi_t, s_mids, t_mids, d_M, wa, wb, bias, A, B);
     BX_LAUNCH_CHECK();

@@ -1,10 +1,7 @@
-// bx_conv_sd.cu -- a8: the cylindrical descriptor convolutions as a SHIFTED-DESCRIPTOR implicit GEMM on tcgen05.
+// bx_conv_sd.cu -- the cylindrical descriptor convolutions as a SHIFTED-DESCRIPTOR implicit GEMM on the Hopper tensor cores (wgmma).
 //
-// Replaces, for the eight layers of Cylindrical_Net (/root/reference/models/patchnet.py:16-84 with the padding of
-// utils/common.py:265-310), the im2col-style loader of bx_conv_tc.cu: there every activation was delivered to the tensor
-// core NINE times (once per 3x3 tap, through registers and tensor memory) and the narrow layers were bound by that
-// delivery.  Here an activation is written to shared memory ONCE per tile and the nine taps are nine VIEWS of the same
-// bytes:
+// For the eight layers of Cylindrical_Net (reference models/patchnet.py:16-84 with the padding of utils/common.py:265-310) an
+// activation is written to shared memory ONCE per tile and the nine 3x3 taps are nine VIEWS of the same bytes:
 //
 //   row space   every sample is a padded (8 x 22) raster: padded row y' = 0 is a zero row (elevation padding, shared with
 //               the previous sample's bottom), y' = 1..7 are the elevations; padded column x' = 0 / 21 are the circular
@@ -18,63 +15,42 @@
 //               slices as three chunks of 16 channels.
 //   precision   fp32-grade results (descriptor parity 1e-4 rel) from fp16 tensor-core operands: x = hi + lo * 2^-11 with
 //               hi = fp16(x), lo = fp16((x - hi) * 2^11) (22 mantissa bits, the same as the 3xTF32 split, at twice the
-//               tensor rate and half the operand bytes):  a*b ~= ah*bh + (al*bh + ah*bl) * 2^-11.  The ah*bh products go to
-//               a ping-pong pair of TMEM accumulator sets [main | cross] cut after every 16-channel chunk (K = 144); a finished
-//               segment's main + cross * 2^-11 is added with round-to-nearest into fp32 running sums in registers (the tensor
-//               core accumulates with truncation: bx_conv_tc.cu header).  Per tap TWO instructions: ah * [bh | bl] as one
-//               N = 2*NT MMA into [main | cross] (the hi activations are fetched from shared memory once for both products --
-//               the kernel is bound by the tensor core's shared-memory operand reads), then al * bh into the cross columns.
+//               tensor rate and half the operand bytes):  a*b ~= ah*bh + (al*bh + ah*bl) * 2^-11.  Per 16-channel chunk
+//               (K = 144) the products go to a fresh accumulator [main | cross]; the finished chunk's main + cross * 2^-11 is
+//               added with round-to-nearest into fp32 running sums that start from the bias, so no accumulation chain is
+//               longer than one chunk.  For Cout <= 64 a tap is TWO instructions: ah * [bh | bl] as one N = 2*NT MMA into
+//               [main | cross] (the hi rows and lo rows of a weight kcore are adjacent) and al * bh into the cross columns;
+//               for Cout 128 the columns are done in two 64-wide blocks of three N = 64 MMAs each.
 //               |x| >= 65504 cannot be represented: the loader raises *flag and the host re-runs the layer on the TF32 kernel.
 //
-// Persistent warp-specialised CTA, one per SM (presplit in and out -- the layer-to-layer case -- 15 warps):
-//   8 epilogue warps  drain finished segments (tcgen05.ld) into fp32 running sums that start from the bias; a finished tile is
-//                     parked as fp32 in a shared-memory staging buffer and the warps go back to draining.
-//   1 A producer      one thread: a chunk = four 2816-byte bulk copies of the previous layer's presplit image (ring of NA chunks).
-//                     (fp32-input variant: 4 loader warps convert channel-blocked activations to fp16 hi/lo instead.)
-//   4 storer warps    staged tile -> ReLU, fp16 hi/lo split, global stores of values, wrap-column copies and zero rows (the
-//                     next layer's operand image) -- off the epilogue warps' critical path.
-//   1 MMA warp        per (chunk, tap): 2 (3 for Cout 128) x tcgen05.mma.kind::f16 (SS form, M = 128, K = 16); probes the barrier the
-//                     next step needs (mbarrier.test_wait) before issuing the current step's MMAs; tcgen05.commit to the slot /
-//                     segment / tile barriers.  No thread ever touches an activation between shared memory and the MMA.
-//   1 weight thread   the host-arranged weight image [chunk][tap][kcore][split][n][8 x fp16]: loaded ONCE and kept resident when
-//                     it fits (Cin * Cout <= 64 * 64), else streamed with cp.async.bulk + mbarrier transaction counts (whole-chunk
-//                     stages for Cout <= 64, three-tap stages for Cout 128).
-// What paces the kernel was measured, not assumed: tools/umma_probe.cu (instruction rates of the SS / TS / pair forms, drain and
-// copy rates) and the -DBX_TC_TRACE build of this file (cycle split of the MMA warp and an epilogue warp); DESIGN.md section 5.1.
+// Persistent warp-specialised CTA, one per SM:
+//   2 MMA warpgroups  warpgroup g owns tile rows 64 g .. 64 g + 63: per (chunk, tap) its wgmmas read the shifted A view and the
+//                     weights straight from shared memory; after a chunk the accumulators are folded into the running sums
+//                     and the A slot / weight stages are released.  A finished tile goes through a shared-memory staging buffer
+//                     (64 columns at a time) so that each thread then stores one row: ReLU, fp16 hi/lo split and the next
+//                     layer's wrap columns and zero rows, or fp32 channel-blocked values.
+//   A producer        presplit input: one thread, a chunk = four 2816-byte bulk copies of the previous layer's presplit image
+//                     (ring of NA chunks).  fp32 input: 4 loader warps convert channel-blocked activations to fp16 hi/lo.
+//   weight thread     the host-arranged weight image [chunk][tap][kcore][split][n][8 x fp16] in stages of three taps with
+//                     cp.async.bulk + mbarrier transaction counts; loaded ONCE and kept resident when the whole image fits
+//                     next to three A chunks, else streamed through a ring.
 #include <cuda_fp16.h>
 
 #include "bx_common.cuh"
-#include "bx_tcgen05.cuh"
+#include "bx_wgmma.cuh"
 
 namespace {
-
-// -DBX_TC_TRACE builds (BX_BUILD_TRACE=1): where the MMA warp and one epilogue warp of the middle CTA spend their cycles
-// (BX_SD_TRACE=<nchunks*1000+Cout> prints the split once per process): [0] MMA warp total, [1] waiting for A chunks, [2] for a
-// free accumulator set, [3] for weights, [4] for the cross accumulator, [5] epilogue warp 0 total, [6] waiting for segments,
-// [7] storing tiles.
-#ifdef BX_TC_TRACE
-__device__ unsigned long long g_sd_trace[8];
-#define SD_TR_DECL long long tr_[8] = {0, 0, 0, 0, 0, 0, 0, 0}; long long t_ = 0; const bool tron_ = blockIdx.x == gridDim.x / 2
-#define SD_TR_T0() do { if (tron_) t_ = clock64(); } while (0)
-#define SD_TR_ADD(i) do { if (tron_) tr_[i] += clock64() - t_; } while (0)
-#define SD_TR_OUT(i) do { if (tron_ && lane == 0) g_sd_trace[i] = (unsigned long long)tr_[i]; } while (0)
-#else
-#define SD_TR_DECL
-#define SD_TR_T0()
-#define SD_TR_ADD(i)
-#define SD_TR_OUT(i)
-#endif
 
 constexpr int SD_BM = 128;                       // GEMM rows per tile
 constexpr int SD_AROWS = 176;                    // tile rows + halo (2*22 + 2 = 46 -> 48)
 constexpr int SD_SROWS = 176;                    // padded rows per sample (8 x 22)
-constexpr int SD_KBYTES = SD_AROWS * 16;         // payload bytes of one (split, kcore) image of a chunk: [row][8 x fp16]
-#ifndef SD_KPAD
-#define SD_KPAD 0
-#endif
-constexpr int SD_KCORE = SD_KBYTES + SD_KPAD;    // its stride in shared memory (experiment: +64 shifts the second K half by 16 banks)
-constexpr int SD_CHUNK = 4 * SD_KCORE;           // [split(hi,lo)][kcore(2)]
-constexpr int SD_NL = 4;                         // loader warps
+constexpr int SD_KBYTES = SD_AROWS * 16;         // one (split, kcore) image of a chunk: [row][8 x fp16]
+constexpr int SD_CHUNK = 4 * SD_KBYTES;          // [split(hi,lo)][kcore(2)]
+constexpr int SD_NL = 4;                         // loader warps (fp32 input)
+constexpr int SD_NC = 8;                         // MMA warps: two warpgroups of 64 tile rows
+constexpr int SD_MAXNA = 12, SD_MAXNBS = 24;     // A chunk slots; weight stages (resident: every stage of up to 8 chunks)
+constexpr int SD_TRING = 32;                     // published tile indices of dynamic scheduling
+constexpr int SD_SMEM = 227 * 1024 - 2048;       // dynamic shared memory of one CTA (the rest: barriers, bias)
 
 struct ConvSdParams {
     const float *in;
@@ -82,55 +58,31 @@ struct ConvSdParams {
     const float *bias;
     float *out;
     int *flag;
-    int n, Cout, nchunks, is3d, S_in, G_in, relu, n_tiles, NA, dbg;
+    int n, Cout, nchunks, is3d, S_in, G_in, relu, n_tiles, NA;
     const int *d_n;            // optional device-side sample count (<= n): the match lists of the cost-volume stack
     const float *fa, *fb;      // COSTAB loader: the factor maps A [n,8,3*20,4], B [n,8,3*18,4] of bx_costvol_ab (else NULL)
     int cyl, rs, W, OD, OW, S_out, rs_out;   // raster geometry: rows per sample, row stride, valid output extent, output rasters
     const __half *in_sd;       // IN_SD: presplit padded input  [nchunks][split,kcore (4)][rows_in][8 x fp16]
     __half *out_sd;            // OUT_SD: presplit padded output [Cout/16][4][rows_out][8 x fp16] = the next layer's in_sd
     long long rows_in, rows_out;
-    int nbs;                   // weight ring length in super-stages (<= SD_MAXNBS); resident: == nchunks * 3, every stage is loaded once
-    int resident;              // the whole weight image stays in shared memory (fits for Cin * Cout <= 64 * 64): no re-streaming per tile
+    int nbs;                   // weight ring length in stages of three taps (resident: == nchunks * 3, every stage is loaded once)
+    int resident;              // the whole weight image stays in shared memory: no re-streaming per tile
     int *tile_ctr;             // dynamic tile scheduling (presplit-input kernels): [0] next tile, [1] CTAs that have finished; NULL = static stride
-    int stage_sync;            // verification form (bx_conv_sd_set_stage_sync / BX_SD_STAGE_SYNC=1): staging hand-over through named barriers (bar.sync / bar.arrive)
-                               // instead of mbarriers -- the form compute-sanitizer's racecheck models; same results
-    int wchunk;                // 1: a weight stage is a whole 16-channel chunk (nine taps, one copy / one barrier per chunk); 0: three taps
-    int stagger;               // experiment (BX_SD_STAGGER=<cycles>): CTA b starts (b % 16) * stagger cycles late so the tile stores of the SMs do not coincide
 };
-constexpr int SD_MAXNBS = 12;
 
-// B ring: one bulk copy / one mbarrier per SUPER-STAGE of three taps (the MMA warp's issue loop is the critical resource:
-// every barrier wait costs it ~90 cycles), NBS super-stages deep.
-// Depth: the ring has to cover the L2 -> shared-memory latency of a bulk copy (~1.5-2 k cycles with all SMs streaming) PLUS the
-// time until the MMAs that read a stage have retired (tcgen05.commit): the trace build showed the MMA warp waiting 400-500
-// cycles per chunk for weights with rings of 1.3 chunks (round 2, first half); now two chunks and more.
-#ifndef SD_NBS_MUL
-#define SD_NBS_MUL 2
-#endif
-template <int NT> struct SdRing { static constexpr int SB = 3, NBS = NT == 128 ? 3 * SD_NBS_MUL : 12; };
+template <int NT, int IN_SD> struct SdCfg {
+    static constexpr int NB = NT < 64 ? NT : 64;                  // accumulator block: output columns per pass
+    static constexpr int NH = NT / NB;                            // passes per chunk
+    static constexpr int NLW = IN_SD ? 1 : SD_NL;                 // A producer warps
+    static constexpr int THREADS = (SD_NC + NLW + 1) * 32;
+    static constexpr int B_STAGE = 3 * 64 * NT;                   // three taps of [kcore][split][n][16 B]
+    static constexpr int STAGE_BYTES = SD_BM * NB * 4;            // fp32 staging of one column block of a tile
+};
 
-__device__ __forceinline__ void mma_f16_ss(uint32_t leader, uint32_t tmem_d, uint32_t a_lo, uint32_t b_lo, uint32_t desc_hi, uint32_t idesc,
-                                           uint32_t accumulate) {
-    asm volatile(
-        "{\n\t"
-        ".reg .pred p, q;\n\t"
-        ".reg .b64 da, db;\n\t"
-        "setp.ne.b32 p, %6, 0;\n\t"
-        "setp.ne.b32 q, %0, 0;\n\t"
-        "mov.b64 da, {%2, %4};\n\t"
-        "mov.b64 db, {%3, %4};\n\t"
-        "@q tcgen05.mma.cta_group::1.kind::f16 [%1], da, db, %5, p;\n\t"
-        "}\n" ::"r"(leader),
-        "r"(tmem_d), "r"(a_lo), "r"(b_lo), "r"(desc_hi), "r"(idesc), "r"(accumulate)
-        : "memory");
-}
-
-// One epilogue thread's share of a finished tile: GEMM row R = t * 128 + 32 * quarter + lane, CW consecutive output channels
-// starting at ecs * CW.  `run` already holds bias + sum (the running sums start from the bias); here: ReLU, then either fp32
-// channel-blocked stores of the valid rows or the presplit images of the next layer (value, wrap-column copies, zero rows).
-// The epilogue warps are the kernel's second critical resource (a tile's store used to cost them as long as three of its
-// four chunks take the tensor core): rows that produce nothing skip the arithmetic, the index arithmetic is 32-bit, the
-// image pointers advance by additions.
+// One thread's share of a finished tile: GEMM row R = t * 128 + row, CW consecutive output channels starting at co0; get8
+// yields bias + sum of eight of them.  Here: ReLU, then either fp32 channel-blocked stores of the valid rows or the presplit
+// images of the next layer (value, wrap-column copies, zero rows).  Rows that produce nothing skip the arithmetic, the index
+// arithmetic is 32-bit, the image pointers advance by additions.
 template <int CW, int OUT_SD, class Get8>
 __device__ __forceinline__ void sd_store_rows(const ConvSdParams &p, int t, int row, int co0, int n_samples, Get8 get8) {
     const uint32_t R = (uint32_t)t * SD_BM + (uint32_t)row;            // host: rows < 2^31
@@ -195,225 +147,153 @@ __device__ __forceinline__ void sd_store_rows(const ConvSdParams &p, int t, int 
     }
 }
 
-// the epilogue warps' own store: values from their running sums
-template <int CW, int OUT_SD>
-__device__ __forceinline__ void sd_store_tile(const ConvSdParams &p, int t, int quarter, int ecs, int lane, int n_samples, const float (&run)[CW]) {
-    sd_store_rows<CW, OUT_SD>(p, t, quarter * 32 + lane, ecs * CW, n_samples, [&](int c, float (&r)[8]) {
-#pragma unroll
-        for (int e = 0; e < 8; ++e) r[e] = run[c + e];
-    });
-}
-
 // IN_SD = 0: fp32 channel-blocked input converted by the loader warps; 1: presplit padded fp16 images fetched with bulk copies.
 // OUT_SD = 0: fp32 channel-blocked output; 1: presplit padded fp16 images (zero rows and wrap columns written here).
-// MERGED (NT <= 64): per tap ah * [bh | bl] as ONE N = 2*NT instruction into [main | cross] + al * bh; both halves are cut
-// and drained per segment.  NT = 128 (N = 256 instructions and twice the drain traffic measured 5 % SLOWER there): three
-// N = 128 instructions per tap, main ping-pong per segment, cross accumulators one chain per tile (ping-pong by tile).
-// STAGED (presplit in and out, the descriptor stack's layer-to-layer case): the epilogue warps only park a finished tile
-// (bias + sum, fp32) in a shared-memory staging buffer and go back to draining; four STORER warps do ReLU, the fp16 split
-// and the global stores (values, wrap copies, zero rows) while the next tile is computed.  Measured before: the store took the
-// epilogue warps 2600 (Cout 64) / 5200 (Cout 128) cycles per tile, mostly waiting for the LSU, and the tensor core stalled on
-// accumulator sets meanwhile.
-template <int NT, int IN_SD, int OUT_SD> struct SdRoles {
-    static constexpr bool STAGED = IN_SD && OUT_SD;
-    static constexpr int NST = 4;          // storer warps, one tile row per thread.  Eight (two per row, half the channels each: 19 warps, 107 registers)
-                                           // measured 15-25 % SLOWER on the Cout 64 layers
-    static constexpr int NLW = STAGED ? 1 + NST : SD_NL;
-};
-
-template <int NT, int ECS, int IN_SD, int OUT_SD>
-__global__ void __launch_bounds__((4 * ECS + SdRoles<NT, IN_SD, OUT_SD>::NLW + 2) * 32, 1) conv_sd_kernel(const ConvSdParams p) {
-    constexpr bool MERGED = NT <= 64;
-    constexpr bool STAGED = SdRoles<NT, IN_SD, OUT_SD>::STAGED;
-    constexpr int NLW = SdRoles<NT, IN_SD, OUT_SD>::NLW;       // warps between the epilogue warps and the MMA warp: loaders, or A producer + storers
-    constexpr int NST = SdRoles<NT, IN_SD, OUT_SD>::NST;
-    constexpr int NE = 4 * ECS, MMA_WARP = NE + NLW, WGT_WARP = NE + NLW + 1;
-    constexpr int CW = NT / ECS;                  // accumulator columns of one epilogue warp
-    constexpr int SB = SdRing<NT>::SB;
-    const int NBS = p.nbs;
-    constexpr int B_STAGE = 64 * NT;              // [kcore][split][n][16 B]
-    constexpr int NSETS = MERGED ? 4 : 2;         // accumulator sets in flight: MERGED four [main | cross] pairs (the epilogue warps may lag
-                                                  // three chunks behind the tensor core, e.g. while they store the previous tile); else main[2], cross[2]
-    constexpr int TMEM_COLS = MERGED ? NSETS * 2 * NT : 4 * NT;
-    constexpr int MAXNA = 12;
-    // barriers
-    constexpr int BAR_AFULL = 0, BAR_AEMPTY = MAXNA, BAR_BFULL = 2 * MAXNA, BAR_BEMPTY = BAR_BFULL + SD_MAXNBS;
-    constexpr int BAR_SEGDONE = BAR_BEMPTY + SD_MAXNBS, BAR_ACCFREE = BAR_SEGDONE + 4, BAR_XDONE = BAR_ACCFREE + 4, BAR_XFREE = BAR_XDONE + 2;
-    constexpr int BAR_STAGED = BAR_XFREE + 2, BAR_STFREE = BAR_STAGED + 1, BAR_TILE = BAR_STFREE + 1;
-    constexpr int TRING = 32;                     // published tile indices: the A producer is at most 12 (one-chunk tiles) + 7 tiles ahead of the storers
-    constexpr int NBARS = BAR_TILE + TRING;
+template <int NT, int IN_SD, int OUT_SD>
+// Registers: the warps of a CTA are spread over the SM's four sub-partitions of 16 K registers each, so the 10 (13) warps
+// put 3 (4) warps on one of them and cap a thread at 168 (128) registers -- the bound __launch_bounds__ gives ptxas.
+__global__ void __launch_bounds__(SdCfg<NT, IN_SD>::THREADS, 1) conv_sd_kernel(const ConvSdParams p) {
+    using C = SdCfg<NT, IN_SD>;
+    constexpr int NB = C::NB, NH = C::NH, WGT_WARP = SD_NC + C::NLW;
+    constexpr int BAR_AFULL = 0, BAR_AEMPTY = SD_MAXNA, BAR_BFULL = 2 * SD_MAXNA, BAR_BEMPTY = BAR_BFULL + SD_MAXNBS;
+    constexpr int BAR_TILE = BAR_BEMPTY + SD_MAXNBS, NBARS = BAR_TILE + SD_TRING;
     extern __shared__ __align__(128) unsigned char smem[];
     __shared__ __align__(8) unsigned long long bars[NBARS];
-    __shared__ int tile_ring[TRING];
-    __shared__ uint32_t tmem_base_s;
+    __shared__ int tile_ring[SD_TRING];
     __shared__ __align__(16) float bias_s[128];        // the running sums of a tile start from the bias
 
-    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-    const int NA = p.NA, nchunks = p.nchunks;
+    const int tid = threadIdx.x, lane = tid & 31;
+    const int warp = __shfl_sync(0xffffffffu, tid >> 5, 0);       // warp-uniform role index (keeps the wgmma issue convergent)
+    const int NA = p.NA, NBS = p.nbs, nchunks = p.nchunks;
+    const bool resident = p.resident != 0;
     const int n_samples = p.d_n ? min(*p.d_n, p.n) : p.n;
     const int n_tiles = (int)(((long long)n_samples * p.rs + SD_BM - 1) / SD_BM);   // <= the host's bound the grid was sized for
-    const int n_stages = nchunks * 9;
-    // staging buffer of one finished tile, fp32 [NT / 4][128 rows][4]: behind the A and B rings
-    float4 *const stage = reinterpret_cast<float4 *>(smem + (size_t)NA * SD_CHUNK + (size_t)p.nbs * (p.wchunk ? 9 : SdRing<NT>::SB) * 64 * NT);
-    const int nseg = nchunks;                    // one accumulator segment per 16-channel chunk (nine main MMAs, K = 144)
+    // shared memory: A ring | weight ring | staging buffer of one column block of a finished tile, fp32 [NB / 4][128 rows][4]
+    float *const stage = reinterpret_cast<float *>(smem + (size_t)NA * SD_CHUNK + (size_t)NBS * C::B_STAGE);
 
-    if (warp == MMA_WARP) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(&tmem_base_s)), "r"(TMEM_COLS) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
     if (tid == 0) {
-        for (int s = 0; s < MAXNA; ++s) {
+        for (int s = 0; s < SD_MAXNA; ++s) {
             mbar_init(smem_u32(&bars[BAR_AFULL + s]), IN_SD ? 1 : SD_NL);
-            mbar_init(smem_u32(&bars[BAR_AEMPTY + s]), 1);
+            mbar_init(smem_u32(&bars[BAR_AEMPTY + s]), SD_NC);
         }
         for (int s = 0; s < SD_MAXNBS; ++s) {
             mbar_init(smem_u32(&bars[BAR_BFULL + s]), 1);
-            mbar_init(smem_u32(&bars[BAR_BEMPTY + s]), 1);
+            mbar_init(smem_u32(&bars[BAR_BEMPTY + s]), SD_NC);
         }
-        for (int s = 0; s < 4; ++s) {
-            mbar_init(smem_u32(&bars[BAR_SEGDONE + s]), 1);
-            mbar_init(smem_u32(&bars[BAR_ACCFREE + s]), NE);
-        }
-        for (int s = 0; s < 2; ++s) {
-            mbar_init(smem_u32(&bars[BAR_XDONE + s]), 1);
-            mbar_init(smem_u32(&bars[BAR_XFREE + s]), NE);
-        }
-        mbar_init(smem_u32(&bars[BAR_STAGED]), NE);
-        mbar_init(smem_u32(&bars[BAR_STFREE]), NST);
-        for (int s = 0; s < TRING; ++s) mbar_init(smem_u32(&bars[BAR_TILE + s]), 1);
+        for (int s = 0; s < SD_TRING; ++s) mbar_init(smem_u32(&bars[BAR_TILE + s]), 1);
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
     if (threadIdx.x < 128) bias_s[threadIdx.x] = (int)threadIdx.x < p.Cout ? __ldg(p.bias + threadIdx.x) : 0.0f;
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
     __syncthreads();
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    uint32_t tmem_base = tmem_base_s;
     uint32_t a_base = smem_u32(smem);
     uint32_t b_base = a_base + (uint32_t)NA * SD_CHUNK;
     uint32_t bar_base = smem_u32(&bars[0]);
-    asm volatile("" : "+r"(tmem_base), "+r"(a_base), "+r"(b_base), "+r"(bar_base));
+    asm volatile("" : "+r"(a_base), "+r"(b_base), "+r"(bar_base));
 
     // Tile sequence of this CTA.  Static: blockIdx.x, + gridDim.x, ...  Dynamic (presplit input, p.tile_ctr): the A producer
     // draws the next tile from a global counter and publishes it in a shared-memory ring; every other role reads the k-th
     // entry (-1 = no more tiles).  With several pairs in flight a convolution often starts with some SMs still held by
-    // another stream's kernels (the FPS clusters keep 16 SMs for 2.2 ms): with the static stride the CTAs that start late
-    // still own 1/148 of the tiles each and the whole launch waits for them (measured: ~0.2-0.4 ms per pair).
+    // another stream's kernels; with the static stride the CTAs that start late still own their share of the tiles and the
+    // whole launch waits for them.
     const bool dyn = IN_SD && p.tile_ctr != nullptr;
     auto tile_of = [&](uint32_t k) -> int {
         if (!dyn) { const long long t = (long long)blockIdx.x + (long long)k * gridDim.x; return t < n_tiles ? (int)t : -1; }
-        mbar_wait(bar_base + 8u * (BAR_TILE + (k & (TRING - 1))), (k / TRING) & 1u);
-        return tile_ring[k & (TRING - 1)];
+        mbar_wait(bar_base + 8u * (BAR_TILE + (k & (SD_TRING - 1))), (k / SD_TRING) & 1u);
+        return tile_ring[k & (SD_TRING - 1)];
     };
 
-    if (STAGED && warp > NE && warp < NE + NLW) {
-        // =========================== storers: staged tile -> ReLU, fp16 split, global stores ========================
-        constexpr int SCW = NT * 4 / NST;                            // channels per storer thread
-        const int sw = warp - NE - 1, row = (sw & 3) * 32 + lane, sc0 = (sw >> 2) * SCW;
-        uint32_t k = 0;
+    if (warp < SD_NC) {
+        // =========================== MMA warpgroups: wgmma, chunk folds, tile stores =====================================
+        const int wg = warp >> 2, tl = tid & 127;
+        const int r0 = wg * 64 + (warp & 3) * 16 + (lane >> 2);         // fragment rows r0 and r0 + 8 of the tile
+        const int cq = 2 * (lane & 3);                                   // fragment column within an 8-column group
+        constexpr uint32_t DESC_HI = 128u >> 4;                          // SBO = 128 B (8 rows x 16 B)
+        constexpr uint32_t A_LBO = ((uint32_t)SD_KBYTES >> 4) << 16;    // K-adjacent core matrices: one kcore image apart
+        constexpr uint32_t B_LBO = ((uint32_t)(2 * NT * 16) >> 4) << 16; // weight image [kcore][split(hi,lo)][n][16 B]
+        constexpr uint32_t A_SPLIT = (2u * SD_KBYTES) >> 4, B_TAP16 = (64u * NT) >> 4, B_LO16 = (uint32_t)(NT * 16) >> 4;
+        const uint32_t a0 = ((a_base + (uint32_t)wg * 64u * 16u) >> 4) | A_LBO;   // this warpgroup's 64 rows
+        const uint32_t b0 = (b_base >> 4) | B_LBO;
+        const uint32_t Wrow = (uint32_t)p.W;                             // tap (g, tt) reads rows R + g * W + tt
+        float run[NT / 2], acc[NB];
+        uint32_t slot = 0, a_par = 0, q = 0, k = 0;
         for (int t = tile_of(0); t >= 0; t = tile_of(++k)) {
-            if (p.stage_sync) asm volatile("bar.sync 1, %0;" ::"r"((NE + NST) * 32) : "memory");       // epilogue warps arrive, storers wait
-            else mbar_wait(bar_base + 8u * BAR_STAGED, k & 1u);
-            sd_store_rows<SCW, OUT_SD>(p, t, row, sc0, n_samples, [&](int c, float (&r)[8]) {
-                const float4 u0 = stage[((sc0 + c) >> 2) * SD_BM + row], u1 = stage[(((sc0 + c) >> 2) + 1) * SD_BM + row];
-                r[0] = u0.x; r[1] = u0.y; r[2] = u0.z; r[3] = u0.w; r[4] = u1.x; r[5] = u1.y; r[6] = u1.z; r[7] = u1.w;
-            });
-            __syncwarp();
-            if (p.stage_sync) asm volatile("bar.arrive 2, %0;" ::"r"((NE + NST) * 32) : "memory");
-            else if (lane == 0) mbar_arrive(bar_base + 8u * BAR_STFREE);
-        }
-    } else if (warp < NE) {
-        // =========================== epilogue: segment drains, bias, ReLU, stores ==========================
-        const int quarter = warp & 3, ecs = warp >> 2;
-        const uint32_t tm_lane = (uint32_t)(quarter * 32) << 16;
-        float run[CW];
-        int seg = 0, k = 0;
-        SD_TR_DECL;
-#ifdef BX_TC_TRACE
-        const long long te0_ = clock64();
-#endif
-        for (int t = tile_of(0); t >= 0; t = tile_of((uint32_t)++k)) {
 #pragma unroll
-            for (int c = 0; c < CW; c += 4) {
-                const float4 b4 = *reinterpret_cast<const float4 *>(&bias_s[ecs * CW + c]);
-                run[c] = b4.x; run[c + 1] = b4.y; run[c + 2] = b4.z; run[c + 3] = b4.w;
-            }
-            for (int jj = 0; jj < nseg; ++jj, ++seg) {
-                const int set = seg & (NSETS - 1);
-                SD_TR_T0();
-                mbar_wait(bar_base + 8u * (BAR_SEGDONE + set), (uint32_t)((seg / NSETS) & 1));
-                SD_TR_ADD(6);
-                asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
+            for (int i = 0; i < NT / 2; ++i) run[i] = bias_s[(i / (NB / 2)) * NB + 8 * ((i % (NB / 2)) >> 2) + cq + (i & 1)];
+            for (int c = 0; c < nchunks; ++c) {
+                mbar_wait(bar_base + 8u * (BAR_AFULL + slot), a_par);
+                const uint32_t ac = a0 + slot * ((uint32_t)SD_CHUNK >> 4);
+                const uint32_t q0 = resident ? (uint32_t)c * 3u : q;    // first weight stage of this chunk
 #pragma unroll
-                for (int c0 = 0; c0 < CW; c0 += 32) {
-                    uint32_t v[32];
-                    if constexpr (MERGED) {
-                        uint32_t u[32];
-                        tmem_ld<32>(tmem_base + tm_lane + (uint32_t)(set * 2 * NT + ecs * CW + c0), v);            // ah*bh
-                        tmem_ld<32>(tmem_base + tm_lane + (uint32_t)(set * 2 * NT + NT + ecs * CW + c0), u);       // (ah*bl + al*bh) * 2^11
-                        asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
+                for (int h = 0; h < NH; ++h) {
+                    wgmma_fence();
 #pragma unroll
-                        for (int c = 0; c < 32; ++c) run[c0 + c] += fmaf(__uint_as_float(u[c]), 0.00048828125f, __uint_as_float(v[c]));
-                    } else {
-                        tmem_ld<32>(tmem_base + tm_lane + (uint32_t)(set * NT + ecs * CW + c0), v);
-                        asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
+                    for (int g = 0; g < 3; ++g) {
+                        const uint32_t sq = q0 + (uint32_t)g, sb = sq % (uint32_t)NBS;
+                        if (h == 0) mbar_wait(bar_base + 8u * (BAR_BFULL + sb), resident ? 0u : (sq / (uint32_t)NBS) & 1u);
+                        const uint32_t bg = b0 + sb * ((uint32_t)C::B_STAGE >> 4);
 #pragma unroll
-                        for (int c = 0; c < 32; ++c) run[c0 + c] += __uint_as_float(v[c]);
+                        for (int tt = 0; tt < 3; ++tt) {
+                            const uint32_t ah = ac + (uint32_t)g * Wrow + (uint32_t)tt, al = ah + A_SPLIT;   // one row = 16 B
+                            const uint32_t bh = bg + (uint32_t)tt * B_TAP16 + (uint32_t)(h * NB * 16 / 16);
+                            const uint32_t acc_on = (g == 0 && tt == 0) ? 0u : 1u;
+                            if constexpr (NH == 1) {     // ah * [bh | bl] -> [main | cross], al * bh -> cross
+                                wgmma_f16<2 * NT>(acc, gmma_desc(ah, DESC_HI), gmma_desc(bh, DESC_HI), acc_on);
+                                wgmma_f16<NT>(acc + NT / 2, gmma_desc(al, DESC_HI), gmma_desc(bh, DESC_HI), 1u);
+                            } else {
+                                wgmma_f16<64>(acc, gmma_desc(ah, DESC_HI), gmma_desc(bh, DESC_HI), acc_on);
+                                wgmma_f16<64>(acc + 32, gmma_desc(al, DESC_HI), gmma_desc(bh, DESC_HI), acc_on);
+                                wgmma_f16<64>(acc + 32, gmma_desc(ah, DESC_HI), gmma_desc(bh + B_LO16, DESC_HI), 1u);
+                            }
+                        }
                     }
-                }
-                asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-                __syncwarp();
-                if (lane == 0) mbar_arrive(bar_base + 8u * (BAR_ACCFREE + set));
-            }
-            if constexpr (!MERGED) {      // the tile's cross accumulator: one read, scaled by 2^-11
-                const int xset = k & 1;
-                mbar_wait(bar_base + 8u * (BAR_XDONE + xset), (uint32_t)((k >> 1) & 1));
-                asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
+                    wgmma_commit();
+                    wgmma_wait<0>();
+                    wgmma_fence_regs<NB>(acc);
 #pragma unroll
-                for (int c0 = 0; c0 < CW; c0 += 32) {
-                    uint32_t u[32];
-                    tmem_ld<32>(tmem_base + tm_lane + (uint32_t)(2 * NT + xset * NT + ecs * CW + c0), u);
-                    asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-#pragma unroll
-                    for (int c = 0; c < 32; ++c) run[c0 + c] = fmaf(__uint_as_float(u[c]), 0.00048828125f, run[c0 + c]);
+                    for (int i = 0; i < NB / 2; ++i) run[h * (NB / 2) + i] += fmaf(acc[NB / 2 + i], 0.00048828125f, acc[i]);
                 }
-                asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
                 __syncwarp();
-                if (lane == 0) mbar_arrive(bar_base + 8u * (BAR_XFREE + xset));
-            }
-            SD_TR_T0();
-            if constexpr (STAGED) {
-                if (k >= 1) {                                                                      // the storers have read the previous tile
-                    if (p.stage_sync) asm volatile("bar.sync 2, %0;" ::"r"((NE + NST) * 32) : "memory");
-                    else mbar_wait(bar_base + 8u * BAR_STFREE, (uint32_t)((k - 1) & 1));
+                if (lane == 0) {
+                    mbar_arrive(bar_base + 8u * (BAR_AEMPTY + slot));
+                    if (!resident)
+                        for (int g = 0; g < 3; ++g) mbar_arrive(bar_base + 8u * (BAR_BEMPTY + (q0 + (uint32_t)g) % (uint32_t)NBS));
                 }
-#pragma unroll
-                for (int c = 0; c < CW; c += 4)
-                    stage[((ecs * CW + c) >> 2) * SD_BM + quarter * 32 + lane] = make_float4(run[c], run[c + 1], run[c + 2], run[c + 3]);
-                __syncwarp();
-                if (p.stage_sync) asm volatile("bar.arrive 1, %0;" ::"r"((NE + NST) * 32) : "memory");
-                else if (lane == 0) mbar_arrive(bar_base + 8u * BAR_STAGED);
-            } else {
-                sd_store_tile<CW, OUT_SD>(p, t, quarter, ecs, lane, n_samples, run);
+                if (++slot == (uint32_t)NA) { slot = 0; a_par ^= 1u; }
+                if (!resident) q += 3;
             }
-            SD_TR_ADD(7);
+            // the finished tile, one column block at a time: fragments -> staging -> one row per thread
+#pragma unroll
+            for (int h = 0; h < NH; ++h) {
+                asm volatile("bar.sync %0, 128;" ::"r"(1 + wg) : "memory");        // this warpgroup's rows of the staging buffer are free
+#pragma unroll
+                for (int i = 0; i < NB / 2; i += 2) {
+                    const int col = 8 * (i >> 2) + cq, row = r0 + ((i & 2) ? 8 : 0);
+                    *reinterpret_cast<float2 *>(stage + ((size_t)(col >> 2) * SD_BM + row) * 4 + (col & 3)) =
+                        make_float2(run[h * (NB / 2) + i], run[h * (NB / 2) + i + 1]);
+                }
+                asm volatile("bar.sync %0, 128;" ::"r"(1 + wg) : "memory");
+                const int row = wg * 64 + (tl & 63), cs = (tl >> 6) * (NB / 2);
+                const float4 *st4 = reinterpret_cast<const float4 *>(stage);
+                sd_store_rows<NB / 2, OUT_SD>(p, t, row, h * NB + cs, n_samples, [&](int cc, float (&r)[8]) {
+                    const float4 u0 = st4[((cs + cc) >> 2) * SD_BM + row], u1 = st4[(((cs + cc) >> 2) + 1) * SD_BM + row];
+                    r[0] = u0.x; r[1] = u0.y; r[2] = u0.z; r[3] = u0.w; r[4] = u1.x; r[5] = u1.y; r[6] = u1.z; r[7] = u1.w;
+                });
+            }
         }
-#ifdef BX_TC_TRACE
-        if (warp == 0) { tr_[5] = clock64() - te0_; SD_TR_OUT(5); SD_TR_OUT(6); SD_TR_OUT(7); }
-#endif
-    } else if (warp < NE + NLW) {
+    } else if (warp < WGT_WARP) {
         if (IN_SD) {
             // =========================== A producer: presplit images by bulk copy =================================
             // A chunk's four (split, kcore) images are four contiguous 2816-byte runs of the previous layer's output: one
             // thread keeps NA chunks in flight; no register staging, no conversion.
-            if (warp == NE && lane == 0) {
+            if (warp == SD_NC && lane == 0) {
                 uint32_t slot = 0, par = 0, round = 0;
                 for (uint32_t k = 0;; ++k) {
                     int t;
                     if (dyn) {           // draw the next tile and publish it to the other roles
                         t = atomicAdd(p.tile_ctr, 1);
                         if (t >= n_tiles) t = -1;
-                        tile_ring[k & (TRING - 1)] = t;
-                        mbar_arrive(bar_base + 8u * (BAR_TILE + (k & (TRING - 1))));
+                        tile_ring[k & (SD_TRING - 1)] = t;
+                        mbar_arrive(bar_base + 8u * (BAR_TILE + (k & (SD_TRING - 1))));
                     } else {
                         t = tile_of(k);
                     }
@@ -424,7 +304,7 @@ __global__ void __launch_bounds__((4 * ECS + SdRoles<NT, IN_SD, OUT_SD>::NLW + 2
                         const unsigned char *src = reinterpret_cast<const unsigned char *>(p.in_sd) + ((size_t)(c * 4) * p.rows_in + (size_t)t * SD_BM) * 16;
 #pragma unroll
                         for (int im = 0; im < 4; ++im)
-                            bulk_g2s(a_base + slot * (uint32_t)SD_CHUNK + (uint32_t)im * SD_KCORE, src + (size_t)im * p.rows_in * 16, (uint32_t)SD_KBYTES,
+                            bulk_g2s(a_base + slot * (uint32_t)SD_CHUNK + (uint32_t)im * SD_KBYTES, src + (size_t)im * p.rows_in * 16, (uint32_t)SD_KBYTES,
                                      bar_base + 8u * (BAR_AFULL + slot));
                         if (++slot == (uint32_t)NA) { slot = 0; par ^= 1u; round = 1; }
                     }
@@ -434,11 +314,10 @@ __global__ void __launch_bounds__((4 * ECS + SdRoles<NT, IN_SD, OUT_SD>::NLW + 2
         } else {
         // =========================== loaders: fp32 activations -> fp16 hi/lo chunk images ====================
             // A chunk image is 2 x 176 items of (row, 8 channels) = two 16-byte loads each; thread `ltid` owns the items ltid,
-            // ltid + 128, ltid + 256 of EVERY chunk.  The activations come from HBM (~1400 cycles): all six loads of a chunk are
-            // issued at once and the loads of chunk j + 1 are in flight while chunk j is converted -- a chunk per thread group
-            // with one exposed round trip each was 3.4x slower than the tensor core needs (measured).
+            // ltid + 128, ltid + 256 of EVERY chunk.  The activations come from HBM: all six loads of a chunk are issued at once
+            // and the loads of chunk j + 1 are in flight while chunk j is converted, so no chunk waits a whole exposed round trip.
             constexpr int ITEMS = (2 * SD_AROWS + SD_NL * 32 - 1) / (SD_NL * 32);      // 3
-            const int ltid = tid - NE * 32;
+            const int ltid = tid - SD_NC * 32;
             const float4 *in4 = reinterpret_cast<const float4 *>(p.in);
             float amax = 0.0f;
             float4 cur[ITEMS][2], nxt[ITEMS][2];
@@ -454,7 +333,7 @@ __global__ void __launch_bounds__((4 * ECS + SdRoles<NT, IN_SD, OUT_SD>::NLW + 2
                         const long long pr = p0 + r;
                         const int s = (int)(pr / p.rs), q = (int)(pr - (long long)s * p.rs);
                         const int yp = q / 22, xp = q - yp * 22;
-                        if (s < n_samples && (yp != 0 || !p.cyl) && !(p.dbg & 1) && !p.fa) {
+                        if (s < n_samples && (yp != 0 || !p.cyl) && !p.fa) {
                             const int xx = xp == 0 ? 19 : (xp == 21 ? 0 : xp - 1);
                             int pos = p.cyl ? (yp - 1) * 20 + xx : q, g0;       // valid rasters: the row IS the input position
                             if (p.is3d) { pos += c * 140; g0 = h * 2; } else { g0 = c * 4 + h * 2; }
@@ -528,8 +407,8 @@ __global__ void __launch_bounds__((4 * ECS + SdRoles<NT, IN_SD, OUT_SD>::NLW + 2
                             lo[e] = *reinterpret_cast<const uint32_t *>(&ll);
                             amax = fmaxf(amax, fmaxf(fabsf(xs[2 * e]), fabsf(xs[2 * e + 1])));
                         }
-                        *reinterpret_cast<uint4 *>(dst + (size_t)h * SD_KCORE + (size_t)r * 16) = make_uint4(hi[0], hi[1], hi[2], hi[3]);
-                        *reinterpret_cast<uint4 *>(dst + (size_t)(2 + h) * SD_KCORE + (size_t)r * 16) = make_uint4(lo[0], lo[1], lo[2], lo[3]);
+                        *reinterpret_cast<uint4 *>(dst + (size_t)h * SD_KBYTES + (size_t)r * 16) = make_uint4(hi[0], hi[1], hi[2], hi[3]);
+                        *reinterpret_cast<uint4 *>(dst + (size_t)(2 + h) * SD_KBYTES + (size_t)r * 16) = make_uint4(lo[0], lo[1], lo[2], lo[3]);
                     }
                 }
                 asm volatile("fence.proxy.async.shared::cta;" ::: "memory");     // generic-proxy stores -> tensor-core (async proxy) reads
@@ -541,504 +420,64 @@ __global__ void __launch_bounds__((4 * ECS + SdRoles<NT, IN_SD, OUT_SD>::NLW + 2
             }
             if (!(amax < 65000.0f) && p.flag) atomicOr(p.flag, 1);   // also true for NaN
         }
-    } else if (warp == WGT_WARP) {
+    } else {
         // =========================== weight producer ========================================================
         if (lane == 0) {
-            const int n_super = p.wchunk ? nchunks : n_stages / SB;
-            int q = 0;
+            const int n_st = nchunks * 3;
+            uint32_t q = 0;
             for (uint32_t k = 0; tile_of(k) >= 0; ++k) {
-                if (p.resident && k >= 1) break;                      // resident weights: loaded by the first tile, never again
-                for (int ss = 0; ss < n_super; ++ss, ++q) {
-                    const int sb = q % NBS;
-                    const uint32_t useb = (uint32_t)(q / NBS);
-                    if (useb > 0) mbar_wait(bar_base + 8u * (BAR_BEMPTY + sb), (useb - 1) & 1);
-                    const uint32_t bytes = (uint32_t)(p.wchunk ? 9 : SB) * (uint32_t)B_STAGE;
-                    mbar_arrive_expect_tx(bar_base + 8u * (BAR_BFULL + sb), bytes);
-                    bulk_g2s(b_base + (uint32_t)sb * bytes, reinterpret_cast<const unsigned char *>(p.w) + (size_t)ss * bytes, bytes,
-                             bar_base + 8u * (BAR_BFULL + sb));
+                if (resident && k >= 1) break;                      // resident weights: loaded by the first tile, never again
+                for (int s = 0; s < n_st; ++s, ++q) {
+                    const uint32_t sb = q % (uint32_t)NBS, use = q / (uint32_t)NBS;
+                    if (use > 0) mbar_wait(bar_base + 8u * (BAR_BEMPTY + sb), (use - 1) & 1u);
+                    mbar_arrive_expect_tx(bar_base + 8u * (BAR_BFULL + sb), (uint32_t)C::B_STAGE);
+                    bulk_g2s(b_base + sb * (uint32_t)C::B_STAGE, reinterpret_cast<const unsigned char *>(p.w) + (size_t)s * C::B_STAGE,
+                             (uint32_t)C::B_STAGE, bar_base + 8u * (BAR_BFULL + sb));
                 }
             }
         }
-        __syncwarp();
-    } else {
-        // =========================== MMA issuer =============================================================
-        // The issue loop is the critical resource of the kernel: everything is compile-time or a running counter (no
-        // divisions / modulo per stage -- a generic loop of ~100 uniform-datapath instructions per stage issued one stage per
-        // ~320 cycles, measured), the nine taps are unrolled with constant descriptor offsets, one weight barrier per
-        // three taps, one segment (= one 16-channel chunk, nine main MMAs) per accumulator set.
-        // instruction descriptor: D = F32, A = B = F16, both K-major, N = NT, M = 128
-        constexpr uint32_t IDESC = (1u << 4) | ((uint32_t)(NT >> 3) << 17) | ((uint32_t)(128 >> 4) << 24);
-        constexpr uint32_t IDESC2 = (1u << 4) | ((uint32_t)((2 * NT) >> 3) << 17) | ((uint32_t)(128 >> 4) << 24);      // N = 2 * NT
-        constexpr uint32_t DESC_HI = (128u >> 4) | (1u << 14);            // SBO = 128 B (8 rows x 16 B), descriptor version 1
-        constexpr uint32_t A_LBO = ((uint32_t)SD_KCORE >> 4) << 16;       // K-adjacent core matrices: one kcore image apart
-        constexpr uint32_t B_LBO = ((uint32_t)(2 * NT * 16) >> 4) << 16;   // weight image [kcore][split(hi,lo)][n][16 B]: K-adjacent core matrices 2*NT rows apart
-        constexpr uint32_t A_SPLIT = (2u * SD_KCORE) >> 4, B_LO16 = (uint32_t)(NT * 16) >> 4;   // hi -> lo image (A), hi -> lo rows (B), 16-byte units
-        constexpr uint32_t B_STAGE16 = (uint32_t)B_STAGE >> 4, A_CHUNK16 = (uint32_t)SD_CHUNK >> 4;
-        const uint32_t leader = elect_leader();
-        const uint32_t a0 = (a_base >> 4) | A_LBO, b0 = (b_base >> 4) | B_LBO;
-        const int Wrow = p.W;                                              // tap (g, tt) reads rows R + g * W + tt
-        const uint32_t shift_on = (p.dbg & 4) ? 0u : 1u;                   // BX_SD_DBG=4: every tap reads the unshifted (128-byte aligned) view (timing experiment)
-        uint32_t slot = 0, a_par = 0, sbq = 0, b_par = 0, seg = 0, k = 0;
-        if (p.stagger > 0) {
-            const long long ts = clock64(), wait = (long long)(blockIdx.x & 15) * p.stagger;
-            while (clock64() - ts < wait) { }
-        }
-        SD_TR_DECL;
-#ifdef BX_TC_TRACE
-        const long long tm0_ = clock64();
-#endif
-        const bool resident = p.resident != 0;
-        // look-ahead probes (mbar_test): the barrier the NEXT step needs is tested before this step's MMAs are issued
-        const uint32_t probe = (p.dbg & 8) ? 0u : 1u;         // BX_SD_DBG=8: blocking waits only (A/B switch)
-        uint32_t pa = probe & mbar_test(bar_base + 8u * (BAR_AFULL + slot), a_par), pc = 1u;
-        uint32_t pb = probe & mbar_test(bar_base + 8u * (BAR_BFULL + sbq), b_par);
-        for (; tile_of(k) >= 0; ++k) {
-            const uint32_t xset = k & 1;
-            if (!MERGED && k >= 2) {
-                SD_TR_T0();
-                mbar_wait(bar_base + 8u * (BAR_XFREE + xset), ((k >> 1) - 1) & 1);
-                SD_TR_ADD(4);
-                asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-            }
-            const uint32_t d_cross = tmem_base + (2u * NT + xset * NT);
-            const bool wait_b = !resident || k == 0;
-            const bool wchunk = p.wchunk != 0;
-            for (int c = 0; c < nchunks; ++c) {
-                const uint32_t set = seg & (uint32_t)(NSETS - 1);
-                SD_TR_T0();
-                if (!pa) mbar_wait(bar_base + 8u * (BAR_AFULL + slot), a_par);
-                SD_TR_ADD(1);
-                SD_TR_T0();
-                if (!pc) mbar_wait(bar_base + 8u * (BAR_ACCFREE + set), ((seg / NSETS) - 1) & 1);
-                SD_TR_ADD(2);
-                asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-                const uint32_t ac = a0 + slot * A_CHUNK16;
-                const uint32_t d_set = tmem_base + set * (2u * NT);      // [main | cross]
-                // the next chunk's A slot and accumulator set
-                uint32_t slot_n = slot + 1, a_par_n = a_par;
-                if (slot_n == (uint32_t)NA) { slot_n = 0; a_par_n ^= 1u; }
-                const uint32_t seg_n = seg + 1, set_n = seg_n & (uint32_t)(NSETS - 1);
-                uint32_t pa_n = 0u, pc_n = 1u;
-#pragma unroll
-                for (int g = 0; g < 3; ++g) {
-                    SD_TR_T0();
-                    if (wait_b && !pb && (!wchunk || g == 0)) mbar_wait(bar_base + 8u * (BAR_BFULL + sbq), b_par);
-                    SD_TR_ADD(3);
-                    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-                    const uint32_t bg = wchunk ? b0 + sbq * (9u * B_STAGE16) + (uint32_t)g * (3u * B_STAGE16) : b0 + sbq * (3u * B_STAGE16);
-                    uint32_t sbq_n = sbq, b_par_n = b_par;
-                    if (!wchunk || g == 2) { if (++sbq_n == (uint32_t)NBS) { sbq_n = 0; b_par_n ^= 1u; } }
-                    const uint32_t pb_n = (!wchunk || g == 2) ? (probe & mbar_test(bar_base + 8u * (BAR_BFULL + sbq_n), b_par_n)) : 1u;
-                    if (g == 2) {
-                        pa_n = probe & mbar_test(bar_base + 8u * (BAR_AFULL + slot_n), a_par_n);
-                        if (seg_n >= (uint32_t)NSETS) pc_n = probe & mbar_test(bar_base + 8u * (BAR_ACCFREE + set_n), ((seg_n / NSETS) - 1) & 1);
-                    }
-#pragma unroll
-                    for (int tt = 0; tt < 3; ++tt) {
-                        const uint32_t ah = ac + shift_on * (uint32_t)(g * Wrow + tt), al = ah + A_SPLIT;    // one row = 16 B = one address unit
-                        const uint32_t bb = bg + (uint32_t)tt * B_STAGE16;                         // rows 0..NT-1 = bh, NT..2NT-1 = bl
-                        // ah * [bh | bl] -> [main | cross] in ONE N = 2*NT instruction (the hi activations are read once for
-                        // both products), then al * bh into the cross columns
-                        if constexpr (MERGED) {
-                            mma_f16_ss(leader, d_set, ah, bb, DESC_HI, IDESC2, (g == 0 && tt == 0) ? 0u : 1u);
-                            mma_f16_ss(leader, d_set + NT, al, bb, DESC_HI, IDESC, 1u);
-                        } else {
-                            const uint32_t first = c == 0 ? 0u : 1u;
-                            if (!(p.dbg & 2)) {      // BX_SD_DBG=2: knock-out experiment (main products only)
-                            mma_f16_ss(leader, d_cross, al, bb, DESC_HI, IDESC, (g == 0 && tt == 0) ? first : 1u);
-                            mma_f16_ss(leader, d_cross, ah, bb + B_LO16, DESC_HI, IDESC, 1u);
-                            }
-                            mma_f16_ss(leader, tmem_base + set * NT, ah, bb, DESC_HI, IDESC, (g == 0 && tt == 0) ? 0u : 1u);
-                        }
-                    }
-                    if (!resident && (!wchunk || g == 2)) mma_commit(leader, bar_base + 8u * (BAR_BEMPTY + sbq));
-                    sbq = sbq_n; b_par = b_par_n; pb = pb_n;
-                }
-                mma_commit(leader, bar_base + 8u * (BAR_SEGDONE + set));
-                mma_commit(leader, bar_base + 8u * (BAR_AEMPTY + slot));     // the chunk's MMAs have read the slot
-                seg = seg_n; slot = slot_n; a_par = a_par_n; pa = pa_n; pc = pc_n;
-            }
-            if (!MERGED) mma_commit(leader, bar_base + 8u * (BAR_XDONE + xset));
-        }
-#ifdef BX_TC_TRACE
-        tr_[0] = clock64() - tm0_; SD_TR_OUT(0); SD_TR_OUT(1); SD_TR_OUT(2); SD_TR_OUT(3); SD_TR_OUT(4);
-#endif
         __syncwarp();
     }
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
     __syncthreads();
-    if (warp == MMA_WARP) {
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(TMEM_COLS) : "memory");
-    }
     if (dyn && tid == 0) {      // the last CTA to finish rewinds the counters for the next launch that uses them
         __threadfence();
         if (atomicAdd(p.tile_ctr + 1, 1) == (int)gridDim.x - 1) { p.tile_ctr[0] = 0; p.tile_ctr[1] = 0; __threadfence(); }
     }
 }
 
-// ---------------------------------------------------------------------------------------------------------------------
-// Macro-tile variant (production for the descriptor stack): TWO adjacent 128-row tiles share every weight chunk.
-// Measured on conv_sd_kernel: with only a third of the MMAs issued the 128 -> 128 layer still took 72 % of its time -- the
-// kernel is bound by what an SM can pull from L2 (~43 B/clk per SM when all 148 do), and 87 % of that was the weight image,
-// re-streamed for every 128-row tile (589 KB per tile against 90 KB of activations).  Here a weight chunk (nine taps) is
-// fetched once per 256 rows: tile u = 0 runs its 27 (18) MMAs of the chunk, then tile u = 1 runs the same taps against the
-// same shared-memory weights.  Cout 128: one main accumulator per tile (while tile 1's MMAs run the epilogue warps of tile 0
-// drain its segment, and vice versa); Cout <= 64: two [main | cross] sets per tile (their 432-864-cycle segments are shorter
-// than a drain).
-// Presplit input only (bulk-copied A chunks); 8 epilogue warps per tile, one A producer, one weight producer, one MMA warp.
-template <int NT, int OUT_SD>
-__global__ void __launch_bounds__(19 * 32, 1) conv_sd2_kernel(const ConvSdParams p) {
-    constexpr bool MERGED = NT <= 64;
-    constexpr int NEW = 8;                        // epilogue warps per tile: 4 lane quarters x 2 column halves
-    constexpr int CW = NT / 2;
-    constexpr int LDW = CW < 32 ? CW : 32;        // columns per tcgen05.ld
-    constexpr int APROD_WARP = 2 * NEW, WGT_WARP = 2 * NEW + 1, MMA_WARP = 2 * NEW + 2;
-    constexpr int B_STAGE = 64 * NT, B_CHUNK = 9 * B_STAGE;   // nine taps of [kcore][split][n][16 B]
-    constexpr int TMEM_COLS = MERGED ? 8 * NT : 4 * NT;   // MERGED: two [main | cross] sets per tile; else main[2 tiles], cross[2 tiles]
-    constexpr int MAXNA = 12;
-    constexpr int BAR_AFULL = 0, BAR_AEMPTY = MAXNA, BAR_BFULL = 2 * MAXNA, BAR_BEMPTY = BAR_BFULL + 2;
-    constexpr int NSET = MERGED ? 2 : 1;          // accumulator sets per tile (MERGED: 4 sets of [main | cross] = 8 * NT <= 512 columns)
-    constexpr int BAR_SEGDONE = BAR_BEMPTY + 2, BAR_ACCFREE = BAR_SEGDONE + 4, BAR_XDONE = BAR_ACCFREE + 4, BAR_XFREE = BAR_XDONE + 2;
-    constexpr int NBARS = BAR_XFREE + 2;
-    extern __shared__ __align__(128) unsigned char smem[];
-    __shared__ __align__(8) unsigned long long bars[NBARS];
-    __shared__ uint32_t tmem_base_s;
-    __shared__ __align__(16) float bias_s[128];        // the running sums of a tile start from the bias
-
-    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-    const int NA = p.NA, nchunks = p.nchunks;
-    const int n_samples = p.d_n ? min(*p.d_n, p.n) : p.n;
-    const int n_tiles = (int)(((long long)n_samples * p.rs + SD_BM - 1) / SD_BM);
-    const int n_macro = (n_tiles + 1) >> 1;
-
-    if (warp == MMA_WARP) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(&tmem_base_s)), "r"(TMEM_COLS) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-    if (tid == 0) {
-        for (int s = 0; s < MAXNA; ++s) {
-            mbar_init(smem_u32(&bars[BAR_AFULL + s]), 1);
-            mbar_init(smem_u32(&bars[BAR_AEMPTY + s]), 1);
-        }
-        for (int s = 0; s < 2; ++s) {
-            mbar_init(smem_u32(&bars[BAR_BFULL + s]), 1);
-            mbar_init(smem_u32(&bars[BAR_BEMPTY + s]), 1);
-            mbar_init(smem_u32(&bars[BAR_SEGDONE + s]), 1);
-            mbar_init(smem_u32(&bars[BAR_SEGDONE + 2 + s]), 1);
-            mbar_init(smem_u32(&bars[BAR_ACCFREE + s]), NEW);
-            mbar_init(smem_u32(&bars[BAR_ACCFREE + 2 + s]), NEW);
-            mbar_init(smem_u32(&bars[BAR_XDONE + s]), 1);
-            mbar_init(smem_u32(&bars[BAR_XFREE + s]), NEW);
-        }
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    }
-    if (threadIdx.x < 128) bias_s[threadIdx.x] = (int)threadIdx.x < p.Cout ? __ldg(p.bias + threadIdx.x) : 0.0f;
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-    __syncthreads();
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    uint32_t tmem_base = tmem_base_s;
-    uint32_t a_base = smem_u32(smem);
-    uint32_t b_base = a_base + (uint32_t)NA * SD_CHUNK;
-    uint32_t bar_base = smem_u32(&bars[0]);
-    asm volatile("" : "+r"(tmem_base), "+r"(a_base), "+r"(b_base), "+r"(bar_base));
-
-    if (warp < 2 * NEW) {
-        // =========================== epilogue warps of tile u ===============================================
-        const int u = warp >> 3, quarter = warp & 3, ecs = (warp >> 2) & 1;
-        const uint32_t tm_lane = (uint32_t)(quarter * 32) << 16;
-        const uint32_t d_main0 = tmem_base + tm_lane + (uint32_t)(MERGED ? u * 4 * NT : u * NT) + (uint32_t)(ecs * CW);
-        const uint32_t d_cross0 = tmem_base + tm_lane + (uint32_t)(MERGED ? u * 4 * NT + NT : 2 * NT + u * NT) + (uint32_t)(ecs * CW);
-        float run[CW];
-        uint32_t seg = 0, k = 0;
-        SD_TR_DECL;
-#ifdef BX_TC_TRACE
-        const long long te0_ = clock64();
-#endif
-        for (int m = blockIdx.x; m < n_macro; m += gridDim.x, ++k) {
-#pragma unroll
-            for (int c = 0; c < CW; c += 4) {
-                const float4 b4 = *reinterpret_cast<const float4 *>(&bias_s[ecs * CW + c]);
-                run[c] = b4.x; run[c + 1] = b4.y; run[c + 2] = b4.z; run[c + 3] = b4.w;
-            }
-            for (int c = 0; c < nchunks; ++c, ++seg) {
-                const uint32_t sp = NSET == 2 ? (seg & 1u) : 0u;                 // which of the tile's sets this segment used
-                const uint32_t bidx = (uint32_t)u * 2u + sp;
-                SD_TR_T0();
-                mbar_wait(bar_base + 8u * (BAR_SEGDONE + bidx), (NSET == 2 ? (seg >> 1) : seg) & 1u);
-                SD_TR_ADD(6);
-                asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-                const uint32_t d_main = d_main0 + sp * (2u * NT), d_cross = d_cross0 + sp * (2u * NT);
-#pragma unroll
-                for (int c0 = 0; c0 < CW; c0 += LDW) {
-                    uint32_t v[LDW];
-                    if constexpr (MERGED) {
-                        uint32_t w[LDW];
-                        tmem_ld<LDW>(d_main + (uint32_t)c0, v);
-                        tmem_ld<LDW>(d_cross + (uint32_t)c0, w);
-                        asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-#pragma unroll
-                        for (int e = 0; e < LDW; ++e) run[c0 + e] += fmaf(__uint_as_float(w[e]), 0.00048828125f, __uint_as_float(v[e]));
-                    } else {
-                        tmem_ld<LDW>(d_main + (uint32_t)c0, v);
-                        asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-#pragma unroll
-                        for (int e = 0; e < LDW; ++e) run[c0 + e] += __uint_as_float(v[e]);
-                    }
-                }
-                asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-                __syncwarp();
-                if (lane == 0) mbar_arrive(bar_base + 8u * (BAR_ACCFREE + bidx));
-            }
-            if constexpr (!MERGED) {      // the tile's cross chain: one read per tile, scaled by 2^-11
-                const uint32_t d_cross = d_cross0;
-                mbar_wait(bar_base + 8u * (BAR_XDONE + u), k & 1u);
-                asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-#pragma unroll
-                for (int c0 = 0; c0 < CW; c0 += LDW) {
-                    uint32_t w[LDW];
-                    tmem_ld<LDW>(d_cross + (uint32_t)c0, w);
-                    asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-#pragma unroll
-                    for (int e = 0; e < LDW; ++e) run[c0 + e] = fmaf(__uint_as_float(w[e]), 0.00048828125f, run[c0 + e]);
-                }
-                asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-                __syncwarp();
-                if (lane == 0) mbar_arrive(bar_base + 8u * (BAR_XFREE + u));
-            }
-            const int t = 2 * m + u;
-            SD_TR_T0();
-            if (t < n_tiles) sd_store_tile<CW, OUT_SD>(p, t, quarter, ecs, lane, n_samples, run);
-            SD_TR_ADD(7);
-        }
-#ifdef BX_TC_TRACE
-        if (warp == 0) { tr_[5] = clock64() - te0_; SD_TR_OUT(5); SD_TR_OUT(6); SD_TR_OUT(7); }
-#endif
-    } else if (warp == APROD_WARP) {
-        // =========================== A producer: chunk c of tile 0, chunk c of tile 1, chunk c + 1 of tile 0, ... ==========
-        if (lane == 0) {
-            uint32_t slot = 0, par = 0, round = 0;
-            for (int m = blockIdx.x; m < n_macro; m += gridDim.x)
-                for (int c = 0; c < nchunks; ++c)
-                    for (int u = 0; u < 2; ++u) {
-                        int t = 2 * m + u;
-                        if (t >= n_tiles) t = n_tiles - 1;       // odd tile count: the partner repeats the last tile (never stored)
-                        if (round) mbar_wait(bar_base + 8u * (BAR_AEMPTY + slot), par ^ 1u);
-                        mbar_arrive_expect_tx(bar_base + 8u * (BAR_AFULL + slot), 4u * (uint32_t)SD_KBYTES);
-                        const unsigned char *src = reinterpret_cast<const unsigned char *>(p.in_sd) + ((size_t)(c * 4) * p.rows_in + (size_t)t * SD_BM) * 16;
-#pragma unroll
-                        for (int im = 0; im < 4; ++im)
-                            bulk_g2s(a_base + slot * (uint32_t)SD_CHUNK + (uint32_t)im * SD_KCORE, src + (size_t)im * p.rows_in * 16, (uint32_t)SD_KBYTES,
-                                     bar_base + 8u * (BAR_AFULL + slot));
-                        if (++slot == (uint32_t)NA) { slot = 0; par ^= 1u; round = 1; }
-                    }
-        }
-        __syncwarp();
-    } else if (warp == WGT_WARP) {
-        // =========================== weight producer: one bulk copy per chunk (nine taps), double-buffered ===============
-        if (lane == 0) {
-            uint32_t q = 0;
-            for (int m = blockIdx.x; m < n_macro; m += gridDim.x)
-                for (int c = 0; c < nchunks; ++c, ++q) {
-                    const uint32_t sb = q & 1u;
-                    if (q >= 2) mbar_wait(bar_base + 8u * (BAR_BEMPTY + sb), ((q >> 1) - 1) & 1u);
-                    mbar_arrive_expect_tx(bar_base + 8u * (BAR_BFULL + sb), (uint32_t)B_CHUNK);
-                    bulk_g2s(b_base + sb * (uint32_t)B_CHUNK, reinterpret_cast<const unsigned char *>(p.w) + (size_t)c * B_CHUNK, (uint32_t)B_CHUNK,
-                             bar_base + 8u * (BAR_BFULL + sb));
-                }
-        }
-        __syncwarp();
-    } else {
-        // =========================== MMA issuer =============================================================
-        constexpr uint32_t IDESC = (1u << 4) | ((uint32_t)(NT >> 3) << 17) | ((uint32_t)(128 >> 4) << 24);
-        constexpr uint32_t IDESC2 = (1u << 4) | ((uint32_t)((2 * NT) >> 3) << 17) | ((uint32_t)(128 >> 4) << 24);
-        constexpr uint32_t DESC_HI = (128u >> 4) | (1u << 14);
-        constexpr uint32_t A_LBO = ((uint32_t)SD_KCORE >> 4) << 16;
-        constexpr uint32_t B_LBO = ((uint32_t)(2 * NT * 16) >> 4) << 16;
-        constexpr uint32_t A_SPLIT = (2u * SD_KCORE) >> 4, B_LO16 = (uint32_t)(NT * 16) >> 4;
-        constexpr uint32_t B_STAGE16 = (uint32_t)B_STAGE >> 4, B_CHUNK16 = (uint32_t)B_CHUNK >> 4, A_CHUNK16 = (uint32_t)SD_CHUNK >> 4;
-        const uint32_t leader = elect_leader();
-        const uint32_t a0 = (a_base >> 4) | A_LBO, b0 = (b_base >> 4) | B_LBO;
-        uint32_t slot = 0, a_par = 0, q = 0, seg = 0, k = 0;      // seg: segments finished per tile (same for both tiles)
-        SD_TR_DECL;
-#ifdef BX_TC_TRACE
-        const long long tm0_ = clock64();
-#endif
-        // look-ahead probes (mbar_test): the barriers of the NEXT step are tested before this step's MMAs are issued
-        const uint32_t probe = (p.dbg & 16) ? 1u : 0u;       // measured: the look-ahead probes do not pay here (A chunks arrive just in time: a failed probe + wait costs more)
-        uint32_t pa = probe & mbar_test(bar_base + 8u * (BAR_AFULL + slot), a_par), pc = probe;
-        uint32_t pb = probe & mbar_test(bar_base + 8u * BAR_BFULL, 0u);
-        for (int m = blockIdx.x; m < n_macro; m += gridDim.x, ++k) {
-            for (int c = 0; c < nchunks; ++c, ++q, ++seg) {
-                const uint32_t sb = q & 1u;
-                SD_TR_T0();
-                if (!pb) mbar_wait(bar_base + 8u * (BAR_BFULL + sb), (q >> 1) & 1u);
-                pb = 0u;
-                SD_TR_ADD(3);
-                const uint32_t bg = b0 + sb * B_CHUNK16;
-#pragma unroll
-                for (int u = 0; u < 2; ++u) {
-                    SD_TR_T0();
-                    if (!pa) mbar_wait(bar_base + 8u * (BAR_AFULL + slot), a_par);
-                    SD_TR_ADD(1);
-                    const uint32_t sp = NSET == 2 ? (seg & 1u) : 0u, bidx = (uint32_t)u * 2u + sp;
-                    SD_TR_T0();
-                    if (!pc && seg >= (uint32_t)NSET) mbar_wait(bar_base + 8u * (BAR_ACCFREE + bidx), (NSET == 2 ? ((seg >> 1) - 1) : (seg - 1)) & 1u);
-                    SD_TR_ADD(2);
-                    SD_TR_T0();
-                    if (!MERGED && c == 0 && k >= 1) mbar_wait(bar_base + 8u * (BAR_XFREE + u), (k - 1) & 1u);
-                    SD_TR_ADD(4);
-                    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-                    const uint32_t ac = a0 + slot * A_CHUNK16;
-                    const uint32_t d_set = tmem_base + (MERGED ? ((uint32_t)u * 2u + sp) * (2u * NT) : (uint32_t)u * NT);
-                    const uint32_t d_cross = tmem_base + (uint32_t)(2 * NT + u * NT);
-                    const uint32_t first = c == 0 ? 0u : 1u;
-                    // probes for the next (tile, chunk) step
-                    uint32_t slot_n = slot + 1, a_par_n = a_par;
-                    if (slot_n == (uint32_t)NA) { slot_n = 0; a_par_n ^= 1u; }
-                    uint32_t pa_n = 0u, pc_n = 0u;
-                    if (probe) {
-                        pa_n = mbar_test(bar_base + 8u * (BAR_AFULL + slot_n), a_par_n);
-                        const uint32_t seg_n = u == 0 ? seg : seg + 1u, u_n = u == 0 ? 1u : 0u;
-                        const uint32_t bidx_n = u_n * 2u + (NSET == 2 ? (seg_n & 1u) : 0u);
-                        pc_n = seg_n >= (uint32_t)NSET ? mbar_test(bar_base + 8u * (BAR_ACCFREE + bidx_n), (NSET == 2 ? ((seg_n >> 1) - 1) : (seg_n - 1)) & 1u) : 1u;
-                        if (u == 1) pb = mbar_test(bar_base + 8u * (BAR_BFULL + ((q + 1u) & 1u)), ((q + 1u) >> 1) & 1u);
-                    }
-#pragma unroll
-                    for (int tap = 0; tap < 9; ++tap) {
-                        const uint32_t ah = ac + (uint32_t)((tap / 3) * 22 + (tap % 3)), al = ah + A_SPLIT;
-                        const uint32_t bb = bg + (uint32_t)tap * B_STAGE16;
-                        if constexpr (MERGED) {
-                            mma_f16_ss(leader, d_set, ah, bb, DESC_HI, IDESC2, tap == 0 ? 0u : 1u);
-                            mma_f16_ss(leader, d_set + NT, al, bb, DESC_HI, IDESC, 1u);
-                        } else {
-                            mma_f16_ss(leader, d_cross, al, bb, DESC_HI, IDESC, tap == 0 ? first : 1u);
-                            mma_f16_ss(leader, d_cross, ah, bb + B_LO16, DESC_HI, IDESC, 1u);
-                            mma_f16_ss(leader, d_set, ah, bb, DESC_HI, IDESC, tap == 0 ? 0u : 1u);
-                        }
-                    }
-                    mma_commit(leader, bar_base + 8u * (BAR_SEGDONE + bidx));
-                    mma_commit(leader, bar_base + 8u * (BAR_AEMPTY + slot));
-                    if (!MERGED && c == nchunks - 1) mma_commit(leader, bar_base + 8u * (BAR_XDONE + u));
-                    slot = slot_n; a_par = a_par_n; pa = pa_n; pc = pc_n;
-                }
-                mma_commit(leader, bar_base + 8u * (BAR_BEMPTY + sb));
-            }
-        }
-#ifdef BX_TC_TRACE
-        tr_[0] = clock64() - tm0_; SD_TR_OUT(0); SD_TR_OUT(1); SD_TR_OUT(2); SD_TR_OUT(3); SD_TR_OUT(4);
-#endif
-        __syncwarp();
-    }
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-    __syncthreads();
-    if (warp == MMA_WARP) {
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(TMEM_COLS) : "memory");
-    }
-}
-
-#ifdef BX_TC_TRACE
-static void sd_trace_print(const ConvSdParams &p, const char *kern, int n_tiles, cudaStream_t st) {
-    static int want = -2, seen[32][2], nseen = 0;    // BX_SD_TRACE=1: every layer shape, at its third launch
-    if (want == -2) { const char *e = getenv("BX_SD_TRACE"); want = e ? atoi(e) : -1; }
-    if (want < 0) return;
-    const int key = p.nchunks * 1000 + p.Cout;
-    int i = 0;
-    while (i < nseen && seen[i][0] != key) ++i;
-    if (i == nseen) { if (nseen == 32) return; seen[nseen][0] = key; seen[nseen++][1] = 0; }
-    if (++seen[i][1] != 3) return;
-    cudaStreamSynchronize(st);
-    unsigned long long h[8];
-    cudaMemcpyFromSymbol(h, g_sd_trace, sizeof(h));
-    const double tiles = (n_tiles + 147) / 148, per = tiles * p.nchunks;
-    printf("[sd trace] %s nchunks %d Cout %d: per chunk-tile  MMA warp %.0f cyc = wait A %.0f + wait acc %.0f + wait W %.0f + wait cross %.0f + issue %.0f | "
-           "epilogue warp %.0f = wait seg %.0f + store %.0f + drain %.0f\n", kern, p.nchunks, p.Cout, h[0] / per, h[1] / per, h[2] / per, h[3] / per, h[4] / per,
-           (h[0] - h[1] - h[2] - h[3] - h[4]) / per, h[5] / per, h[6] / per, h[7] / per, (h[5] - h[6] - h[7]) / per);
-    fflush(stdout);
-}
-#else
-static inline void sd_trace_print(const ConvSdParams &, const char *, int, cudaStream_t) {}
-#endif
-
-template <int NT, int OUT_SD>
-int launch_sd2(ConvSdParams p, cudaStream_t st) {
-    constexpr int B_RING = 2 * 9 * 64 * NT;
-    int na = (227 * 1024 - 1024 - B_RING) / SD_CHUNK;
-    if (na > 12) na = 12;
-    { static int cap = -1; if (cap < 0) { const char *e = getenv("BX_SD_NA"); cap = e ? atoi(e) : 0; } if (cap >= 2 && na > cap) na = cap; }
-    na &= ~1;                                   // chunks alternate between the two tiles
-    p.NA = na;
-    const int smem = na * SD_CHUNK + B_RING;
-    static BxPerDevice attr = {};
-    if (bx_needs_attr(attr, (size_t)smem))
-        BX_CUDA(cudaFuncSetAttribute(conv_sd2_kernel<NT, OUT_SD>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-    int sms = bx_device_sm_count();
-    if (sms <= 0) sms = 148;
-    const int n_macro = (p.n_tiles + 1) / 2;
-    const int grid = n_macro < sms ? n_macro : sms;
-    conv_sd2_kernel<NT, OUT_SD><<<grid, 19 * 32, smem, st>>>(p);
-    BX_LAUNCH_CHECK();
-    sd_trace_print(p, "conv_sd2", p.n_tiles, st);
-    return BX_OK;
-}
-
-int g_sd_stage_sync = -1;      // -1: follow BX_SD_STAGE_SYNC
-
-template <int NT, int ECS, int IN_SD, int OUT_SD>
+template <int NT, int IN_SD, int OUT_SD>
 int launch_sd(ConvSdParams p, cudaStream_t st) {
-    { static int env = -1; if (env < 0) { const char *e = getenv("BX_SD_STAGE_SYNC"); env = e ? atoi(e) : 0; } p.stage_sync = g_sd_stage_sync >= 0 ? g_sd_stage_sync : env; }
-    // the whole weight image resident in shared memory when it leaves room for >= 6 A chunks (Cin * Cout <= 64 * 64: 144 KB),
-    // else a ring of SdRing<NT>::NBS super-stages of three taps
-    constexpr int B_SUPER = SdRing<NT>::SB * 64 * NT;
-    static int res_mode = -1;      // BX_SD_RESIDENT=0 disables (A/B switch)
-    if (res_mode < 0) { const char *e = getenv("BX_SD_RESIDENT"); res_mode = e ? atoi(e) : 1; }
-    const int n_super = p.nchunks * 3;
-    constexpr int STAGE_BYTES = SdRoles<NT, IN_SD, OUT_SD>::STAGED ? NT * SD_BM * 4 : 0;
-    p.resident = res_mode && n_super <= SD_MAXNBS && (227 * 1024 - 2048 - STAGE_BYTES - n_super * B_SUPER) / SD_CHUNK >= 4;
-    p.nbs = p.resident ? n_super : (SdRing<NT>::NBS < SD_MAXNBS ? SdRing<NT>::NBS : SD_MAXNBS);
-    while (!p.resident && p.nbs > 3 && (227 * 1024 - 2048 - STAGE_BYTES - p.nbs * B_SUPER) / SD_CHUNK < 4) --p.nbs;   // leave room for four A chunks
-    // streamed weights of the narrow layers: whole-chunk stages (one 36 KB copy and one barrier per chunk instead of three of 12 KB)
-    static int wc_mode = -1;
-    if (wc_mode < 0) { const char *e = getenv("BX_SD_WCHUNK"); wc_mode = e ? atoi(e) : 1; }
-    p.wchunk = wc_mode && !p.resident && NT <= 64;
-    if (p.wchunk) { p.nbs /= 3; if (p.nbs > 4) p.nbs = 4; if (p.nbs < 2) p.nbs = 2; }
-    { static int stg = -1; if (stg < 0) { const char *e = getenv("BX_SD_STAGGER"); stg = e ? atoi(e) : 0; } p.stagger = stg; }
-    const int B_RING = p.nbs * B_SUPER * (p.wchunk ? 3 : 1);
-    int na = 2 * p.nchunks;
-    const int na_max = (227 * 1024 - 2048 - STAGE_BYTES - B_RING) / SD_CHUNK;
-    if (na > na_max) na = na_max;
-    if (na > 12) na = 12;
-    { static int cap = -1; if (cap < 0) { const char *e = getenv("BX_SD_NA"); cap = e ? atoi(e) : 0; } if (cap >= 2 && na > cap) na = cap; }
+    using C = SdCfg<NT, IN_SD>;
+    // the whole weight image resident in shared memory when it leaves room for three A chunks, else a ring of six stages
+    // (two chunks) or as many as leave room for four A chunks
+    const int budget = SD_SMEM - C::STAGE_BYTES, n_st = p.nchunks * 3;
+    p.resident = n_st <= SD_MAXNBS && budget - n_st * C::B_STAGE >= 3 * SD_CHUNK;
+    p.nbs = p.resident ? n_st : 6;
+    while (!p.resident && p.nbs > 3 && budget - p.nbs * C::B_STAGE < 4 * SD_CHUNK) --p.nbs;
+    int na = (budget - p.nbs * C::B_STAGE) / SD_CHUNK;
+    if (na > 2 * p.nchunks) na = 2 * p.nchunks;
+    if (na > SD_MAXNA) na = SD_MAXNA;
+    BX_REQUIRE(na >= 2, "bx_conv_layer_sd: no room for the activation ring");
     p.NA = na;
-    const int smem = na * SD_CHUNK + B_RING + STAGE_BYTES;
+    const int smem = na * SD_CHUNK + p.nbs * C::B_STAGE + C::STAGE_BYTES;
     static BxPerDevice attr = {};
     if (bx_needs_attr(attr, (size_t)smem))
-        BX_CUDA(cudaFuncSetAttribute(conv_sd_kernel<NT, ECS, IN_SD, OUT_SD>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+        BX_CUDA(cudaFuncSetAttribute(conv_sd_kernel<NT, IN_SD, OUT_SD>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
     int sms = bx_device_sm_count();
-    if (sms <= 0) sms = 148;
-    { static int gcap = -1; if (gcap < 0) { const char *e = getenv("BX_SD_GRID"); gcap = e ? atoi(e) : 0; } if (gcap > 0 && sms > gcap) sms = gcap; }   // experiment
+    if (sms <= 0) sms = 132;
     const int grid = p.n_tiles < sms ? p.n_tiles : sms;
-    conv_sd_kernel<NT, ECS, IN_SD, OUT_SD><<<grid, (4 * ECS + SdRoles<NT, IN_SD, OUT_SD>::NLW + 2) * 32, smem, st>>>(p);
+    conv_sd_kernel<NT, IN_SD, OUT_SD><<<grid, C::THREADS, smem, st>>>(p);
     BX_LAUNCH_CHECK();
-    sd_trace_print(p, "conv_sd", p.n_tiles, st);
     return BX_OK;
 }
 
-template <int NT, int ECS>
+template <int NT>
 int dispatch_sd(const ConvSdParams &p, int in_sd, int out_sd, cudaStream_t st) {
-    if (in_sd) return out_sd ? launch_sd<NT, ECS, 1, 1>(p, st) : launch_sd<NT, ECS, 1, 0>(p, st);
-    return out_sd ? launch_sd<NT, ECS, 0, 1>(p, st) : launch_sd<NT, ECS, 0, 0>(p, st);
+    if (in_sd) return out_sd ? launch_sd<NT, 1, 1>(p, st) : launch_sd<NT, 1, 0>(p, st);
+    return out_sd ? launch_sd<NT, 0, 1>(p, st) : launch_sd<NT, 0, 0>(p, st);
 }
 
 }  // namespace
-
-// Staging hand-over between the epilogue and the storer warps of conv_sd_kernel: 0 = mbarriers (production), 1 = named barriers
-// (bar.arrive / bar.sync: the form compute-sanitizer racecheck models; bit-identical results), -1 = follow BX_SD_STAGE_SYNC.
-// Returns the previous value.
-BX_API int bx_conv_sd_set_stage_sync(int mode) {
-    const int old = g_sd_stage_sync;
-    g_sd_stage_sync = mode;
-    return old;
-}
 
 // rows of a presplit activation image: n samples of rows_per_sample raster rows (176 for the cylindrical layers: 8 x 22),
 // rounded to whole 128-row tiles, + the 48-row halo a tile's operand fetch reaches past its last row
@@ -1076,27 +515,15 @@ BX_API int bx_conv_layer_sd(int geom, const void *in, int in_presplit, const voi
         p.rs = D * W; p.W = W; p.OD = D - 2; p.OW = W - 2; p.S_out = p.OD * p.OW; p.rs_out = p.S_out;
         p.S_in = D * W;
     }
-    { static int dbg = -1; if (dbg < 0) { const char *e = getenv("BX_SD_DBG"); dbg = e ? atoi(e) : 0; } p.dbg = dbg; }
     const long long rows = (long long)n * p.rs;
     BX_REQUIRE(rows + 4 * SD_BM < 0x7fffffffLL, "bx_conv_layer_sd: too many samples (raster rows must stay below 2^31)");
     p.n_tiles = (int)((rows + SD_BM - 1) / SD_BM);
     p.rows_in = bx_conv_sd_rows(n, p.rs);
     p.rows_out = bx_conv_sd_rows(n, p.rs_out);
     cudaStream_t st = bx_stream(stream);
-    static int macro = -1;       // BX_SD_MACRO=0: one 128-row tile per weight pass everywhere (A/B switch, experiments)
-    if (macro < 0) { const char *e = getenv("BX_SD_MACRO"); macro = e ? atoi(e) : 0; }
-    // Two tiles per weight chunk (conv_sd2_kernel) where it measured faster at K = 9000 patches: 128->128 (1019 -> 980 us) and
-    // Cout 32 (64->32: 219 -> 190 us, 32->32: 120 -> 98 us).  64->128 (560 vs 572 us) and the Cout 64 layers (305 vs 323 us, with
-    // two accumulator sets per tile) are not: their weight stream is small against the per-tile costs.  BX_SD_MACRO=2 forces
-    // the macro-tile kernel everywhere, 0 disables it.
-    if (macro && p.cyl && in_presplit && p.n_tiles >= 2) {
-        if (Cout > 64) { if (macro >= 2 || p.nchunks >= 8) return out_presplit ? launch_sd2<128, 1>(p, st) : launch_sd2<128, 0>(p, st); }
-        else if (Cout > 32) { if (macro >= 2) return out_presplit ? launch_sd2<64, 1>(p, st) : launch_sd2<64, 0>(p, st); }
-        else return out_presplit ? launch_sd2<32, 1>(p, st) : launch_sd2<32, 0>(p, st);
-    }
-    if (Cout > 64) return dispatch_sd<128, 2>(p, in_presplit, out_presplit, st);
-    if (Cout > 32) return dispatch_sd<64, 2>(p, in_presplit, out_presplit, st);
-    return dispatch_sd<32, 1>(p, in_presplit, out_presplit, st);
+    if (Cout > 64) return dispatch_sd<128>(p, in_presplit, out_presplit, st);
+    if (Cout > 32) return dispatch_sd<64>(p, in_presplit, out_presplit, st);
+    return dispatch_sd<32>(p, in_presplit, out_presplit, st);
 }
 
 /* Second CostNet layer on the shifted-descriptor kernel: conv 32 -> 64, k = 3x3x3 over the regenerated first activation
@@ -1118,9 +545,8 @@ BX_API int bx_conv_layer_sd_costab(const float *fa, const float *fb, const void 
     p.n = n; p.Cout = 64; p.relu = relu;
     p.is3d = 0; p.cyl = 0; p.nchunks = 6; p.G_in = 8;
     p.rs = 324; p.W = 18; p.OD = 16; p.OW = 16; p.S_out = 256; p.rs_out = 256; p.S_in = 324;
-    p.dbg = 0;
     p.n_tiles = (int)(((long long)n * p.rs + SD_BM - 1) / SD_BM);
     p.rows_in = bx_conv_sd_rows(n, p.rs);
     p.rows_out = bx_conv_sd_rows(n, p.rs_out);
-    return dispatch_sd<64, 2>(p, 0, out_presplit, bx_stream(stream));
+    return dispatch_sd<64>(p, 0, out_presplit, bx_stream(stream));
 }

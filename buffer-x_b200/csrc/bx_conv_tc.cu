@@ -1,43 +1,29 @@
-// bx_conv_tc.cu -- a8/a11 convolution stacks on the 5th-generation tensor cores (tcgen05 + TMEM).
+// bx_conv_tc.cu -- a8/a11 convolution stacks on the Hopper tensor cores (wgmma, TF32 operands).
 //
 // Same implicit GEMM as bx_conv.cu (rows = (sample, output position), cols = Cout, K = taps*Cin, padding
-// geometry folded into the loader), but the inner product runs as tcgen05.mma kind::tf32 with fp32
-// accumulators in tensor memory.  fp32-grade accuracy (descriptor parity 1e-4 rel) needs two things:
-//   1. the 3xTF32 split  x = hi + lo  (hi = x with the 13 low mantissa bits cleared -- the tensor core ignores them,
-//      so the hi operand is x itself -- lo = x - hi, exact):
+// geometry folded into the loader), but the inner product runs as wgmma .tf32 with fp32 accumulators in registers.
+// fp32-grade accuracy (descriptor parity 1e-4 rel) needs two things:
+//   1. the 3xTF32 split  x = hi + lo  (hi = x with the 13 low mantissa bits cleared, lo = x - hi, exact):
 //          a*b ~= ah*bh + ah*bl + al*bh          (dropped al*bl ~ 2^-20 relative)
-//   2. short accumulation chains: the tensor core accumulates with truncation, so the error of a chain grows
-//      linearly with its length (measured on B200, K = 1152: 5x the fp32-FFMA error for one chain, below it
-//      for chains of 12 MMAs; tools/tc_precision.py).  The ah*bh products therefore go to a PING-PONG pair
-//      of TMEM accumulators that is cut every seg_len stages (default 6 = 12 MMAs); finished segments are added with
-//      round-to-nearest into fp32 running sums held in the loader threads' registers while the tensor core
-//      already fills the other accumulator.  The cross terms (2^-11 smaller) keep one long chain.
+//   2. short accumulation chains: the tensor core does not round its internal accumulation to nearest, so the error of a
+//      chain grows with its length.  The products of seg_len stages (default 4 = 24 MMAs) go to a fresh accumulator that
+//      is then added with round-to-nearest into fp32 running sums (tools/tc_precision.py measures the effect of seg_len).
 //
-// Warp-specialised CTA (LG*128 + 64 threads, 128 GEMM rows = one M=128 tile, N = NT columns):
-//   loader warps  LG groups of four warps; group g owns the stages it = g, g+LG, ... so a warp touches a barrier once
-//               per LG stages.  thread -> row = t & 127.  Per owned stage (16 input channels of one tap; chunk-outer /
-//               tap-inner order keeps a chunk's activations in L1 across its taps; tap geometry from a shared table)
-//               a thread fetches its row's 16 activations with four 16-byte loads (channel-blocked activations
-//               [n][C/4][position][4]), splits them and writes hi/lo with tcgen05.st (32x32b.x8) into the A ring in
-//               TENSOR MEMORY (4 stages x 32 columns: [kstep][hi,lo][8 values]); the MMAs read A from TMEM (TS
-//               form), which takes the activation operand off the shared-memory read port -- with A in shared
-//               memory the kernel was bound by smem bandwidth (3 MMAs re-read the same 128x8 tile).
-//               Every seg_len stages each loader warp drains its 32 lanes x NT/LG columns of the finished main
-//               accumulator (tcgen05.ld) into its running sums and releases the accumulator (accfree barrier).
-//   weight warp   streams the host-arranged B (weight) images
+// Warp-specialised CTA (416 threads, 128 GEMM rows = one tile, N = NT columns):
+//   loader warps  four warps, thread -> row.  Per stage (16 input channels of one tap; chunk-outer / tap-inner order keeps a
+//               chunk's activations in L1 across its taps; tap geometry from a shared table) a thread fetches its row's 16
+//               activations with four 16-byte loads (channel-blocked activations [n][C/4][position][4]), splits them and
+//               writes hi / lo into the A ring in shared memory, the canonical K-major no-swizzle image
+//               [split][kq(4)][row(128)][4 x fp32] (LBO = one kq image = 2 KB, SBO = 128 B).
+//   weight thread streams the host-arranged B (weight) images
 //                   [kstep][split][kunit][n(NT)][16 B]      K-major no-swizzle, LBO = NT*16 B, SBO = 128 B
-//               through a shared-memory ring with cp.async.bulk + mbarrier transaction counts, 8-12 stages AHEAD of
-//               the tensor core and independent of the A slots (the weights never touch registers and their L2
-//               latency is off the slot turnaround path).
-//   MMA warp      waits a_full[stage] (and b_full once per weight super-stage), issues 6 tcgen05.mma
-//               (2 k-steps x {al*bh, ah*bl, ah*bh}), tcgen05.commit -> a_empty / b_empty; no __syncthreads in the
-//               main loop.
-//   epilogue    running sums (+ cross accumulator) + bias (+ReLU) -> 16-byte channel-blocked stores.
-// Configurations (dispatch_nt): Cout 128 -> LG=4, ping-pong main + separate cross accumulator, 1 CTA/SM;
-// Cout 64 -> LG=2, ping-pong accumulators that also take the cross terms (segments of 4 stages), 2 CTAs/SM;
-// Cout <= 32 -> LG=2, ping-pong + separate cross, 2 CTAs/SM.  -DBX_TC_TRACE adds a clock64 stage timeline.
+//               through a shared-memory ring with cp.async.bulk + mbarrier transaction counts, up to TC_NBS stages ahead.
+//   2 MMA warpgroups  warpgroup g owns tile rows 64 g .. 64 g + 63: per stage 6 wgmmas (2 k-steps x {al*bh, ah*bl, ah*bh},
+//               small terms first); a stage's slots are released once the NEXT stage's MMAs are in flight (wgmma.wait_group 1),
+//               every seg_len stages the accumulators are folded into the running sums; epilogue: bias (+ReLU) ->
+//               channel-blocked stores.
 #include "bx_common.cuh"
-#include "bx_tcgen05.cuh"
+#include "bx_wgmma.cuh"
 
 namespace {
 
@@ -48,63 +34,38 @@ struct ConvTcParams {
     const int *d_n;
     int Cin, Cout, D, H, W, kd, kh, kw, relu;
     int S_in, S_out, OD, OH, OW, T;
-    int seg_len;  // stages per main-accumulator segment
-    long long *trace;   // -DBX_TC_TRACE builds only: clock64 stamps of one CTA
+    int seg_len;  // stages per accumulator segment
     const float *equi_s, *equi_t;
     const int *s_mids, *t_mids;
 };
 
 constexpr int TC_BM = 128;
-constexpr int TC_STAGES = 4;      // A ring (tensor memory)
-// B ring (shared memory): weights are prefetched independently of the A slots, TC_SB stages per bulk copy and per
-// barrier ("super-stage"), TC_NBS super-stages.  Narrow layers: 4 x 3 (one mbarrier wait per four stages -- the MMA
-// warp's per-stage latency is what bounds them); wide layers: 1 x 8.
-template <int NT> struct BRing { static constexpr int SB = NT == 128 ? 1 : 4, NBS = NT == 128 ? 8 : 3; };
+constexpr int TC_STAGES = 4;              // A ring (shared memory)
+constexpr int TC_NBS = 8;                 // B ring: weights are prefetched independently of the A slots
 constexpr int TC_MAX_TAPS = 128;
-constexpr int A_STAGE_COLS = 32;  // TMEM columns of one A stage: [kstep(2)][split(hi,lo)][8 tf32 values]
+constexpr int TC_NC = 8, TC_NL = 4;       // MMA warps (two warpgroups), loader warps
+constexpr int TC_THREADS = (TC_NC + TC_NL + 1) * 32;
+constexpr int TC_AIMG = TC_BM * 64;       // one split of an A stage: [kq(4)][row(128)][4 x fp32] = 8 KB
+constexpr int TC_ASTAGE = 2 * TC_AIMG;
 
-// LG = loader groups of 4 warps (group g fills the stages it = g, g+LG, ...); NSETS = main accumulators (2 = ping-pong,
-// 1 = the tensor core waits for the drain).  Wide layers (NT = 128) run LG = 4, NSETS = 2, one CTA per SM (384 of the 512
-// TMEM columns).  Narrow layers (NT <= 64) are dominated by per-tile latencies (pipeline fill, drains, epilogue), not
-// by tensor time, so they run LG = 2 (288 threads) with at most 256 TMEM columns: TWO CTAs per SM overlap one tile's
-// prologue / drain bubbles / epilogue with the other tile's MMAs.
-template <int GEOM, int NT, int LG, int NSETS, int MINB, int XSEP>
-__global__ void __launch_bounds__(LG * 128 + 64, MINB) conv_tc_kernel(const ConvTcParams p) {
-    constexpr int TC_LOADERS = LG * 128;
-    constexpr int MMA_WARP = LG * 4;
-    constexpr int WGT_WARP = LG * 4 + 1;   // weight producer: streams the B images through the shared-memory ring
-    constexpr int TC_SB = BRing<NT>::SB, TC_NBS = BRing<NT>::NBS, TC_BSTAGES = TC_SB * TC_NBS;
-    constexpr int B_STAGE_BYTES = 2 * 2 * 2 * NT * 16;  // [kstep][split][kunit][n][16B]
-    constexpr int STAGE_BYTES = B_STAGE_BYTES;      // shared memory holds only the weights; A lives in tensor memory
-    constexpr int A_RING = (NSETS + XSEP) * NT;     // TMEM columns: main[0..NSETS), [cross], then the A ring
-    constexpr int TMEM_NEED = A_RING + TC_STAGES * A_STAGE_COLS;
-    constexpr int TMEM_COLS = TMEM_NEED <= 256 ? 256 : 512;
-    static_assert(MINB == 1 || TMEM_NEED <= 256, "two CTAs per SM need <= 256 TMEM columns each");
-    constexpr int CW = NT / LG;         // accumulator columns owned by one loader warp
-    // barriers: full[ST] (4 loader-warp arrivals + 1 expect_tx arrival), empty[ST], segdone[2], accfree[2]
-    constexpr int BAR_EMPTY = TC_STAGES, BAR_SEGDONE = 2 * TC_STAGES, BAR_ACCFREE = 2 * TC_STAGES + 2;
-    constexpr int BAR_BFULL = 2 * TC_STAGES + 4, BAR_BEMPTY = BAR_BFULL + TC_NBS;
+template <int NT> constexpr int tc_smem() { return TC_STAGES * TC_ASTAGE + TC_NBS * (2 * 2 * 2 * NT * 16); }
+
+template <int GEOM, int NT>
+__global__ void __launch_bounds__(TC_THREADS, 1) conv_tc_kernel(const ConvTcParams p) {
+    constexpr int B_STAGE = 2 * 2 * 2 * NT * 16;  // [kstep][split][kunit][n][16B]
+    constexpr int BAR_AEMPTY = TC_STAGES, BAR_BFULL = 2 * TC_STAGES, BAR_BEMPTY = BAR_BFULL + TC_NBS;
     extern __shared__ __align__(128) unsigned char smem[];
-    __shared__ __align__(8) unsigned long long bars[2 * TC_STAGES + 4 + 2 * TC_NBS];
-    __shared__ uint32_t tmem_base_s;
+    __shared__ __align__(8) unsigned long long bars[2 * TC_STAGES + 2 * TC_NBS];
     __shared__ int4 tap_tab[TC_MAX_TAPS];
 
     const int n_samples = p.d_n ? *p.d_n : p.n;
     const long long Mtotal = (long long)n_samples * p.S_out;
     const long long row0 = (long long)blockIdx.x * TC_BM;
-    if (row0 >= Mtotal) return;  // uniform per CTA, before any barrier / TMEM allocation
-    const int tid = threadIdx.x, warp = tid >> 5;
-#ifdef BX_TC_TRACE
-    if (p.trace && blockIdx.x == gridDim.x / 2 && tid == 0) p.trace[4000] = clock64();   // CTA start
-#endif
+    if (row0 >= Mtotal) return;  // uniform per CTA, before any barrier
+    const int tid = threadIdx.x;
+    const int warp = __shfl_sync(0xffffffffu, tid >> 5, 0);       // warp-uniform role index (keeps the wgmma issue convergent)
     const int n_iters = (p.Cin / 16) * p.T;  // stage = (16-channel chunk, tap); chunk outer, tap inner
-    const int G = XSEP ? p.seg_len : (p.seg_len < 4 ? p.seg_len : 4);   // merged cross terms: 6 MMAs per stage in one chain
-    const int nseg = (n_iters + G - 1) / G;
 
-    if (warp == MMA_WARP) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(&tmem_base_s)), "r"(TMEM_COLS) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
     if (tid < p.T) {   // tap geometry table: no counter arithmetic in the loader loop
         const int dz = tid / (p.kh * p.kw), r = tid - dz * (p.kh * p.kw), dy = r / p.kw, dx = r - dy * p.kw;
         int base = 0;
@@ -114,32 +75,24 @@ __global__ void __launch_bounds__(LG * 128 + 64, MINB) conv_tc_kernel(const Conv
     }
     if (tid == 0) {
         for (int s = 0; s < TC_STAGES; ++s) {
-            mbar_init(smem_u32(&bars[s]), 4);                // A full: the 4 warps of the owning group
-            mbar_init(smem_u32(&bars[BAR_EMPTY + s]), 1);
+            mbar_init(smem_u32(&bars[s]), TC_NL);            // A full: the four loader warps
+            mbar_init(smem_u32(&bars[BAR_AEMPTY + s]), TC_NC);
         }
         for (int s = 0; s < TC_NBS; ++s) {
             mbar_init(smem_u32(&bars[BAR_BFULL + s]), 1);    // B full: the producer's expect_tx arrival + the bulk copy's bytes
-            mbar_init(smem_u32(&bars[BAR_BEMPTY + s]), 1);
-        }
-        for (int s = 0; s < 2; ++s) {
-            mbar_init(smem_u32(&bars[BAR_SEGDONE + s]), 1);
-            mbar_init(smem_u32(&bars[BAR_ACCFREE + s]), TC_LOADERS / 32);
+            mbar_init(smem_u32(&bars[BAR_BEMPTY + s]), TC_NC);
         }
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
     __syncthreads();
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    uint32_t tmem_base = tmem_base_s;
-    uint32_t smem_base = smem_u32(smem);
+    uint32_t a_base = smem_u32(smem);
+    uint32_t b_base = a_base + (uint32_t)(TC_STAGES * TC_ASTAGE);
     uint32_t bar_base = smem_u32(&bars[0]);
-    // opaque to the compiler: keep the three bases in registers instead of re-deriving the shared-window address
-    // (S2R SR_CgaCtaId + LEA chains) in front of every barrier operation of the loader loop
-    asm volatile("" : "+r"(tmem_base), "+r"(smem_base), "+r"(bar_base));
+    asm volatile("" : "+r"(a_base), "+r"(b_base), "+r"(bar_base));
 
-    if (warp < MMA_WARP) {
+    if (warp >= TC_NC && warp < TC_NC + TC_NL) {
         // =========================== loaders ===========================================================
-        const int row = tid & 127, grp = tid >> 7;       // grp: which stages (it % LG == grp) this thread fills
+        const int row = tid - TC_NC * 32;
         const long long lm = row0 + row;
         const bool lvalid = lm < Mtotal;
         int ln = 0, oz = 0, oy = 0, ox = 0;
@@ -169,12 +122,8 @@ __global__ void __launch_bounds__(LG * 128 + 64, MINB) conv_tc_kernel(const Conv
             pa = p.in + (size_t)ln * p.S_in * p.Cin;      // activations are channel-blocked: [n][Cin/4][position][4]
         }
         constexpr int cstride = 140;   // channel-first equivariant maps of the direct cost-volume loader
-        // (chunk, tap) of the stage this group fills next; the tap geometry comes from the shared table
-        int chunk = grp / p.T, t = grp - chunk * p.T;
-        auto advance_lg = [&]() {
-            t += LG;
-            while (t >= p.T) { t -= p.T; ++chunk; }
-        };
+        // (chunk, tap) of the stage filled next; the tap geometry comes from the shared table
+        int chunk = 0, t = 0;
         const int oy20 = oy * 20;
         const int rowbase = (oz * p.H + oy) * p.W + ox;   // VALID3D
         float a_reg[16];
@@ -233,264 +182,153 @@ __global__ void __launch_bounds__(LG * 128 + 64, MINB) conv_tc_kernel(const Conv
                 }
             }
         };
-        const uint32_t a_lane = (uint32_t)((warp & 3) * 32) << 16;   // this warp's TMEM lanes = its 32 GEMM rows
-        // registers -> tensor memory: [kstep][hi,lo][8].  The hi operand is the fp32 value itself: kind::tf32 reads only the
-        // upper 19 bits of a 32-bit operand (truncation -- verified by the 2e-5 layer tests, which fail if the hardware
-        // rounded), so x and (x & 0xFFFFE000) are the same operand and lo = x - (x & 0xFFFFE000) stays exact.
+        // registers -> shared memory: hi = x with the low 13 mantissa bits cleared, lo = x - hi (exact)
         auto store_stage = [&](int s) {
+            unsigned char *dst = smem + (size_t)s * TC_ASTAGE + (size_t)row * 16;
 #pragma unroll
-            for (int ks = 0; ks < 2; ++ks) {
-                float xr[8], lo[8];
+            for (int kq = 0; kq < 4; ++kq) {
+                float hi[4], lo[4];
 #pragma unroll
-                for (int j = 0; j < 8; ++j) {
-                    xr[j] = a_reg[ks * 8 + j];
-                    lo[j] = xr[j] - __uint_as_float(__float_as_uint(xr[j]) & 0xFFFFE000u);
+                for (int j = 0; j < 4; ++j) {
+                    hi[j] = __uint_as_float(__float_as_uint(a_reg[kq * 4 + j]) & 0xFFFFE000u);
+                    lo[j] = a_reg[kq * 4 + j] - hi[j];
                 }
-                const uint32_t col = (uint32_t)(A_RING + s * A_STAGE_COLS + ks * 16);
-                tmem_st8(tmem_base + a_lane + col, xr);
-                tmem_st8(tmem_base + a_lane + col + 8, lo);
+                *reinterpret_cast<float4 *>(dst + (size_t)kq * TC_BM * 16) = make_float4(hi[0], hi[1], hi[2], hi[3]);
+                *reinterpret_cast<float4 *>(dst + TC_AIMG + (size_t)kq * TC_BM * 16) = make_float4(lo[0], lo[1], lo[2], lo[3]);
             }
         };
-
-        // ---- accumulator ownership of this warp: TMEM lanes 32*(warp&3).., columns CW*(warp>>2).. ----------
-        const int eq = warp & 3, ecs = warp >> 2;
-        const uint32_t tm_lane = (uint32_t)(eq * 32) << 16;
-        float run[CW];
-#pragma unroll
-        for (int j = 0; j < CW; ++j) run[j] = 0.0f;
-        auto drain = [&](int j, bool release) {       // add finished segment j (main set j&1) into the running sums
-            const int set = j % NSETS;
-            mbar_wait(bar_base + 8u * (BAR_SEGDONE + set), (uint32_t)((j / NSETS) & 1));
-            asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-            uint32_t v[CW];
-            tmem_ld<CW>(tmem_base + tm_lane + (uint32_t)(set * NT + ecs * CW), v);
-            asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-#pragma unroll
-            for (int c = 0; c < CW; ++c) run[c] += __uint_as_float(v[c]);
-            if (release) {
-                asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-                __syncwarp();
-                if ((tid & 31) == 0) mbar_arrive(bar_base + 8u * (BAR_ACCFREE + set));
-            }
-        };
-
-        if (grp < n_iters) load_stage();
-        int next_drain = 0;
-#ifdef BX_TC_TRACE
-        const bool tr = p.trace && blockIdx.x == gridDim.x / 2 && (tid & 127) == 0;
-        long long *tb = p.trace + (size_t)grp * 3 * 64;
-        int trk = 0;
-#endif
-        for (int it = grp; it < n_iters; it += LG) {
-#ifdef BX_TC_TRACE
-            if (tr && trk < 64) tb[trk * 3 + 0] = clock64();
-#endif
-            if (next_drain < nseg - 1 && it >= (next_drain + 1) * G + (G < TC_STAGES ? G : TC_STAGES)) {
-                drain(next_drain, true);                  // its MMAs are several stages behind us: short wait
-                ++next_drain;
-            }
+        load_stage();
+        for (int it = 0; it < n_iters; ++it) {
             const int s = it % TC_STAGES;
-            const uint32_t use = (uint32_t)(it / TC_STAGES);   // how many times slot s has been filled before
-            if (use > 0) mbar_wait(bar_base + 8u * (BAR_EMPTY + s), (use - 1) & 1);  // tensor core has read the slot
-#ifdef BX_TC_TRACE
-            if (tr && trk < 64) tb[trk * 3 + 1] = clock64();
-#endif
-            store_stage(s);                               // tcgen05.st issued (sources are read at issue) ...
-            if (it + LG < n_iters) {                      // ... this group's next activations go in flight behind them ...
-                advance_lg();
+            if (it >= TC_STAGES) mbar_wait(bar_base + 8u * (BAR_AEMPTY + s), (uint32_t)((it / TC_STAGES - 1) & 1));   // the MMAs have read the slot
+            store_stage(s);
+            if (it + 1 < n_iters) {                       // the next stage's activations go in flight behind the stores
+                if (++t == p.T) { t = 0; ++chunk; }
                 load_stage();
             }
-            asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory");      // ... and only then wait for the stores
-            asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");  // tcgen05.st ordered before the arrive
+            asm volatile("fence.proxy.async.shared::cta;" ::: "memory");     // generic-proxy stores -> tensor-core (async proxy) reads
             __syncwarp();
             if ((tid & 31) == 0) mbar_arrive(bar_base + 8u * s);
-#ifdef BX_TC_TRACE
-            if (tr && trk < 64) { tb[trk * 3 + 2] = clock64(); ++trk; }
-#endif
         }
-#ifdef BX_TC_TRACE
-        if (tr) p.trace[4002] = clock64();               // loader group: main loop done
-#endif
-        while (next_drain < nseg) {                      // a set must still be released if a later segment reuses it
-            drain(next_drain, next_drain + NSETS < nseg);
-            ++next_drain;
-        }
-        // ---- epilogue: running sums + cross accumulator + bias (+ReLU) ------------------------------------
-        {
-            uint32_t u[CW];
-            if (XSEP) {
-                tmem_ld<CW>(tmem_base + tm_lane + (uint32_t)(NSETS * NT + ecs * CW), u);
-                asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-            } else {
+    } else if (warp < TC_NC) {
+        // =========================== MMA warpgroups ======================================================
+        const int lane = tid & 31, wg = warp >> 2;
+        const int r0 = wg * 64 + (warp & 3) * 16 + (lane >> 2);         // fragment rows r0 and r0 + 8 of the tile
+        const int cq = 2 * (lane & 3);                                   // fragment column within an 8-column group
+        constexpr uint32_t DESC_HI = 128u >> 4;                          // SBO = 128 B
+        constexpr uint32_t A_LBO = ((uint32_t)(TC_BM * 16) >> 4) << 16, B_LBO = ((uint32_t)(NT * 16) >> 4) << 16;
+        constexpr uint32_t B_IMG = (2u * NT * 16) >> 4;                  // one (kstep, split) image of B, in 16-byte units
+        const uint32_t a0 = ((a_base + (uint32_t)wg * 64u * 16u) >> 4) | A_LBO;
+        const uint32_t b0 = (b_base >> 4) | B_LBO;
+        const int G = p.seg_len;
+        float run[NT / 2], acc[NT / 2];
 #pragma unroll
-                for (int c = 0; c < CW; ++c) u[c] = 0u;   // cross terms were accumulated with the main products
+        for (int i = 0; i < NT / 2; ++i) run[i] = 0.0f;
+        int in_seg = 0, pend = -1;                      // pend: the stage whose slots are released after the next wait
+        auto release = [&](int it) {
+            __syncwarp();
+            if (lane == 0) {
+                mbar_arrive(bar_base + 8u * (BAR_AEMPTY + it % TC_STAGES));
+                mbar_arrive(bar_base + 8u * (BAR_BEMPTY + it % TC_NBS));
             }
-            const long long em = row0 + eq * 32 + (tid & 31);
+        };
+        for (int it = 0; it < n_iters; ++it) {
+            const int s = it % TC_STAGES, sb = it % TC_NBS;
+            mbar_wait(bar_base + 8u * (BAR_BFULL + sb), (uint32_t)((it / TC_NBS) & 1));
+            mbar_wait(bar_base + 8u * s, (uint32_t)((it / TC_STAGES) & 1));
+            wgmma_fence();
+#pragma unroll
+            for (int ks = 0; ks < 2; ++ks) {
+                const uint32_t ah = a0 + (uint32_t)(s * TC_ASTAGE + ks * 2 * TC_BM * 16) / 16u, al = ah + (uint32_t)TC_AIMG / 16u;
+                const uint32_t bh = b0 + (uint32_t)sb * ((uint32_t)B_STAGE >> 4) + (uint32_t)(ks * 2) * B_IMG, bl = bh + B_IMG;
+                wgmma_tf32<NT>(acc, gmma_desc(al, DESC_HI), gmma_desc(bh, DESC_HI), (in_seg == 0 && ks == 0) ? 0u : 1u);
+                wgmma_tf32<NT>(acc, gmma_desc(ah, DESC_HI), gmma_desc(bl, DESC_HI), 1u);
+                wgmma_tf32<NT>(acc, gmma_desc(ah, DESC_HI), gmma_desc(bh, DESC_HI), 1u);
+            }
+            wgmma_commit();
+            if (++in_seg == G || it == n_iters - 1) {      // segment done: fold it into the running sums
+                wgmma_wait<0>();
+                wgmma_fence_regs<NT / 2>(acc);
+                if (pend >= 0) release(pend);
+                release(it);
+                pend = -1;
+#pragma unroll
+                for (int i = 0; i < NT / 2; ++i) run[i] += acc[i];
+                in_seg = 0;
+            } else {
+                wgmma_wait<1>();                            // the previous stage's MMAs are done
+                if (pend >= 0) release(pend);
+                pend = it;
+            }
+        }
+        // ---- epilogue: running sums + bias (+ReLU) -> channel-blocked [n][Cout/4][position][4] ----------------------
+#pragma unroll
+        for (int half = 0; half < 2; ++half) {
+            const long long em = row0 + r0 + 8 * half;
             if (em < Mtotal) {
                 const int en = (int)(em / p.S_out);
                 const int epos = (int)(em - (long long)en * p.S_out);
-                // channel-blocked output [n][Cout/4][position][4]: one 16-byte store per group of 4 channels, coalesced
-                // across the warp's 32 consecutive rows
-                float4 *eo = reinterpret_cast<float4 *>(p.out) + ((size_t)en * (p.Cout >> 2) + ((ecs * CW) >> 2)) * p.S_out + epos;
+                float *eo = p.out + ((size_t)en * (p.Cout >> 2) * p.S_out + epos) * 4;
 #pragma unroll
-                for (int c = 0; c < CW; c += 4) {
-                    const int co = ecs * CW + c;
+                for (int j = 0; j < NT / 8; ++j) {
+                    const int co = 8 * j + cq;
                     if (co < p.Cout) {
-                        const float4 b4 = __ldg(reinterpret_cast<const float4 *>(p.bias + co));
-                        float4 r;
-                        r.x = (run[c] + __uint_as_float(u[c])) + b4.x;
-                        r.y = (run[c + 1] + __uint_as_float(u[c + 1])) + b4.y;
-                        r.z = (run[c + 2] + __uint_as_float(u[c + 2])) + b4.z;
-                        r.w = (run[c + 3] + __uint_as_float(u[c + 3])) + b4.w;
-                        if (p.relu) { r.x = fmaxf(r.x, 0.0f); r.y = fmaxf(r.y, 0.0f); r.z = fmaxf(r.z, 0.0f); r.w = fmaxf(r.w, 0.0f); }
-                        eo[(size_t)(c >> 2) * p.S_out] = r;
+                        float2 r = make_float2(run[4 * j + 2 * half] + __ldg(p.bias + co), run[4 * j + 2 * half + 1] + __ldg(p.bias + co + 1));
+                        if (p.relu) { r.x = fmaxf(r.x, 0.0f); r.y = fmaxf(r.y, 0.0f); }
+                        *reinterpret_cast<float2 *>(eo + (size_t)(co >> 2) * p.S_out * 4 + (co & 3)) = r;
                     }
                 }
             }
         }
-    } else if (warp == WGT_WARP) {
+    } else {
         // =========================== weight producer ====================================================
         // The weight image of stage `it` is one contiguous block; its order is known in advance, so the producer runs
-        // up to TC_BSTAGES stages ahead of the tensor core, independent of the activation slots: the L2 -> shared
-        // memory latency of the bulk copy (~1 us) is off the stage turnaround path.
+        // up to TC_NBS stages ahead of the tensor core, independent of the activation slots.
         if ((tid & 31) == 0) {
-            const int n_super = (n_iters + TC_SB - 1) / TC_SB;
-            for (int q = 0; q < n_super; ++q) {
-                const int sb = q % TC_NBS;
-                const uint32_t useb = (uint32_t)(q / TC_NBS);
-                if (useb > 0) mbar_wait(bar_base + 8u * (BAR_BEMPTY + sb), (useb - 1) & 1);
-                const int nst = (n_iters - q * TC_SB) < TC_SB ? (n_iters - q * TC_SB) : TC_SB;
-                const uint32_t bytes = (uint32_t)nst * (uint32_t)B_STAGE_BYTES;
-                mbar_arrive_expect_tx(bar_base + 8u * (BAR_BFULL + sb), bytes);
-                bulk_g2s(smem_base + (uint32_t)(sb * TC_SB) * STAGE_BYTES,
-                         reinterpret_cast<const unsigned char *>(p.w) + (size_t)q * TC_SB * B_STAGE_BYTES, bytes, bar_base + 8u * (BAR_BFULL + sb));
+            for (int it = 0; it < n_iters; ++it) {
+                const int sb = it % TC_NBS;
+                const uint32_t use = (uint32_t)(it / TC_NBS);
+                if (use > 0) mbar_wait(bar_base + 8u * (BAR_BEMPTY + sb), (use - 1) & 1);
+                mbar_arrive_expect_tx(bar_base + 8u * (BAR_BFULL + sb), (uint32_t)B_STAGE);
+                bulk_g2s(b_base + (uint32_t)(sb * B_STAGE), reinterpret_cast<const unsigned char *>(p.w) + (size_t)it * B_STAGE, (uint32_t)B_STAGE,
+                         bar_base + 8u * (BAR_BFULL + sb));
             }
         }
         __syncwarp();
-    } else {
-        // =========================== MMA issuer ==========================================================
-        // instruction descriptor: D=F32, A=B=TF32, both K-major, N = NT, M = 128
-        constexpr uint32_t IDESC = (1u << 4) | (2u << 7) | (2u << 10) | ((uint32_t)(NT >> 3) << 17) | ((uint32_t)(128 >> 4) << 24);
-        constexpr uint32_t DESC_HI = (128u >> 4) | (1u << 14);                 // SBO = 128 B, descriptor version 1
-        constexpr uint32_t B_LBO = ((uint32_t)(NT * 16) >> 4) << 16;
-        constexpr uint32_t B_IMG = (2u * NT * 16) >> 4;                         // one (kstep, split) image of B, in 16-byte units
-        const uint32_t leader = elect_leader();
-        const uint32_t b0 = (smem_base >> 4) | B_LBO;                            // stage 0, kstep 0, hi
-        const uint32_t d_cross = tmem_base + (uint32_t)(NSETS * NT);
-        int s = 0, sb = 0, seg = 0, in_seg = 0;
-        uint32_t use = 0, useb = 0;
-#ifdef BX_TC_TRACE
-        const bool trm = p.trace && blockIdx.x == gridDim.x / 2 && (tid & 31) == 0;
-        long long *tm = p.trace + 4 * 3 * 64;
-#endif
-        for (int it = 0; it < n_iters; ++it) {
-#ifdef BX_TC_TRACE
-            if (trm && it < 128) tm[it * 3 + 0] = clock64();
-#endif
-            if (in_seg == 0 && seg >= NSETS) {
-                // segment `seg` reuses main set seg % NSETS: segment seg-NSETS must have been drained
-                mbar_wait(bar_base + 8u * (BAR_ACCFREE + (seg % NSETS)), (uint32_t)(((seg - NSETS) / NSETS) & 1));
-                asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-            }
-            if (sb % TC_SB == 0)                                      // weights: one wait per TC_SB stages (usually long since there)
-                mbar_wait(bar_base + 8u * (BAR_BFULL + sb / TC_SB), useb & 1);
-#ifdef BX_TC_TRACE
-            if (trm && it < 128) tm[it * 3 + 1] = clock64();
-#endif
-            mbar_wait(bar_base + 8u * s, use & 1);                    // activations
-            asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-#ifdef BX_TC_TRACE
-            if (trm && it < 128) tm[it * 3 + 2] = clock64();
-#endif
-            const uint32_t so = (uint32_t)sb * (uint32_t)(STAGE_BYTES >> 4);
-            const uint32_t d_main = tmem_base + (uint32_t)((seg % NSETS) * NT);
-#pragma unroll
-            for (int ks = 0; ks < 2; ++ks) {
-                const uint32_t ah = tmem_base + (uint32_t)(A_RING + s * A_STAGE_COLS + ks * 16), al = ah + 8;
-                const uint32_t bh = b0 + so + (uint32_t)(ks * 2 + 0) * B_IMG, bl = b0 + so + (uint32_t)(ks * 2 + 1) * B_IMG;
-                if (XSEP) {
-                    mma_tf32_ts(leader, d_cross, al, bh, DESC_HI, IDESC, (it == 0 && ks == 0) ? 0u : 1u);
-                    mma_tf32_ts(leader, d_cross, ah, bl, DESC_HI, IDESC, 1u);
-                    mma_tf32_ts(leader, d_main, ah, bh, DESC_HI, IDESC, (in_seg == 0 && ks == 0) ? 0u : 1u);
-                } else {   // one accumulator per segment takes all three products (small terms first)
-                    mma_tf32_ts(leader, d_main, al, bh, DESC_HI, IDESC, (in_seg == 0 && ks == 0) ? 0u : 1u);
-                    mma_tf32_ts(leader, d_main, ah, bl, DESC_HI, IDESC, 1u);
-                    mma_tf32_ts(leader, d_main, ah, bh, DESC_HI, IDESC, 1u);
-                }
-            }
-            mma_commit(leader, bar_base + 8u * (BAR_EMPTY + s));   // slot s may be refilled once these MMAs have read it
-            if (sb % TC_SB == TC_SB - 1 || it == n_iters - 1)
-                mma_commit(leader, bar_base + 8u * (BAR_BEMPTY + sb / TC_SB));   // the whole super-stage has been read
-            if (++s == TC_STAGES) { s = 0; ++use; }
-            if (++sb == TC_BSTAGES) { sb = 0; ++useb; }
-            if (++in_seg == G || it == n_iters - 1) {
-                mma_commit(leader, bar_base + 8u * (BAR_SEGDONE + (seg % NSETS)));
-                in_seg = 0;
-                ++seg;
-            }
-        }
-        __syncwarp();
-    }
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-    __syncthreads();
-#ifdef BX_TC_TRACE
-    if (p.trace && blockIdx.x == gridDim.x / 2 && tid == 0) p.trace[4001] = clock64();   // CTA end (before dealloc)
-#endif
-    if (warp == MMA_WARP) {
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(TMEM_COLS) : "memory");
     }
 }
 
-template <int GEOM, int NT, int LG, int NSETS, int MINB, int XSEP>
+template <int GEOM, int NT>
 int launch_tc(const ConvTcParams &p, int max_n, cudaStream_t st) {
     const long long maxM = (long long)max_n * p.S_out;
     const unsigned gx = (unsigned)((maxM + TC_BM - 1) / TC_BM);
     if (gx == 0) return BX_OK;
-    constexpr int smem = BRing<NT>::SB * BRing<NT>::NBS * (2 * 2 * 2 * NT * 16);
+    constexpr int smem = tc_smem<NT>();
     static BxPerDevice attr_done = {};
     if (bx_needs_attr(attr_done))
-        BX_CUDA(cudaFuncSetAttribute(conv_tc_kernel<GEOM, NT, LG, NSETS, MINB, XSEP>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-    conv_tc_kernel<GEOM, NT, LG, NSETS, MINB, XSEP><<<gx, LG * 128 + 64, smem, st>>>(p);
+        BX_CUDA(cudaFuncSetAttribute(conv_tc_kernel<GEOM, NT>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+    conv_tc_kernel<GEOM, NT><<<gx, TC_THREADS, smem, st>>>(p);
     BX_LAUNCH_CHECK();
     return BX_OK;
 }
 
-int g_tc_mode = -1;   // -1: read BX_TC_MODE once (debug / A-B switch): 0 default, 1 = every layer one CTA per SM (LG=4),
-                      // 2 = narrow layers two CTAs per SM with 16 loader warps each (60 registers per thread)
-
 template <int GEOM>
 int dispatch_nt(const ConvTcParams &p, int max_n, cudaStream_t st) {
-    if (g_tc_mode < 0) {
-        const char *e = getenv("BX_TC_MODE");
-        g_tc_mode = e ? atoi(e) : 0;
-    }
-    if (p.Cout > 64) return launch_tc<GEOM, 128, 4, 2, 1, 1>(p, max_n, st);
-    if (g_tc_mode == 1) {           // every layer one CTA per SM
-        if (p.Cout > 32) return launch_tc<GEOM, 64, 4, 2, 1, 1>(p, max_n, st);
-        return launch_tc<GEOM, 32, 4, 2, 1, 1>(p, max_n, st);
-    }
-    if (g_tc_mode == 2) {           // narrow layers: two CTAs per SM with 16 loader warps each (56 registers per thread)
-        if (p.Cout > 32) return launch_tc<GEOM, 64, 4, 2, 2, 0>(p, max_n, st);
-        return launch_tc<GEOM, 32, 4, 2, 2, 1>(p, max_n, st);
-    }
-    if (g_tc_mode == 3) {           // Cout 64: single main accumulator + separate cross accumulator (drain bubble)
-        if (p.Cout > 32) return launch_tc<GEOM, 64, 2, 1, 2, 1>(p, max_n, st);
-        return launch_tc<GEOM, 32, 2, 2, 2, 1>(p, max_n, st);
-    }
-    if (p.Cout > 32) return launch_tc<GEOM, 64, 2, 2, 2, 0>(p, max_n, st);
-    return launch_tc<GEOM, 32, 2, 2, 2, 1>(p, max_n, st);
+    if (p.Cout > 64) return launch_tc<GEOM, 128>(p, max_n, st);
+    if (p.Cout > 32) return launch_tc<GEOM, 64>(p, max_n, st);
+    return launch_tc<GEOM, 32>(p, max_n, st);
 }
 
 }  // namespace
 
 BX_API int bx_conv_tc_ntile(int Cout) { return Cout > 64 ? 128 : (Cout > 32 ? 64 : 32); }
 
-// Tuning knob (experiments / tests): maximum number of 16-channel stages accumulated in tensor memory
-// before the accumulators are drained with a rounded fp32 add.  <= 0 restores the default.
-static int g_tc_max_stages = 6;
+// Tuning knob (experiments / tests): maximum number of 16-channel stages accumulated by the tensor core before the
+// accumulators are folded into the running sums with a rounded fp32 add.  <= 0 restores the default.
+static int g_tc_max_stages = 4;
 BX_API int bx_conv_tc_set_segment_stages(int stages) {
     const int old = g_tc_max_stages;
-    g_tc_max_stages = stages > 0 ? stages : 6;
+    g_tc_max_stages = stages > 0 ? stages : 4;
     return old;
 }
 
@@ -509,17 +347,7 @@ BX_API int bx_conv_layer_tc(int geom, const float *in, const float *w_tc, const 
     p.Cin = Cin; p.Cout = Cout; p.D = D; p.H = H; p.W = W; p.kd = kd; p.kh = kh; p.kw = kw; p.relu = relu;
     p.equi_s = equi_s; p.equi_t = equi_t; p.s_mids = s_mids; p.t_mids = t_mids;
     p.T = kd * kh * kw;
-    p.seg_len = g_tc_max_stages;   // main-accumulator segment: 6 stages = 12 truncating accumulations
-#ifdef BX_TC_TRACE
-    static long long *d_trace = nullptr;
-    const char *te = getenv("BX_TC_TRACE");
-    const bool do_trace = te && atoi(te) == Cin * 1000 + Cout;
-    if (do_trace) {
-        if (!d_trace) cudaMalloc(&d_trace, sizeof(long long) * 4096);
-        cudaMemset(d_trace, 0, sizeof(long long) * 4096);
-        p.trace = d_trace;
-    }
-#endif
+    p.seg_len = g_tc_max_stages;
     cudaStream_t st = bx_stream(stream);
     switch (geom) {
         case BX_GEOM_CYL3D:
@@ -529,33 +357,7 @@ BX_API int bx_conv_layer_tc(int geom, const float *in, const float *w_tc, const 
         case BX_GEOM_CYL2D:
             BX_REQUIRE(in && D == 1 && H == 7 && W == 20 && kd == 1 && kh == 3 && kw == 3, "bx_conv_layer_tc: CYL2D expects [C,7,20], k=3x3");
             p.S_in = 140; p.S_out = 140; p.OD = 1; p.OH = 7; p.OW = 20;
-#ifdef BX_TC_TRACE
-            {   // debugging aid: BX_TC_TRACE=<Cin*1000+Cout> prints the stage timeline of the middle CTA of that layer once
-                const int rc = dispatch_nt<BX_GEOM_CYL2D>(p, n, st);
-                static int printed = 0;
-                if (do_trace && printed < 1) {
-                    ++printed;
-                    cudaDeviceSynchronize();
-                    static long long h[4096];
-                    cudaMemcpy(h, d_trace, sizeof(h), cudaMemcpyDeviceToHost);
-                    const long long t00 = h[0];
-                    for (int g = 0; g < 4; ++g)
-                        for (int k = 0; k < 24; ++k) {
-                            const long long *r = h + (g * 64 + k) * 3;
-                            if (r[2]) printf("L g%d k%2d top %7lld  empty-wait %5lld  fill %5lld\n", g, k, r[0] - t00, r[1] - r[0], r[2] - r[1]);
-                        }
-                    printf("CTA start %lld  end %lld  (total %lld cycles); a loader group left its main loop at %lld\n", h[4000] - t00, h[4001] - t00,
-                           h[4001] - h[4000], h[4002] - t00);
-                    const long long *m = h + 4 * 3 * 64;
-                    for (int it = 0; it < 72 && m[it * 3]; ++it)
-                        printf("M it%3d top %7lld (+%5lld)  acc/b-wait %5lld  a-wait %5lld\n", it, m[it * 3] - t00, it ? m[it * 3] - m[it * 3 - 3] : 0,
-                               m[it * 3 + 1] - m[it * 3], m[it * 3 + 2] - m[it * 3 + 1]);
-                }
-                return rc;
-            }
-#else
             return dispatch_nt<BX_GEOM_CYL2D>(p, n, st);
-#endif
         case BX_GEOM_VALID3D:
             BX_REQUIRE(in && D >= kd && H >= kh && W >= kw && kd >= 1 && kh >= 1 && kw >= 1, "bx_conv_layer_tc: VALID3D kernel larger than input");
             p.OD = D - kd + 1; p.OH = H - kh + 1; p.OW = W - kw + 1;

@@ -47,8 +47,8 @@ __device__ __forceinline__ Cand warp_best(const Cand c) {
 }
 
 // ---- cluster exchange without cluster.sync: remote stores + remote mbarrier arrive (release.cluster), local wait
-//      (acquire.cluster).  A cluster.sync costs ~380 cycles per FPS iteration and flushes L1; this costs one DSMEM
-//      round (~215 cycles).
+//      (acquire.cluster).  A cluster.sync per FPS iteration is a full cluster barrier and flushes L1; this costs one
+//      DSMEM round.
 __device__ __forceinline__ uint32_t fps_smem_u32(const void *p) { return (uint32_t)__cvta_generic_to_shared(p); }
 __device__ __forceinline__ uint32_t fps_mapa(uint32_t saddr, uint32_t cta) {
     uint32_t r;
@@ -285,10 +285,10 @@ BX_API int bx_fps(const float *xyz, const int32_t *h_offsets, int B, int npoint,
 }
 
 // max_cluster > 0: THROUGHPUT form -- at most that many CTAs per cloud (2 or 4), more points per thread.  An iteration is a
-// latency chain (reductions + cluster exchange, ~1.1 us) whatever the cluster size, so the default form spreads a cloud over
-// 8 SMs only to shorten the register scan; when several pairs are in flight the 16 SMs of a pair's two clouds are taken from
-// the other pairs' convolutions for 2.2 ms (measured: 7 % of the pipelined rate).  Two CTAs per cloud hold 10 points per
-// thread: 1.4x the latency on a quarter of the SMs.  Same indices in every form (the tie rank does not depend on the layout).
+// latency chain (reductions + cluster exchange) whatever the cluster size, so the default form spreads a cloud over 8 SMs
+// only to shorten the register scan; when several pairs are in flight the 16 SMs of a pair's two clouds are taken from the
+// other pairs' convolutions for the whole sampling.  Two CTAs per cloud hold 10 points per thread: a longer chain on a
+// quarter of the SMs.  Same indices in every form (the tie rank does not depend on the layout).
 BX_API int bx_fps_ex(const float *xyz, const int32_t *h_offsets, int B, int npoint, int32_t *idx, float *kpts, int max_cluster,
                      void *stream) {
     BX_REQUIRE(xyz && h_offsets && idx, "bx_fps: null pointer");

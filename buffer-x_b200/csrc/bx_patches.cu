@@ -324,8 +324,8 @@ __global__ void __launch_bounds__(1024) hg_scan_batched_kernel(const HgJobs J) {
     int *cnt = J.cnt[blockIdx.x];
     hg_scan_body(cnt, cnt + HG_CELLS, cnt + 2 * HG_CELLS + 4);
 }
-// The same scan spread over HG_CHUNKS CTAs per job (one CTA per job scanning 131072 buckets is a 80 us latency chain on six
-// SMs -- as long as the query itself): chunk totals first, then every chunk scans its 4096 buckets from the sum of the
+// The same scan spread over HG_CHUNKS CTAs per job (one CTA per job scanning 131072 buckets is a long latency chain on six
+// SMs): chunk totals first, then every chunk scans its 4096 buckets from the sum of the
 // totals before it.  Totals live behind the cursor array (workspace ints [3 * HG_CELLS + 8, + HG_CHUNKS)).
 constexpr int HG_CHUNK = 4096, HG_CHUNKS = HG_CELLS / HG_CHUNK, HG_SCAN_THREADS = 256;
 __global__ void __launch_bounds__(HG_SCAN_THREADS) hg_chunksum_batched_kernel(const HgJobs J) {
@@ -388,8 +388,8 @@ __global__ void __launch_bounds__(HG_THREADS) hg_query_batched_kernel(const HgJo
 //           d2 < r2 test, so every index and coordinate is what the serial scan produces; the task of segment 0 also writes
 //           the padding slots.
 // No early exit (scale 0 does up to twice the distance tests), but 10-60x more independent warps and no block barriers.
-// Measured on C2 (1500 key-points x 20000 points): 78 us per call against 74 us for the streaming kernel -- not faster, so the
-// streaming kernel stays the production path; kept as the independently written second implementation the tests compare.
+// It was not faster than the streaming kernel on the B200 (not re-measured on the H100), so the streaming kernel stays the
+// production path; kept as the independently written second implementation the tests compare.
 constexpr int SG_SEG = 2048;                 // points per segment
 constexpr int SG_WORDS = SG_SEG / 32;        // 64 mask words per task
 constexpr int SG_WARPS = 8;                  // tasks (consecutive key-points, same segment) per CTA

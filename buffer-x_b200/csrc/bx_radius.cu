@@ -145,7 +145,7 @@ BX_API int bx_radius_estimate(const float *kpts, int Kr, const float *pts, int N
     if (bx_needs_attr(attr_done))
         BX_CUDA(cudaFuncSetAttribute(radius_hist_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     int sms = bx_device_sm_count();
-    if (sms <= 0) sms = 148;
+    if (sms <= 0) sms = 132;
     const int gy = (Kr + KT - 1) / KT;
     int gx = (N + HT - 1) / HT;
     const int cap = (4 * sms + gy - 1) / gy;  // ~4 CTAs per SM overall; beyond that grid-stride

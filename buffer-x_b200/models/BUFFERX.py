@@ -1,4 +1,4 @@
-"""BufferX on B200: the per-pair registration ``forward()``.
+"""BufferX on H100: the per-pair registration ``forward()``.
 
 Mirrors ``BufferX`` of /root/reference/models/BUFFERX.py (constructor :72-84, inference branch of
 ``forward`` :257-467, ``mutual_matching`` :469-496, ``post_refinement`` :522-556): same attribute names
@@ -249,9 +249,9 @@ class BufferX(nn.Module):
         self._slots_per_shape = int(slots_per_shape)
         # three or more pairs in flight: the key-point sampling of a pair runs beside the other pairs' convolutions; bx_fps_ex offers
         # a 2- / 4-CTA-per-cloud form (fewer SMs, longer)
-        # (measured on C2 with six pairs in flight: 2 CTAs per cloud 5.1 ms per FPS and 163 pairs/s, 8 CTAs 2.2 ms and 177 -- what the
-        # other streams lose is governed by how LONG the sampling holds its SMs, not by how many, so the default stays the
-        # latency form; BX_FPS_CLUSTER=2|4 selects the throughput form for experiments)
+        # (what the other streams lose is governed by how LONG the sampling holds its SMs, not by how many, so the default stays
+        # the latency form; this choice was measured on the B200 and has not been re-measured on the H100; BX_FPS_CLUSTER=2|4
+        # selects the throughput form for experiments)
         self._fps_cluster = int(os.environ.get("BX_FPS_CLUSTER", "0")) if (flag and self._slots_per_shape >= 3) else 0
         self._slots.clear()
         self._rr.clear()

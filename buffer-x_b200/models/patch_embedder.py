@@ -1,4 +1,4 @@
-"""Mini-SpinNet patch descriptor on B200 kernels.
+"""Mini-SpinNet patch descriptor on H100 kernels.
 
 Mirrors ``MiniSpinNet`` of /root/reference/models/patch_embedder.py (constructor :16-42, forward :44-90,
 same sub-module names -> same state_dict keys ``pnt_layer.{0,1}``, ``pool_layer.{0,1,3,4}``,

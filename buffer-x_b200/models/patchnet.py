@@ -14,14 +14,15 @@ import os
 from bufferx_b200 import ops
 
 # Debug switch only: BX_CONV=ffma routes the conv stacks through the fp32 CUDA-core kernel (bx_conv.cu)
-# instead of the tcgen05 kernel (bx_conv_tc.cu).  Both are sm_100a kernels of this library.
+# instead of the tensor-core kernel (bx_conv_tc.cu).  Both are sm_90a kernels of this library.
 USE_FFMA = os.environ.get("BX_CONV", "sd").lower() == "ffma"
-# BX_CONV=tc: the descriptor stack on the round-1 TF32 kernel (bx_conv_tc.cu) instead of the shifted-descriptor fp16-split
+# BX_CONV=tc: the descriptor stack on the TF32 kernel (bx_conv_tc.cu) instead of the shifted-descriptor fp16-split
 # kernel (bx_conv_sd.cu, the default).  The TF32 kernel is also the automatic fall-back when an activation leaves fp16 range.
 USE_TF32_DESC = os.environ.get("BX_CONV", "sd").lower() == "tc"
 # BX_SD_DYNAMIC=1: the persistent conv kernels draw their tiles from a device-side counter (bx_conv_layer_sd d_tile_ctr) instead
-# of the static stride.  Measured with six pairs in flight: 170.1 vs 170.5 pairs/s -- no gain (a launch whose CTAs start late
-# still cannot finish before they have been scheduled), so the static stride stays the default; the path is kept and tested.
+# of the static stride.  It brought no gain with six pairs in flight (a launch whose CTAs start late still cannot finish before
+# they have been scheduled), so the static stride stays the default; that was measured on the B200 and has not been
+# re-measured on the H100.  The path is kept and tested.
 DYNAMIC_TILES = os.environ.get("BX_SD_DYNAMIC", "0") == "1"
 # Debug switch only: BX_COSTVOL=direct runs the first CostNet layer as a convolution over the on-the-fly cost volume
 # (GEOM_COSTVOL) instead of its factorised form (bx_costvol_ab + GEOM_COSTAB).

@@ -23,11 +23,11 @@ SYMBOLS = [
     "bx_pool_desc", "bx_mutual_nn",
     "bx_hypotheses", "bx_consensus", "bx_ransac_workspace_bytes", "bx_ransac", "bx_refine", "bx_conv_tc_set_segment_stages",
     "bx_radius_neighbors", "bx_grid_subsample", "bx_costvol_ab", "bx_concat_matches",
-    "bx_pca_analysis", "bx_project_range", "bx_voxel_down_sample", "bx_conv_layer_sd", "bx_conv_sd_rows", "bx_spt_pnt_sd", "bx_fps_set_sync_mode", "bx_select_patches_seg", "bx_select_patches_workspace_bytes", "bx_conv_layer_sd_costab", "bx_lrf_batched", "bx_select_patches_batched", "bx_fps_ex", "bx_conv_sd_set_stage_sync", "bx_select_patches_grid", "bx_select_patches_grid_workspace_bytes", "bx_select_patches_grid_batched",
+    "bx_pca_analysis", "bx_project_range", "bx_voxel_down_sample", "bx_conv_layer_sd", "bx_conv_sd_rows", "bx_spt_pnt_sd", "bx_fps_set_sync_mode", "bx_select_patches_seg", "bx_select_patches_workspace_bytes", "bx_conv_layer_sd_costab", "bx_lrf_batched", "bx_select_patches_batched", "bx_fps_ex", "bx_select_patches_grid", "bx_select_patches_grid_workspace_bytes", "bx_select_patches_grid_batched",
 ]
 
 GEOM_CYL3D, GEOM_CYL2D, GEOM_VALID3D, GEOM_COSTVOL, GEOM_COSTAB = 0, 1, 2, 3, 4
-# BX_PATCHES=seg: segmented two-pass form of select_patches (measured equal to the streaming scan: 78 vs 74 us per launch)
+# BX_PATCHES=seg: segmented two-pass form of select_patches (an independently written cross-check of the streaming scan)
 SELECT_PATCHES_SCAN = os.environ.get("BX_PATCHES", "scan").lower() != "seg"
 RADIUS_BINS = 8192
 
@@ -80,7 +80,6 @@ def load_library():
     lib.bx_conv_sd_rows.argtypes = [c_int, c_int]
     lib.bx_conv_layer_sd_costab.argtypes = [P, P, P, P, P, c_int, c_int, P, c_int, P, P]
     lib.bx_fps_set_sync_mode.argtypes = [c_int]
-    lib.bx_conv_sd_set_stage_sync.argtypes = [c_int]
     lib.bx_spt_pnt_sd.argtypes = [P, c_int, c_int, P, c_int, c_int, P, c_float, c_int, P, P, P, c_int64, P, P]
     lib.bx_conv_sd_rows.restype = c_int64
     lib.bx_costvol_ab.argtypes = [P, P, P, P, P, c_int, P, P, P, P, P, P]
@@ -251,8 +250,8 @@ def select_patches(pts4: torch.Tensor, kpts: torch.Tensor, radius, P: int, want_
 
 
 # clouds of at least this many points gather their patches through the spatial hash grid (bx_select_patches_grid) instead of the
-# streaming scan: a ball then holds so small a part of the cloud that reading the cloud front to back costs more than binning it
-# (measured: C3 2 x 120 k points 102 -> 120 pairs/s; C2 2 x 20 k points 171.8 -> 176.5 pairs/s with six pairs in flight)
+# streaming scan: a ball then holds so small a part of the cloud that reading the cloud front to back costs more than binning it.
+# The threshold was chosen on the B200 and has not been re-measured on the H100.
 GRID_MIN_POINTS = int(os.environ.get("BX_PATCHES_GRID_MIN", "12000"))
 
 
@@ -369,7 +368,7 @@ def tf32_split(w: torch.Tensor):
 
 
 def conv_tc_weights(Wt: torch.Tensor) -> torch.Tensor:
-    """[T, Cin, Cout] folded fp32 weights -> the tcgen05 operand image of ``bx_conv_layer_tc``:
+    """[T, Cin, Cout] folded fp32 weights -> the wgmma operand image of ``bx_conv_layer_tc``:
     [chunk(Cin/16)][tap][kstep(2)][split(hi,lo)][kunit(2)][n(NT)][4]."""
     T, Cin, Cout = Wt.shape
     assert Cin % 16 == 0 and Cout <= 128

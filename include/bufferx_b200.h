@@ -1,5 +1,5 @@
 /*
- * bufferx_b200.h -- C-ABI of the B200-native (sm_100a) BUFFER-X per-pair registration hot path.
+ * bufferx_b200.h -- C-ABI of the H100-native (sm_90a) BUFFER-X per-pair registration hot path.
  *
  * Boundary contract
  *   - extern "C", plain pointers and sizes only.  Every pointer is a DEVICE pointer unless the
@@ -38,7 +38,7 @@ extern "C" {
 /* ---- library ------------------------------------------------------------------------------ */
 const char *bx_last_error(void);
 int bx_version(void);          /* 10000*major + 100*minor + patch */
-int bx_device_sm_count(void);  /* SM count of the current device (148 on B200), <0 on error */
+int bx_device_sm_count(void);  /* SM count of the current device (132 on an H100 SXM), <0 on error */
 unsigned long long bx_launch_count(void); /* kernels launched by this library since it was loaded */
 
 /* ---- a1: farthest point sampling ------------------------------------------------------------
@@ -179,24 +179,20 @@ int bx_conv_layer_sd(int geom, const void *in, int in_presplit, const void *w_sd
                      int n, const int32_t *d_n, int Cin, int Cout, int D, int W, int relu, int32_t *d_flag, int32_t *d_tile_ctr,
                      void *stream);
 long long bx_conv_sd_rows(int n, int rows_per_sample);
-/* Verification switch: how the epilogue warps of the shifted-descriptor kernel hand a finished tile to its storer warps --
- * 0 mbarriers (production), 1 named barriers (the form compute-sanitizer's racecheck models), -1 follow BX_SD_STAGE_SYNC.
- * Identical results; returns the previous value. */
-int bx_conv_sd_set_stage_sync(int mode);
 /* The second CostNet layer (32 -> 64, k = 3x3x3 over relu(A - B) regenerated from the factor maps of bx_costvol_ab) as a
  * 96 -> 64, k = (3,1,3) convolution over the 18 x 18 (n, l) raster on the same kernel.  fa [n,8,60,4], fb [n,8,54,4] fp32;
  * w_sd: ops.conv_sd_weights_costab; out: fp32 [n,16,256,4] or presplit over the 16 x 16 raster (rows = bx_conv_sd_rows(n, 256)). */
 int bx_conv_layer_sd_costab(const float *fa, const float *fb, const void *w_sd, const float *bias, void *out, int out_presplit, int n,
                             const int32_t *d_n, int relu, int32_t *d_flag, void *stream);
 
-/* Tensor-core variant (tcgen05.mma kind::tf32, 3xTF32 split, fp32 accumulators in TMEM; same geometry
+/* Tensor-core variant (wgmma .tf32, 3xTF32 split, fp32 accumulators in registers; same geometry
  * arguments).  Activations are CHANNEL-BLOCKED here: in [n][Cin/4][S_in][4], out [n][Cout/4][S_out][4] (a GEMM row
  * fetches its 16 input channels with four 16-byte loads that coalesce across the warp's 32 consecutive rows; the
  * epilogue stores the same way); Cout % 4 == 0; in, out, bias 16-byte aligned.  w_tc is the host-prepared operand image: for every stage it = chunk*T + tap (chunk = 16
  * input channels) the block [kstep(2)][split(2: hi,lo)][kunit(2)][n(NT)][4 floats], NT = bx_conv_tc_ntile(Cout),
  * rows n >= Cout zero, hi = round-to-nearest tf32 of the folded weight, lo = w - hi.  Cin % 16 == 0, Cout <= 128. */
 int bx_conv_tc_ntile(int Cout);
-/* Tuning knob: stages (16 channels x 1 tap) accumulated per TMEM segment before the fp32 drain (default 6);
+/* Tuning knob: stages (16 channels x 1 tap) accumulated per tensor-core segment before the rounded fp32 add (default 4);
  * returns the previous value.  Used by tools/tc_precision.py. */
 int bx_conv_tc_set_segment_stages(int stages);
 int bx_conv_layer_tc(int geom, const float *in, const float *w_tc, const float *bias, float *out, int n,

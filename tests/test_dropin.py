@@ -60,19 +60,7 @@ def test_documented_pythonpath_resolves_reference_and_mirror_modules(tmp_path):
               "dataset.dataloader", "config"):
         assert res[n] is not None and res[n].startswith(os.path.realpath(str(ref))), f"{n} must come from the reference checkout, got {res[n]}"
     for n in ("models.BUFFERX", "models.patchnet", "models.patch_embedder", "models.pose_estimator"):
-        assert res[n] is not None and res[n].startswith(ours), f"{n} must resolve to the B200 mirror, got {res[n]}"
-
-
-@pytest.mark.skipif(not os.path.isdir("/root/reference/utils"), reason="needs the reference checkout (build container only)")
-def test_real_reference_checkout_utils_are_not_shadowed():
-    code = ("import importlib.util as u, os; "
-            "print([os.path.realpath(u.find_spec(n).origin) for n in ('utils.timer','utils.SE3','utils.tools','models.BUFFERX')])")
-    env = dict(os.environ)
-    env["PYTHONPATH"] = os.pathsep.join([os.path.join(ROOT, "buffer-x_b200"), ROOT])
-    out = subprocess.run([sys.executable, "-c", code], cwd="/root/reference", env=env, capture_output=True, text=True, timeout=300)
-    assert out.returncode == 0, out.stderr
-    paths = eval(out.stdout.strip().splitlines()[-1])
-    assert all(p.startswith("/root/reference/utils/") for p in paths[:3]) and paths[3].startswith(os.path.realpath(ROOT))
+        assert res[n] is not None and res[n].startswith(ours), f"{n} must resolve to the H100 mirror, got {res[n]}"
 
 
 # ------------------------------------------------------------------------------------------------ GPU

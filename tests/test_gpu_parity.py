@@ -54,7 +54,7 @@ def test_fps_bit_exact(dev, oracle, n, m, kind):
 @pytest.mark.parametrize("n,m", [(20000, 1500), (120000, 300), (5000, 512)])
 def test_fps_mbarrier_exchange_equals_cluster_sync_exchange(dev, oracle, n, m):
     """The production cluster exchange (remote st.shared::cluster + mbarrier.arrive.release.cluster, local acquire wait) and
-    the verification form (the same stores ordered by cluster.sync(), which racecheck models; profiles/r02_sanitizer_*)
+    the verification form (the same stores ordered by cluster.sync(), which racecheck models)
     give the same indices -- and both equal the oracle."""
     from bufferx_b200 import ops
     lib = ops.load_library()
@@ -763,26 +763,6 @@ def test_conv_layer_kernels(dev, geom, Cin, Cout, dims, k, n, impl):
     got = out.cpu().numpy().reshape(ref.shape)
     err = np.abs(got - ref.numpy()).max() / np.abs(ref.numpy()).max()
     assert err < 2e-5, f"{impl} {geom} Cin={Cin} Cout={Cout}: rel err {err}"     # fp32-grade (3xTF32 / FFMA) vs torch fp32
-
-
-def test_conv_sd_stage_handover_forms_same_bits(dev):
-    """The epilogue -> storer staging hand-over with mbarriers (production) and with named barriers (the form racecheck models,
-    profiles/r02_sanitizer_racecheck_*.txt) writes the same bits, for a narrow and a wide layer."""
-    from bufferx_b200 import ops
-    lib = ops.load_library()
-    torch.manual_seed(6)
-    for Cin, Cout, n in ((64, 64, 500), (64, 128, 300)):
-        x = ops.sd_pack(torch.relu(torch.randn(n, Cin, 7, 20, device=dev)))
-        w, b = ops.conv_sd_weights(torch.randn(9, Cin, Cout, device=dev) * 0.05), torch.randn(Cout, device=dev) * 0.1
-        outs = []
-        old = lib.bx_conv_sd_set_stage_sync(0)
-        try:
-            for mode in (0, 1):
-                lib.bx_conv_sd_set_stage_sync(mode)
-                outs.append(ops.conv_layer_sd(ops.GEOM_CYL2D, x, w, b, ops.conv_sd_buffer(n, Cout, dev).zero_(), n, Cin, Cout, True, None))
-        finally:
-            lib.bx_conv_sd_set_stage_sync(old)
-        assert torch.equal(outs[0].view(torch.int16), outs[1].view(torch.int16))
 
 
 def test_conv_sd_dynamic_tiles_same_bits(dev):

@@ -8,7 +8,7 @@ import bufferx_b200 as bx
 from bufferx_b200 import ops
 from bufferx_b200.synth import init_synthetic_weights, workload_cfg
 
-MODE = os.environ.get("BX_CONV", "sd").lower()          # sd (shifted-descriptor fp16-split kernel) | tc (round-1 TF32 kernel)
+MODE = os.environ.get("BX_CONV", "sd").lower()          # sd (shifted-descriptor fp16-split kernel) | tc (TF32 tensor-core kernel)
 K = int(sys.argv[1]) if len(sys.argv) > 1 else 1500
 reps = int(sys.argv[2]) if len(sys.argv) > 2 else 10
 cfg = workload_cfg("C2")
@@ -50,15 +50,7 @@ for i, l in enumerate(L):
     taps = l["k"][0] * l["k"][1] * l["k"][2]
     fl = 2.0 * K * 140 * l["cin"] * l["cout"] * taps
     stages = l["cin"] // 16 * taps
-    nt = 128 if l["cout"] > 64 else (64 if l["cout"] > 32 else 32)
-    tiles = (K * 140 + 127) // 128
-    if MODE == "sd":        # 3 fp16 MMAs (K = 16) per stage, N/2 cycles each; tiles of 128 padded rows (176 per sample)
-        tiles = (K * 176 + 127) // 128
-        tensor_min_us = stages * 3 * (nt / 2) * ((tiles + 147) // 148) / 1965.0
-    else:
-        tensor_min_us = stages * 6 * (nt / 2) * ((tiles + 147) // 148) / 1965.0     # 6 MMAs/stage, N/2 cycles each at 1.965 GHz
     tot_ms += ms
     tot_fl += fl
-    print(f"L{i}: {l['cin']:3d}->{l['cout']:3d} taps {taps:2d} stages {stages:3d}  {ms * 1e3:7.1f} us  {fl / ms / 1e9:6.1f} TFLOP/s  "
-          f"tensor-min {tensor_min_us:6.1f} us ({100 * tensor_min_us / (ms * 1e3):4.1f} %)")
+    print(f"L{i}: {l['cin']:3d}->{l['cout']:3d} taps {taps:2d} stages {stages:3d}  {ms * 1e3:7.1f} us  {fl / ms / 1e9:6.1f} TFLOP/s")
 print(f"[{MODE}] stack: {tot_ms * 1e3:.1f} us  {tot_fl / tot_ms / 1e9:.1f} TFLOP/s fp32-equivalent")
