@@ -18,19 +18,22 @@
 //               tensor rate and half the operand bytes):  a*b ~= ah*bh + (al*bh + ah*bl) * 2^-11.  Per 16-channel chunk
 //               (K = 144) the products go to a fresh accumulator [main | cross]; the finished chunk's main + cross * 2^-11 is
 //               added with round-to-nearest into fp32 running sums that start from the bias, so no accumulation chain is
-//               longer than one chunk.  For Cout <= 64 a tap is TWO instructions: ah * [bh | bl] as one N = 2*NT MMA into
-//               [main | cross] (the hi rows and lo rows of a weight kcore are adjacent) and al * bh into the cross columns;
-//               for Cout 128 the columns are done in two 64-wide blocks of three N = 64 MMAs each.
+//               longer than one chunk.  A tap is three N = Cout MMAs: ah * bh into main, ah * bl and al * bh into cross.
+//               main and cross are disjoint register blocks, each written only by whole wgmmas: a wgmma that accumulates
+//               into a sub-range of another in-flight wgmma's registers makes ptxas wait for each wgmma before issuing the
+//               next.  Cout 128 takes a chunk in one pass (128 accumulators + 64 running sums per thread, see the register
+//               split below), except with fp32 input, which does two 64-column passes.
 //               |x| >= 65504 cannot be represented: the loader raises *flag and the host re-runs the layer on the TF32 kernel.
 //
-// Persistent warp-specialised CTA, one per SM:
+// Persistent warp-specialised CTA, one per SM, of three warpgroups:
 //   2 MMA warpgroups  warpgroup g owns tile rows 64 g .. 64 g + 63: per (chunk, tap) its wgmmas read the shifted A view and the
 //                     weights straight from shared memory; after a chunk the accumulators are folded into the running sums
 //                     and the A slot / weight stages are released.  A finished tile goes through a shared-memory staging buffer
 //                     (64 columns at a time) so that each thread then stores one row: ReLU, fp16 hi/lo split and the next
 //                     layer's wrap columns and zero rows, or fp32 channel-blocked values.
+//   producer warpgroup, warps 0-2 = A producer, warp 3 = weight thread:
 //   A producer        presplit input: one thread, a chunk = four 2816-byte bulk copies of the previous layer's presplit image
-//                     (ring of NA chunks).  fp32 input: 4 loader warps convert channel-blocked activations to fp16 hi/lo.
+//                     (ring of NA chunks).  fp32 input: 3 loader warps convert channel-blocked activations to fp16 hi/lo.
 //   weight thread     the host-arranged weight image [chunk][tap][kcore][split][n][8 x fp16] in stages of three taps with
 //                     cp.async.bulk + mbarrier transaction counts; loaded ONCE and kept resident when the whole image fits
 //                     next to three A chunks, else streamed through a ring.
@@ -46,8 +49,9 @@ constexpr int SD_AROWS = 176;                    // tile rows + halo (2*22 + 2 =
 constexpr int SD_SROWS = 176;                    // padded rows per sample (8 x 22)
 constexpr int SD_KBYTES = SD_AROWS * 16;         // one (split, kcore) image of a chunk: [row][8 x fp16]
 constexpr int SD_CHUNK = 4 * SD_KBYTES;          // [split(hi,lo)][kcore(2)]
-constexpr int SD_NL = 4;                         // loader warps (fp32 input)
+constexpr int SD_NL = 3;                         // loader warps (fp32 input)
 constexpr int SD_NC = 8;                         // MMA warps: two warpgroups of 64 tile rows
+constexpr int SD_WGT_WARP = SD_NC + 3;           // weight thread: last warp of the producer warpgroup
 constexpr int SD_MAXNA = 12, SD_MAXNBS = 24;     // A chunk slots; weight stages (resident: every stage of up to 8 chunks)
 constexpr int SD_TRING = 32;                     // published tile indices of dynamic scheduling
 constexpr int SD_SMEM = 227 * 1024 - 2048;       // dynamic shared memory of one CTA (the rest: barriers, bias)
@@ -71,13 +75,25 @@ struct ConvSdParams {
 };
 
 template <int NT, int IN_SD> struct SdCfg {
-    static constexpr int NB = NT < 64 ? NT : 64;                  // accumulator block: output columns per pass
+    // accumulator block: output columns per pass over a chunk.  All of them, except for Cout 128 with fp32 input, whose
+    // loader warps keep more registers than the 128 accumulators + 64 running sums of a single pass would leave room for.
+    static constexpr int NB = (NT == 128 && !IN_SD) ? 64 : NT;
     static constexpr int NH = NT / NB;                            // passes per chunk
-    static constexpr int NLW = IN_SD ? 1 : SD_NL;                 // A producer warps
-    static constexpr int THREADS = (SD_NC + NLW + 1) * 32;
+    static constexpr int SB = NT < 64 ? NT : 64;                  // output columns per staging round of a finished tile
+    static constexpr int THREADS = (SD_NC + 4) * 32;              // two MMA warpgroups + one producer warpgroup
+    // per-thread registers after setmaxnreg: 128 * PROD_REGS + 256 * MMA_REGS = 384 * 168, the CTA's allocation at launch
+    // (ptxas reports 168 for every instantiation; a split that asked for more would leave setmaxnreg.inc waiting forever)
+    static constexpr int PROD_REGS = IN_SD ? 56 : 136, MMA_REGS = IN_SD ? 224 : 184;
     static constexpr int B_STAGE = 3 * 64 * NT;                   // three taps of [kcore][split][n][16 B]
-    static constexpr int STAGE_BYTES = SD_BM * NB * 4;            // fp32 staging of one column block of a tile
+    static constexpr int STAGE_BYTES = SD_BM * SB * 4;            // fp32 staging of one column block of a tile
 };
+static_assert(128 * SdCfg<64, 1>::PROD_REGS + 256 * SdCfg<64, 1>::MMA_REGS == 384 * 168, "register split of the presplit kernels");
+static_assert(128 * SdCfg<64, 0>::PROD_REGS + 256 * SdCfg<64, 0>::MMA_REGS == 384 * 168, "register split of the fp32-input kernels");
+
+// Moves registers between warpgroups (all threads of a warpgroup execute it with the same count, a multiple of 8): the
+// producer warpgroup gives back what the MMA warpgroups take.  .inc waits until the registers are free.
+template <int R> __device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(R)); }
+template <int R> __device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(R)); }
 
 // One thread's share of a finished tile: GEMM row R = t * 128 + row, CW consecutive output channels starting at co0; get8
 // yields bias + sum of eight of them.  Here: ReLU, then either fp32 channel-blocked stores of the valid rows or the presplit
@@ -150,11 +166,13 @@ __device__ __forceinline__ void sd_store_rows(const ConvSdParams &p, int t, int 
 // IN_SD = 0: fp32 channel-blocked input converted by the loader warps; 1: presplit padded fp16 images fetched with bulk copies.
 // OUT_SD = 0: fp32 channel-blocked output; 1: presplit padded fp16 images (zero rows and wrap columns written here).
 template <int NT, int IN_SD, int OUT_SD>
-// Registers: the warps of a CTA are spread over the SM's four sub-partitions of 16 K registers each, so the 10 (13) warps
-// put 3 (4) warps on one of them and cap a thread at 168 (128) registers -- the bound __launch_bounds__ gives ptxas.
+// Registers: 12 warps = 3 per sub-partition of 16 K registers, so every thread starts at 168 (the bound __launch_bounds__
+// gives ptxas).  The producer warpgroup then drops to PROD_REGS (56 for the bulk-copy and weight threads, 136 for the fp32
+// loaders) and the MMA warpgroups rise to MMA_REGS (224 / 184): room for a whole Cout 128 chunk's accumulators
+// [main 64 | cross 64] next to the 64 running sums, and enough for ptxas to keep the wgmma chain of a chunk in flight.
 __global__ void __launch_bounds__(SdCfg<NT, IN_SD>::THREADS, 1) conv_sd_kernel(const ConvSdParams p) {
     using C = SdCfg<NT, IN_SD>;
-    constexpr int NB = C::NB, NH = C::NH, WGT_WARP = SD_NC + C::NLW;
+    constexpr int NB = C::NB, NH = C::NH, SB = C::SB, WGT_WARP = SD_WGT_WARP;
     constexpr int BAR_AFULL = 0, BAR_AEMPTY = SD_MAXNA, BAR_BFULL = 2 * SD_MAXNA, BAR_BEMPTY = BAR_BFULL + SD_MAXNBS;
     constexpr int BAR_TILE = BAR_BEMPTY + SD_MAXNBS, NBARS = BAR_TILE + SD_TRING;
     extern __shared__ __align__(128) unsigned char smem[];
@@ -202,8 +220,11 @@ __global__ void __launch_bounds__(SdCfg<NT, IN_SD>::THREADS, 1) conv_sd_kernel(c
         return tile_ring[k & (SD_TRING - 1)];
     };
 
+    // Each role branch starts with its warpgroup's setmaxnreg (one instruction for all threads of a warpgroup): the MMA
+    // warpgroups take the registers the producer warpgroup gives up.
     if (warp < SD_NC) {
         // =========================== MMA warpgroups: wgmma, chunk folds, tile stores =====================================
+        setmaxnreg_inc<C::MMA_REGS>();
         const int wg = warp >> 2, tl = tid & 127;
         const int r0 = wg * 64 + (warp & 3) * 16 + (lane >> 2);         // fragment rows r0 and r0 + 8 of the tile
         const int cq = 2 * (lane & 3);                                   // fragment column within an 8-column group
@@ -214,7 +235,7 @@ __global__ void __launch_bounds__(SdCfg<NT, IN_SD>::THREADS, 1) conv_sd_kernel(c
         const uint32_t a0 = ((a_base + (uint32_t)wg * 64u * 16u) >> 4) | A_LBO;   // this warpgroup's 64 rows
         const uint32_t b0 = (b_base >> 4) | B_LBO;
         const uint32_t Wrow = (uint32_t)p.W;                             // tap (g, tt) reads rows R + g * W + tt
-        float run[NT / 2], acc[NB];
+        float run[NT / 2], acc[NB];      // acc = [main NB / 2 | cross NB / 2]: disjoint blocks, each written by whole wgmmas
         uint32_t slot = 0, a_par = 0, q = 0, k = 0;
         for (int t = tile_of(0); t >= 0; t = tile_of(++k)) {
 #pragma unroll
@@ -234,15 +255,18 @@ __global__ void __launch_bounds__(SdCfg<NT, IN_SD>::THREADS, 1) conv_sd_kernel(c
 #pragma unroll
                         for (int tt = 0; tt < 3; ++tt) {
                             const uint32_t ah = ac + (uint32_t)g * Wrow + (uint32_t)tt, al = ah + A_SPLIT;   // one row = 16 B
-                            const uint32_t bh = bg + (uint32_t)tt * B_TAP16 + (uint32_t)(h * NB * 16 / 16);
+                            const uint32_t bh = bg + (uint32_t)tt * B_TAP16 + (uint32_t)(h * NB), bl = bh + B_LO16;   // n rows of 16 B
                             const uint32_t acc_on = (g == 0 && tt == 0) ? 0u : 1u;
-                            if constexpr (NH == 1) {     // ah * [bh | bl] -> [main | cross], al * bh -> cross
-                                wgmma_f16<2 * NT>(acc, gmma_desc(ah, DESC_HI), gmma_desc(bh, DESC_HI), acc_on);
-                                wgmma_f16<NT>(acc + NT / 2, gmma_desc(al, DESC_HI), gmma_desc(bh, DESC_HI), 1u);
+                            // ah * bh -> main; al * bh and ah * bl -> cross.  The cross products keep the order of the
+                            // earlier forms of this kernel (Cout <= 64: ah * bl first; Cout 128: al * bh first), so the
+                            // rounding of every element is unchanged.
+                            wgmma_f16<NB>(acc, gmma_desc(ah, DESC_HI), gmma_desc(bh, DESC_HI), acc_on);
+                            if constexpr (NT < 128) {
+                                wgmma_f16<NB>(acc + NB / 2, gmma_desc(ah, DESC_HI), gmma_desc(bl, DESC_HI), acc_on);
+                                wgmma_f16<NB>(acc + NB / 2, gmma_desc(al, DESC_HI), gmma_desc(bh, DESC_HI), 1u);
                             } else {
-                                wgmma_f16<64>(acc, gmma_desc(ah, DESC_HI), gmma_desc(bh, DESC_HI), acc_on);
-                                wgmma_f16<64>(acc + 32, gmma_desc(al, DESC_HI), gmma_desc(bh, DESC_HI), acc_on);
-                                wgmma_f16<64>(acc + 32, gmma_desc(ah, DESC_HI), gmma_desc(bh + B_LO16, DESC_HI), 1u);
+                                wgmma_f16<NB>(acc + NB / 2, gmma_desc(al, DESC_HI), gmma_desc(bh, DESC_HI), acc_on);
+                                wgmma_f16<NB>(acc + NB / 2, gmma_desc(ah, DESC_HI), gmma_desc(bl, DESC_HI), 1u);
                             }
                         }
                     }
@@ -263,180 +287,185 @@ __global__ void __launch_bounds__(SdCfg<NT, IN_SD>::THREADS, 1) conv_sd_kernel(c
             }
             // the finished tile, one column block at a time: fragments -> staging -> one row per thread
 #pragma unroll
-            for (int h = 0; h < NH; ++h) {
+            for (int h = 0; h < NT / SB; ++h) {
                 asm volatile("bar.sync %0, 128;" ::"r"(1 + wg) : "memory");        // this warpgroup's rows of the staging buffer are free
 #pragma unroll
-                for (int i = 0; i < NB / 2; i += 2) {
+                for (int i = 0; i < SB / 2; i += 2) {
                     const int col = 8 * (i >> 2) + cq, row = r0 + ((i & 2) ? 8 : 0);
                     *reinterpret_cast<float2 *>(stage + ((size_t)(col >> 2) * SD_BM + row) * 4 + (col & 3)) =
-                        make_float2(run[h * (NB / 2) + i], run[h * (NB / 2) + i + 1]);
+                        make_float2(run[h * (SB / 2) + i], run[h * (SB / 2) + i + 1]);
                 }
                 asm volatile("bar.sync %0, 128;" ::"r"(1 + wg) : "memory");
-                const int row = wg * 64 + (tl & 63), cs = (tl >> 6) * (NB / 2);
+                const int row = wg * 64 + (tl & 63), cs = (tl >> 6) * (SB / 2);
                 const float4 *st4 = reinterpret_cast<const float4 *>(stage);
-                sd_store_rows<NB / 2, OUT_SD>(p, t, row, h * NB + cs, n_samples, [&](int cc, float (&r)[8]) {
+                sd_store_rows<SB / 2, OUT_SD>(p, t, row, h * SB + cs, n_samples, [&](int cc, float (&r)[8]) {
                     const float4 u0 = st4[((cs + cc) >> 2) * SD_BM + row], u1 = st4[(((cs + cc) >> 2) + 1) * SD_BM + row];
                     r[0] = u0.x; r[1] = u0.y; r[2] = u0.z; r[3] = u0.w; r[4] = u1.x; r[5] = u1.y; r[6] = u1.z; r[7] = u1.w;
                 });
             }
         }
-    } else if (warp < WGT_WARP) {
-        if (IN_SD) {
-            // =========================== A producer: presplit images by bulk copy =================================
-            // A chunk's four (split, kcore) images are four contiguous 2816-byte runs of the previous layer's output: one
-            // thread keeps NA chunks in flight; no register staging, no conversion.
-            if (warp == SD_NC && lane == 0) {
-                uint32_t slot = 0, par = 0, round = 0;
-                for (uint32_t k = 0;; ++k) {
-                    int t;
-                    if (dyn) {           // draw the next tile and publish it to the other roles
-                        t = atomicAdd(p.tile_ctr, 1);
-                        if (t >= n_tiles) t = -1;
-                        tile_ring[k & (SD_TRING - 1)] = t;
-                        mbar_arrive(bar_base + 8u * (BAR_TILE + (k & (SD_TRING - 1))));
-                    } else {
-                        t = tile_of(k);
-                    }
-                    if (t < 0) break;
-                    for (int c = 0; c < nchunks; ++c) {
-                        if (round) mbar_wait(bar_base + 8u * (BAR_AEMPTY + slot), par ^ 1u);
-                        mbar_arrive_expect_tx(bar_base + 8u * (BAR_AFULL + slot), 4u * (uint32_t)SD_KBYTES);
-                        const unsigned char *src = reinterpret_cast<const unsigned char *>(p.in_sd) + ((size_t)(c * 4) * p.rows_in + (size_t)t * SD_BM) * 16;
+    } else {
+        setmaxnreg_dec<C::PROD_REGS>();
+        if (warp < WGT_WARP) {
+            if (IN_SD) {
+                // =========================== A producer: presplit images by bulk copy =================================
+                // A chunk's four (split, kcore) images are four contiguous 2816-byte runs of the previous layer's output: one
+                // thread keeps NA chunks in flight; no register staging, no conversion.  The other two warps before the weight
+                // warp have no work.
+                if (warp == SD_NC && lane == 0) {
+                    uint32_t slot = 0, par = 0, round = 0;
+                    for (uint32_t k = 0;; ++k) {
+                        int t;
+                        if (dyn) {           // draw the next tile and publish it to the other roles
+                            t = atomicAdd(p.tile_ctr, 1);
+                            if (t >= n_tiles) t = -1;
+                            tile_ring[k & (SD_TRING - 1)] = t;
+                            mbar_arrive(bar_base + 8u * (BAR_TILE + (k & (SD_TRING - 1))));
+                        } else {
+                            t = tile_of(k);
+                        }
+                        if (t < 0) break;
+                        for (int c = 0; c < nchunks; ++c) {
+                            if (round) mbar_wait(bar_base + 8u * (BAR_AEMPTY + slot), par ^ 1u);
+                            mbar_arrive_expect_tx(bar_base + 8u * (BAR_AFULL + slot), 4u * (uint32_t)SD_KBYTES);
+                            const unsigned char *src = reinterpret_cast<const unsigned char *>(p.in_sd) + ((size_t)(c * 4) * p.rows_in + (size_t)t * SD_BM) * 16;
 #pragma unroll
-                        for (int im = 0; im < 4; ++im)
-                            bulk_g2s(a_base + slot * (uint32_t)SD_CHUNK + (uint32_t)im * SD_KBYTES, src + (size_t)im * p.rows_in * 16, (uint32_t)SD_KBYTES,
-                                     bar_base + 8u * (BAR_AFULL + slot));
-                        if (++slot == (uint32_t)NA) { slot = 0; par ^= 1u; round = 1; }
+                            for (int im = 0; im < 4; ++im)
+                                bulk_g2s(a_base + slot * (uint32_t)SD_CHUNK + (uint32_t)im * SD_KBYTES, src + (size_t)im * p.rows_in * 16, (uint32_t)SD_KBYTES,
+                                         bar_base + 8u * (BAR_AFULL + slot));
+                            if (++slot == (uint32_t)NA) { slot = 0; par ^= 1u; round = 1; }
+                        }
+                    }
+                }
+                __syncwarp();
+            } else {
+            // =========================== loaders: fp32 activations -> fp16 hi/lo chunk images ====================
+                // A chunk image is 2 x 176 items of (row, 8 channels) = two 16-byte loads each; thread `ltid` owns the items ltid,
+                // ltid + 96, ltid + 192, ltid + 288 of EVERY chunk.  The activations come from HBM: all eight loads of a chunk are
+                // issued at once and the loads of chunk j + 1 are in flight while chunk j is converted, so no chunk waits a whole
+                // exposed round trip.
+                constexpr int ITEMS = (2 * SD_AROWS + SD_NL * 32 - 1) / (SD_NL * 32);      // 4
+                const int ltid = tid - SD_NC * 32;
+                const float4 *in4 = reinterpret_cast<const float4 *>(p.in);
+                float amax = 0.0f;
+                float4 cur[ITEMS][2], nxt[ITEMS][2];
+                auto issue = [&](int t, int c, float4 (&v)[ITEMS][2]) {
+                    const long long p0 = (long long)t * SD_BM;
+#pragma unroll
+                    for (int m = 0; m < ITEMS; ++m) {
+                        const int idx = ltid + m * SD_NL * 32;
+                        v[m][0] = make_float4(0.f, 0.f, 0.f, 0.f);
+                        v[m][1] = v[m][0];
+                        if (idx < 2 * SD_AROWS) {
+                            const int h = idx >= SD_AROWS ? 1 : 0, r = idx - h * SD_AROWS;
+                            const long long pr = p0 + r;
+                            const int s = (int)(pr / p.rs), q = (int)(pr - (long long)s * p.rs);
+                            const int yp = q / 22, xp = q - yp * 22;
+                            if (s < n_samples && (yp != 0 || !p.cyl) && !p.fa) {
+                                const int xx = xp == 0 ? 19 : (xp == 21 ? 0 : xp - 1);
+                                int pos = p.cyl ? (yp - 1) * 20 + xx : q, g0;       // valid rasters: the row IS the input position
+                                if (p.is3d) { pos += c * 140; g0 = h * 2; } else { g0 = c * 4 + h * 2; }
+                                const float4 *src = in4 + ((size_t)s * p.G_in + g0) * p.S_in + pos;
+                                v[m][0] = __ldg(src);
+                                v[m][1] = __ldg(src + p.S_in);
+                            }
+                        }
+                    }
+                };
+                int j = 0;
+                int t = blockIdx.x, c = 0;
+                if (t < n_tiles) issue(t, 0, cur);
+                while (t < n_tiles) {
+                    // position of the chunk after this one
+                    int tn = t, cn = c + 1;
+                    if (cn == nchunks) { cn = 0; tn = t + gridDim.x; }
+                    if (tn < n_tiles) issue(tn, cn, nxt);
+                    const int slot = j % NA;
+                    if (j >= NA) mbar_wait(bar_base + 8u * (BAR_AEMPTY + slot), (uint32_t)(((j / NA) - 1) & 1));
+                    unsigned char *dst = smem + (size_t)slot * SD_CHUNK;
+                    if (p.fa) {
+                        // second CostNet layer: the first layer's activation relu(A[c][k][(l - n) mod 20] - B[c][k][l]) is regenerated
+                        // here from the factor maps (models/BUFFERX.py:39-69 + patchnet.py:192-198, factorised by bx_costvol_ab).  Raster
+                        // row q = (n, l) of the 18 x 18 grid; chunk c = (k = c / 2, channels 16 * (c % 2) ...): the k dimension of the
+                        // 3x3x3 kernel is folded into the channels, the taps are (dn, dl).  The 14.6 KB of factors per match are L2
+                        // hits, so all loads of the chunk are issued here, no cross-chunk prefetch.
+                        const long long p0 = (long long)t * SD_BM;
+                        const int kk = c >> 1, cb = (c & 1) * 4;
+                        float4 va[ITEMS][2], vb[ITEMS][2];
+#pragma unroll
+                        for (int m = 0; m < ITEMS; ++m) {
+                            const int idx = ltid + m * SD_NL * 32;
+                            va[m][0] = va[m][1] = vb[m][0] = vb[m][1] = make_float4(0.f, 0.f, 0.f, 0.f);
+                            if (idx < 2 * SD_AROWS) {
+                                const int h = idx >= SD_AROWS ? 1 : 0, r = idx - h * SD_AROWS;
+                                const long long pr = p0 + r;
+                                const int s = (int)(pr / 324), q = (int)(pr - (long long)s * 324);
+                                const int nn = q / 18, ll = q - nn * 18;
+                                if (s < n_samples) {
+                                    int sh = ll - nn;
+                                    sh = sh < 0 ? sh + 20 : sh;
+                                    const float4 *sa = reinterpret_cast<const float4 *>(p.fa) + ((size_t)s * 8 + cb + h * 2) * 60 + kk * 20 + sh;
+                                    const float4 *sb = reinterpret_cast<const float4 *>(p.fb) + ((size_t)s * 8 + cb + h * 2) * 54 + kk * 18 + ll;
+                                    va[m][0] = __ldg(sa); va[m][1] = __ldg(sa + 60);
+                                    vb[m][0] = __ldg(sb); vb[m][1] = __ldg(sb + 54);
+                                }
+                            }
+                        }
+#pragma unroll
+                        for (int m = 0; m < ITEMS; ++m) {
+                            cur[m][0] = make_float4(fmaxf(va[m][0].x - vb[m][0].x, 0.f), fmaxf(va[m][0].y - vb[m][0].y, 0.f), fmaxf(va[m][0].z - vb[m][0].z, 0.f),
+                                                    fmaxf(va[m][0].w - vb[m][0].w, 0.f));
+                            cur[m][1] = make_float4(fmaxf(va[m][1].x - vb[m][1].x, 0.f), fmaxf(va[m][1].y - vb[m][1].y, 0.f), fmaxf(va[m][1].z - vb[m][1].z, 0.f),
+                                                    fmaxf(va[m][1].w - vb[m][1].w, 0.f));
+                        }
+                    }
+#pragma unroll
+                    for (int m = 0; m < ITEMS; ++m) {
+                        const int idx = ltid + m * SD_NL * 32;
+                        if (idx < 2 * SD_AROWS) {
+                            const int h = idx >= SD_AROWS ? 1 : 0, r = idx - h * SD_AROWS;
+                            const float xs[8] = {cur[m][0].x, cur[m][0].y, cur[m][0].z, cur[m][0].w, cur[m][1].x, cur[m][1].y, cur[m][1].z, cur[m][1].w};
+                            uint32_t hi[4], lo[4];
+#pragma unroll
+                            for (int e = 0; e < 4; ++e) {
+                                const __half2 hh = __floats2half2_rn(xs[2 * e], xs[2 * e + 1]);
+                                const float2 hf = __half22float2(hh);
+                                const __half2 ll = __floats2half2_rn((xs[2 * e] - hf.x) * 2048.0f, (xs[2 * e + 1] - hf.y) * 2048.0f);
+                                hi[e] = *reinterpret_cast<const uint32_t *>(&hh);
+                                lo[e] = *reinterpret_cast<const uint32_t *>(&ll);
+                                amax = fmaxf(amax, fmaxf(fabsf(xs[2 * e]), fabsf(xs[2 * e + 1])));
+                            }
+                            *reinterpret_cast<uint4 *>(dst + (size_t)h * SD_KBYTES + (size_t)r * 16) = make_uint4(hi[0], hi[1], hi[2], hi[3]);
+                            *reinterpret_cast<uint4 *>(dst + (size_t)(2 + h) * SD_KBYTES + (size_t)r * 16) = make_uint4(lo[0], lo[1], lo[2], lo[3]);
+                        }
+                    }
+                    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");     // generic-proxy stores -> tensor-core (async proxy) reads
+                    __syncwarp();
+                    if (lane == 0) mbar_arrive(bar_base + 8u * (BAR_AFULL + slot));
+#pragma unroll
+                    for (int m = 0; m < ITEMS; ++m) { cur[m][0] = nxt[m][0]; cur[m][1] = nxt[m][1]; }
+                    t = tn; c = cn; ++j;
+                }
+                if (!(amax < 65000.0f) && p.flag) atomicOr(p.flag, 1);   // also true for NaN
+            }
+        } else {
+            // =========================== weight producer ========================================================
+            if (lane == 0) {
+                const int n_st = nchunks * 3;
+                uint32_t q = 0;
+                for (uint32_t k = 0; tile_of(k) >= 0; ++k) {
+                    if (resident && k >= 1) break;                      // resident weights: loaded by the first tile, never again
+                    for (int s = 0; s < n_st; ++s, ++q) {
+                        const uint32_t sb = q % (uint32_t)NBS, use = q / (uint32_t)NBS;
+                        if (use > 0) mbar_wait(bar_base + 8u * (BAR_BEMPTY + sb), (use - 1) & 1u);
+                        mbar_arrive_expect_tx(bar_base + 8u * (BAR_BFULL + sb), (uint32_t)C::B_STAGE);
+                        bulk_g2s(b_base + sb * (uint32_t)C::B_STAGE, reinterpret_cast<const unsigned char *>(p.w) + (size_t)s * C::B_STAGE,
+                                 (uint32_t)C::B_STAGE, bar_base + 8u * (BAR_BFULL + sb));
                     }
                 }
             }
             __syncwarp();
-        } else {
-        // =========================== loaders: fp32 activations -> fp16 hi/lo chunk images ====================
-            // A chunk image is 2 x 176 items of (row, 8 channels) = two 16-byte loads each; thread `ltid` owns the items ltid,
-            // ltid + 128, ltid + 256 of EVERY chunk.  The activations come from HBM: all six loads of a chunk are issued at once
-            // and the loads of chunk j + 1 are in flight while chunk j is converted, so no chunk waits a whole exposed round trip.
-            constexpr int ITEMS = (2 * SD_AROWS + SD_NL * 32 - 1) / (SD_NL * 32);      // 3
-            const int ltid = tid - SD_NC * 32;
-            const float4 *in4 = reinterpret_cast<const float4 *>(p.in);
-            float amax = 0.0f;
-            float4 cur[ITEMS][2], nxt[ITEMS][2];
-            auto issue = [&](int t, int c, float4 (&v)[ITEMS][2]) {
-                const long long p0 = (long long)t * SD_BM;
-#pragma unroll
-                for (int m = 0; m < ITEMS; ++m) {
-                    const int idx = ltid + m * SD_NL * 32;
-                    v[m][0] = make_float4(0.f, 0.f, 0.f, 0.f);
-                    v[m][1] = v[m][0];
-                    if (idx < 2 * SD_AROWS) {
-                        const int h = idx >= SD_AROWS ? 1 : 0, r = idx - h * SD_AROWS;
-                        const long long pr = p0 + r;
-                        const int s = (int)(pr / p.rs), q = (int)(pr - (long long)s * p.rs);
-                        const int yp = q / 22, xp = q - yp * 22;
-                        if (s < n_samples && (yp != 0 || !p.cyl) && !p.fa) {
-                            const int xx = xp == 0 ? 19 : (xp == 21 ? 0 : xp - 1);
-                            int pos = p.cyl ? (yp - 1) * 20 + xx : q, g0;       // valid rasters: the row IS the input position
-                            if (p.is3d) { pos += c * 140; g0 = h * 2; } else { g0 = c * 4 + h * 2; }
-                            const float4 *src = in4 + ((size_t)s * p.G_in + g0) * p.S_in + pos;
-                            v[m][0] = __ldg(src);
-                            v[m][1] = __ldg(src + p.S_in);
-                        }
-                    }
-                }
-            };
-            int j = 0;
-            int t = blockIdx.x, c = 0;
-            if (t < n_tiles) issue(t, 0, cur);
-            while (t < n_tiles) {
-                // position of the chunk after this one
-                int tn = t, cn = c + 1;
-                if (cn == nchunks) { cn = 0; tn = t + gridDim.x; }
-                if (tn < n_tiles) issue(tn, cn, nxt);
-                const int slot = j % NA;
-                if (j >= NA) mbar_wait(bar_base + 8u * (BAR_AEMPTY + slot), (uint32_t)(((j / NA) - 1) & 1));
-                unsigned char *dst = smem + (size_t)slot * SD_CHUNK;
-                if (p.fa) {
-                    // second CostNet layer: the first layer's activation relu(A[c][k][(l - n) mod 20] - B[c][k][l]) is regenerated
-                    // here from the factor maps (models/BUFFERX.py:39-69 + patchnet.py:192-198, factorised by bx_costvol_ab).  Raster
-                    // row q = (n, l) of the 18 x 18 grid; chunk c = (k = c / 2, channels 16 * (c % 2) ...): the k dimension of the
-                    // 3x3x3 kernel is folded into the channels, the taps are (dn, dl).  The 14.6 KB of factors per match are L2
-                    // hits, so all loads of the chunk are issued here, no cross-chunk prefetch.
-                    const long long p0 = (long long)t * SD_BM;
-                    const int kk = c >> 1, cb = (c & 1) * 4;
-                    float4 va[ITEMS][2], vb[ITEMS][2];
-#pragma unroll
-                    for (int m = 0; m < ITEMS; ++m) {
-                        const int idx = ltid + m * SD_NL * 32;
-                        va[m][0] = va[m][1] = vb[m][0] = vb[m][1] = make_float4(0.f, 0.f, 0.f, 0.f);
-                        if (idx < 2 * SD_AROWS) {
-                            const int h = idx >= SD_AROWS ? 1 : 0, r = idx - h * SD_AROWS;
-                            const long long pr = p0 + r;
-                            const int s = (int)(pr / 324), q = (int)(pr - (long long)s * 324);
-                            const int nn = q / 18, ll = q - nn * 18;
-                            if (s < n_samples) {
-                                int sh = ll - nn;
-                                sh = sh < 0 ? sh + 20 : sh;
-                                const float4 *sa = reinterpret_cast<const float4 *>(p.fa) + ((size_t)s * 8 + cb + h * 2) * 60 + kk * 20 + sh;
-                                const float4 *sb = reinterpret_cast<const float4 *>(p.fb) + ((size_t)s * 8 + cb + h * 2) * 54 + kk * 18 + ll;
-                                va[m][0] = __ldg(sa); va[m][1] = __ldg(sa + 60);
-                                vb[m][0] = __ldg(sb); vb[m][1] = __ldg(sb + 54);
-                            }
-                        }
-                    }
-#pragma unroll
-                    for (int m = 0; m < ITEMS; ++m) {
-                        cur[m][0] = make_float4(fmaxf(va[m][0].x - vb[m][0].x, 0.f), fmaxf(va[m][0].y - vb[m][0].y, 0.f), fmaxf(va[m][0].z - vb[m][0].z, 0.f),
-                                                fmaxf(va[m][0].w - vb[m][0].w, 0.f));
-                        cur[m][1] = make_float4(fmaxf(va[m][1].x - vb[m][1].x, 0.f), fmaxf(va[m][1].y - vb[m][1].y, 0.f), fmaxf(va[m][1].z - vb[m][1].z, 0.f),
-                                                fmaxf(va[m][1].w - vb[m][1].w, 0.f));
-                    }
-                }
-#pragma unroll
-                for (int m = 0; m < ITEMS; ++m) {
-                    const int idx = ltid + m * SD_NL * 32;
-                    if (idx < 2 * SD_AROWS) {
-                        const int h = idx >= SD_AROWS ? 1 : 0, r = idx - h * SD_AROWS;
-                        const float xs[8] = {cur[m][0].x, cur[m][0].y, cur[m][0].z, cur[m][0].w, cur[m][1].x, cur[m][1].y, cur[m][1].z, cur[m][1].w};
-                        uint32_t hi[4], lo[4];
-#pragma unroll
-                        for (int e = 0; e < 4; ++e) {
-                            const __half2 hh = __floats2half2_rn(xs[2 * e], xs[2 * e + 1]);
-                            const float2 hf = __half22float2(hh);
-                            const __half2 ll = __floats2half2_rn((xs[2 * e] - hf.x) * 2048.0f, (xs[2 * e + 1] - hf.y) * 2048.0f);
-                            hi[e] = *reinterpret_cast<const uint32_t *>(&hh);
-                            lo[e] = *reinterpret_cast<const uint32_t *>(&ll);
-                            amax = fmaxf(amax, fmaxf(fabsf(xs[2 * e]), fabsf(xs[2 * e + 1])));
-                        }
-                        *reinterpret_cast<uint4 *>(dst + (size_t)h * SD_KBYTES + (size_t)r * 16) = make_uint4(hi[0], hi[1], hi[2], hi[3]);
-                        *reinterpret_cast<uint4 *>(dst + (size_t)(2 + h) * SD_KBYTES + (size_t)r * 16) = make_uint4(lo[0], lo[1], lo[2], lo[3]);
-                    }
-                }
-                asm volatile("fence.proxy.async.shared::cta;" ::: "memory");     // generic-proxy stores -> tensor-core (async proxy) reads
-                __syncwarp();
-                if (lane == 0) mbar_arrive(bar_base + 8u * (BAR_AFULL + slot));
-#pragma unroll
-                for (int m = 0; m < ITEMS; ++m) { cur[m][0] = nxt[m][0]; cur[m][1] = nxt[m][1]; }
-                t = tn; c = cn; ++j;
-            }
-            if (!(amax < 65000.0f) && p.flag) atomicOr(p.flag, 1);   // also true for NaN
         }
-    } else {
-        // =========================== weight producer ========================================================
-        if (lane == 0) {
-            const int n_st = nchunks * 3;
-            uint32_t q = 0;
-            for (uint32_t k = 0; tile_of(k) >= 0; ++k) {
-                if (resident && k >= 1) break;                      // resident weights: loaded by the first tile, never again
-                for (int s = 0; s < n_st; ++s, ++q) {
-                    const uint32_t sb = q % (uint32_t)NBS, use = q / (uint32_t)NBS;
-                    if (use > 0) mbar_wait(bar_base + 8u * (BAR_BEMPTY + sb), (use - 1) & 1u);
-                    mbar_arrive_expect_tx(bar_base + 8u * (BAR_BFULL + sb), (uint32_t)C::B_STAGE);
-                    bulk_g2s(b_base + sb * (uint32_t)C::B_STAGE, reinterpret_cast<const unsigned char *>(p.w) + (size_t)s * C::B_STAGE,
-                             (uint32_t)C::B_STAGE, bar_base + 8u * (BAR_BFULL + sb));
-                }
-            }
-        }
-        __syncwarp();
     }
     __syncthreads();
     if (dyn && tid == 0) {      // the last CTA to finish rewinds the counters for the next launch that uses them
