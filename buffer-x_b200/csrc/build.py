@@ -20,7 +20,7 @@ OUT = os.path.join(PKG, "libbufferx_b200.so")
 OBJ = os.path.join(HERE, "_obj")
 
 EXACT = ["bx_api.cu", "bx_fps.cu", "bx_radius.cu", "bx_patches.cu", "bx_spt.cu", "bx_match.cu", "bx_ransac.cu", "bx_neighbors.cu",
-         "bx_bootstrap.cu"]
+         "bx_bootstrap.cu", "bx_train.cu"]
 FAST = ["bx_conv.cu", "bx_conv_tc.cu", "bx_conv_sd.cu"]
 ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 COMMON = ["-O3", "-lineinfo", "-std=c++17", "-Xcompiler", "-fPIC,-fvisibility=hidden", "--expt-relaxed-constexpr"]

@@ -1,4 +1,4 @@
-"""BufferX on H100: the per-pair registration ``forward()``.
+"""BufferX on H100: the per-pair registration ``forward()`` and, in eval mode, the training stages' validation forward.
 
 Mirrors ``BufferX`` of /root/reference/models/BUFFERX.py (constructor :72-84, inference branch of
 ``forward`` :257-467, ``mutual_matching`` :469-496, ``post_refinement`` :522-556): same attribute names
@@ -465,10 +465,105 @@ class BufferX(nn.Module):
         net.overflow_flag(next(self.parameters()).device).zero_()
         return self.forward(data_source, perms=perms, ransac_seed=ransac_seed, debug=debug)
 
-    def forward(self, data_source, perms=None, ransac_seed=None, debug=False):
+    # ------------------------------------------------------------------------------------------------
+    def _draw_des_r(self):
+        """Descriptor radius of the training branch (reference BUFFERX.py:175-198), drawn from NumPy's global RNG."""
+        cfg = self.config
+        name, center = cfg.data.dataset, cfg.patch.des_r
+        if name == "3DMatch":
+            lo, hi = center * 0.5, center * 1.5
+            return np.round(np.clip(np.random.normal(center, (hi - lo) / 6, 1), lo, hi), 2)[0]
+        if name == "KITTI":
+            values = {3.0: [2.0, 2.5, 3.0, 3.5, 4.0], 0.3: [0.2, 0.25, 0.3, 0.35, 0.4]}.get(center)
+            if values is None:
+                raise ValueError(f"KITTI training radii are defined for des_r 3.0 and 0.3, not {center}")
+            return np.random.choice(values, p=[0.2, 0.2, 0.2, 0.2, 0.2])
+        return center
+
+    def _train_forward(self, data_source, perms=None, aug_angles=None, match_choice=None):
+        """Validation forward of cfg.stage "Desc" / "Pose" in eval mode (reference BUFFERX.py:148-255): ground-truth
+        correspondences on the second-level clouds, descriptors of the (sub-sampled) matched key-points, then EquiMatch
+        score + integer SO(2) label ("Desc") or CostNet soft arg-max + float SO(2) label of the augmented target ("Pose").
+        NumPy's global RNG is consumed like the reference: match sub-sampling (only beyond cfg.train.pos_num), des_r,
+        source permutation, target permutation, augmentation angles.  ``perms`` = (src, tgt) permutations, ``aug_angles``
+        [K] and ``match_choice`` (rows of the match list) replace the respective draws.  Device->host reads: the number of
+        ground-truth matches (it sizes the draw), and at the end the fp16-range flag of the convolution kernels."""
+        cfg = self.config
+        stage = cfg.stage
+        dev = next(self.parameters()).device
+        azi_n = cfg.patch.azi_n
+
+        def _pts(x, shape=(-1, 3)):
+            return torch.as_tensor(x).to(dev, dtype=torch.float32, non_blocking=True).reshape(*shape).contiguous()
+
+        rng_state = np.random.get_state()     # replayed if the pair has to be recomputed on the TF32 kernels
+        with torch.cuda.device(dev):
+            src, tgt = _pts(data_source["src_fds_pcd"]), _pts(data_source["tgt_fds_pcd"])
+            src_sds, tgt_sds = _pts(data_source["src_sds_pcd"]), _pts(data_source["tgt_sds_pcd"])
+            T = _pts(data_source["relt_pose"], (4, 4))
+            vs = data_source["voxel_sizes"]
+            voxel = float(vs.reshape(-1)[0].item() if isinstance(vs, torch.Tensor) else np.asarray(vs, dtype=np.float32).reshape(-1)[0])
+            pairs, d_cnt = ops.gt_matches(src_sds, tgt_sds, T, voxel)
+            n_match = int(d_cnt.item())
+            match = pairs[:n_match]
+            if match_choice is not None:
+                match = match[torch.as_tensor(np.asarray(match_choice), dtype=torch.long).to(dev)]
+            elif n_match > cfg.train.pos_num:
+                rand_ind = np.random.choice(range(n_match), cfg.train.pos_num, replace=False)
+                match = match[torch.from_numpy(rand_ind).to(dev)]
+            if match.shape[0] == 0:
+                print(f"{data_source.get('src_id')} {data_source.get('tgt_id')} has no keypts")
+                return None
+            match = match.long()
+            src_kpt, tgt_kpt = src_sds[match[:, 0]].contiguous(), tgt_sds[match[:, 1]].contiguous()
+            des_r = self._draw_des_r()
+            aligned = bool(data_source["is_aligned_to_global_z"])
+            ps, pt = (None, None) if perms is None else perms
+            src_d = self.Desc(src[None], src_kpt[None], des_r, aligned, perm=ps)
+            tgt_d = self.Desc(tgt[None], tgt_kpt[None], des_r, aligned, None, stage == "Pose", perm=pt, aug_angles=aug_angles)
+            K = src_kpt.shape[0]
+            if K < 2:
+                print(f"{data_source.get('src_id')} {data_source.get('tgt_id')} don't have enough patches")
+                return None
+            if stage == "Desc":
+                out = {"src_kpt": src_kpt, "tgt_kpt": tgt_kpt, "src_des": src_d["desc"], "tgt_des": tgt_d["desc"],
+                       "equi_score": ops.equi_match(src_d["equi"], tgt_d["equi"]),
+                       "gt_label": ops.so2_gt(src_d["rand_axis"], src_d["R"], tgt_d["R"], T, azi_n, True)}
+            else:
+                # patch i of the source against patch i of the target: identity match lists through CostNet, the soft
+                # arg-max from the hypothesis kernel (its pose outputs land in scratch buffers)
+                ids = torch.arange(K, dtype=torch.int32, device=dev)
+                d_K = torch.full((1,), K, dtype=torch.int32, device=dev)
+                logits = self.Pose.logits(src_d["equi"], tgt_d["equi"], ids, ids, d_K, K)
+                pred = torch.empty(K, dtype=torch.float32, device=dev)
+                offs = torch.zeros(2, dtype=torch.int32, device=dev)
+                scratch = [torch.empty((K, 3, 3), dtype=torch.float32, device=dev)] + \
+                          [torch.empty((K, 3), dtype=torch.float32, device=dev) for _ in range(3)]
+                ops.hypotheses(logits, azi_n, src_kpt, tgt_kpt, src_d["R"], tgt_d["R"], ids, ids, d_K, K, offs[0:1], offs[1:2], pred,
+                               *scratch)
+                out = {"pred_ind": pred,
+                       "gt_ind": ops.so2_gt(src_d["rand_axis"], src_d["R"], tgt_d["R"], T, azi_n, False, aug_R=tgt_d["aug_rotation"])}
+            overflow = self.Desc.conv_net.overflow_flag(dev).item() != 0
+        if overflow:      # an activation left fp16 range: recompute the pair with the TF32 kernels and the same draws
+            np.random.set_state(rng_state)
+            net = self.Desc.conv_net
+            net.force_tf32 = True
+            self.Pose.conv.force_tf32 = True
+            self._drop_captured_state()
+            net.overflow_flag(dev).zero_()
+            return self._train_forward(data_source, perms, aug_angles, match_choice)
+        return out
+
+    def forward(self, data_source, perms=None, ransac_seed=None, debug=False, aug_angles=None, match_choice=None):
         cfg = self.config
         if cfg.stage != "test":
-            raise NotImplementedError("bufferx_b200 implements the inference hot path (cfg.stage == 'test')")
+            if cfg.stage not in ("Desc", "Pose") or self.training:
+                raise NotImplementedError(
+                    "bufferx_b200 runs cfg.stage 'test' and, in eval mode, the validation forward of the training stages "
+                    "'Desc' / 'Pose'; training-mode BatchNorm and the backward pass are not built (call model.eval())")
+            if next(self.parameters()).device.type != "cuda":
+                raise ops.BufferXError("BufferX.forward needs the model on a CUDA device: there is no CPU path")
+            return self._train_forward(data_source, perms, aug_angles, match_choice)
         dev = next(self.parameters()).device
         if dev.type != "cuda":
             raise ops.BufferXError("BufferX.forward needs the model on a CUDA device: there is no CPU path")

@@ -2,7 +2,7 @@
 
 Mirrors ``MiniSpinNet`` of /root/reference/models/patch_embedder.py (constructor :16-42, forward :44-90,
 same sub-module names -> same state_dict keys ``pnt_layer.{0,1}``, ``pool_layer.{0,1,3,4}``,
-``conv_net.ops.*``).  Inference only: select_patches -> axis_align -> normalize -> SPT -> pnt_layer+max ->
+``conv_net.ops.*``).  Eval mode only: select_patches -> axis_align -> normalize -> SPT -> pnt_layer+max ->
 Cylindrical_Net -> attention pooling, every stage a hand-written CUDA kernel behind the C-ABI.
 """
 import numpy as np
@@ -78,11 +78,14 @@ class MiniSpinNet(nn.Module):
             )
         return self._prep
 
-    def forward(self, pts, kpts, des_r, is_aligned_to_global_z, z_axis=None, is_aug=False, perm=None, debug=False):
+    def forward(self, pts, kpts, des_r, is_aligned_to_global_z, z_axis=None, is_aug=False, perm=None, debug=False, aug_angles=None):
         """pts [1,N,3], kpts [1,K,3] CUDA f32; des_r python float or 1-element CUDA tensor.
-        ``perm`` (optional int32 [N]) replaces the host draw of the reference (patch_embedder.py:96)."""
-        if z_axis is not None or is_aug:
-            raise NotImplementedError("training-time options (z_axis / SO(2) augmentation) are outside the inference hot path")
+        ``perm`` (optional int32 [N]) replaces the host draw of the reference (patch_embedder.py:96).
+        ``is_aug``: SO(2) augmentation of the normalised patches and rand_axis (patch_embedder.py:54-67), one z-rotation per
+        patch; the angles are drawn from NumPy's global RNG after the permutation, like the reference, unless ``aug_angles``
+        ([K] fp32) are given.  ``aug_rotation`` is then the [K,3,3] rotations (None without augmentation)."""
+        if z_axis is not None:
+            raise NotImplementedError("an externally supplied z_axis is a training-time option outside the forward built here")
         pts = pts[0].contiguous()
         kpts = kpts[0].contiguous()
         dev = pts.device
@@ -96,6 +99,13 @@ class MiniSpinNet(nn.Module):
         pts4 = ops.permute_cloud(pts, perm)
         patches, idx = ops.select_patches(pts4, kpts, des_r, self.patch_sample, want_idx=debug)
         delta, R, rand_axis = ops.lrf(patches, des_r, bool(is_aligned_to_global_z))
+        aug_R = None
+        if is_aug:
+            if aug_angles is None:
+                # the reference draws angles = r * 2 * pi in fp64 and casts them to fp32
+                aug_angles = (np.random.random([kpts.shape[0], 1]) * 2 * np.pi)[:, 0].astype(np.float32)
+            ang = torch.as_tensor(np.ascontiguousarray(aug_angles, dtype=np.float32)).to(dev, non_blocking=True)
+            aug_R = ops.so2_augment(delta, rand_axis, ang)
         res = ops.spt_pnt(delta, prep["voxels"], prep["rot"], self.delta / self.rad_n, self.voxel_sample, prep["w_pnt"],
                           prep["b_pnt"], self.azi_n, debug=debug)
         feat = res[0] if debug else res                                  # [K,4,V,4] channel-blocked
@@ -106,7 +116,7 @@ class MiniSpinNet(nn.Module):
         else:
             x, _ = self.conv_net(feat)                                   # [K,8,140,4] channel-blocked
             desc, equi = ops.pool_desc(x, prep["w1"], prep["b1"], prep["w2"], prep["b2"], channels_last=True)
-        out = {"desc": desc, "equi": equi, "rand_axis": rand_axis, "R": R, "patches": delta, "aug_rotation": None}
+        out = {"desc": desc, "equi": equi, "rand_axis": rand_axis, "R": R, "patches": delta, "aug_rotation": aug_R}
         if debug:
             x_cf = x if pn.USE_FFMA else ops.from_blocked(x).view(K, -1, self.ele_n, self.azi_n)
             out.update(idx=idx, raw_patches=patches, vidx=res[1], inv=res[2], feat=ops.from_blocked(feat), x=x_cf)

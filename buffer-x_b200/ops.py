@@ -24,6 +24,7 @@ SYMBOLS = [
     "bx_hypotheses", "bx_consensus", "bx_ransac_workspace_bytes", "bx_ransac", "bx_refine", "bx_conv_tc_set_segment_stages",
     "bx_radius_neighbors", "bx_grid_subsample", "bx_costvol_ab", "bx_concat_matches",
     "bx_pca_analysis", "bx_project_range", "bx_voxel_down_sample", "bx_conv_layer_sd", "bx_conv_sd_rows", "bx_spt_pnt_sd", "bx_fps_set_sync_mode", "bx_select_patches_seg", "bx_select_patches_workspace_bytes", "bx_conv_layer_sd_costab", "bx_lrf_batched", "bx_select_patches_batched", "bx_fps_ex", "bx_select_patches_grid", "bx_select_patches_grid_workspace_bytes", "bx_select_patches_grid_batched",
+    "bx_gt_matches", "bx_so2_augment", "bx_equi_match", "bx_so2_gt",
 ]
 
 GEOM_CYL3D, GEOM_CYL2D, GEOM_VALID3D, GEOM_COSTVOL, GEOM_COSTAB = 0, 1, 2, 3, 4
@@ -95,6 +96,10 @@ def load_library():
     lib.bx_refine.argtypes = [P, P, P, c_int, P, c_float, P, P, P]
     lib.bx_radius_neighbors.argtypes = [P, c_int, P, c_int, P, c_int, P, c_int, c_float, P, c_int, P, P, P, P]
     lib.bx_grid_subsample.argtypes = [P, c_int, c_float, P, P, c_int, P, P, P, P, P, P]
+    lib.bx_gt_matches.argtypes = [P, c_int, P, c_int, P, c_float, P, P, P, P]
+    lib.bx_so2_augment.argtypes = [P, c_int, c_int, P, P, P, P]
+    lib.bx_equi_match.argtypes = [P, P, c_int, c_int, c_int, c_int, P, P]
+    lib.bx_so2_gt.argtypes = [P, P, P, P, P, c_int, c_int, P, P, P]
     _lib = lib
     return lib
 
@@ -735,3 +740,51 @@ def voxel_down_sample(points: torch.Tensor, voxel: float):
                                     _dp(cnt), _dp(dm), _stream()), "bx_voxel_down_sample")
     m = int(dm.item())
     return keys[:m], xyz[:m], cnt[:m]
+
+
+# --------------------------------------------------------------------------- #
+# training stages' validation forward (cfg.stage "Desc" / "Pose", eval mode)
+# --------------------------------------------------------------------------- #
+def gt_matches(src: torch.Tensor, tgt: torch.Tensor, T: torch.Tensor, voxel: float):
+    """Ground-truth correspondences: src [N,3], tgt [M,3], T [4,4] f32 -> (pairs [N,2] int32, count [1] int32 on the device);
+    rows >= count are undefined."""
+    N, M = src.shape[0], tgt.shape[0]
+    dev = src.device
+    nn = torch.empty(max(N, 1), dtype=I32, device=dev)
+    pairs = torch.empty((max(N, 1), 2), dtype=I32, device=dev)
+    cnt = torch.zeros(1, dtype=I32, device=dev)
+    _check(load_library().bx_gt_matches(_dp(src, F32, "src"), N, _dp(tgt, F32, "tgt"), M, _dp(T, F32, "T"), float(voxel), _dp(nn), _dp(pairs),
+                                        _dp(cnt), _stream()), "bx_gt_matches")
+    return pairs, cnt
+
+
+def so2_augment(delta: torch.Tensor, rand_axis: torch.Tensor, angles: torch.Tensor, aug_R: torch.Tensor | None = None):
+    """Rotates delta [K,P,3] and rand_axis [K,3] in place about z by angles [K] (f32); returns aug_R [K,3,3]."""
+    K, P, _ = delta.shape
+    if aug_R is None:
+        aug_R = torch.empty((K, 3, 3), dtype=F32, device=delta.device)
+    _check(load_library().bx_so2_augment(_dp(delta, F32, "delta"), K, P, _dp(rand_axis, F32, "rand_axis"), _dp(angles, F32, "angles"), _dp(aug_R),
+                                         _stream()), "bx_so2_augment")
+    return aug_R
+
+
+def equi_match(d1: torch.Tensor, d2: torch.Tensor, out: torch.Tensor | None = None):
+    """EquiMatch score of two [B,C,K,L] equivariant maps -> [B,L]."""
+    B, C, K, L = d1.shape
+    if tuple(d2.shape) != (B, C, K, L):
+        raise BufferXError(f"equi_match: shapes {tuple(d1.shape)} and {tuple(d2.shape)} differ")
+    if out is None:
+        out = torch.empty((B, L), dtype=F32, device=d1.device)
+    _check(load_library().bx_equi_match(_dp(d1, F32, "d1"), _dp(d2, F32, "d2"), B, C, K, L, _dp(out, F32, "out"), _stream()), "bx_equi_match")
+    return out
+
+
+def so2_gt(s_rand_axis, s_R, t_R, T, azi_n: int, integer: bool, aug_R=None):
+    """SO(2) label of every patch: int64 [P] (integer=True) or float32 [P]."""
+    P = s_rand_axis.shape[0]
+    dev = s_rand_axis.device
+    out = torch.empty(P, dtype=torch.int64 if integer else F32, device=dev)
+    li, lf = (_dp(out), None) if integer else (None, _dp(out))
+    _check(load_library().bx_so2_gt(_dp(s_rand_axis, F32, "s_rand_axis"), _dp(s_R, F32, "s_R"), _dp(t_R, F32, "t_R"), _dp(T, F32, "T"),
+                                    _dp(aug_R, F32, "aug_R"), P, int(azi_n), li, lf, _stream()), "bx_so2_gt")
+    return out

@@ -30,7 +30,7 @@ import numpy as np
 
 from .config import make_cfg
 
-__all__ = ["make_pair", "workload_cfg", "WORKLOADS"]
+__all__ = ["make_pair", "workload_cfg", "add_training_clouds", "WORKLOADS"]
 
 WORKLOADS = ("C1", "C2", "C3", "C5")
 
@@ -247,6 +247,40 @@ def make_pair(name: str = "C2", seed: int = 0, n_src: int | None = None, n_tgt: 
         "sphericity": np.array([0.0], dtype=np.float32),
         "is_aligned_to_global_z": aligned,
     }
+
+
+def _voxel_means(pts, voxel):
+    """Voxel grid down-sample (Open3D's voxel_down_sample rule: cells of ``voxel`` from min - voxel/2, fp64 mean of the
+    points of a cell), cells in ascending (ix, iy, iz) key order, fp32 out."""
+    P = np.asarray(pts, dtype=np.float64)
+    iv = np.floor((P - (P.min(axis=0) - voxel * 0.5)) / voxel).astype(np.int64)
+    keys = iv[:, 0] | (iv[:, 1] << 21) | (iv[:, 2] << 42)
+    uk, inv, cnt = np.unique(keys, return_inverse=True, return_counts=True)
+    sums = np.zeros((len(uk), 3))
+    np.add.at(sums, inv, P)
+    return (sums / cnt[:, None]).astype(np.float32)
+
+
+def add_training_clouds(data, cfg, voxel=None, isolated=False):
+    """Make a synthetic pair look like the training loader's collate dict: ``src_sds_pcd`` / ``tgt_sds_pcd`` (second-level
+    clouds, voxel down-sample of the first-level clouds at ``cfg.data.voxel_size_0`` unless ``voxel`` is given) and
+    ``voxel_sizes`` = [voxel].  ``isolated=True`` appends one corresponding point pair (p and relt_pose p) at least 2 m
+    away from both first-level clouds: a key-point whose ball query comes back empty."""
+    v = float(cfg.data.voxel_size_0 if voxel is None else voxel)
+    out = dict(data)
+    src_sds, tgt_sds = _voxel_means(data["src_fds_pcd"], v), _voxel_means(data["tgt_fds_pcd"], v)
+    if isolated:
+        T = np.asarray(data["relt_pose"], dtype=np.float64)
+        p = np.asarray(data["src_fds_pcd"], dtype=np.float64).max(axis=0) + 3.0
+        q = T[:3, :3] @ p + T[:3, 3]
+        for cloud, x in ((data["src_fds_pcd"], p), (data["tgt_fds_pcd"], q)):
+            if np.sqrt(((np.asarray(cloud, dtype=np.float64) - x) ** 2).sum(1)).min() < 2.0:
+                raise RuntimeError("isolated point is not isolated")
+        src_sds = np.concatenate([src_sds, p[None].astype(np.float32)])
+        tgt_sds = np.concatenate([tgt_sds, q[None].astype(np.float32)])
+    out["src_sds_pcd"], out["tgt_sds_pcd"] = src_sds, tgt_sds
+    out["voxel_sizes"] = np.array([v], dtype=np.float32)
+    return out
 
 
 POSE_TRAINED = os.path.join(os.path.dirname(os.path.abspath(__file__)), "data", "pose_synth_trained.npz")

@@ -307,6 +307,26 @@ int bx_voxel_down_sample(const float *pts, int n, double voxel, unsigned long lo
                          int table_cap, unsigned long long *minmax6, unsigned long long *keys_out, float *xyz_out,
                          int32_t *cnt_out, int32_t *d_m, void *stream);
 
+/* ---- SURVEY 8(f) row 3: the training stages' validation forward (cfg.stage "Desc" / "Pose", eval mode) ----------
+ * bx_gt_matches replaces BufferX.get_matching_indices (models/BUFFERX.py:498-520): every source point is moved by the
+ * row-major 4x4 T (utils/SE3.transform, each row ((r0*x + r1*y) + r2*z) + t), its nearest target point is found by a
+ * brute-force scan (knn_cuda k = 1: the first minimum in target order wins ties) and [i, nn(i)] is kept when
+ * sqrt(d2) < voxel.  nn_ws [N] int32 workspace; pairs [N,2] int32 in source order; *d_count = pairs kept.
+ * bx_so2_augment is the SO(2) augmentation of MiniSpinNet.forward (models/patch_embedder.py:54-67): patch k of delta
+ * [K,P,3] and rand_axis [K,3] are rotated in place by the kornia axis-angle matrix of (0, 0, angles[k]); aug_R [K,3,3]
+ * (may be NULL) receives the rotations.
+ * bx_equi_match is EquiMatch (models/BUFFERX.py:16-36): cor[b,a] = sum_{c,k,l} D1[b,c,k,(l-a) mod L] * D2[b,c,k,l] over
+ * [B,C,K,L] maps (L <= 32, both maps of a patch in shared memory), fixed fp32 summation order.
+ * bx_so2_gt is BufferX.cal_so2_gt (models/BUFFERX.py:86-126) on s_rand_axis [P,3], the LRFs s_R / t_R [P,3,3], the
+ * ground-truth pose T [4,4] and optional aug_R [P,3,3]: exactly one of label_int [P] (rounded, azi_n -> 0) and
+ * label_float [P] is written. */
+int bx_gt_matches(const float *src, int N, const float *tgt, int M, const float *T, float voxel, int32_t *nn_ws,
+                  int32_t *pairs, int32_t *d_count, void *stream);
+int bx_so2_augment(float *delta, int K, int P, float *rand_axis, const float *angles, float *aug_R, void *stream);
+int bx_equi_match(const float *D1, const float *D2, int B, int C, int K, int L, float *cor, void *stream);
+int bx_so2_gt(const float *s_rand_axis, const float *s_R, const float *t_R, const float *T, const float *aug_R, int P,
+              int azi_n, long long *label_int, float *label_float, void *stream);
+
 #ifdef __cplusplus
 }
 #endif
