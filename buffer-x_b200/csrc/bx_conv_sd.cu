@@ -18,25 +18,45 @@
 //               tensor rate and half the operand bytes):  a*b ~= ah*bh + (al*bh + ah*bl) * 2^-11.  Per 16-channel chunk
 //               (K = 144) the products go to a fresh accumulator [main | cross]; the finished chunk's main + cross * 2^-11 is
 //               added with round-to-nearest into fp32 running sums that start from the bias, so no accumulation chain is
-//               longer than one chunk.  A tap is three N = Cout MMAs: ah * bh into main, ah * bl and al * bh into cross.
-//               main and cross are disjoint register blocks, each written only by whole wgmmas: a wgmma that accumulates
-//               into a sub-range of another in-flight wgmma's registers makes ptxas wait for each wgmma before issuing the
-//               next.  Cout 128 takes a chunk in one pass (128 accumulators + 64 running sums per thread, see the register
-//               split below), except with fp32 input, which does two 64-column passes.
+//               longer than one chunk.  main and cross are disjoint register blocks, each written only by whole wgmmas: a
+//               wgmma that accumulates into a sub-range of another in-flight wgmma's registers makes ptxas wait for each
+//               wgmma before issuing the next.
 //               |x| >= 65504 cannot be represented: the loader raises *flag and the host re-runs the layer on the TF32 kernel.
 //
+// Two mainloops, both with the shifted activation views as one operand and the weights as the other:
+//   rows-as-M         (Cout 128, and every fp32-input kernel)  M = 64 tile rows per warpgroup, N = Cout.  A tap is three
+//                     m64nCout wgmmas: ah * bh into main, ah * bl and al * bh into cross.  Cout 128 takes a chunk in one pass
+//                     (128 accumulators + 64 running sums per thread, see the register split below), except with fp32 input,
+//                     which does two 64-column passes.
+//   channels-as-M     (presplit input, Cout <= 64)  M = 64 output channels, N = a whole 128-row tile per warpgroup, so every
+//                     wgmma is m64n128k16 whatever Cout is (a narrow N re-reads the activation tile once per few MACs).  The
+//                     weight image is the A operand and the activation view the B operand; both have the same K-major
+//                     no-swizzle core-matrix layout as before, so a tap is still "base descriptor + (W dy + dx) rows".
+//                     Cout 64: three wgmmas per tap, Wh * ah into main, then Wl * ah and Wh * al into cross.  Cout <= 32: the
+//                     weight image holds, per (chunk, tap, kcore), two 64-row blocks P and Q; in each 16-row group w, P rows
+//                     0-7 / 8-15 are hi / lo of channels 8w .. 8w + 7 and Q rows 0-7 / 8-15 are zero / hi.  P * ah then Q * al
+//                     into ONE accumulator leaves main (Wh * ah + exact zeros) in fragment rows r and cross (Wl * ah, then
+//                     Wh * al) in rows r + 8 of the same thread: two wgmmas per tap and a thread-local fold.  The cross
+//                     products keep the order of the rows-as-M form (ah * bl first), so every element rounds as before.
+//
 // Persistent warp-specialised CTA, one per SM, of three warpgroups:
-//   2 MMA warpgroups  warpgroup g owns tile rows 64 g .. 64 g + 63: per (chunk, tap) its wgmmas read the shifted A view and the
-//                     weights straight from shared memory; after a chunk the accumulators are folded into the running sums
-//                     and the A slot / weight stages are released.  A finished tile goes through a shared-memory staging buffer
-//                     (64 columns at a time) so that each thread then stores one row: ReLU, fp16 hi/lo split and the next
-//                     layer's wrap columns and zero rows, or fp32 channel-blocked values.
+//   2 MMA warpgroups  rows-as-M: warpgroup g owns tile rows 64 g .. 64 g + 63 of the CTA's tile.  channels-as-M: the CTA works
+//                     on a unit of two tiles 2u, 2u + 1 and warpgroup g owns tile 2u + g (for an odd tile count the last unit's
+//                     second warpgroup recomputes tile 2u and stores nothing).  Per (chunk, tap) the wgmmas read the shifted
+//                     activation view and the weights straight from shared memory; after a chunk the accumulators are folded
+//                     into the running sums and the A slot / weight stages are released.  Both warpgroups walk the chunks in
+//                     step, so a streamed weight stage is released when both have used it.  A finished tile goes through a
+//                     shared-memory staging buffer (64 columns, or 64 rows of every channel, at a time) so that each thread
+//                     then stores (half) a row: ReLU, fp16 hi/lo split and the next layer's wrap columns and zero rows, or
+//                     fp32 channel-blocked values.
 //   producer warpgroup, warps 0-2 = A producer, warp 3 = weight thread:
 //   A producer        presplit input: one thread, a chunk = four 2816-byte bulk copies of the previous layer's presplit image
-//                     (ring of NA chunks).  fp32 input: 3 loader warps convert channel-blocked activations to fp16 hi/lo.
-//   weight thread     the host-arranged weight image [chunk][tap][kcore][split][n][8 x fp16] in stages of three taps with
-//                     cp.async.bulk + mbarrier transaction counts; loaded ONCE and kept resident when the whole image fits
-//                     next to three A chunks, else streamed through a ring.
+//                     (ring of NA chunk slots; channels-as-M: slots 2s and 2s + 1 hold the same chunk of the unit's two
+//                     tiles).  fp32 input: 3 loader warps convert channel-blocked activations to fp16 hi/lo.
+//   weight thread     the host-arranged weight image [chunk][tap][kcore][split][n][8 x fp16] (Cout <= 32: [chunk][tap][kcore]
+//                     [P | Q][64][8 x fp16]) in stages of three taps with cp.async.bulk + mbarrier transaction counts; loaded
+//                     ONCE and kept resident when the whole image fits next to three A chunks (four for channels-as-M), else
+//                     streamed through a ring.
 #include <cuda_fp16.h>
 
 #include "bx_common.cuh"
@@ -75,8 +95,12 @@ struct ConvSdParams {
 };
 
 template <int NT, int IN_SD> struct SdCfg {
-    // accumulator block: output columns per pass over a chunk.  All of them, except for Cout 128 with fp32 input, whose
-    // loader warps keep more registers than the 128 accumulators + 64 running sums of a single pass would leave room for.
+    // channels-as-M mainloop (see the header): presplit input with Cout <= 64.  The fp32-input kernels keep rows-as-M: their
+    // MMA threads have 184 registers, too few for 128 accumulators + 64 running sums.
+    static constexpr bool CM = IN_SD && NT < 128;
+    static constexpr int TPU = CM ? 2 : 1;                        // tiles per unit of work of a CTA
+    // rows-as-M accumulator block: output columns per pass over a chunk.  All of them, except for Cout 128 with fp32 input,
+    // whose loader warps keep more registers than the 128 accumulators + 64 running sums of a single pass would leave room for.
     static constexpr int NB = (NT == 128 && !IN_SD) ? 64 : NT;
     static constexpr int NH = NT / NB;                            // passes per chunk
     static constexpr int SB = NT < 64 ? NT : 64;                  // output columns per staging round of a finished tile
@@ -84,8 +108,11 @@ template <int NT, int IN_SD> struct SdCfg {
     // per-thread registers after setmaxnreg: 128 * PROD_REGS + 256 * MMA_REGS = 384 * 168, the CTA's allocation at launch
     // (ptxas reports 168 for every instantiation; a split that asked for more would leave setmaxnreg.inc waiting forever)
     static constexpr int PROD_REGS = IN_SD ? 56 : 136, MMA_REGS = IN_SD ? 224 : 184;
-    static constexpr int B_STAGE = 3 * 64 * NT;                   // three taps of [kcore][split][n][16 B]
-    static constexpr int STAGE_BYTES = SD_BM * SB * 4;            // fp32 staging of one column block of a tile
+    static constexpr int WR = NT < 64 ? 64 : NT;                  // weight rows per (tap, kcore, split): Cout <= 32 is [P | Q] x 64
+    static constexpr int B_STAGE = 3 * 64 * WR;                   // three taps of [kcore][split][WR][16 B]
+    // fp32 staging of a finished tile: rows-as-M, one column block of the CTA's tile [SB / 4][128 rows][4]; channels-as-M (SB
+    // = NT), 64 rows of every channel of each warpgroup's tile, [warpgroup][NT / 4][64 rows][4] -- the same size
+    static constexpr int STAGE_BYTES = SD_BM * SB * 4;
 };
 static_assert(128 * SdCfg<64, 1>::PROD_REGS + 256 * SdCfg<64, 1>::MMA_REGS == 384 * 168, "register split of the presplit kernels");
 static_assert(128 * SdCfg<64, 0>::PROD_REGS + 256 * SdCfg<64, 0>::MMA_REGS == 384 * 168, "register split of the fp32-input kernels");
@@ -186,13 +213,14 @@ __global__ void __launch_bounds__(SdCfg<NT, IN_SD>::THREADS, 1) conv_sd_kernel(c
     const bool resident = p.resident != 0;
     const int n_samples = p.d_n ? min(*p.d_n, p.n) : p.n;
     const int n_tiles = (int)(((long long)n_samples * p.rs + SD_BM - 1) / SD_BM);   // <= the host's bound the grid was sized for
-    // shared memory: A ring | weight ring | staging buffer of one column block of a finished tile, fp32 [NB / 4][128 rows][4]
+    const int n_units = (n_tiles + C::TPU - 1) / C::TPU;
+    // shared memory: A ring | weight ring | staging buffer of a finished tile (C::STAGE_BYTES)
     float *const stage = reinterpret_cast<float *>(smem + (size_t)NA * SD_CHUNK + (size_t)NBS * C::B_STAGE);
 
     if (tid == 0) {
         for (int s = 0; s < SD_MAXNA; ++s) {
             mbar_init(smem_u32(&bars[BAR_AFULL + s]), IN_SD ? 1 : SD_NL);
-            mbar_init(smem_u32(&bars[BAR_AEMPTY + s]), SD_NC);
+            mbar_init(smem_u32(&bars[BAR_AEMPTY + s]), C::CM ? 4 : SD_NC);     // channels-as-M: a slot is one warpgroup's
         }
         for (int s = 0; s < SD_MAXNBS; ++s) {
             mbar_init(smem_u32(&bars[BAR_BFULL + s]), 1);
@@ -208,14 +236,14 @@ __global__ void __launch_bounds__(SdCfg<NT, IN_SD>::THREADS, 1) conv_sd_kernel(c
     uint32_t bar_base = smem_u32(&bars[0]);
     asm volatile("" : "+r"(a_base), "+r"(b_base), "+r"(bar_base));
 
-    // Tile sequence of this CTA.  Static: blockIdx.x, + gridDim.x, ...  Dynamic (presplit input, p.tile_ctr): the A producer
-    // draws the next tile from a global counter and publishes it in a shared-memory ring; every other role reads the k-th
-    // entry (-1 = no more tiles).  With several pairs in flight a convolution often starts with some SMs still held by
-    // another stream's kernels; with the static stride the CTAs that start late still own their share of the tiles and the
-    // whole launch waits for them.
+    // Unit sequence of this CTA (a unit is C::TPU tiles).  Static: blockIdx.x, + gridDim.x, ...  Dynamic (presplit input,
+    // p.tile_ctr): the A producer draws the next unit from a global counter and publishes it in a shared-memory ring; every
+    // other role reads the k-th entry (-1 = no more units).  With several pairs in flight a convolution often starts with some
+    // SMs still held by another stream's kernels; with the static stride the CTAs that start late still own their share of
+    // the tiles and the whole launch waits for them.
     const bool dyn = IN_SD && p.tile_ctr != nullptr;
     auto tile_of = [&](uint32_t k) -> int {
-        if (!dyn) { const long long t = (long long)blockIdx.x + (long long)k * gridDim.x; return t < n_tiles ? (int)t : -1; }
+        if (!dyn) { const long long t = (long long)blockIdx.x + (long long)k * gridDim.x; return t < n_units ? (int)t : -1; }
         mbar_wait(bar_base + 8u * (BAR_TILE + (k & (SD_TRING - 1))), (k / SD_TRING) & 1u);
         return tile_ring[k & (SD_TRING - 1)];
     };
@@ -226,83 +254,175 @@ __global__ void __launch_bounds__(SdCfg<NT, IN_SD>::THREADS, 1) conv_sd_kernel(c
         // =========================== MMA warpgroups: wgmma, chunk folds, tile stores =====================================
         setmaxnreg_inc<C::MMA_REGS>();
         const int wg = warp >> 2, tl = tid & 127;
-        const int r0 = wg * 64 + (warp & 3) * 16 + (lane >> 2);         // fragment rows r0 and r0 + 8 of the tile
-        const int cq = 2 * (lane & 3);                                   // fragment column within an 8-column group
         constexpr uint32_t DESC_HI = 128u >> 4;                          // SBO = 128 B (8 rows x 16 B)
         constexpr uint32_t A_LBO = ((uint32_t)SD_KBYTES >> 4) << 16;    // K-adjacent core matrices: one kcore image apart
-        constexpr uint32_t B_LBO = ((uint32_t)(2 * NT * 16) >> 4) << 16; // weight image [kcore][split(hi,lo)][n][16 B]
-        constexpr uint32_t A_SPLIT = (2u * SD_KBYTES) >> 4, B_TAP16 = (64u * NT) >> 4, B_LO16 = (uint32_t)(NT * 16) >> 4;
-        const uint32_t a0 = ((a_base + (uint32_t)wg * 64u * 16u) >> 4) | A_LBO;   // this warpgroup's 64 rows
-        const uint32_t b0 = (b_base >> 4) | B_LBO;
+        constexpr uint32_t A_SPLIT = (2u * SD_KBYTES) >> 4;
+        // weight image [kcore][split][WR][16 B]: K-adjacent core matrices one kcore (2 WR rows) apart, taps 64 WR rows apart
+        constexpr uint32_t B_LBO = ((uint32_t)(2 * C::WR * 16) >> 4) << 16, B_TAP16 = (64u * C::WR) >> 4;
         const uint32_t Wrow = (uint32_t)p.W;                             // tap (g, tt) reads rows R + g * W + tt
-        float run[NT / 2], acc[NB];      // acc = [main NB / 2 | cross NB / 2]: disjoint blocks, each written by whole wgmmas
         uint32_t slot = 0, a_par = 0, q = 0, k = 0;
-        for (int t = tile_of(0); t >= 0; t = tile_of(++k)) {
-#pragma unroll
-            for (int i = 0; i < NT / 2; ++i) run[i] = bias_s[(i / (NB / 2)) * NB + 8 * ((i % (NB / 2)) >> 2) + cq + (i & 1)];
-            for (int c = 0; c < nchunks; ++c) {
-                mbar_wait(bar_base + 8u * (BAR_AFULL + slot), a_par);
-                const uint32_t ac = a0 + slot * ((uint32_t)SD_CHUNK >> 4);
+        if constexpr (C::CM) {
+            // ---- channels-as-M: warpgroup wg owns tile 2u + wg; weights = A operand (64 channel rows), activations = B (128 rows)
+            // Fragment of thread (warp w = warp & 3, lane): acc[4j + e] is M row 16 w + lane / 4 + 8 (e / 2), tile row
+            // 8 j + 2 (lane % 4) + e % 2.  Cout 64: acc = [main 64 | cross 64], M row = channel.  Cout <= 32: M rows r / r + 8
+            // of a 16-row group are main / cross of channel 8 w + lane / 4.  run[i]: channel ch(i), tile row col(i).
+            constexpr int NACC = NT == 64 ? 128 : 64;
+            constexpr uint32_t W_LO16 = (64u * 16u) >> 4;                // lo (Cout 64) / Q (Cout <= 32): 64 rows after hi / P
+            const int wq = warp & 3;
+            auto ch = [&](int i) { return NT == 64 ? 16 * wq + (lane >> 2) + 8 * ((i & 3) >> 1) : 8 * wq + (lane >> 2); };
+            auto col = [&](int i) { return (NT == 64 ? 8 * (i >> 2) : 8 * (i >> 1)) + 2 * (lane & 3) + (i & 1); };
+            auto mi = [](int i) { return NT == 64 ? i : 4 * (i >> 1) + (i & 1); };              // main accumulator of run[i]
+            auto xi = [](int i) { return NT == 64 ? 64 + i : 4 * (i >> 1) + 2 + (i & 1); };     // cross accumulator of run[i]
+            const uint32_t x0 = ((a_base + (uint32_t)wg * SD_CHUNK) >> 4) | A_LBO;   // slot 2 s + wg: this warpgroup's tile
+            const uint32_t w0 = (b_base >> 4) | B_LBO;
+            const uint32_t nslots = (uint32_t)NA / 2u;
+            float run[NT], acc[NACC];
+            // one chunk of this warpgroup's tile: 27 (Cout 64) or 18 (Cout <= 32) wgmmas, one wait, the fold, the release
+            auto chunk = [&](int c) {
+                const uint32_t cs = 2u * slot + (uint32_t)wg;
+                mbar_wait(bar_base + 8u * (BAR_AFULL + cs), a_par);
+                const uint32_t xc = x0 + slot * ((2u * SD_CHUNK) >> 4);
                 const uint32_t q0 = resident ? (uint32_t)c * 3u : q;    // first weight stage of this chunk
+                wgmma_fence();
 #pragma unroll
-                for (int h = 0; h < NH; ++h) {
-                    wgmma_fence();
+                for (int g = 0; g < 3; ++g) {
+                    const uint32_t sq = q0 + (uint32_t)g, sb = sq % (uint32_t)NBS;
+                    mbar_wait(bar_base + 8u * (BAR_BFULL + sb), resident ? 0u : (sq / (uint32_t)NBS) & 1u);
+                    const uint32_t wgt = w0 + sb * ((uint32_t)C::B_STAGE >> 4);
 #pragma unroll
-                    for (int g = 0; g < 3; ++g) {
-                        const uint32_t sq = q0 + (uint32_t)g, sb = sq % (uint32_t)NBS;
-                        if (h == 0) mbar_wait(bar_base + 8u * (BAR_BFULL + sb), resident ? 0u : (sq / (uint32_t)NBS) & 1u);
-                        const uint32_t bg = b0 + sb * ((uint32_t)C::B_STAGE >> 4);
-#pragma unroll
-                        for (int tt = 0; tt < 3; ++tt) {
-                            const uint32_t ah = ac + (uint32_t)g * Wrow + (uint32_t)tt, al = ah + A_SPLIT;   // one row = 16 B
-                            const uint32_t bh = bg + (uint32_t)tt * B_TAP16 + (uint32_t)(h * NB), bl = bh + B_LO16;   // n rows of 16 B
-                            const uint32_t acc_on = (g == 0 && tt == 0) ? 0u : 1u;
-                            // ah * bh -> main; al * bh and ah * bl -> cross.  The cross products keep the order of the
-                            // earlier forms of this kernel (Cout <= 64: ah * bl first; Cout 128: al * bh first), so the
-                            // rounding of every element is unchanged.
-                            wgmma_f16<NB>(acc, gmma_desc(ah, DESC_HI), gmma_desc(bh, DESC_HI), acc_on);
-                            if constexpr (NT < 128) {
-                                wgmma_f16<NB>(acc + NB / 2, gmma_desc(ah, DESC_HI), gmma_desc(bl, DESC_HI), acc_on);
-                                wgmma_f16<NB>(acc + NB / 2, gmma_desc(al, DESC_HI), gmma_desc(bh, DESC_HI), 1u);
-                            } else {
-                                wgmma_f16<NB>(acc + NB / 2, gmma_desc(al, DESC_HI), gmma_desc(bh, DESC_HI), acc_on);
-                                wgmma_f16<NB>(acc + NB / 2, gmma_desc(ah, DESC_HI), gmma_desc(bl, DESC_HI), 1u);
-                            }
+                    for (int tt = 0; tt < 3; ++tt) {
+                        const uint32_t xh = xc + (uint32_t)g * Wrow + (uint32_t)tt, xl = xh + A_SPLIT;   // one row = 16 B
+                        const uint32_t wh = wgt + (uint32_t)tt * B_TAP16, wl = wh + W_LO16;
+                        const uint32_t acc_on = (g == 0 && tt == 0) ? 0u : 1u;
+                        if constexpr (NT == 64) {
+                            wgmma_f16<128>(acc, gmma_desc(wh, DESC_HI), gmma_desc(xh, DESC_HI), acc_on);
+                            wgmma_f16<128>(acc + 64, gmma_desc(wl, DESC_HI), gmma_desc(xh, DESC_HI), acc_on);
+                            wgmma_f16<128>(acc + 64, gmma_desc(wh, DESC_HI), gmma_desc(xl, DESC_HI), 1u);
+                        } else {      // wh = P, wl = Q
+                            wgmma_f16<128>(acc, gmma_desc(wh, DESC_HI), gmma_desc(xh, DESC_HI), acc_on);
+                            wgmma_f16<128>(acc, gmma_desc(wl, DESC_HI), gmma_desc(xl, DESC_HI), 1u);
                         }
                     }
-                    wgmma_commit();
-                    wgmma_wait<0>();
-                    wgmma_fence_regs<NB>(acc);
-#pragma unroll
-                    for (int i = 0; i < NB / 2; ++i) run[h * (NB / 2) + i] += fmaf(acc[NB / 2 + i], 0.00048828125f, acc[i]);
                 }
+                wgmma_commit();
+                wgmma_wait<0>();
+                wgmma_fence_regs<NACC>(acc);
+#pragma unroll
+                for (int i = 0; i < NT; ++i) run[i] += fmaf(acc[xi(i)], 0.00048828125f, acc[mi(i)]);
                 __syncwarp();
                 if (lane == 0) {
-                    mbar_arrive(bar_base + 8u * (BAR_AEMPTY + slot));
+                    mbar_arrive(bar_base + 8u * (BAR_AEMPTY + cs));
                     if (!resident)
                         for (int g = 0; g < 3; ++g) mbar_arrive(bar_base + 8u * (BAR_BEMPTY + (q0 + (uint32_t)g) % (uint32_t)NBS));
                 }
-                if (++slot == (uint32_t)NA) { slot = 0; a_par ^= 1u; }
+                if (++slot == nslots) { slot = 0; a_par ^= 1u; }
                 if (!resident) q += 3;
-            }
-            // the finished tile, one column block at a time: fragments -> staging -> one row per thread
+            };
+            float *const st = stage + (size_t)wg * 64 * NT;                  // this warpgroup's [NT / 4][64 rows][4]
+            const float4 *st4 = reinterpret_cast<const float4 *>(st);
+            for (int u = tile_of(0); u >= 0; u = tile_of(++k)) {
 #pragma unroll
-            for (int h = 0; h < NT / SB; ++h) {
-                asm volatile("bar.sync %0, 128;" ::"r"(1 + wg) : "memory");        // this warpgroup's rows of the staging buffer are free
-#pragma unroll
-                for (int i = 0; i < SB / 2; i += 2) {
-                    const int col = 8 * (i >> 2) + cq, row = r0 + ((i & 2) ? 8 : 0);
-                    *reinterpret_cast<float2 *>(stage + ((size_t)(col >> 2) * SD_BM + row) * 4 + (col & 3)) =
-                        make_float2(run[h * (SB / 2) + i], run[h * (SB / 2) + i + 1]);
+                for (int i = 0; i < NT; ++i) run[i] = bias_s[ch(i)];
+                // Two chunks per iteration, the second one guarded: the code of a chunk appears twice, so a Cout <= 32 kernel
+                // shows a chain of 36 HGMMAs (2 waits) in its SASS, which tests/test_conv_sd_ptxas_cpu.py checks for.
+                for (int c = 0; c < nchunks; c += 2) {
+                    chunk(c);
+                    if (c + 1 < nchunks) chunk(c + 1);
                 }
-                asm volatile("bar.sync %0, 128;" ::"r"(1 + wg) : "memory");
-                const int row = wg * 64 + (tl & 63), cs = (tl >> 6) * (SB / 2);
-                const float4 *st4 = reinterpret_cast<const float4 *>(stage);
-                sd_store_rows<SB / 2, OUT_SD>(p, t, row, h * SB + cs, n_samples, [&](int cc, float (&r)[8]) {
-                    const float4 u0 = st4[((cs + cc) >> 2) * SD_BM + row], u1 = st4[(((cs + cc) >> 2) + 1) * SD_BM + row];
-                    r[0] = u0.x; r[1] = u0.y; r[2] = u0.z; r[3] = u0.w; r[4] = u1.x; r[5] = u1.y; r[6] = u1.z; r[7] = u1.w;
-                });
+                const int t = 2 * u + wg;
+                if (t >= n_tiles) continue;                                   // the recomputed tile 2u of an odd tile count
+                // the finished tile, 64 rows at a time: fragments -> staging -> half a row (NT / 2 channels) per thread
+#pragma unroll
+                for (int h = 0; h < 2; ++h) {
+                    asm volatile("bar.sync %0, 128;" ::"r"(1 + wg) : "memory");    // this warpgroup's staging buffer is free
+#pragma unroll
+                    for (int i = 0; i < NT; ++i)
+                        if ((col(i) >> 6) == h) st[((ch(i) >> 2) * 64 + (col(i) & 63)) * 4 + (ch(i) & 3)] = run[i];
+                    asm volatile("bar.sync %0, 128;" ::"r"(1 + wg) : "memory");
+                    const int row = tl & 63, cs = (tl >> 6) * (NT / 2);
+                    sd_store_rows<NT / 2, OUT_SD>(p, t, h * 64 + row, cs, n_samples, [&](int cc, float (&r)[8]) {
+                        const float4 u0 = st4[((cs + cc) >> 2) * 64 + row], u1 = st4[(((cs + cc) >> 2) + 1) * 64 + row];
+                        r[0] = u0.x; r[1] = u0.y; r[2] = u0.z; r[3] = u0.w; r[4] = u1.x; r[5] = u1.y; r[6] = u1.z; r[7] = u1.w;
+                    });
+                }
             }
+        } else {
+            // ---- rows-as-M: warpgroup wg owns rows 64 wg .. 64 wg + 63 of tile t; activations = A operand, weights = B (N = Cout)
+            const int r0 = wg * 64 + (warp & 3) * 16 + (lane >> 2);         // fragment rows r0 and r0 + 8 of the tile
+            const int cq = 2 * (lane & 3);                                   // fragment column within an 8-column group
+            // Cout <= 32 (fp32 input): hi / lo of the B operand are rows 0-7 / 8-15 of each 16-row group of P, so its 8-row core
+            // matrices are 256 B apart and lo starts 128 B after hi
+            constexpr uint32_t B_DESC_HI = (NT < 64 ? 256u : 128u) >> 4, B_LO16 = (NT < 64 ? 128u : (uint32_t)NT * 16u) >> 4;
+            const uint32_t a0 = ((a_base + (uint32_t)wg * 64u * 16u) >> 4) | A_LBO;   // this warpgroup's 64 rows
+            const uint32_t b0 = (b_base >> 4) | B_LBO;
+            float run[NT / 2], acc[NB];      // acc = [main NB / 2 | cross NB / 2]: disjoint blocks, each written by whole wgmmas
+            for (int t = tile_of(0); t >= 0; t = tile_of(++k)) {
+#pragma unroll
+                for (int i = 0; i < NT / 2; ++i) run[i] = bias_s[(i / (NB / 2)) * NB + 8 * ((i % (NB / 2)) >> 2) + cq + (i & 1)];
+                for (int c = 0; c < nchunks; ++c) {
+                    mbar_wait(bar_base + 8u * (BAR_AFULL + slot), a_par);
+                    const uint32_t ac = a0 + slot * ((uint32_t)SD_CHUNK >> 4);
+                    const uint32_t q0 = resident ? (uint32_t)c * 3u : q;    // first weight stage of this chunk
+#pragma unroll
+                    for (int h = 0; h < NH; ++h) {
+                        wgmma_fence();
+#pragma unroll
+                        for (int g = 0; g < 3; ++g) {
+                            const uint32_t sq = q0 + (uint32_t)g, sb = sq % (uint32_t)NBS;
+                            if (h == 0) mbar_wait(bar_base + 8u * (BAR_BFULL + sb), resident ? 0u : (sq / (uint32_t)NBS) & 1u);
+                            const uint32_t bg = b0 + sb * ((uint32_t)C::B_STAGE >> 4);
+#pragma unroll
+                            for (int tt = 0; tt < 3; ++tt) {
+                                const uint32_t ah = ac + (uint32_t)g * Wrow + (uint32_t)tt, al = ah + A_SPLIT;   // one row = 16 B
+                                const uint32_t bh = bg + (uint32_t)tt * B_TAP16 + (uint32_t)(h * NB), bl = bh + B_LO16;   // n rows of 16 B
+                                const uint32_t acc_on = (g == 0 && tt == 0) ? 0u : 1u;
+                                // ah * bh -> main; al * bh and ah * bl -> cross.  The cross products keep the order of the
+                                // earlier forms of this kernel (Cout <= 64: ah * bl first; Cout 128: al * bh first), so the
+                                // rounding of every element is unchanged.
+                                wgmma_f16<NB>(acc, gmma_desc(ah, DESC_HI), gmma_desc(bh, B_DESC_HI), acc_on);
+                                if constexpr (NT < 128) {
+                                    wgmma_f16<NB>(acc + NB / 2, gmma_desc(ah, DESC_HI), gmma_desc(bl, B_DESC_HI), acc_on);
+                                    wgmma_f16<NB>(acc + NB / 2, gmma_desc(al, DESC_HI), gmma_desc(bh, B_DESC_HI), 1u);
+                                } else {
+                                    wgmma_f16<NB>(acc + NB / 2, gmma_desc(al, DESC_HI), gmma_desc(bh, B_DESC_HI), acc_on);
+                                    wgmma_f16<NB>(acc + NB / 2, gmma_desc(ah, DESC_HI), gmma_desc(bl, B_DESC_HI), 1u);
+                                }
+                            }
+                        }
+                        wgmma_commit();
+                        wgmma_wait<0>();
+                        wgmma_fence_regs<NB>(acc);
+#pragma unroll
+                        for (int i = 0; i < NB / 2; ++i) run[h * (NB / 2) + i] += fmaf(acc[NB / 2 + i], 0.00048828125f, acc[i]);
+                    }
+                    __syncwarp();
+                    if (lane == 0) {
+                        mbar_arrive(bar_base + 8u * (BAR_AEMPTY + slot));
+                        if (!resident)
+                            for (int g = 0; g < 3; ++g) mbar_arrive(bar_base + 8u * (BAR_BEMPTY + (q0 + (uint32_t)g) % (uint32_t)NBS));
+                    }
+                    if (++slot == (uint32_t)NA) { slot = 0; a_par ^= 1u; }
+                    if (!resident) q += 3;
+                }
+                // the finished tile, one column block at a time: fragments -> staging -> one row per thread
+#pragma unroll
+                for (int h = 0; h < NT / SB; ++h) {
+                    asm volatile("bar.sync %0, 128;" ::"r"(1 + wg) : "memory");        // this warpgroup's rows of the staging buffer are free
+#pragma unroll
+                    for (int i = 0; i < SB / 2; i += 2) {
+                        const int col = 8 * (i >> 2) + cq, row = r0 + ((i & 2) ? 8 : 0);
+                        *reinterpret_cast<float2 *>(stage + ((size_t)(col >> 2) * SD_BM + row) * 4 + (col & 3)) =
+                            make_float2(run[h * (SB / 2) + i], run[h * (SB / 2) + i + 1]);
+                    }
+                    asm volatile("bar.sync %0, 128;" ::"r"(1 + wg) : "memory");
+                    const int row = wg * 64 + (tl & 63), cs = (tl >> 6) * (SB / 2);
+                    const float4 *st4 = reinterpret_cast<const float4 *>(stage);
+                    sd_store_rows<SB / 2, OUT_SD>(p, t, row, h * SB + cs, n_samples, [&](int cc, float (&r)[8]) {
+                        const float4 u0 = st4[((cs + cc) >> 2) * SD_BM + row], u1 = st4[(((cs + cc) >> 2) + 1) * SD_BM + row];
+                        r[0] = u0.x; r[1] = u0.y; r[2] = u0.z; r[3] = u0.w; r[4] = u1.x; r[5] = u1.y; r[6] = u1.z; r[7] = u1.w;
+                    });
+                }
+        }
         }
     } else {
         setmaxnreg_dec<C::PROD_REGS>();
@@ -310,30 +430,38 @@ __global__ void __launch_bounds__(SdCfg<NT, IN_SD>::THREADS, 1) conv_sd_kernel(c
             if (IN_SD) {
                 // =========================== A producer: presplit images by bulk copy =================================
                 // A chunk's four (split, kcore) images are four contiguous 2816-byte runs of the previous layer's output: one
-                // thread keeps NA chunks in flight; no register staging, no conversion.  The other two warps before the weight
-                // warp have no work.
+                // thread keeps NA chunks in flight; no register staging, no conversion.  Channels-as-M: chunk c of the unit's
+                // tile 2u + g goes to slot 2 s + g (tile 2u again when 2u + 1 does not exist).  The other two warps before the
+                // weight warp have no work.
                 if (warp == SD_NC && lane == 0) {
+                    constexpr uint32_t TPU = C::TPU;
+                    const uint32_t nslots = (uint32_t)NA / TPU;
                     uint32_t slot = 0, par = 0, round = 0;
                     for (uint32_t k = 0;; ++k) {
-                        int t;
-                        if (dyn) {           // draw the next tile and publish it to the other roles
-                            t = atomicAdd(p.tile_ctr, 1);
-                            if (t >= n_tiles) t = -1;
-                            tile_ring[k & (SD_TRING - 1)] = t;
+                        int u;
+                        if (dyn) {           // draw the next unit and publish it to the other roles
+                            u = atomicAdd(p.tile_ctr, 1);
+                            if (u >= n_units) u = -1;
+                            tile_ring[k & (SD_TRING - 1)] = u;
                             mbar_arrive(bar_base + 8u * (BAR_TILE + (k & (SD_TRING - 1))));
                         } else {
-                            t = tile_of(k);
+                            u = tile_of(k);
                         }
-                        if (t < 0) break;
+                        if (u < 0) break;
                         for (int c = 0; c < nchunks; ++c) {
-                            if (round) mbar_wait(bar_base + 8u * (BAR_AEMPTY + slot), par ^ 1u);
-                            mbar_arrive_expect_tx(bar_base + 8u * (BAR_AFULL + slot), 4u * (uint32_t)SD_KBYTES);
-                            const unsigned char *src = reinterpret_cast<const unsigned char *>(p.in_sd) + ((size_t)(c * 4) * p.rows_in + (size_t)t * SD_BM) * 16;
 #pragma unroll
-                            for (int im = 0; im < 4; ++im)
-                                bulk_g2s(a_base + slot * (uint32_t)SD_CHUNK + (uint32_t)im * SD_KBYTES, src + (size_t)im * p.rows_in * 16, (uint32_t)SD_KBYTES,
-                                         bar_base + 8u * (BAR_AFULL + slot));
-                            if (++slot == (uint32_t)NA) { slot = 0; par ^= 1u; round = 1; }
+                            for (uint32_t g = 0; g < TPU; ++g) {
+                                const uint32_t cs = slot * TPU + g;
+                                const int t = (int)(TPU * (uint32_t)u + g) < n_tiles ? (int)(TPU * (uint32_t)u + g) : (int)(TPU * (uint32_t)u);
+                                if (round) mbar_wait(bar_base + 8u * (BAR_AEMPTY + cs), par ^ 1u);
+                                mbar_arrive_expect_tx(bar_base + 8u * (BAR_AFULL + cs), 4u * (uint32_t)SD_KBYTES);
+                                const unsigned char *src = reinterpret_cast<const unsigned char *>(p.in_sd) + ((size_t)(c * 4) * p.rows_in + (size_t)t * SD_BM) * 16;
+#pragma unroll
+                                for (int im = 0; im < 4; ++im)
+                                    bulk_g2s(a_base + cs * (uint32_t)SD_CHUNK + (uint32_t)im * SD_KBYTES, src + (size_t)im * p.rows_in * 16, (uint32_t)SD_KBYTES,
+                                             bar_base + 8u * (BAR_AFULL + cs));
+                            }
+                            if (++slot == nslots) { slot = 0; par ^= 1u; round = 1; }
                         }
                     }
                 }
@@ -477,16 +605,18 @@ __global__ void __launch_bounds__(SdCfg<NT, IN_SD>::THREADS, 1) conv_sd_kernel(c
 template <int NT, int IN_SD, int OUT_SD>
 int launch_sd(ConvSdParams p, cudaStream_t st) {
     using C = SdCfg<NT, IN_SD>;
-    // the whole weight image resident in shared memory when it leaves room for three A chunks, else a ring of six stages
-    // (two chunks) or as many as leave room for four A chunks
+    // the whole weight image resident in shared memory when it leaves room for three A chunks (channels-as-M: two per
+    // warpgroup), else a ring of six stages (two chunks) or as many as leave room for four A chunks.  Channels-as-M slots come
+    // in pairs, one per warpgroup.
     const int budget = SD_SMEM - C::STAGE_BYTES, n_st = p.nchunks * 3;
-    p.resident = n_st <= SD_MAXNBS && budget - n_st * C::B_STAGE >= 3 * SD_CHUNK;
+    p.resident = n_st <= SD_MAXNBS && budget - n_st * C::B_STAGE >= (C::CM ? 4 : 3) * SD_CHUNK;
     p.nbs = p.resident ? n_st : 6;
     while (!p.resident && p.nbs > 3 && budget - p.nbs * C::B_STAGE < 4 * SD_CHUNK) --p.nbs;
     int na = (budget - p.nbs * C::B_STAGE) / SD_CHUNK;
-    if (na > 2 * p.nchunks) na = 2 * p.nchunks;
+    if (na > 2 * C::TPU * p.nchunks) na = 2 * C::TPU * p.nchunks;
     if (na > SD_MAXNA) na = SD_MAXNA;
-    BX_REQUIRE(na >= 2, "bx_conv_layer_sd: no room for the activation ring");
+    na -= na % C::TPU;
+    BX_REQUIRE(na >= 2 * C::TPU, "bx_conv_layer_sd: no room for the activation ring");
     p.NA = na;
     const int smem = na * SD_CHUNK + p.nbs * C::B_STAGE + C::STAGE_BYTES;
     static BxPerDevice attr = {};
@@ -494,7 +624,8 @@ int launch_sd(ConvSdParams p, cudaStream_t st) {
         BX_CUDA(cudaFuncSetAttribute(conv_sd_kernel<NT, IN_SD, OUT_SD>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
     int sms = bx_device_sm_count();
     if (sms <= 0) sms = 132;
-    const int grid = p.n_tiles < sms ? p.n_tiles : sms;
+    const int units = (p.n_tiles + C::TPU - 1) / C::TPU;
+    const int grid = units < sms ? units : sms;
     conv_sd_kernel<NT, IN_SD, OUT_SD><<<grid, C::THREADS, smem, st>>>(p);
     BX_LAUNCH_CHECK();
     return BX_OK;

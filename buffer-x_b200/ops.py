@@ -420,8 +420,10 @@ def conv_layer_tc(geom, x, w_tc, bias, out, n, Cin, Cout, D, H, W, kd, kh, kw, r
 
 def conv_sd_weights(Wt: torch.Tensor) -> torch.Tensor:
     """[T, Cin, Cout] folded fp32 weights (T = 9: 3x3, or 27: 3x3x3 with Cin = 16) -> the fp16 operand image of
-    ``bx_conv_layer_sd``: [chunk][tap(9)][kcore(2)][split(hi,lo)][n(NT)][8], w = hi + lo * 2^-11 (hi and lo rows of a kcore are
-    adjacent, so [hi | lo] is one N = 2*NT operand)."""
+    ``bx_conv_layer_sd``: [chunk][tap(9)][kcore(2)][split(hi,lo)][n(NT)][8], w = hi + lo * 2^-11.  Cout <= 32 (NT = 32):
+    [chunk][tap][kcore][P | Q][64][8], where in each 16-row group w of P rows 0-7 / 8-15 are hi / lo of channels 8w..8w+7 and
+    in Q they are zero / hi (the 64-row A operand of the channels-as-M mainloop; the rows-as-M mainloop reads hi and lo out of
+    P with a 256-byte core-matrix stride)."""
     T, Cin, Cout = Wt.shape
     assert T in (9, 27) and Cin % 16 == 0 and Cout <= 128 and (T == 9 or Cin == 16)
     NT = 128 if Cout > 64 else (64 if Cout > 32 else 32)
@@ -433,8 +435,14 @@ def conv_sd_weights(Wt: torch.Tensor) -> torch.Tensor:
         W = W.view(9, Cin // 16, 16, NT).permute(1, 0, 2, 3)          # [chunk, tap, 16, NT]
     hi = W.half()
     lo = ((W - hi.float()) * 2048.0).half()
+    nch = W.shape[0]
+    if NT == 32:
+        grp = lambda x: x.reshape(nch, 9, 2, 8, 4, 8).permute(0, 1, 2, 4, 5, 3)   # [chunk, tap, kcore, w, channel, 8]
+        h, l = grp(hi), grp(lo)
+        P = torch.stack([h, l], dim=4)                                # [chunk, tap, kcore, w, split, channel, 8]
+        Q = torch.stack([torch.zeros_like(h), h], dim=4)
+        return torch.stack([P, Q], dim=3).contiguous().view(-1)       # [chunk, tap, kcore, P|Q, w, split, channel, 8]
     both = torch.stack([hi, lo], dim=2)                               # [chunk, tap, split, 16, NT]
-    nch = both.shape[0]
     both = both.reshape(nch, 9, 2, 2, 8, NT).permute(0, 1, 3, 2, 5, 4).contiguous()   # [chunk, tap, kcore, split, NT, 8]
     return both.view(-1)
 

@@ -168,11 +168,13 @@ int bx_conv_layer(int geom, const float *in, const float *w, const float *bias, 
  *                 2 wrap columns, written by the producing kernel; valid: D*W rows per sample), rows =
  *                 bx_conv_sd_rows(n, rows per sample).  The consumer's operand tiles are plain cp.async.bulk copies.
  * n = sample capacity; *d_n (optional, device) = the number of samples actually present (match count).
- * w_sd: fp16 hi/lo weight image [chunk][tap][kcore][split][NT][8] (ops.conv_sd_weights; NT = bx_conv_tc_ntile(Cout));
+ * w_sd: fp16 hi/lo weight image [chunk][tap][kcore][split][NT][8] (ops.conv_sd_weights; NT = bx_conv_tc_ntile(Cout)); for
+ * Cout <= 32 it is [chunk][tap][kcore][P | Q][64][8] (hi / lo and zero / hi of 8 channels per 16-row group, see bx_conv_sd.cu);
  * bias fp32 [Cout].  An activation with |x| >= 65000 cannot be split into fp16 operands -> *d_flag |= 1 (d_flag may be
  * NULL) and the caller re-runs the stack with bx_conv_layer_tc.
  * d_tile_ctr (optional, device, int32[2], zero before its first use): dynamic tile scheduling for presplit-input layers --
- * the persistent CTAs draw 128-row tiles from the counter instead of a fixed stride, so a launch that starts while other
+ * the persistent CTAs draw units of work (one 128-row tile, or two for Cout <= 64) from the counter instead of a fixed
+ * stride, so a launch that starts while other
  * streams still hold some SMs is not held up by its late CTAs; the kernel rewinds the counter when it finishes.  One
  * counter pair per launch in flight (the callers keep one per layer and stream). */
 int bx_conv_layer_sd(int geom, const void *in, int in_presplit, const void *w_sd, const float *bias, void *out, int out_presplit,
