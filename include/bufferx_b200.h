@@ -207,7 +207,8 @@ int bx_conv_layer_tc(int geom, const float *in, const float *w_tc, const float *
  * A/B small convolutions of the source/target equivariant maps (60 + 54 positions per match instead of 972).
  * wa: [32 c][3 dk][5 e][32 co] = sum over (dn,dl) with dl-dn = e-2 of the folded weight; wb: [32][3][3 dl][32] = sum
  * over dn; bias [32] is added into A.  A: [maxM][8][3*20][4], B: [maxM][8][3*18][4] (channel-blocked like the
- * activations of bx_conv_layer_tc; 16-byte aligned); rows >= *d_M untouched. */
+ * activations of bx_conv_layer_tc; 16-byte aligned); rows >= *d_M untouched.  *d_M <= maxM is the caller's to keep:
+ * the kernel does not clamp it. */
 int bx_costvol_ab(const float *equi_s, const float *equi_t, const int32_t *s_mids, const int32_t *t_mids,
                   const int32_t *d_M, int maxM, const float *wa, const float *wb, const float *bias, float *A,
                   float *B, void *stream);
@@ -238,7 +239,8 @@ int bx_concat_matches(const int32_t *s_lists, const int32_t *t_lists, const int3
 /* ---- a11 tail + a12: soft arg-max and pose hypotheses ---------------------------------------
  * Replaces softmax/expectation of CostVolume.forward (models/BUFFERX.py:66-69) and the hypothesis
  * build (:382-389, kornia axis_angle_to_rotation_matrix).  logits: [maxM, azi_n].
- * Appends M = *d_M rows at row offset *d_off of the accumulators and writes *d_off_out = off + M. */
+ * Appends M = *d_M rows at row offset *d_off of the accumulators and writes *d_off_out = off + M.  *d_M <= maxM is the
+ * caller's to keep: the kernel does not clamp it. */
 int bx_hypotheses(const float *logits, int azi_n, const float *kpts_s, const float *kpts_t, const float *Rt_s,
                   const float *Rt_t, const int32_t *s_mids, const int32_t *t_mids, const int32_t *d_M, int maxM,
                   const int32_t *d_off, int32_t *d_off_out, float *ind_out, float *R_acc, float *t_acc,

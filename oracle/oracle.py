@@ -329,22 +329,49 @@ def desc_fp64(feat: torch.Tensor, sd, rad_n=3, ele_n=7, azi_n=20) -> torch.Tenso
 _COST_CONVS = [0, 3, 6, 9, 12, 15, 18, 21, 24, 27]
 
 
+def _cost_net(d1: torch.Tensor, d2: torch.Tensor, sd, azi_n, pfx, keep=False):
+    """The cost volume of d1,d2 [M,32,5,20] through CostNet in the dtype of the inputs and ``sd`` -> (logits [M,azi_n],
+    post-ReLU activations of the nine hidden layers if ``keep``)."""
+    M = d1.shape[0]
+    l = torch.arange(azi_n)
+    idx = (l[None, :] - l[:, None]) % azi_n          # idx[n][l] = (l - n) mod azi_n  (BUFFERX.py:43-48)
+    x = d1[:, :, :, idx.reshape(-1)].reshape(M, d1.shape[1], d1.shape[2], azi_n, azi_n)
+    x = x.permute(0, 1, 3, 2, 4) - d2.unsqueeze(2)   # [M,C,n,k,l]
+    acts = []
+    for i in _COST_CONVS:
+        x = F.conv3d(x, sd[pfx + f"ops.{i}.weight"], sd[pfx + f"ops.{i}.bias"])
+        if i != 27:
+            x = F.relu(_bn(x, sd, pfx + f"ops.{i + 1}", False))
+            if keep:
+                acts.append(x)
+    return x.reshape(M, azi_n), acts
+
+
 def cost_volume(d1: torch.Tensor, d2: torch.Tensor, sd, azi_n=20, pfx="Pose.conv.") -> torch.Tensor:
     """a11: d1,d2 [M,32,5,20] -> soft arg-max azimuth bin [M] (float)."""
     M = d1.shape[0]
     if M == 0:
         return torch.zeros(0)
-    l = torch.arange(azi_n)
-    idx = (l[None, :] - l[:, None]) % azi_n          # idx[n][l] = (l - n) mod azi_n  (BUFFERX.py:43-48)
-    x = d1[:, :, :, idx.reshape(-1)].reshape(M, d1.shape[1], d1.shape[2], azi_n, azi_n)
-    x = x.permute(0, 1, 3, 2, 4) - d2.unsqueeze(2)   # [M,C,n,k,l]
-    for i in _COST_CONVS:
-        x = F.conv3d(x, sd[pfx + f"ops.{i}.weight"], sd[pfx + f"ops.{i}.bias"])
-        if i != 27:
-            x = F.relu(_bn(x, sd, pfx + f"ops.{i + 1}", False))
-    cost = x.reshape(M, azi_n)
+    cost, _ = _cost_net(d1, d2, sd, azi_n, pfx)
     prob = F.softmax(cost, dim=-1)
     return torch.sum(prob * torch.arange(0, azi_n)[None], dim=-1)
+
+
+def costnet_fp64(d1: torch.Tensor, d2: torch.Tensor, sd, keep=False, azi_n=20, pfx="Pose.conv."):
+    """a11 evaluated in float64 on the (fp32) maps d1,d2 [M,32,5,20] -> logits [M,azi_n] float64; with ``keep`` also the
+    post-ReLU activation of every hidden layer.  The ground truth against which the fp32 oracle and every CostNet kernel
+    are measured (tests/test_costnet_fp64_*.py)."""
+    sd64 = {k: (v.double() if v.is_floating_point() else v) for k, v in sd.items() if k.startswith(pfx)}
+    with torch.no_grad():
+        logits, acts = _cost_net(d1.double(), d2.double(), sd64, azi_n, pfx, keep)
+    return (logits, acts) if keep else logits
+
+
+def soft_argmax(logits: torch.Tensor) -> torch.Tensor:
+    """The reference's non-circular expectation sum(softmax(logits) * arange) (BUFFERX.py:66-69), in float64."""
+    lg = torch.as_tensor(logits).double()
+    prob = F.softmax(lg, dim=-1)
+    return torch.sum(prob * torch.arange(lg.shape[-1], dtype=torch.float64)[None], dim=-1)
 
 
 def azimuth_rotation(angle: torch.Tensor) -> torch.Tensor:
