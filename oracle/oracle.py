@@ -294,36 +294,88 @@ def pnt_max(inv_patches: torch.Tensor, sd, pfx="Desc.") -> torch.Tensor:
 _CYL_CONVS = [0, 3, 6, 9, 12, 15, 18, 21]
 
 
-def cyl_net(x: torch.Tensor, sd, pfx="Desc.conv_net.") -> torch.Tensor:
-    """a8: [K,16,3,7,20] -> [K,32,7,20]."""
+def _cyl_layers(x: torch.Tensor, sd, pfx, keep=False):
+    """The eight Cylindrical_Net layers in the dtype of x and ``sd`` -> (output [K,32,7,20], the activation after each
+    layer if ``keep``: post-ReLU for the first seven, the plain convolution for the last)."""
     x = F.conv3d(_pad_cyl(x), sd[pfx + "ops.0.weight"], sd[pfx + "ops.0.bias"])
     x = F.relu(_bn(x, sd, pfx + "ops.1", False)).squeeze(2)
+    acts = [x] if keep else []
     for i in _CYL_CONVS[1:]:
         x = F.conv2d(_pad_cyl(x), sd[pfx + f"ops.{i}.weight"], sd[pfx + f"ops.{i}.bias"])
         if i != 21:
             x = F.relu(_bn(x, sd, pfx + f"ops.{i + 1}", False))
-    return x
+        if keep:
+            acts.append(x)
+    return x, acts
 
 
-def pool_desc(x: torch.Tensor, sd, pfx="Desc."):
-    """a9: x [K,32,7,20] -> desc [K,32] (L2-normalised attention-pooled), equi [K,32,7,20]."""
+def cyl_net(x: torch.Tensor, sd, pfx="Desc.conv_net.") -> torch.Tensor:
+    """a8: [K,16,3,7,20] -> [K,32,7,20]."""
+    return _cyl_layers(x, sd, pfx)[0]
+
+
+def _pool(x: torch.Tensor, sd, pfx):
+    """a9 -> (desc [K,32], equi [K,32,7,20], attention map [K,1,7,20], pooled vector before the normalisation [K,32])."""
     w = F.conv2d(x, sd[pfx + "pool_layer.0.weight"], sd[pfx + "pool_layer.0.bias"])
     w = F.relu(_bn(w, sd, pfx + "pool_layer.1", True))
     w = F.conv2d(w, sd[pfx + "pool_layer.3.weight"], sd[pfx + "pool_layer.3.bias"])
     w = F.relu(_bn(w, sd, pfx + "pool_layer.4", True))
-    f = F.avg_pool2d(x * w, kernel_size=(x.shape[2], x.shape[3]))
-    f = F.normalize(f.view(f.shape[0], -1), p=2, dim=1)
-    return f, F.normalize(x, p=2, dim=1)
+    f = F.avg_pool2d(x * w, kernel_size=(x.shape[2], x.shape[3])).view(x.shape[0], -1)
+    return F.normalize(f, p=2, dim=1), F.normalize(x, p=2, dim=1), w, f
 
 
-def desc_fp64(feat: torch.Tensor, sd, rad_n=3, ele_n=7, azi_n=20) -> torch.Tensor:
-    """a8+a9 evaluated in float64 on the (fp32) point-layer features [k,16,V]: the ground truth against which the fp32
-    oracle and the GPU path are both measured where a descriptor is ill-conditioned (tests/test_gpu_parity.py)."""
-    sd64 = {k: (v.double() if v.is_floating_point() else v) for k, v in sd.items() if k.startswith("Desc.")}
+def pool_desc(x: torch.Tensor, sd, pfx="Desc."):
+    """a9: x [K,32,7,20] -> desc [K,32] (L2-normalised attention-pooled), equi [K,32,7,20]."""
+    d, e, _, _ = _pool(x, sd, pfx)
+    return d, e
+
+
+def _sd64(sd, pfx, device):
+    return {k: (v.double() if v.is_floating_point() else v).to(device) for k, v in sd.items() if k.startswith(pfx)}
+
+
+def desc_fp64(feat: torch.Tensor, sd, keep=False, rad_n=3, ele_n=7, azi_n=20):
+    """a8+a9 evaluated in float64 on the point-layer features [k,16,V] (on their device: torch's own float64 kernels): the
+    ground truth against which the fp32 oracle and the GPU path are both measured (tests/test_gpu_parity.py,
+    tests/test_descnet_fp64_*.py).  -> desc [k,32] float64; with ``keep`` also a dict: ``acts`` (the eight layer outputs of
+    _cyl_layers), ``equi``, ``att`` (attention map [k,1,7,20]) and ``pooled`` (the vector before its L2 normalisation)."""
+    sd64 = _sd64(sd, "Desc.", feat.device)
     with torch.no_grad():
-        x = cyl_net(feat.double().view(feat.shape[0], feat.shape[1], rad_n, ele_n, azi_n), sd64)
-        d, _ = pool_desc(x, sd64)
-    return d
+        x, acts = _cyl_layers(feat.double().view(feat.shape[0], feat.shape[1], rad_n, ele_n, azi_n), sd64, "Desc.conv_net.", keep)
+        d, equi, att, pooled = _pool(x, sd64, "Desc.")
+    return (d, dict(acts=acts, equi=equi, att=att, pooled=pooled)) if keep else d
+
+
+def pnt_fp64(delta, vidx, sd, absref=False, azi_n=20, pfx="Desc."):
+    """a7 in float64 on an integer voxel selection: delta [K,P,3] fp32 patches, vidx [K,V,nv] (oracle.spt's) -> the
+    point-layer features [K,16,V] float64.  The samples are de-rotated in float64 (angle -a 2 pi / azi_n) from the fp32
+    coordinates; a slot is zero where oracle.spt zeroes it (slot 0 holding index 0, padding slots repeating slot 0).  With
+    ``absref`` also max over the samples of |W| |x'| + |b| (conv + BN folded in float64; |x'| from |x| |cos| + |y| |sin|, so
+    that a cancelling de-rotation does not shrink the bound), on the same device as the features."""
+    delta = torch.as_tensor(np.asarray(delta) if not isinstance(delta, torch.Tensor) else delta)
+    vidx = torch.as_tensor(np.asarray(vidx) if not isinstance(vidx, torch.Tensor) else vidx).long().to(delta.device)
+    K, V, nv = vidx.shape
+    dev = delta.device
+    d = delta.double()
+    pts = torch.gather(d, 1, vidx.view(K, V * nv, 1).expand(K, V * nv, 3)).view(K, V, nv, 3)
+    zero = torch.zeros((K, V, nv), dtype=torch.bool, device=dev)
+    zero[:, :, 0] = vidx[:, :, 0] == 0
+    zero[:, :, 1:] = vidx[:, :, 1:] == vidx[:, :, :1]
+    pts = torch.where(zero[..., None], torch.zeros((), dtype=torch.float64, device=dev), pts)
+    ang = -torch.arange(azi_n, dtype=torch.float64, device=dev) * (2 * math.pi / azi_n)
+    a = torch.arange(V, device=dev) % azi_n
+    c, s = torch.cos(ang)[a].view(1, V, 1), torch.sin(ang)[a].view(1, V, 1)
+    x, y, z = pts[..., 0], pts[..., 1], pts[..., 2]
+    inv = torch.stack([x * c - y * s, x * s + y * c, z], dim=-1)                  # [K,V,nv,3]
+    g = lambda k: sd[pfx + k].detach().double().to(dev)
+    sc = g("pnt_layer.1.weight") / torch.sqrt(g("pnt_layer.1.running_var") + 1e-5)
+    W = g("pnt_layer.0.weight").view(16, 3) * sc[:, None]
+    b = (g("pnt_layer.0.bias") - g("pnt_layer.1.running_mean")) * sc + g("pnt_layer.1.bias")
+    feat = torch.relu(inv @ W.t() + b).amax(dim=2).permute(0, 2, 1).contiguous()
+    if not absref:
+        return feat
+    ax = torch.stack([x.abs() * c.abs() + y.abs() * s.abs(), x.abs() * s.abs() + y.abs() * c.abs(), z.abs()], dim=-1)
+    return feat, (ax @ W.abs().t() + b.abs()).amax(dim=2).permute(0, 2, 1).contiguous()
 
 
 _COST_CONVS = [0, 3, 6, 9, 12, 15, 18, 21, 24, 27]
