@@ -820,9 +820,9 @@ BX_API int bx_lrf(const float *patches, int K, int P, float des_r, const float *
 
 BX_API int bx_lrf_batched(const float *patches, int K, int P, float des_r, const float *d_des_r, int r_group, int flags, float *delta,
                           float *Rt, float *rand_axis, void *stream) {
-    BX_REQUIRE(patches && delta && Rt && rand_axis, "bx_lrf: null pointer");
     BX_REQUIRE(K >= 0 && P >= 1 && r_group >= 0, "bx_lrf: bad sizes");
-    if (K == 0) return BX_OK;
+    if (K == 0) return BX_OK;                 // an empty batch: torch hands empty tensors over as null pointers
+    BX_REQUIRE(patches && delta && Rt && rand_axis, "bx_lrf: null pointer");
     lrf_kernel<<<(K + LRF_WARPS - 1) / LRF_WARPS, LRF_WARPS * 32, 0, bx_stream(stream)>>>(patches, K, P, des_r, d_des_r,
                                                                                            flags, delta, Rt, rand_axis, r_group);
     BX_LAUNCH_CHECK();

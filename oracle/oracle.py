@@ -144,6 +144,57 @@ def lrf(patches, des_r: float, aligned: bool, z_axis=None, want_z=False):
     return delta, Rt, ra
 
 
+def rodrigues_fp64(z, stable=False):
+    """The rotation of ``lrf`` taking unit z [K,3] (float64) onto +e_z, evaluated in float64 -> (R [K,3,3], rand_axis
+    [K,3]).  theta = arccos(z_z) (the literal form) or cos = z_z, sin = |z x e_z| (stable); axis a = (z_1, -z_0) /
+    max(sn, 1e-12) with sn = |z x e_z|, R = I + sin [a]x + (1 - cos) [a]x^2 written out like the kernel, so that sn = 0
+    gives R = I."""
+    z = np.asarray(z, dtype=np.float64)
+    sn = np.hypot(z[:, 0], z[:, 1])
+    if stable:
+        ct, st = z[:, 2], sn
+    else:
+        th = np.arccos(np.clip(z[:, 2], -1.0, 1.0))
+        ct, st = np.cos(th), np.sin(th)
+    den = np.maximum(sn, 1e-12)
+    a0, a1 = z[:, 1] / den, -z[:, 0] / den
+    kk = 1.0 - ct
+    R = np.empty((len(z), 3, 3))
+    R[:, 0, 0], R[:, 0, 1], R[:, 0, 2] = 1.0 - kk * a1 * a1, kk * a0 * a1, st * a1
+    R[:, 1, 0], R[:, 1, 1], R[:, 1, 2] = kk * a0 * a1, 1.0 - kk * a0 * a0, -st * a0
+    R[:, 2, 0], R[:, 2, 1], R[:, 2, 2] = -st * a1, st * a0, 1.0 - kk * (a0 * a0 + a1 * a1)
+    return R, np.stack([a0, a1, np.zeros_like(a0)], axis=1)
+
+
+def lrf_fp64(patches, des_r, aligned: bool, stable: bool = False):
+    """a4+a5 in float64 on the fp32 patches [K,P,3] (key point last): the covariance of p - c about the key point c,
+    numpy's eigh and its eigenvector of the smallest eigenvalue, the sign rule of ``lrf`` (flip when -z . c < 0), then
+    ``rodrigues_fp64`` and delta = R (p - c) / r.  ``des_r``: a scalar or one radius per patch, used at its fp32 value (the
+    value the kernel divides by).  An all-zero covariance gets e_x before the sign rule, the choice of the kernel's
+    Jacobi (no rotation, first minimum); the reference leaves it open.
+    -> dict(C, lam (ascending), gap = lam_2 - lam_1, z (sign ruled, unit), margin = |z . c|, sn = |z x e_z|, R (applied to
+    delta, R z = e_z), Rt (the transpose, what ``lrf`` returns), rand_axis, delta), float64 throughout."""
+    pt = np.asarray(patches, dtype=np.float32).astype(np.float64)
+    K = pt.shape[0]
+    c = pt[:, -1, :]
+    d = pt - c[:, None, :]
+    r = np.broadcast_to(np.asarray(des_r, dtype=np.float32).astype(np.float64), (K,))
+    C = np.einsum("kpi,kpj->kij", d, d)
+    lam, V = np.linalg.eigh(C) if K else (np.zeros((0, 3)), np.zeros((0, 3, 3)))
+    z = V[:, :, 0].copy()
+    zero = ~C.reshape(K, 9).any(axis=1)
+    z[zero] = (1.0, 0.0, 0.0)
+    dot = np.einsum("ki,ki->k", z, c)
+    z[-dot < 0] *= -1.0
+    if aligned:
+        R, ra = np.broadcast_to(np.eye(3), (K, 3, 3)).copy(), np.broadcast_to([1.0, 0.0, 0.0], (K, 3)).copy()
+    else:
+        R, ra = rodrigues_fp64(z, stable)
+    delta = np.einsum("kij,kpj->kpi", R, d) / r[:, None, None]
+    return dict(C=C, lam=lam, gap=lam[:, 1] - lam[:, 0], z=z, margin=np.abs(dot), sn=np.hypot(z[:, 0], z[:, 1]), R=R,
+                Rt=R.transpose(0, 2, 1).copy(), rand_axis=ra, delta=delta)
+
+
 def voxel_table(rad_n=3, azi_n=20, ele_n=7) -> np.ndarray:
     """[rad_n*ele_n*azi_n, 3] fp32 voxel centres, built in fp64 exactly like
     ``utils/common.py:248-262, 392-405, 422-428`` (s2_grid -> change_coordinates -> shell scale)."""
