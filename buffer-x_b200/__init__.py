@@ -35,4 +35,4 @@ from .models.BUFFERX import BufferX  # noqa: E402,F401
 from . import driver, bootstrap, evaluation  # noqa: E402,F401
 _alias()
 
-__version__ = "0.1.0"
+__version__ = "0.2.0"

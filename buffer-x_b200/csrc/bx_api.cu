@@ -16,7 +16,7 @@ void bx_set_error(const char *fmt, ...) {
 
 BX_API const char *bx_last_error(void) { return g_err; }
 
-BX_API int bx_version(void) { return 100; }
+BX_API int bx_version(void) { return 200; }
 
 BX_API unsigned long long bx_launch_count(void) { return g_bx_launches; }
 

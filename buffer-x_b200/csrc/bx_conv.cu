@@ -1,208 +1,15 @@
-// bx_conv.cu -- a8/a11 convolution stacks as ONE implicit-GEMM kernel, a9 attention pooling.
+// bx_conv.cu -- a9 attention pooling and the factorised first CostNet layer.
 //
-// Replaces the cuDNN Conv3d/Conv2d + BatchNorm + ReLU chains of Cylindrical_Net
-// (/root/reference/models/patchnet.py:16-84; nine torch.cat padding copies per call,
-// /root/reference/utils/common.py:265-310) and of CostNet (patchnet.py:151-210) whose input, the
-// [M,32,20,5,20] cost volume (256 KB per match, /root/reference/models/BUFFERX.py:51-65), is never
-// materialised here: the A-operand loader generates it from the two [32,5,20] equivariant maps.
-//
-// GEMM view: rows = (sample, output position), cols = Cout, K = taps*Cin.  The circular-azimuth /
-// zero-elevation padding and the valid-convolution geometry are folded into the per-row, per-tap input
-// offset computed by the loader (no padded copies).  BatchNorm (eval) is folded into weights/bias on
-// the host; weights are stored [tap][Cin][Cout].  fp32 FFMA with fp32 accumulation (tolerance parity
-// 1e-4 rel against the torch-CPU oracle); CTA tile 256 x (8*TN), k-tile 8, 8x8 (or 8x4) register tile,
-// register-staged double buffering, one barrier per k-tile.
+// bx_pool_desc replaces pool_layer / avg-pool / F.normalize of the descriptor network (models/patch_embedder.py:32-39,
+// 80-83): one CTA per patch turns the last Cylindrical_Net activation into the unit descriptor and the unit-normalised
+// equivariant map.
+// bx_costvol_ab computes the first CostNet layer (models/patchnet.py:196) over the cost volume of models/BUFFERX.py:51-65
+// in factorised form: two small convolutions of the source / target equivariant maps, from which the next layer's loader
+// regenerates the activation (the COSTAB loaders of bx_conv_tc.cu and bx_conv_sd.cu), so the cost volume is never
+// materialised.  CUDA-core fp32 arithmetic with fp32 accumulation.
 #include "bx_common.cuh"
 
 namespace {
-
-struct ConvParams {
-    const float *in, *w, *bias;
-    float *out;
-    int n;
-    const int *d_n;
-    int Cin, Cout, D, H, W, kd, kh, kw, relu;
-    int S_in, S_out, OD, OH, OW, T;
-    const float *equi_s, *equi_t;
-    const int *s_mids, *t_mids;
-};
-
-constexpr int BM = 256, BK = 8, CT = 256;
-
-template <int GEOM, int TN>
-__global__ void __launch_bounds__(CT, 2) conv_gemm_kernel(const ConvParams p) {
-    constexpr int BN = 8 * TN;
-    __shared__ __align__(16) float As[2][BK][BM];
-    __shared__ __align__(16) float Bs[2][BK][BN];
-
-    const int n_samples = p.d_n ? *p.d_n : p.n;
-    const long long Mtotal = (long long)n_samples * p.S_out;
-    const long long row0 = (long long)blockIdx.x * BM;
-    if (row0 >= Mtotal) return;
-    const int co0 = blockIdx.y * BN;
-    const int tid = threadIdx.x;
-
-    // ---- loader role: this thread fetches row (row0 + tid) of the A tile for all 8 k of a k-tile ----
-    const long long lm = row0 + tid;
-    const bool lvalid = lm < Mtotal;
-    int ln = 0, oz = 0, oy = 0, ox = 0;
-    if (lvalid) {
-        ln = (int)(lm / p.S_out);
-        const int pos = (int)(lm - (long long)ln * p.S_out);
-        if (GEOM == BX_GEOM_CYL3D || GEOM == BX_GEOM_CYL2D) {
-            oy = pos / 20;
-            ox = pos - oy * 20;
-        } else {
-            oz = pos / (p.OH * p.OW);
-            const int rem = pos - oz * (p.OH * p.OW);
-            oy = rem / p.OW;
-            ox = rem - oy * p.OW;
-        }
-    }
-    const float *pa = p.in, *pb = nullptr;
-    if (GEOM == BX_GEOM_COSTVOL) {
-        if (lvalid) {
-            pa = p.equi_s + (size_t)p.s_mids[ln] * 32 * 140;
-            pb = p.equi_t + (size_t)p.t_mids[ln] * 32 * 140;
-        }
-    } else {
-        pa = p.in + (size_t)ln * p.Cin * p.S_in;
-    }
-    const int cstride = (GEOM == BX_GEOM_COSTVOL) ? 140 : p.S_in;
-    const int kchunks = p.Cin / BK;
-    const int nk = p.T * kchunks;
-
-    // B loader role
-    const int b_kk = tid / (BN / 4), b_j4 = tid % (BN / 4);
-    const bool b_role = tid < BK * (BN / 4);
-    const bool b_ok = b_role && (co0 + 4 * b_j4 < p.Cout);
-
-    float a_reg[BK];
-    float4 b_reg = make_float4(0.f, 0.f, 0.f, 0.f);
-    int offA = 0, offB = 0;
-    bool tap_ok = false;
-    int cur_tap = -1;
-
-    auto load_tile = [&](int kt) {
-        const int t = kt / kchunks;
-        const int ci0 = (kt - t * kchunks) * BK;
-        if (t != cur_tap) {
-            cur_tap = t;
-            const int dz = t / (p.kh * p.kw);
-            const int r2 = t - dz * (p.kh * p.kw);
-            const int dy = r2 / p.kw;
-            const int dx = r2 - dy * p.kw;
-            if (GEOM == BX_GEOM_CYL3D || GEOM == BX_GEOM_CYL2D) {
-                const int yy = oy + dy - 1;
-                int xx = ox + dx - 1;
-                xx = xx < 0 ? xx + 20 : (xx >= 20 ? xx - 20 : xx);
-                tap_ok = lvalid && yy >= 0 && yy < 7;
-                offA = dz * 140 + yy * 20 + xx;
-            } else if (GEOM == BX_GEOM_VALID3D) {
-                tap_ok = lvalid;
-                offA = ((oz + dz) * p.H + (oy + dy)) * p.W + (ox + dx);
-            } else {  // COSTVOL: value(c, n, k, l) = d1[c][1+k][(l-n) mod 20] - d2[c][1+k][l]
-                tap_ok = lvalid;
-                const int nn = oz + dz, kk = oy + dy, ll = ox + dx;
-                int sh = ll - nn;
-                sh = sh < 0 ? sh + 20 : sh;
-                offA = (1 + kk) * 20 + sh;
-                offB = (1 + kk) * 20 + ll;
-            }
-        }
-#pragma unroll
-        for (int kk = 0; kk < BK; ++kk) {
-            float v = 0.0f;
-            if (tap_ok) {
-                const size_t o = (size_t)(ci0 + kk) * cstride;
-                if (GEOM == BX_GEOM_COSTVOL) v = pa[o + offA] - pb[o + offB];
-                else v = __ldg(pa + o + offA);
-            }
-            a_reg[kk] = v;
-        }
-        if (b_role) {
-            b_reg = make_float4(0.f, 0.f, 0.f, 0.f);
-            if (b_ok) b_reg = *reinterpret_cast<const float4 *>(p.w + ((size_t)(t * p.Cin + ci0 + b_kk) * p.Cout + co0 + 4 * b_j4));
-        }
-    };
-    auto store_tile = [&](int buf) {
-#pragma unroll
-        for (int kk = 0; kk < BK; ++kk) As[buf][kk][tid] = a_reg[kk];
-        if (b_role) *reinterpret_cast<float4 *>(&Bs[buf][b_kk][4 * b_j4]) = b_reg;
-    };
-
-    // ---- compute role ----
-    const int ty = tid >> 3, tx = tid & 7;
-    float acc[8][TN];
-#pragma unroll
-    for (int i = 0; i < 8; ++i)
-#pragma unroll
-        for (int j = 0; j < TN; ++j) acc[i][j] = 0.0f;
-
-    load_tile(0);
-    store_tile(0);
-    __syncthreads();
-    for (int kt = 0; kt < nk; ++kt) {
-        const int cur = kt & 1;
-        if (kt + 1 < nk) load_tile(kt + 1);
-#pragma unroll
-        for (int kk = 0; kk < BK; ++kk) {
-            const float4 a0 = *reinterpret_cast<const float4 *>(&As[cur][kk][ty * 8]);
-            const float4 a1 = *reinterpret_cast<const float4 *>(&As[cur][kk][ty * 8 + 4]);
-            const float a[8] = {a0.x, a0.y, a0.z, a0.w, a1.x, a1.y, a1.z, a1.w};
-            float b[TN];
-            {
-                const float4 b0 = *reinterpret_cast<const float4 *>(&Bs[cur][kk][tx * 4]);
-                b[0] = b0.x; b[1] = b0.y; b[2] = b0.z; b[3] = b0.w;
-                if (TN == 8) {
-                    const float4 b1 = *reinterpret_cast<const float4 *>(&Bs[cur][kk][32 + tx * 4]);
-                    b[TN - 4] = b1.x; b[TN - 3] = b1.y; b[TN - 2] = b1.z; b[TN - 1] = b1.w;
-                }
-            }
-#pragma unroll
-            for (int i = 0; i < 8; ++i)
-#pragma unroll
-                for (int j = 0; j < TN; ++j) acc[i][j] = fmaf(a[i], b[j], acc[i][j]);
-        }
-        if (kt + 1 < nk) store_tile(cur ^ 1);
-        __syncthreads();
-    }
-
-    // ---- epilogue: bias (+ReLU), out[n][co][pos] ----
-#pragma unroll
-    for (int i = 0; i < 8; ++i) {
-        const long long m = row0 + ty * 8 + i;
-        if (m >= Mtotal) continue;
-        const int n = (int)(m / p.S_out);
-        const int pos = (int)(m - (long long)n * p.S_out);
-        float *o = p.out + (size_t)n * p.Cout * p.S_out + pos;
-#pragma unroll
-        for (int j = 0; j < TN; ++j) {
-            const int co = co0 + ((TN == 8 && j >= 4) ? 32 + tx * 4 + (j - 4) : tx * 4 + j);
-            if (co < p.Cout) {
-                float v = acc[i][j] + p.bias[co];
-                if (p.relu) v = fmaxf(v, 0.0f);
-                o[(size_t)co * p.S_out] = v;
-            }
-        }
-    }
-}
-
-template <int GEOM>
-int launch_conv(const ConvParams &p, int max_n, cudaStream_t st) {
-    const long long maxM = (long long)max_n * p.S_out;
-    const unsigned gx = (unsigned)((maxM + BM - 1) / BM);
-    if (gx == 0) return BX_OK;
-    if (p.Cout > 32) {
-        dim3 grid(gx, (unsigned)((p.Cout + 63) / 64));
-        conv_gemm_kernel<GEOM, 8><<<grid, CT, 0, st>>>(p);
-    } else {
-        dim3 grid(gx, 1);
-        conv_gemm_kernel<GEOM, 4><<<grid, CT, 0, st>>>(p);
-    }
-    BX_LAUNCH_CHECK();
-    return BX_OK;
-}
 
 // ---- a9: attention pooling ------------------------------------------------------------------------
 // one CTA per patch; thread = spatial position (S <= 160).
@@ -382,44 +189,6 @@ costvol_ab_kernel(const float *__restrict__ equi_s, const float *__restrict__ eq
 }
 
 }  // namespace
-
-BX_API int bx_conv_layer(int geom, const float *in, const float *w, const float *bias, float *out, int n,
-                         const int32_t *d_n, int Cin, int Cout, int D, int H, int W, int kd, int kh, int kw, int relu,
-                         const float *equi_s, const float *equi_t, const int32_t *s_mids, const int32_t *t_mids,
-                         void *stream) {
-    BX_REQUIRE(w && bias && out, "bx_conv_layer: null pointer");
-    BX_REQUIRE(n >= 0 && Cin >= 8 && Cin % 8 == 0 && Cout >= 1 && Cout % 4 == 0, "bx_conv_layer: bad channels Cin=%d Cout=%d", Cin, Cout);
-    BX_REQUIRE((reinterpret_cast<uintptr_t>(w) & 15) == 0, "bx_conv_layer: weights must be 16-byte aligned");
-    ConvParams p = {};
-    p.in = in; p.w = w; p.bias = bias; p.out = out; p.n = n; p.d_n = d_n;
-    p.Cin = Cin; p.Cout = Cout; p.D = D; p.H = H; p.W = W; p.kd = kd; p.kh = kh; p.kw = kw; p.relu = relu;
-    p.equi_s = equi_s; p.equi_t = equi_t; p.s_mids = s_mids; p.t_mids = t_mids;
-    p.T = kd * kh * kw;
-    cudaStream_t st = bx_stream(stream);
-    switch (geom) {
-        case BX_GEOM_CYL3D:
-            BX_REQUIRE(in && D == 3 && H == 7 && W == 20 && kd == 3 && kh == 3 && kw == 3, "bx_conv_layer: CYL3D expects [C,3,7,20], k=3x3x3");
-            p.S_in = 420; p.S_out = 140; p.OD = 1; p.OH = 7; p.OW = 20;
-            return launch_conv<BX_GEOM_CYL3D>(p, n, st);
-        case BX_GEOM_CYL2D:
-            BX_REQUIRE(in && D == 1 && H == 7 && W == 20 && kd == 1 && kh == 3 && kw == 3, "bx_conv_layer: CYL2D expects [C,7,20], k=3x3");
-            p.S_in = 140; p.S_out = 140; p.OD = 1; p.OH = 7; p.OW = 20;
-            return launch_conv<BX_GEOM_CYL2D>(p, n, st);
-        case BX_GEOM_VALID3D:
-            BX_REQUIRE(in && D >= kd && H >= kh && W >= kw && kd >= 1 && kh >= 1 && kw >= 1, "bx_conv_layer: VALID3D kernel larger than input");
-            p.OD = D - kd + 1; p.OH = H - kh + 1; p.OW = W - kw + 1;
-            p.S_in = D * H * W; p.S_out = p.OD * p.OH * p.OW;
-            return launch_conv<BX_GEOM_VALID3D>(p, n, st);
-        case BX_GEOM_COSTVOL:
-            BX_REQUIRE(equi_s && equi_t && s_mids && t_mids, "bx_conv_layer: COSTVOL needs equi maps and match lists");
-            BX_REQUIRE(Cin == 32 && D == 20 && H == 5 && W == 20 && kd == 3 && kh == 3 && kw == 3, "bx_conv_layer: COSTVOL expects the [32,20,5,20] volume, k=3x3x3");
-            p.OD = 18; p.OH = 3; p.OW = 18; p.S_in = 2000; p.S_out = 972;
-            return launch_conv<BX_GEOM_COSTVOL>(p, n, st);
-        default:
-            bx_set_error("bx_conv_layer: unknown geometry %d", geom);
-            return BX_ERR_INVALID_ARG;
-    }
-}
 
 BX_API int bx_pool_desc(const float *x, int K, int C, int S, int channels_last, const float *w1, const float *b1,
                         const float *w2, const float *b2, float *desc, float *equi, void *stream) {

@@ -1,7 +1,9 @@
 // bx_conv_tc.cu -- a8/a11 convolution stacks on the Hopper tensor cores (wgmma, TF32 operands).
 //
-// Same implicit GEMM as bx_conv.cu (rows = (sample, output position), cols = Cout, K = taps*Cin, padding
-// geometry folded into the loader), but the inner product runs as wgmma .tf32 with fp32 accumulators in registers.
+// Implicit GEMM: rows = (sample, output position), cols = Cout, K = taps*Cin.  The circular-azimuth / zero-elevation
+// padding and the valid-convolution geometry are folded into the per-row, per-tap input offset computed by the loader (no
+// padded copies); BatchNorm (eval) is folded into the weights and bias on the host.  The inner product runs as wgmma .tf32
+// with fp32 accumulators in registers.
 // fp32-grade accuracy (descriptor parity 1e-4 rel) needs two things:
 //   1. the 3xTF32 split  x = hi + lo  (hi = x with the 13 low mantissa bits cleared, lo = x - hi, exact):
 //          a*b ~= ah*bh + ah*bl + al*bh          (dropped al*bl ~ 2^-20 relative)
@@ -35,8 +37,10 @@ struct ConvTcParams {
     int Cin, Cout, D, H, W, kd, kh, kw, relu;
     int S_in, S_out, OD, OH, OW, T;
     int seg_len;  // stages per accumulator segment
-    const float *equi_s, *equi_t;
-    const int *s_mids, *t_mids;
+    const float *equi_s, *equi_t;  // COSTAB: the factor maps A and B of bx_costvol_ab
+    // Unused.  Without these 16 bytes ptxas schedules every instantiation differently; they keep the generated code the
+    // one whose speed the project has measured.
+    const void *reserved[2];
 };
 
 constexpr int TC_BM = 128;
@@ -110,18 +114,12 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv_tc_kernel(const ConvTcPara
             }
         }
         const float *pa = p.in, *pb = nullptr;
-        if (GEOM == BX_GEOM_COSTVOL) {
-            if (lvalid) {
-                pa = p.equi_s + (size_t)p.s_mids[ln] * 32 * 140;
-                pb = p.equi_t + (size_t)p.t_mids[ln] * 32 * 140;
-            }
-        } else if (GEOM == BX_GEOM_COSTAB) {
+        if (GEOM == BX_GEOM_COSTAB) {
             pa = p.equi_s + (size_t)ln * 32 * 60;     // A, channel-blocked [8][3*20][4]
             pb = p.equi_t + (size_t)ln * 32 * 54;     // B, channel-blocked [8][3*18][4]
         } else {
             pa = p.in + (size_t)ln * p.S_in * p.Cin;      // activations are channel-blocked: [n][Cin/4][position][4]
         }
-        constexpr int cstride = 140;   // channel-first equivariant maps of the direct cost-volume loader
         // (chunk, tap) of the stage filled next; the tap geometry comes from the shared table
         int chunk = 0, t = 0;
         const int oy20 = oy * 20;
@@ -140,12 +138,6 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv_tc_kernel(const ConvTcPara
                 offA = tp.w + oy20 + xx;
             } else if (GEOM == BX_GEOM_VALID3D) {
                 offA = rowbase + tp.w;
-            } else if (GEOM == BX_GEOM_COSTVOL) {  // value(c, n, k, l) = d1[c][1+k][(l-n) mod 20] - d2[c][1+k][l]
-                const int nn = oz + tp.x, kk = oy + tp.y, ll = ox + tp.z;
-                int sh = ll - nn;
-                sh = sh < 0 ? sh + 20 : sh;
-                offA = (1 + kk) * 20 + sh;
-                offB = (1 + kk) * 20 + ll;
             } else {  // COSTAB: value(c, n, k, l) = relu(A[c][k][(l-n) mod 20] - B[c][k][l])
                 const int nn = oz + tp.x, kk = oy + tp.y, ll = ox + tp.z;
                 int sh = ll - nn;
@@ -154,15 +146,7 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv_tc_kernel(const ConvTcPara
                 offB = kk * 18 + ll;
             }
             const int c0 = chunk * 16;
-            if (GEOM == BX_GEOM_COSTVOL) {
-                const float *src = pa + (size_t)c0 * cstride + offA;
-#pragma unroll
-                for (int kk = 0; kk < 16; ++kk) {
-                    float v = 0.0f;
-                    if (ok) v = src[kk * cstride] - pb[(size_t)(c0 + kk) * 140 + offB];
-                    a_reg[kk] = v;
-                }
-            } else if (GEOM == BX_GEOM_COSTAB) {   // relu(A - B) from the channel-blocked factors: 2 x four 16-byte loads
+            if (GEOM == BX_GEOM_COSTAB) {   // relu(A - B) from the channel-blocked factors: 2 x four 16-byte loads
                 const float4 *sa = reinterpret_cast<const float4 *>(pa) + (chunk * 4) * 60 + offA;
                 const float4 *sb4 = reinterpret_cast<const float4 *>(pb) + (chunk * 4) * 54 + offB;
 #pragma unroll
@@ -334,8 +318,7 @@ BX_API int bx_conv_tc_set_segment_stages(int stages) {
 
 BX_API int bx_conv_layer_tc(int geom, const float *in, const float *w_tc, const float *bias, float *out, int n,
                             const int32_t *d_n, int Cin, int Cout, int D, int H, int W, int kd, int kh, int kw, int relu,
-                            const float *equi_s, const float *equi_t, const int32_t *s_mids, const int32_t *t_mids,
-                            void *stream) {
+                            const float *equi_s, const float *equi_t, void *stream) {
     BX_REQUIRE(w_tc && bias && out, "bx_conv_layer_tc: null pointer");
     BX_REQUIRE(n >= 0 && Cin >= 16 && Cin % 16 == 0 && Cout >= 4 && Cout % 4 == 0 && Cout <= 128, "bx_conv_layer_tc: bad channels Cin=%d Cout=%d", Cin, Cout);
     BX_REQUIRE((reinterpret_cast<uintptr_t>(w_tc) & 15) == 0, "bx_conv_layer_tc: weights must be 16-byte aligned");
@@ -345,7 +328,7 @@ BX_API int bx_conv_layer_tc(int geom, const float *in, const float *w_tc, const 
     ConvTcParams p = {};
     p.in = in; p.w = w_tc; p.bias = bias; p.out = out; p.n = n; p.d_n = d_n;
     p.Cin = Cin; p.Cout = Cout; p.D = D; p.H = H; p.W = W; p.kd = kd; p.kh = kh; p.kw = kw; p.relu = relu;
-    p.equi_s = equi_s; p.equi_t = equi_t; p.s_mids = s_mids; p.t_mids = t_mids;
+    p.equi_s = equi_s; p.equi_t = equi_t;
     p.T = kd * kh * kw;
     p.seg_len = g_tc_max_stages;
     cudaStream_t st = bx_stream(stream);
@@ -363,11 +346,6 @@ BX_API int bx_conv_layer_tc(int geom, const float *in, const float *w_tc, const 
             p.OD = D - kd + 1; p.OH = H - kh + 1; p.OW = W - kw + 1;
             p.S_in = D * H * W; p.S_out = p.OD * p.OH * p.OW;
             return dispatch_nt<BX_GEOM_VALID3D>(p, n, st);
-        case BX_GEOM_COSTVOL:
-            BX_REQUIRE(equi_s && equi_t && s_mids && t_mids, "bx_conv_layer_tc: COSTVOL needs equi maps and match lists");
-            BX_REQUIRE(Cin == 32 && D == 20 && H == 5 && W == 20 && kd == 3 && kh == 3 && kw == 3, "bx_conv_layer_tc: COSTVOL expects the [32,20,5,20] volume, k=3x3x3");
-            p.OD = 18; p.OH = 3; p.OW = 18; p.S_in = 2000; p.S_out = 972;
-            return dispatch_nt<BX_GEOM_COSTVOL>(p, n, st);
         case BX_GEOM_COSTAB:
             BX_REQUIRE(equi_s && equi_t, "bx_conv_layer_tc: COSTAB needs the A and B factors");
             BX_REQUIRE(Cin == 32 && D == 18 && H == 3 && W == 18 && kd == 3 && kh == 3 && kw == 3, "bx_conv_layer_tc: COSTAB expects the [32,18,3,18] activation, k=3x3x3");

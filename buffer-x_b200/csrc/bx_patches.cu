@@ -379,116 +379,6 @@ __global__ void __launch_bounds__(HG_THREADS) hg_query_batched_kernel(const HgJo
                   patches + (size_t)J.koff[j] * P * 3, (int)blockIdx.x - J.koff[j]);
 }
 
-// ---- segmented form of select_patches (alternative, BX_PATCHES=seg): the same ordered "first P hits", fully parallel ------
-// The streaming kernel above is one dependent scan per key-point (early exit included) with three block barriers per 2048
-// points.  Here the scan is cut into independent (key-point, 2048-point segment) tasks:
-//   pass 1  one warp per task: 64 ballots, the hit masks (64 words) and the hit count go to a workspace;
-//   pass 2  one warp per task: offset = hits of the earlier segments of its key-point (a 32-lane sum over <= 256 segments);
-//           if the offset is below P the task re-reads its masks and writes its hits at offset + rank -- same order, same
-//           d2 < r2 test, so every index and coordinate is what the serial scan produces; the task of segment 0 also writes
-//           the padding slots.
-// No early exit (scale 0 does up to twice the distance tests), but 10-60x more independent warps and no block barriers.
-// It was not faster than the streaming kernel on the B200 (not re-measured on the H100), so the streaming kernel stays the
-// production path; kept as the independently written second implementation the tests compare.
-constexpr int SG_SEG = 2048;                 // points per segment
-constexpr int SG_WORDS = SG_SEG / 32;        // 64 mask words per task
-constexpr int SG_WARPS = 8;                  // tasks (consecutive key-points, same segment) per CTA
-
-__global__ void __launch_bounds__(SG_WARPS * 32)
-sp_seg_count_kernel(const float4 *__restrict__ pts4, int N, const float *__restrict__ kpts, int K, float radius,
-                    const float *__restrict__ d_radius, int nseg, unsigned *__restrict__ masks, int *__restrict__ counts) {
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    const int k = blockIdx.x * SG_WARPS + warp, g = blockIdx.y;
-    if (k >= K) return;
-    const float r = d_radius ? *d_radius : radius;
-    const float r2 = r * r;
-    const float qx = kpts[3 * (size_t)k], qy = kpts[3 * (size_t)k + 1], qz = kpts[3 * (size_t)k + 2];
-    const int base = g * SG_SEG;
-    unsigned *mrow = masks + ((size_t)k * nseg + g) * SG_WORDS;
-    int cnt = 0;
-    unsigned mine0 = 0u, mine1 = 0u;         // lane l keeps words l and 32 + l
-#pragma unroll 4
-    for (int it = 0; it < SG_WORDS; ++it) {
-        const int j = base + it * 32 + lane;
-        float4 p = make_float4(0.f, 0.f, 0.f, 0.f);
-        if (j < N) p = __ldg(pts4 + j);
-        const float d2 = bx_d2(qx - p.x, qy - p.y, qz - p.z);
-        const unsigned m = __ballot_sync(BX_FULL, (j < N) && (d2 < r2));
-        cnt += __popc(m);
-        if ((it & 31) == lane) { if (it < 32) mine0 = m; else mine1 = m; }
-    }
-    mrow[lane] = mine0;
-    mrow[32 + lane] = mine1;
-    if (lane == 0) counts[(size_t)k * nseg + g] = cnt;
-}
-
-__global__ void __launch_bounds__(SG_WARPS * 32)
-sp_seg_emit_kernel(const float4 *__restrict__ pts4, int N, const float *__restrict__ kpts, int K, int P, int nseg,
-                   const unsigned *__restrict__ masks, const int *__restrict__ counts, int *__restrict__ idx, float *__restrict__ patches) {
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    const int k = blockIdx.x * SG_WARPS + warp, g = blockIdx.y;
-    if (k >= K) return;
-    const int *crow = counts + (size_t)k * nseg;
-    int before = 0, total = 0;
-    for (int s = lane; s < nseg; s += 32) {
-        const int c = crow[s];
-        total += c;
-        if (s < g) before += c;
-    }
-#pragma unroll
-    for (int o = 16; o >= 1; o >>= 1) {
-        before += __shfl_xor_sync(BX_FULL, before, o);
-        total += __shfl_xor_sync(BX_FULL, total, o);
-    }
-    const float qx = kpts[3 * (size_t)k], qy = kpts[3 * (size_t)k + 1], qz = kpts[3 * (size_t)k + 2];
-    int *row = idx ? idx + (size_t)k * P : nullptr;
-    float *out = patches + (size_t)k * P * 3;
-    const unsigned *mrow = masks + ((size_t)k * nseg + g) * SG_WORDS;
-    if (before < P && crow[g] > 0) {
-        int off = before;
-        for (int it = 0; it < SG_WORDS && off < P; ++it) {
-            const unsigned m = mrow[it];
-            if (!m) continue;
-            const int slot = off + __popc(m & ((1u << lane) - 1u));
-            if (((m >> lane) & 1u) && slot < P) {
-                const int j = g * SG_SEG + it * 32 + lane;
-                const float4 p = __ldg(pts4 + j);
-                if (row) row[slot] = j;
-                const bool centre = (slot == P - 1);          // slot P-1 always holds the key-point itself (patch_embedder.py:109)
-                out[3 * slot] = centre ? qx : p.x;
-                out[3 * slot + 1] = centre ? qy : p.y;
-                out[3 * slot + 2] = centre ? qz : p.z;
-            }
-            off += __popc(m);
-        }
-    }
-    if (g != 0) return;
-    // padding (task of segment 0): ball_query repeats the first hit; the fix-up replaces those slots by the key-point.
-    // No hit at all: index row = 0, slot 0 = point 0 of the permuted cloud, every other slot = key-point.
-    const int cnt = total < P ? total : P;
-    if (cnt >= P) return;
-    int first = 0;
-    if (total > 0 && row) {                   // index of the first hit: first set bit of the first non-empty segment
-        int sg = 0;
-        while (crow[sg] == 0) ++sg;
-        const unsigned *mr = masks + ((size_t)k * nseg + sg) * SG_WORDS;
-        int w = 0;
-        while (mr[w] == 0u) ++w;
-        first = sg * SG_SEG + w * 32 + (__ffs(mr[w]) - 1);
-    }
-    for (int s = cnt + lane; s < P; s += 32) {
-        if (row) row[s] = first;
-        float x = qx, y = qy, z = qz;
-        if (cnt == 0 && s == 0 && P > 1) {
-            const float4 p0 = pts4[0];
-            x = p0.x; y = p0.y; z = p0.z;
-        }
-        out[3 * s] = x;
-        out[3 * s + 1] = y;
-        out[3 * s + 2] = z;
-    }
-}
-
 // plain ordered ball query over a packed [n,3] cloud (pointnet2_ops.ball_query semantics)
 __global__ void __launch_bounds__(BQ_WARPS * 32)
 ball_query_kernel(const float *__restrict__ xyz, int n, const float *__restrict__ qry, int m, float radius, int nsample,
@@ -774,31 +664,6 @@ BX_API int bx_select_patches_grid_batched(int njobs, const void *const *pts4, co
     if (bx_needs_attr(attr, bitmap))
         BX_CUDA(cudaFuncSetAttribute(hg_query_batched_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(200 * 1024)));
     hg_query_batched_kernel<<<koff, HG_THREADS, bitmap, st>>>(J, P, patches);
-    BX_LAUNCH_CHECK();
-    return BX_OK;
-}
-
-BX_API long long bx_select_patches_workspace_bytes(int N, int K) {
-    const long long nseg = (N + SG_SEG - 1) / SG_SEG;
-    return (long long)K * nseg * (SG_WORDS + 1) * 4;
-}
-
-BX_API int bx_select_patches_seg(const float *pts4, int N, const float *kpts, int K, float radius, const float *d_radius, int P,
-                                 int32_t *idx, float *patches, void *workspace, void *stream) {
-    BX_REQUIRE(pts4 && kpts && patches && workspace, "bx_select_patches_seg: null pointer");
-    BX_REQUIRE(N >= 1 && K >= 0 && P >= 1, "bx_select_patches_seg: bad sizes N=%d K=%d P=%d", N, K, P);
-    BX_REQUIRE((reinterpret_cast<uintptr_t>(pts4) & 15) == 0, "bx_select_patches_seg: pts4 must be 16-byte aligned");
-    if (K == 0) return BX_OK;
-    const int nseg = (N + SG_SEG - 1) / SG_SEG;
-    BX_REQUIRE(nseg <= 65535, "bx_select_patches_seg: cloud too large");
-    unsigned *masks = reinterpret_cast<unsigned *>(workspace);
-    int *counts = reinterpret_cast<int *>(masks + (size_t)K * nseg * SG_WORDS);
-    const dim3 grid((unsigned)((K + SG_WARPS - 1) / SG_WARPS), (unsigned)nseg);
-    sp_seg_count_kernel<<<grid, SG_WARPS * 32, 0, bx_stream(stream)>>>(reinterpret_cast<const float4 *>(pts4), N, kpts, K, radius, d_radius, nseg,
-                                                                       masks, counts);
-    BX_LAUNCH_CHECK();
-    sp_seg_emit_kernel<<<grid, SG_WARPS * 32, 0, bx_stream(stream)>>>(reinterpret_cast<const float4 *>(pts4), N, kpts, K, P, nseg, masks, counts,
-                                                                      idx, patches);
     BX_LAUNCH_CHECK();
     return BX_OK;
 }

@@ -110,16 +110,12 @@ class MiniSpinNet(nn.Module):
                           prep["b_pnt"], self.azi_n, debug=debug)
         feat = res[0] if debug else res                                  # [K,4,V,4] channel-blocked
         K = kpts.shape[0]
-        if pn.USE_FFMA:   # CUDA-core debug path works channel-first
-            x, _ = self.conv_net(ops.from_blocked(feat).view(K, 16, self.rad_n, self.ele_n, self.azi_n))
-            desc, equi = ops.pool_desc(x, prep["w1"], prep["b1"], prep["w2"], prep["b2"])
-        else:
-            x, _ = self.conv_net(feat)                                   # [K,8,140,4] channel-blocked
-            desc, equi = ops.pool_desc(x, prep["w1"], prep["b1"], prep["w2"], prep["b2"], channels_last=True)
+        x, _ = self.conv_net(feat)                                       # [K,8,140,4] channel-blocked
+        desc, equi = ops.pool_desc(x, prep["w1"], prep["b1"], prep["w2"], prep["b2"], channels_last=True)
         out = {"desc": desc, "equi": equi, "rand_axis": rand_axis, "R": R, "patches": delta, "aug_rotation": aug_R}
         if debug:
-            x_cf = x if pn.USE_FFMA else ops.from_blocked(x).view(K, -1, self.ele_n, self.azi_n)
-            out.update(idx=idx, raw_patches=patches, vidx=res[1], inv=res[2], feat=ops.from_blocked(feat), x=x_cf)
+            out.update(idx=idx, raw_patches=patches, vidx=res[1], inv=res[2], feat=ops.from_blocked(feat),
+                       x=ops.from_blocked(x).view(K, -1, self.ele_n, self.azi_n))
         return out
 
     def forward_multi(self, jobs, is_aligned_to_global_z, radii=None):
@@ -142,7 +138,7 @@ class MiniSpinNet(nn.Module):
         # `radii` = the contiguous device array of per-scale radii when the jobs are (src, tgt) per scale with equal key-point
         # counts: the local reference frames of all jobs then run in ONE launch (patch k uses radii[k // (2 K)])
         one_lrf = radii is not None and len(set(Ks)) == 1 and len(jobs) == 2 * radii.numel()
-        one_sel = len(jobs) <= 16 and ops.SELECT_PATCHES_SCAN and all(isinstance(j[2], torch.Tensor) for j in jobs)   # all patch gatherings of the pair in one launch
+        one_sel = len(jobs) <= 16 and all(isinstance(j[2], torch.Tensor) for j in jobs)   # all patch gatherings of the pair in one launch
         sel = []
         for (pts, kpts, des_r, perm), K in zip(jobs, Ks):
             sel.append((ops.permute_cloud(pts.contiguous(), perm), kpts.contiguous(), des_r))
@@ -167,19 +163,15 @@ class MiniSpinNet(nn.Module):
         if one_lrf:
             ops.lrf(patches, radii, bool(is_aligned_to_global_z), delta=delta, Rt=R_all, ra=ra_all, r_group=2 * Ks[0])
         net = self.conv_net
-        if not pn.USE_FFMA and not net.force_tf32 and self.rad_n * self.ele_n * self.azi_n == 420 and self.azi_n == 20:
+        if not net.force_tf32 and self.rad_n * self.ele_n * self.azi_n == 420 and self.azi_n == 20:
             # production: features straight into the presplit fp16 format the first conv layer fetches with bulk copies
             feat = ops.spt_pnt_sd(delta, prep["voxels"], prep["rot"], self.delta / self.rad_n, self.voxel_sample, prep["w_pnt"],
                                   prep["b_pnt"], self.azi_n, net.overflow_flag(dev))
         else:
             feat = ops.spt_pnt(delta, prep["voxels"], prep["rot"], self.delta / self.rad_n, self.voxel_sample, prep["w_pnt"],
                                prep["b_pnt"], self.azi_n)
-        if pn.USE_FFMA:
-            x, _ = self.conv_net(ops.from_blocked(feat).view(Kt, 16, self.rad_n, self.ele_n, self.azi_n))
-            desc, equi = ops.pool_desc(x, prep["w1"], prep["b1"], prep["w2"], prep["b2"])
-        else:
-            x, _ = self.conv_net(feat, K=Kt)
-            desc, equi = ops.pool_desc(x, prep["w1"], prep["b1"], prep["w2"], prep["b2"], channels_last=True)
+        x, _ = self.conv_net(feat, K=Kt)
+        desc, equi = ops.pool_desc(x, prep["w1"], prep["b1"], prep["w2"], prep["b2"], channels_last=True)
         outs, o = [], 0
         for K, R, ra in zip(Ks, Rs, axes):
             outs.append({"desc": desc[o:o + K], "equi": equi[o:o + K], "rand_axis": ra, "R": R, "patches": delta[o:o + K],

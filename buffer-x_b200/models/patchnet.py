@@ -3,8 +3,9 @@
 Mirrors the state_dict layout of /root/reference/models/patchnet.py: ``Cylindrical_Net``
 (:68-84, ops.{0,1,3,4,...,21}) and ``CostNet`` (:192-210, ops.{0,1,...,27}); BatchNorm layers in the
 stacks have ``affine=False`` (:28,31).  The modules hold parameters only -- the arithmetic runs in
-``bx_conv_layer`` (buffer-x_b200/csrc/bx_conv.cu).  ``folded()`` returns, per conv layer, the weight
-re-laid as [tap][Cin][Cout] with the eval-mode BatchNorm folded in (computed in fp64, stored fp32).
+the library's convolution kernels (``bx_conv_layer_sd``, ``bx_conv_layer_tc``, ``bx_costvol_ab``).  ``folded()``
+returns, per conv layer, the weight re-laid as [tap][Cin][Cout] with the eval-mode BatchNorm folded in (computed in
+fp64, stored fp32), and the kernels' operand images of it.
 """
 import torch
 import torch.nn as nn
@@ -13,9 +14,6 @@ import os
 
 from bufferx_b200 import ops
 
-# Debug switch only: BX_CONV=ffma routes the conv stacks through the fp32 CUDA-core kernel (bx_conv.cu)
-# instead of the tensor-core kernel (bx_conv_tc.cu).  Both are sm_90a kernels of this library.
-USE_FFMA = os.environ.get("BX_CONV", "sd").lower() == "ffma"
 # BX_CONV=tc: the descriptor stack on the TF32 kernel (bx_conv_tc.cu) instead of the shifted-descriptor fp16-split
 # kernel (bx_conv_sd.cu, the default).  The TF32 kernel is also the automatic fall-back when an activation leaves fp16 range.
 USE_TF32_DESC = os.environ.get("BX_CONV", "sd").lower() == "tc"
@@ -24,9 +22,6 @@ USE_TF32_DESC = os.environ.get("BX_CONV", "sd").lower() == "tc"
 # they have been scheduled), so the static stride stays the default; that was measured on the B200 and has not been
 # re-measured on the H100.  The path is kept and tested.
 DYNAMIC_TILES = os.environ.get("BX_SD_DYNAMIC", "0") == "1"
-# Debug switch only: BX_COSTVOL=direct runs the first CostNet layer as a convolution over the on-the-fly cost volume
-# (GEOM_COSTVOL) instead of its factorised form (bx_costvol_ab + GEOM_COSTAB).
-DIRECT_COSTVOL = os.environ.get("BX_COSTVOL", "factored").lower() == "direct"
 
 
 def fold_conv_bn(conv_w, conv_b, bn_mean=None, bn_var=None, bn_w=None, bn_b=None, eps=1e-5):
@@ -121,33 +116,31 @@ class Cylindrical_Net(_ConvStack):
         return self._flag
 
     def forward(self, x, K=None):
-        """Tensor-core path (default): x [K,4,420,4] channel-blocked (or the presplit image of K patches) -> x_out [K,8,140,4].
-        CUDA-core debug path (BX_CONV=ffma): x [K,16,3,7,20] -> [K,32,7,20].  Returns (x_out, None)."""
+        """x [K,4,420,4] channel-blocked (or the presplit image of K patches) -> (x_out [K,8,140,4], None)."""
         presplit_in = x.dtype == torch.float16             # [3, 4, rows, 8] from bx_spt_pnt_sd: K is passed separately
         K = x.shape[0] if not presplit_in else int(K)
         dev = x.device
         L = self.folded()
         cur = x.contiguous()
-        use_sd = not USE_FFMA and not self.force_tf32
+        use_sd = not self.force_tf32
         assert use_sd or not presplit_in
         flag = self.overflow_flag(dev) if use_sd else None
         # dynamic tile scheduling of the persistent conv kernels: one zeroed counter pair per layer (and per call = per stream)
         ctrs = torch.zeros(2 * len(L), dtype=torch.int32, device=dev) if (use_sd and DYNAMIC_TILES) else None
         for i, l in enumerate(L):
-            out = torch.empty((K, l["cout"], 140) if USE_FFMA else (K, l["cout"] // 4, 140, 4), dtype=torch.float32, device=dev)
+            out = torch.empty((K, l["cout"] // 4, 140, 4), dtype=torch.float32, device=dev)
             if use_sd:       # layer-to-layer activations in the presplit padded fp16 format; fp32 in at the first, fp32 out at the last layer
                 out = out if i == len(L) - 1 else ops.conv_sd_buffer(K, l["cout"], dev)
                 ops.conv_layer_sd(ops.GEOM_CYL3D if i == 0 else ops.GEOM_CYL2D, cur, l["w_sd"], l["b"], out, K, l["cin"], l["cout"], l["relu"], flag,
                                   tile_ctr=None if ctrs is None else ctrs[2 * i:2 * i + 2])
                 cur = out
                 continue
-            conv, w = (ops.conv_layer, l["w"]) if USE_FFMA else (ops.conv_layer_tc, l["w_tc"])
             if i == 0:
-                conv(ops.GEOM_CYL3D, cur, w, l["b"], out, K, l["cin"], l["cout"], 3, 7, 20, 3, 3, 3, l["relu"])
+                ops.conv_layer_tc(ops.GEOM_CYL3D, cur, l["w_tc"], l["b"], out, K, l["cin"], l["cout"], 3, 7, 20, 3, 3, 3, l["relu"])
             else:
-                conv(ops.GEOM_CYL2D, cur, w, l["b"], out, K, l["cin"], l["cout"], 1, 7, 20, 1, 3, 3, l["relu"])
+                ops.conv_layer_tc(ops.GEOM_CYL2D, cur, l["w_tc"], l["b"], out, K, l["cin"], l["cout"], 1, 7, 20, 1, 3, 3, l["relu"])
             cur = out
-        return (cur.view(K, L[-1]["cout"], 7, 20) if USE_FFMA else cur), None
+        return cur, None
 
 
 class CostNet(_ConvStack):
@@ -172,8 +165,7 @@ class CostNet(_ConvStack):
         L = self.folded()
         D, H, W = 20, 5, 20
         cur = None
-        factored = (not USE_FFMA) and not DIRECT_COSTVOL
-        use_sd = not USE_FFMA and not self.force_tf32
+        use_sd = not self.force_tf32
         flag = self.flag_source(dev) if (use_sd and self.flag_source is not None) else None
         ctrs = torch.zeros(2 * len(L), dtype=torch.int32, device=dev) if (use_sd and DYNAMIC_TILES) else None
         for i, l in enumerate(L):
@@ -188,8 +180,7 @@ class CostNet(_ConvStack):
                                   tile_ctr=None if ctrs is None else ctrs[2 * i:2 * i + 2])
                 cur, D, H, W = out, OD, OH, OW
                 continue
-            conv, w = (ops.conv_layer, l["w"]) if USE_FFMA else (ops.conv_layer_tc, l["w_tc"])
-            if factored and i == 0:
+            if i == 0:
                 # first layer is linear in the cost volume before its ReLU: two small convolutions of the equivariant
                 # maps (bx_costvol_ab); the second layer's loader rebuilds relu(A - B) on the fly (GEOM_COSTAB)
                 if "wa" not in l:
@@ -199,8 +190,8 @@ class CostNet(_ConvStack):
                 continue
             # tensor-core layers exchange channel-blocked activations [maxM, C/4, positions, 4]
             def _f32_out():
-                return torch.empty((maxM, l["cout"], OD * OH * OW) if USE_FFMA else (maxM, l["cout"] // 4, OD * OH * OW, 4), dtype=torch.float32, device=dev)
-            if factored and i == 1 and use_sd:       # regenerated first activation -> 96 -> 64 conv over the 18 x 18 raster
+                return torch.empty((maxM, l["cout"] // 4, OD * OH * OW, 4), dtype=torch.float32, device=dev)
+            if i == 1 and use_sd:       # regenerated first activation -> 96 -> 64 conv over the 18 x 18 raster
                 if "w_sd_ab" not in l:
                     l["w_sd_ab"] = ops.conv_sd_weights_costab(l["w"])
                 out = ops.conv_sd_buffer(maxM, 64, dev, 256) if L[2].get("w_sd") is not None else _f32_out()
@@ -208,13 +199,11 @@ class CostNet(_ConvStack):
                 cur, D, H, W = out, OD, OH, OW
                 continue
             out = _f32_out()
-            if factored and i == 1:
-                conv(ops.GEOM_COSTAB, None, w, l["b"], out, maxM, l["cin"], l["cout"], D, H, W, kd, kh, kw, l["relu"],
-                     d_n=d_M, equi_s=fa, equi_t=fb)
-            elif i == 0:
-                conv(ops.GEOM_COSTVOL, None, w, l["b"], out, maxM, l["cin"], l["cout"], D, H, W, kd, kh, kw, l["relu"],
-                     d_n=d_M, equi_s=equi_s, equi_t=equi_t, s_mids=s_mids, t_mids=t_mids)
+            if i == 1:
+                ops.conv_layer_tc(ops.GEOM_COSTAB, None, l["w_tc"], l["b"], out, maxM, l["cin"], l["cout"], D, H, W, kd, kh, kw, l["relu"],
+                                  d_n=d_M, equi_s=fa, equi_t=fb)
             else:
-                conv(ops.GEOM_VALID3D, cur, w, l["b"], out, maxM, l["cin"], l["cout"], D, H, W, kd, kh, kw, l["relu"], d_n=d_M)
+                ops.conv_layer_tc(ops.GEOM_VALID3D, cur, l["w_tc"], l["b"], out, maxM, l["cin"], l["cout"], D, H, W, kd, kh, kw, l["relu"],
+                                  d_n=d_M)
             cur, D, H, W = out, OD, OH, OW
         return cur.view(maxM, L[-1]["cout"])      # one output position: blocked [maxM, C/4, 1, 4] == [maxM, C]

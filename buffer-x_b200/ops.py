@@ -19,17 +19,15 @@ LIB_PATH = os.path.join(_PKG, "libbufferx_b200.so")
 
 SYMBOLS = [
     "bx_last_error", "bx_version", "bx_device_sm_count", "bx_launch_count", "bx_fps", "bx_radius_estimate", "bx_permute_cloud",
-    "bx_select_patches", "bx_ball_query", "bx_lrf", "bx_spt_pnt", "bx_conv_layer", "bx_conv_tc_ntile", "bx_conv_layer_tc",
+    "bx_select_patches", "bx_ball_query", "bx_lrf", "bx_spt_pnt", "bx_conv_tc_ntile", "bx_conv_layer_tc",
     "bx_pool_desc", "bx_mutual_nn",
     "bx_hypotheses", "bx_consensus", "bx_ransac_workspace_bytes", "bx_ransac", "bx_refine", "bx_conv_tc_set_segment_stages",
     "bx_radius_neighbors", "bx_grid_subsample", "bx_costvol_ab", "bx_concat_matches",
-    "bx_pca_analysis", "bx_project_range", "bx_voxel_down_sample", "bx_conv_layer_sd", "bx_conv_sd_rows", "bx_spt_pnt_sd", "bx_fps_set_sync_mode", "bx_select_patches_seg", "bx_select_patches_workspace_bytes", "bx_conv_layer_sd_costab", "bx_lrf_batched", "bx_select_patches_batched", "bx_fps_ex", "bx_select_patches_grid", "bx_select_patches_grid_workspace_bytes", "bx_select_patches_grid_batched",
+    "bx_pca_analysis", "bx_project_range", "bx_voxel_down_sample", "bx_conv_layer_sd", "bx_conv_sd_rows", "bx_spt_pnt_sd", "bx_fps_set_sync_mode", "bx_conv_layer_sd_costab", "bx_lrf_batched", "bx_select_patches_batched", "bx_fps_ex", "bx_select_patches_grid", "bx_select_patches_grid_workspace_bytes", "bx_select_patches_grid_batched",
     "bx_gt_matches", "bx_so2_augment", "bx_equi_match", "bx_so2_gt",
 ]
 
-GEOM_CYL3D, GEOM_CYL2D, GEOM_VALID3D, GEOM_COSTVOL, GEOM_COSTAB = 0, 1, 2, 3, 4
-# BX_PATCHES=seg: segmented two-pass form of select_patches (an independently written cross-check of the streaming scan)
-SELECT_PATCHES_SCAN = os.environ.get("BX_PATCHES", "scan").lower() != "seg"
+GEOM_CYL3D, GEOM_CYL2D, GEOM_VALID3D, GEOM_COSTAB = 0, 1, 2, 4
 RADIUS_BINS = 8192
 
 _lib = None
@@ -62,9 +60,6 @@ def load_library():
     lib.bx_radius_estimate.argtypes = [P, c_int, P, c_int, c_int64, P, c_int, c_double, P, P, P, P, P]
     lib.bx_permute_cloud.argtypes = [P, P, c_int, P, P]
     lib.bx_select_patches.argtypes = [P, c_int, P, c_int, c_float, P, c_int, P, P, P]
-    lib.bx_select_patches_seg.argtypes = [P, c_int, P, c_int, c_float, P, c_int, P, P, P, P]
-    lib.bx_select_patches_workspace_bytes.argtypes = [c_int, c_int]
-    lib.bx_select_patches_workspace_bytes.restype = c_int64
     lib.bx_select_patches_batched.argtypes = [c_int, P, P, P, P, P, c_int, P, P]
     lib.bx_select_patches_grid.argtypes = [P, c_int, P, c_int, P, c_int, P, P, P, P]
     lib.bx_select_patches_grid_workspace_bytes.argtypes = [c_int]
@@ -74,8 +69,7 @@ def load_library():
     lib.bx_lrf.argtypes = [P, c_int, c_int, c_float, P, c_int, P, P, P, P]
     lib.bx_lrf_batched.argtypes = [P, c_int, c_int, c_float, P, c_int, c_int, P, P, P, P]
     lib.bx_spt_pnt.argtypes = [P, c_int, c_int, P, c_int, c_int, P, c_float, c_int, P, P, P, P, P, P]
-    lib.bx_conv_layer.argtypes = [c_int, P, P, P, P, c_int, P] + [c_int] * 9 + [P, P, P, P, P]
-    lib.bx_conv_layer_tc.argtypes = [c_int, P, P, P, P, c_int, P] + [c_int] * 9 + [P, P, P, P, P]
+    lib.bx_conv_layer_tc.argtypes = [c_int, P, P, P, P, c_int, P] + [c_int] * 9 + [P, P, P]
     lib.bx_conv_tc_ntile.argtypes = [c_int]
     lib.bx_conv_layer_sd.argtypes = [c_int, P, c_int, P, P, P, c_int, c_int, P, c_int, c_int, c_int, c_int, c_int, P, P, P]
     lib.bx_conv_sd_rows.argtypes = [c_int, c_int]
@@ -242,13 +236,8 @@ def select_patches(pts4: torch.Tensor, kpts: torch.Tensor, radius, P: int, want_
     ev = profiler.span("select_patches", 16.0 * N + 12.0 * K + K * P * (12.0 + (4.0 if want_idx else 0.0))) if profiler else None
     if ev:
         ev[0].record()
-    if SELECT_PATCHES_SCAN:      # the streaming kernel (one ordered scan per key-point with early exit; production)
-        _check(load_library().bx_select_patches(_dp(pts4, F32, "pts4"), N, _dp(kpts, F32, "kpts"), K, rv, rp, P, _dp(idx), _dp(patches), _stream()),
-               "bx_select_patches")
-    else:
-        ws = torch.empty((int(load_library().bx_select_patches_workspace_bytes(N, K)) + 3) // 4, dtype=I32, device=pts4.device)
-        _check(load_library().bx_select_patches_seg(_dp(pts4, F32, "pts4"), N, _dp(kpts, F32, "kpts"), K, rv, rp, P, _dp(idx), _dp(patches), _dp(ws),
-                                                    _stream()), "bx_select_patches_seg")
+    _check(load_library().bx_select_patches(_dp(pts4, F32, "pts4"), N, _dp(kpts, F32, "kpts"), K, rv, rp, P, _dp(idx), _dp(patches), _stream()),
+           "bx_select_patches")
     if ev:
         ev[1].record()
     return patches, idx
@@ -345,24 +334,6 @@ def spt_pnt(delta, voxels, rot, voxel_r: float, nv: int, w, b, azi_n: int, debug
     return (feat, vidx, inv) if debug else feat
 
 
-def conv_layer(geom, x, w, bias, out, n, Cin, Cout, D, H, W, kd, kh, kw, relu, d_n=None, equi_s=None, equi_t=None,
-               s_mids=None, t_mids=None):
-    ev = None
-    if profiler is not None and d_n is None:
-        OD, OH, OW = (1, 7, 20) if geom in (GEOM_CYL3D, GEOM_CYL2D) else (D - kd + 1, H - kh + 1, W - kw + 1)
-        ev = profiler.span("conv_desc", 2.0 * n * OD * OH * OW * Cout * Cin * kd * kh * kw)
-        ev[0].record()
-    elif profiler is not None:
-        ev = profiler.span("conv_cost", 0.0)
-        ev[0].record()
-    _check(load_library().bx_conv_layer(geom, _dp(x, F32, "x"), _dp(w, F32, "w"), _dp(bias, F32, "bias"), _dp(out, F32, "out"), int(n),
-                                        _dp(d_n, I32, "d_n"), Cin, Cout, D, H, W, kd, kh, kw, int(bool(relu)), _dp(equi_s, F32), _dp(equi_t, F32),
-                                        _dp(s_mids, I32), _dp(t_mids, I32), _stream()), "bx_conv_layer")
-    if ev:
-        ev[1].record()
-    return out
-
-
 def tf32_split(w: torch.Tensor):
     """hi = round-to-nearest (ties away) TF32 of w (10-bit mantissa), lo = w - hi (exact in fp32)."""
     bits = w.contiguous().view(torch.int32).to(torch.int64) & 0xFFFFFFFF
@@ -399,8 +370,7 @@ def from_blocked(x: torch.Tensor) -> torch.Tensor:
     return x.permute(0, 1, 3, 2).reshape(n, G * 4, S).contiguous()
 
 
-def conv_layer_tc(geom, x, w_tc, bias, out, n, Cin, Cout, D, H, W, kd, kh, kw, relu, d_n=None, equi_s=None, equi_t=None,
-                  s_mids=None, t_mids=None):
+def conv_layer_tc(geom, x, w_tc, bias, out, n, Cin, Cout, D, H, W, kd, kh, kw, relu, d_n=None, equi_s=None, equi_t=None):
     """x / out are channel-blocked: [n, Cin/4, S_in, 4] / [n, Cout/4, S_out, 4]."""
     ev = None
     if profiler is not None and d_n is None:
@@ -412,7 +382,7 @@ def conv_layer_tc(geom, x, w_tc, bias, out, n, Cin, Cout, D, H, W, kd, kh, kw, r
         ev[0].record()
     _check(load_library().bx_conv_layer_tc(geom, _dp(x, F32, "x"), _dp(w_tc, F32, "w_tc"), _dp(bias, F32, "bias"), _dp(out, F32, "out"), int(n),
                                            _dp(d_n, I32, "d_n"), Cin, Cout, D, H, W, kd, kh, kw, int(bool(relu)), _dp(equi_s, F32), _dp(equi_t, F32),
-                                           _dp(s_mids, I32), _dp(t_mids, I32), _stream()), "bx_conv_layer_tc")
+                                           _stream()), "bx_conv_layer_tc")
     if ev:
         ev[1].record()
     return out

@@ -87,11 +87,6 @@ int bx_select_patches(const float *pts4, int N, const float *kpts, int K, float 
  * [sum_{i<j} K[i], ...) of `patches`.  The pointer arrays are HOST arrays of device pointers (<= 16 jobs). */
 int bx_select_patches_batched(int njobs, const void *const *pts4, const int32_t *N, const void *const *kpts, const int32_t *K,
                               const void *const *d_radius, int P, float *patches, void *stream);
-/* Same result, segmented form (alternative implementation, not faster; cross-checked in the tests): independent (key-point, 2048-point segment) tasks write hit masks and counts
- * into `workspace` (bx_select_patches_workspace_bytes(N, K) bytes), a second pass places the hits at their ordered offsets. */
-int bx_select_patches_seg(const float *pts4, int N, const float *kpts, int K, float radius, const float *d_radius, int P,
-                          int32_t *idx, float *patches, void *workspace, void *stream);
-long long bx_select_patches_workspace_bytes(int N, int K);
 /* Hash-grid form for large clouds (N >= ~50 k points): the permuted cloud is binned into a spatial hash of cells of edge >=
  * radius, a key-point tests the 27 cells around it only, hits set bits in a per-key-point bitmap over the point indices that
  * is read back in index order -- same contract and bit-identical output as bx_select_patches (device-side radius required).
@@ -140,23 +135,18 @@ int bx_spt_pnt_sd(const float *delta, int K, int P, const float *voxels, int V, 
                   void *stream);
 
 /* ---- a8/a11: convolution stacks -------------------------------------------------------------
- * One implicit-GEMM kernel serves every conv layer of Cylindrical_Net (models/patchnet.py:16-84,
- * circular-azimuth / zero-elevation padding of utils/common.py:265-310) and CostNet
- * (models/patchnet.py:151-210, un-padded).  Weights are [taps][Cin][Cout] with BatchNorm folded.
- * geom: BX_GEOM_*; in: [n][Cin][S_in]; out: [n][Cout][S_out]; n = *d_n if d_n != NULL else n. */
+ * Every conv layer of Cylindrical_Net (models/patchnet.py:16-84, circular-azimuth / zero-elevation padding of
+ * utils/common.py:265-310) and CostNet (models/patchnet.py:151-210, un-padded) is an implicit GEMM, rows = (sample,
+ * output position), cols = Cout, K = taps*Cin, on bx_conv_layer_sd (production) or bx_conv_layer_tc (TF32 fall-back).
+ * BatchNorm is folded into the weights.  geom: BX_GEOM_*; n = *d_n if d_n != NULL else n. */
 #define BX_GEOM_CYL3D 0    /* in [C,3,7,20] -> out [C,7,20], taps 27 */
 #define BX_GEOM_CYL2D 1    /* in [C,7,20]   -> out [C,7,20], taps 9  */
 #define BX_GEOM_VALID3D 2  /* in [C,D,H,W]  -> out [C,D-kd+1,H-kh+1,W-kw+1] */
-#define BX_GEOM_COSTVOL 3  /* VALID3D 3x3x3 whose input is the on-the-fly cost volume (models/BUFFERX.py:51-65) */
 #define BX_GEOM_COSTAB 4   /* VALID3D 3x3x3 on [32,18,3,18] whose input is the first CostNet activation regenerated from
                               bx_costvol_ab's factors: relu(A[c][k][(l-n) mod 20] - B[c][k][l]); equi_s = A, equi_t = B
-                              (channel-blocked [n][8][3*20][4] / [n][8][3*18][4]), s_mids/t_mids unused (bx_conv_layer_tc only) */
-int bx_conv_layer(int geom, const float *in, const float *w, const float *bias, float *out, int n, const int32_t *d_n,
-                  int Cin, int Cout, int D, int H, int W, int kd, int kh, int kw, int relu,
-                  const float *equi_s, const float *equi_t, const int32_t *s_mids, const int32_t *t_mids,
-                  void *stream);
+                              (channel-blocked [n][8][3*20][4] / [n][8][3*18][4]) (bx_conv_layer_tc only) */
 
-/* ---- a8 / a11: shifted-descriptor implicit GEMM, fp16-split operands ------------------------------------------
+/* Shifted-descriptor implicit GEMM, fp16-split operands.
  * The production kernel of the eight Cylindrical_Net layers (models/patchnet.py:16-84; padding utils/common.py:265-310)
  * and of the k = (3,1,3) layers of CostNet (models/patchnet.py:151-210).
  * geom = BX_GEOM_CYL3D (16 channels x 3 radial slices, k=3x3x3), BX_GEOM_CYL2D (k=3x3; circular azimuth / zero elevation
@@ -199,8 +189,7 @@ int bx_conv_tc_ntile(int Cout);
 int bx_conv_tc_set_segment_stages(int stages);
 int bx_conv_layer_tc(int geom, const float *in, const float *w_tc, const float *bias, float *out, int n,
                      const int32_t *d_n, int Cin, int Cout, int D, int H, int W, int kd, int kh, int kw, int relu,
-                     const float *equi_s, const float *equi_t, const int32_t *s_mids, const int32_t *t_mids,
-                     void *stream);
+                     const float *equi_s, const float *equi_t, void *stream);
 
 /* Factorised first CostNet layer (models/patchnet.py:196 applied to the cost volume of models/BUFFERX.py:51-65):
  * the layer is linear before its ReLU, so out0[co][n][k][l] = relu(A[co][k][(l-n) mod 20] - B[co][k][l]) with

@@ -125,14 +125,9 @@ def test_select_patches_bit_exact(dev, oracle, radius, P):
     pts4 = ops.permute_cloud(cu(pts, dev), cu(perm, dev))
     assert (pts4[:, :3].cpu().numpy() == pts[perm]).all()
     eidx, epat = oracle.select_patches(pts, perm, kp, radius, P)
-    for scan in (True, False):          # streaming (production) and segmented two-pass form
-        ops.SELECT_PATCHES_SCAN = scan
-        try:
-            pat, idx = ops.select_patches(pts4, cu(kp, dev), radius, P, want_idx=True)
-        finally:
-            ops.SELECT_PATCHES_SCAN = True
-        assert (idx.cpu().numpy() == eidx).all(), f"scan={scan}"
-        assert (pat.cpu().numpy() == epat).all(), f"scan={scan}"
+    pat, idx = ops.select_patches(pts4, cu(kp, dev), radius, P, want_idx=True)
+    assert (idx.cpu().numpy() == eidx).all()
+    assert (pat.cpu().numpy() == epat).all()
     # device-side radius gives the same result
     pat2, _ = ops.select_patches(pts4, cu(kp, dev), torch.tensor([radius], dtype=torch.float32, device=dev), P)
     assert (pat2.cpu().numpy() == epat).all()
@@ -242,31 +237,27 @@ def test_spt_presplit_output_is_the_split_of_the_fp32_features(dev, oracle, c1):
     c1["model"].cpu()
 
 
-def test_cylindrical_net_and_pooling(dev, oracle, c1):
+def test_cylindrical_net_and_both_pooling_layouts(dev, oracle, c1):
+    """The descriptor stack (channel-blocked fp32 in / out) against the oracle, and the pooling kernel from the channel-first
+    and the channel-blocked input layout: both against the oracle, and bit-identical to each other."""
     from bufferx_b200 import ops
     aux = c1["res"][5]
     s = aux["scales"][0]["src"]
     model = c1["model"].to(dev)
     K = s["feat"].shape[0]
-    from bufferx_b200.models import patchnet as pn
     f = cu(s["feat"].numpy(), dev)                                   # oracle layout: [K,16,420]
     ex = s["x"].numpy()
     prep = model.Desc.prepared(dev)
-    if pn.USE_FFMA:
-        x, _ = model.Desc.conv_net(f.view(K, 16, 3, 7, 20))
-        xcf = x
-    else:
-        x, _ = model.Desc.conv_net(ops.to_blocked(f))                # channel-blocked in / out: [K,8,140,4]
-        assert x.shape == (K, 8, 140, 4)
-        xcf = ops.from_blocked(x).reshape(K, 32, 7, 20)
-        d2, e2 = ops.pool_desc(ops.to_blocked(cu(ex, dev).reshape(K, 32, 140)), prep["w1"], prep["b1"], prep["w2"], prep["b2"],
-                               channels_last=True)
+    x, _ = model.Desc.conv_net(ops.to_blocked(f))                    # channel-blocked in / out: [K,8,140,4]
+    assert x.shape == (K, 8, 140, 4)
+    xcf = ops.from_blocked(x).reshape(K, 32, 7, 20)
+    d2, e2 = ops.pool_desc(ops.to_blocked(cu(ex, dev).reshape(K, 32, 140)), prep["w1"], prep["b1"], prep["w2"], prep["b2"],
+                           channels_last=True)
     assert relerr(xcf.cpu().numpy(), ex) < 1e-4                      # 8 stacked fp32 convs vs torch CPU
     desc, equi = ops.pool_desc(cu(ex, dev), prep["w1"], prep["b1"], prep["w2"], prep["b2"])
     assert np.abs(desc.cpu().numpy() - s["desc"].numpy()).max() < 1e-5
     assert np.abs(equi.cpu().numpy() - s["equi"].numpy()).max() < 1e-5
-    if not pn.USE_FFMA:                                              # both input layouts of the pooling kernel agree bit for bit
-        assert (d2 == desc).all() and (e2 == equi).all()
+    assert (d2 == desc).all() and (e2 == equi).all()                 # both input layouts of the pooling kernel agree bit for bit
     model.cpu()
 
 
@@ -716,12 +707,14 @@ def _torch_layer(geom, x, W, b, relu, kd, kh, kw):
     return F.relu(y) if relu else y
 
 
-@pytest.mark.parametrize("impl", ["sd", "tc", "ffma"])
+@pytest.mark.parametrize("impl", ["sd", "tc"])
 @pytest.mark.parametrize("geom,Cin,Cout,dims,k,n", [
     ("cyl3d", 16, 64, (3, 7, 20), (3, 3, 3), 37), ("cyl2d", 64, 128, (1, 7, 20), (1, 3, 3), 41),
     ("cyl2d", 128, 128, (1, 7, 20), (1, 3, 3), 19), ("cyl2d", 64, 32, (1, 7, 20), (1, 3, 3), 300),
     ("cyl2d", 32, 32, (1, 7, 20), (1, 3, 3), 5), ("valid3d", 32, 64, (18, 3, 18), (3, 3, 3), 9),
-    ("valid3d", 64, 128, (14, 1, 14), (3, 1, 3), 13), ("valid3d", 32, 20, (2, 1, 2), (2, 1, 2), 77)])
+    ("valid3d", 64, 128, (14, 1, 14), (3, 1, 3), 13), ("valid3d", 32, 20, (2, 1, 2), (2, 1, 2), 77),
+    ("cyl2d", 64, 64, (1, 7, 20), (1, 3, 3), 23), ("cyl2d", 128, 64, (1, 7, 20), (1, 3, 3), 7),
+    ("valid3d", 128, 128, (12, 1, 12), (3, 1, 3), 11), ("valid3d", 64, 32, (6, 1, 6), (3, 1, 3), 50)])
 def test_conv_layer_kernels(dev, geom, Cin, Cout, dims, k, n, impl):
     from bufferx_b200 import ops
     from bufferx_b200.models.patchnet import fold_conv_bn
@@ -743,7 +736,6 @@ def test_conv_layer_kernels(dev, geom, Cin, Cout, dims, k, n, impl):
     Wt, bf = fold_conv_bn(Wc, b)
     G = {"cyl3d": ops.GEOM_CYL3D, "cyl2d": ops.GEOM_CYL2D, "valid3d": ops.GEOM_VALID3D}[geom]
     OD, OH, OW = (1, 7, 20) if geom != "valid3d" else (D - kd + 1, H - kh + 1, W_ - kw + 1)
-    out = torch.full((n, Cout, OD * OH * OW), float("nan"), device=dev)
     xin = x.to(dev).reshape(n, Cin, -1).contiguous()
     if impl == "sd":                                                  # shifted-descriptor fp16-split kernel (production)
         out_cb = torch.full((n, Cout // 4, OD * OH * OW, 4), float("nan"), device=dev)
@@ -753,16 +745,14 @@ def test_conv_layer_kernels(dev, geom, Cin, Cout, dims, k, n, impl):
                           flag, d_n=d_n, D=D, W=W_)
         out = ops.from_blocked(out_cb)
         assert int(flag.item()) == 0
-    elif impl == "tc":                                                # tensor-core kernel: channel-blocked activations
+    else:                                                             # TF32 tensor-core kernel: channel-blocked activations
         out_cb = torch.full((n, Cout // 4, OD * OH * OW, 4), float("nan"), device=dev)
         ops.conv_layer_tc(G, ops.to_blocked(xin), ops.conv_tc_weights(Wt.to(dev)), bf.to(dev), out_cb, n, Cin, Cout, D, H, W_,
                           kd, kh, kw, relu)
         out = ops.from_blocked(out_cb)
-    else:
-        ops.conv_layer(G, xin, Wt.to(dev), bf.to(dev), out, n, Cin, Cout, D, H, W_, kd, kh, kw, relu)
     got = out.cpu().numpy().reshape(ref.shape)
     err = np.abs(got - ref.numpy()).max() / np.abs(ref.numpy()).max()
-    assert err < 2e-5, f"{impl} {geom} Cin={Cin} Cout={Cout}: rel err {err}"     # fp32-grade (3xTF32 / FFMA) vs torch fp32
+    assert err < 2e-5, f"{impl} {geom} Cin={Cin} Cout={Cout}: rel err {err}"     # fp32-grade (fp16 / 3xTF32 split) vs torch fp32
 
 
 def test_conv_sd_dynamic_tiles_same_bits(dev):
@@ -892,61 +882,6 @@ def test_conv_sd_fp16_range_flag_and_fallback(dev):
     big = torch.full((9, Cin, Cout), 500.0, device=dev)
     ops.conv_layer_sd(ops.GEOM_CYL2D, ops.to_blocked(x), ops.conv_sd_weights(big), torch.zeros(Cout, device=dev), ops.conv_sd_buffer(n, Cout, dev), n, Cin, Cout, True, flag)
     assert int(flag.item()) == 1
-
-
-def test_cost_volume_first_layer_tc_vs_ffma(dev, oracle, c1):
-    """COSTVOL geometry (on-the-fly cost volume + match gather): tensor-core kernel against the CUDA-core kernel."""
-    from bufferx_b200 import ops
-    sc = c1["res"][5]["scales"][0]
-    model = c1["model"].to(dev)
-    L = model.Pose.conv.folded()[0]
-    es, et = cu(sc["src"]["equi"].numpy(), dev), cu(sc["tgt"]["equi"].numpy(), dev)
-    M = len(sc["s_mids"])
-    sm, tm = cu(sc["s_mids"], dev, torch.int32), cu(sc["t_mids"], dev, torch.int32)
-    dM = torch.tensor([M - 3], dtype=torch.int32, device=dev)
-    a = torch.zeros((M, 32, 972), device=dev)
-    b = torch.zeros((M, 8, 972, 4), device=dev)                       # tensor-core kernel writes channel-blocked
-    ops.conv_layer(ops.GEOM_COSTVOL, None, L["w"], L["b"], a, M, 32, 32, 20, 5, 20, 3, 3, 3, True, d_n=dM, equi_s=es, equi_t=et, s_mids=sm, t_mids=tm)
-    ops.conv_layer_tc(ops.GEOM_COSTVOL, None, L["w_tc"], L["b"], b, M, 32, 32, 20, 5, 20, 3, 3, 3, True, d_n=dM, equi_s=es, equi_t=et, s_mids=sm, t_mids=tm)
-    assert (b[M - 3:] == 0).all()                                     # rows beyond the device-side count are untouched
-    assert relerr(ops.from_blocked(b).cpu().numpy(), a.cpu().numpy()) < 2e-5
-    model.cpu()
-
-
-def test_cost_volume_factorised_first_layer(dev, oracle, c1):
-    """bx_costvol_ab + GEOM_COSTAB (first CostNet layer as two small convolutions, second layer regenerating
-    relu(A - B) in its loader) against the direct COSTVOL -> VALID3D chain of the CUDA-core kernel."""
-    from bufferx_b200 import ops
-    sc = c1["res"][5]["scales"][0]
-    model = c1["model"].to(dev)
-    L0, L1 = model.Pose.conv.folded()[0], model.Pose.conv.folded()[1]
-    es, et = cu(sc["src"]["equi"].numpy(), dev), cu(sc["tgt"]["equi"].numpy(), dev)
-    M = len(sc["s_mids"])
-    sm, tm = cu(sc["s_mids"], dev, torch.int32), cu(sc["t_mids"], dev, torch.int32)
-    dM = torch.tensor([M - 2], dtype=torch.int32, device=dev)
-    a0 = torch.zeros((M, 32, 972), device=dev)
-    ops.conv_layer(ops.GEOM_COSTVOL, None, L0["w"], L0["b"], a0, M, 32, 32, 20, 5, 20, 3, 3, 3, True, d_n=dM, equi_s=es, equi_t=et, s_mids=sm, t_mids=tm)
-    a1 = torch.zeros((M, 64, 256), device=dev)
-    ops.conv_layer(ops.GEOM_VALID3D, a0, L1["w"], L1["b"], a1, M, 32, 64, 18, 3, 18, 3, 3, 3, True, d_n=dM)
-    wa, wb = ops.costvol_factor_weights(L0["w"])
-    Ab = torch.zeros((M, 8, 60, 4), device=dev)                      # channel-blocked factors
-    Bb = torch.zeros((M, 8, 54, 4), device=dev)
-    ops.costvol_ab(es, et, sm, tm, dM, M, wa, wb, L0["b"], Ab, Bb)
-    assert (Ab[M - 2:] == 0).all() and (Bb[M - 2:] == 0).all()      # rows beyond the device-side count are untouched
-    A, B = ops.from_blocked(Ab).view(M, 32, 3, 20), ops.from_blocked(Bb).view(M, 32, 3, 18)
-    # rebuild the first activation from the factors on the host: out0[n,k,l] = relu(A[k,(l-n) mod 20] - B[k,l])
-    n = torch.arange(18, device=dev).view(18, 1, 1)
-    l = torch.arange(18, device=dev).view(1, 1, 18)
-    sh = ((l - n) % 20).expand(18, 3, 18)
-    kk = torch.arange(3, device=dev).view(1, 3, 1).expand(18, 3, 18)
-    re0 = torch.relu(A[:, :, kk, sh] - B[:, :, kk, l.expand(18, 3, 18)]).reshape(M, 32, 972)
-    ref0 = a0.cpu().numpy()[: M - 2]
-    assert np.abs(re0.cpu().numpy()[: M - 2] - ref0).max() < 2e-5 * max(1.0, np.abs(ref0).max())
-    b1 = torch.zeros((M, 16, 256, 4), device=dev)                     # channel-blocked
-    ops.conv_layer_tc(ops.GEOM_COSTAB, None, L1["w_tc"], L1["b"], b1, M, 32, 64, 18, 3, 18, 3, 3, 3, True, d_n=dM, equi_s=Ab, equi_t=Bb)
-    assert (b1[M - 2:] == 0).all()
-    assert relerr(ops.from_blocked(b1).cpu().numpy(), a1.cpu().numpy()) < 2e-5
-    model.cpu()
 
 
 # ------------------------------------------------------------------------------ graphs / async pairs

@@ -1,5 +1,6 @@
-"""GPU experiment: per-descriptor relative error of the CUDA path against the CPU oracle for both conv kernels.
-    BX_CONV=tc|ffma python tests/tools/desc_error.py C3"""
+"""GPU experiment: per-descriptor relative error of the CUDA path against the CPU oracle, on the default conv kernel or,
+with BX_CONV=tc, on the TF32 one.
+    BX_CONV=tc python tests/tools/desc_error.py C3"""
 import os, sys
 import numpy as np, torch
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.dirname(os.path.abspath(__file__)))))

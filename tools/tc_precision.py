@@ -11,7 +11,7 @@ lib = ops.load_library()
 g = torch.Generator().manual_seed(0)
 
 
-def run(K, Cout, n, S, seg, relu_like=True, impl="tc"):
+def run(K, Cout, n, S, seg, relu_like=True):
     x = torch.randn((n, K, S), generator=g)
     if relu_like:
         x = x.abs()
@@ -19,24 +19,20 @@ def run(K, Cout, n, S, seg, relu_like=True, impl="tc"):
     b = torch.zeros(Cout)
     ref = torch.einsum("ok,nks->nos", W.double(), x.double())
     Wt = W.t().contiguous()[None]                      # [T=1, Cin, Cout]
-    out = torch.empty((n, Cout, S), device=dev)
-    if impl == "tc":                                   # tensor-core kernel: channel-blocked activations
-        lib.bx_conv_tc_set_segment_stages(seg)
-        out_cb = torch.empty((n, Cout // 4, S, 4), device=dev)
-        ops.conv_layer_tc(ops.GEOM_VALID3D, ops.to_blocked(x.to(dev)), ops.conv_tc_weights(Wt.to(dev)), b.to(dev), out_cb, n, K, Cout,
-                          1, 1, S, 1, 1, 1, False)
-        out = ops.from_blocked(out_cb)
-    else:
-        ops.conv_layer(ops.GEOM_VALID3D, x.to(dev), Wt.to(dev), b.to(dev), out, n, K, Cout, 1, 1, S, 1, 1, 1, False)
+    lib.bx_conv_tc_set_segment_stages(seg)
+    out_cb = torch.empty((n, Cout // 4, S, 4), device=dev)             # the tensor-core kernel takes channel-blocked activations
+    ops.conv_layer_tc(ops.GEOM_VALID3D, ops.to_blocked(x.to(dev)), ops.conv_tc_weights(Wt.to(dev)), b.to(dev), out_cb, n, K, Cout,
+                      1, 1, S, 1, 1, 1, False)
+    out = ops.from_blocked(out_cb)
     err = (out.cpu().double() - ref)
     scale = ref.abs().mean()
     return float(err.abs().max() / scale), float(err.abs().mean() / scale), float(err.mean() / scale), float(ref.mean() / scale)
 
 
-print("impl K Cout seg  max/mean|ref|  mean|err|/mean|ref|  mean(err)/mean|ref| (bias)   mean(ref)")
+print("K Cout seg  max/mean|ref|  mean|err|/mean|ref|  mean(err)/mean|ref| (bias)   mean(ref)")
 for K in (128, 576, 1152):
     for Cout in (64, 128):
-        for impl, seg in (("ffma", 0), ("tc", 100000), ("tc", 24), ("tc", 6), ("tc", 2)):
+        for seg in (100000, 24, 6, 2):
             for relu_like in (True, False):
-                r = run(K, Cout, 64, 140, seg, relu_like, impl)
-                print(f"{impl:5s} K={K:5d} N={Cout:4d} seg={seg:6d} relu={int(relu_like)}  max={r[0]:.3e} mean={r[1]:.3e} bias={r[2]:+.3e} ref={r[3]:+.2f}")
+                r = run(K, Cout, 64, 140, seg, relu_like)
+                print(f"K={K:5d} N={Cout:4d} seg={seg:6d} relu={int(relu_like)}  max={r[0]:.3e} mean={r[1]:.3e} bias={r[2]:+.3e} ref={r[3]:+.2f}")
