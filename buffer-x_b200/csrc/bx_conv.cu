@@ -18,8 +18,9 @@ constexpr int POOL_T = 160;
 __global__ void __launch_bounds__(POOL_T)
 pool_desc_kernel(const float *__restrict__ x, int K, int C, int S, int channels_last, const float *__restrict__ w1,
                  const float *__restrict__ b1, const float *__restrict__ w2, const float *__restrict__ b2,
-                 float *__restrict__ desc, float *__restrict__ equi) {
+                 float *__restrict__ desc, float *__restrict__ equi, const int *__restrict__ d_K) {
     __shared__ float sw1[32 * 16], sb1[16], sw2[16], sb2;
+    if (d_K && (int)blockIdx.x >= *d_K) return;            // beyond the device-side count: the whole CTA, before any barrier
     __shared__ float xw[32][POOL_T + 1];
     __shared__ float fsum[32];
     const int k = blockIdx.x, tid = threadIdx.x;
@@ -192,11 +193,16 @@ costvol_ab_kernel(const float *__restrict__ equi_s, const float *__restrict__ eq
 
 BX_API int bx_pool_desc(const float *x, int K, int C, int S, int channels_last, const float *w1, const float *b1,
                         const float *w2, const float *b2, float *desc, float *equi, void *stream) {
+    return bx_pool_desc_n(x, K, C, S, channels_last, w1, b1, w2, b2, desc, equi, nullptr, stream);
+}
+
+BX_API int bx_pool_desc_n(const float *x, int K, int C, int S, int channels_last, const float *w1, const float *b1,
+                          const float *w2, const float *b2, float *desc, float *equi, const int32_t *d_K, void *stream) {
     BX_REQUIRE(x && w1 && b1 && w2 && b2 && desc && equi, "bx_pool_desc: null pointer");
     BX_REQUIRE(C == 32 && S >= 1 && S <= POOL_T && K >= 0, "bx_pool_desc: expects C=32, S<=%d", POOL_T);
     if (K == 0) return BX_OK;
     BX_REQUIRE(!channels_last || (reinterpret_cast<uintptr_t>(x) & 15) == 0, "bx_pool_desc: x must be 16-byte aligned");
-    pool_desc_kernel<<<K, POOL_T, 0, bx_stream(stream)>>>(x, K, C, S, channels_last ? 1 : 0, w1, b1, w2, b2, desc, equi);
+    pool_desc_kernel<<<K, POOL_T, 0, bx_stream(stream)>>>(x, K, C, S, channels_last ? 1 : 0, w1, b1, w2, b2, desc, equi, d_K);
     BX_LAUNCH_CHECK();
     return BX_OK;
 }

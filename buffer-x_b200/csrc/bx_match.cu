@@ -19,6 +19,9 @@ constexpr int NN_TI = 64;   // rows of a per CTA
 constexpr int NN_TJ = 64;   // cols of b per CTA
 constexpr int NN_C = 32;    // descriptor length (fixed by the network)
 
+// rows present this launch: min(*d_n, n), or n without a device count
+__device__ __forceinline__ int nn_count(const int *d_n, int n) { return d_n ? min(max(*d_n, 0), n) : n; }
+
 __global__ void nn_init_kernel(unsigned long long *keys, int n) {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i < n) keys[i] = ~0ull;
@@ -27,11 +30,15 @@ __global__ void nn_init_kernel(unsigned long long *keys, int n) {
 // grid (ceil(Ka/64), ceil(Kb/64)), 256 threads: thread (ti = tid/4 .. handles 1 row, 16 cols)
 __global__ void __launch_bounds__(256)
 nn_tile_kernel(const float *__restrict__ a, int Ka, const float *__restrict__ b, int Kb,
-               unsigned long long *__restrict__ row_keys, unsigned long long *__restrict__ col_keys) {
+               unsigned long long *__restrict__ row_keys, unsigned long long *__restrict__ col_keys, const int *__restrict__ d_Ka,
+               const int *__restrict__ d_Kb) {
     __shared__ float sa[NN_TI][NN_C + 1];
     __shared__ float sb[NN_TJ][NN_C + 1];
     __shared__ unsigned long long scol[NN_TJ];
     const int i0 = blockIdx.x * NN_TI, j0 = blockIdx.y * NN_TJ;
+    Ka = nn_count(d_Ka, Ka);
+    Kb = nn_count(d_Kb, Kb);
+    if (i0 >= Ka || j0 >= Kb) return;             // the whole CTA: before any barrier
     const int tid = threadIdx.x;
     for (int e = tid; e < NN_TI * NN_C; e += 256) {
         const int r = e / NN_C, c = e % NN_C;
@@ -74,8 +81,14 @@ nn_tile_kernel(const float *__restrict__ a, int Ka, const float *__restrict__ b,
 __global__ void __launch_bounds__(1024)
 nn_select_kernel(const unsigned long long *__restrict__ row_keys, const unsigned long long *__restrict__ col_keys,
                  int Ka, int Kb, int *__restrict__ s_mids, int *__restrict__ t_mids, int *__restrict__ d_M,
-                 int *__restrict__ snn, int *__restrict__ tnn) {
+                 int *__restrict__ snn, int *__restrict__ tnn, const int *__restrict__ d_Ka, const int *__restrict__ d_Kb) {
     __shared__ int sh[33];
+    Ka = nn_count(d_Ka, Ka);
+    Kb = nn_count(d_Kb, Kb);
+    if (Ka == 0 || Kb == 0) {                     // a side without key-points: no match, nothing else written
+        if (threadIdx.x == 0) *d_M = 0;
+        return;
+    }
     int run = 0;
     for (int base = 0; base < Ka; base += 1024) {
         const int i = base + threadIdx.x;
@@ -271,6 +284,12 @@ consensus_select_kernel(const float *__restrict__ ss, const float *__restrict__ 
 
 BX_API int bx_mutual_nn(const float *a, int Ka, const float *b, int Kb, int C, unsigned long long *keys, int32_t *s_mids,
                         int32_t *t_mids, int32_t *d_M, int32_t *snn, int32_t *tnn, void *stream) {
+    return bx_mutual_nn_n(a, Ka, b, Kb, C, nullptr, nullptr, keys, s_mids, t_mids, d_M, snn, tnn, stream);
+}
+
+BX_API int bx_mutual_nn_n(const float *a, int Ka, const float *b, int Kb, int C, const int32_t *d_Ka, const int32_t *d_Kb,
+                          unsigned long long *keys, int32_t *s_mids, int32_t *t_mids, int32_t *d_M, int32_t *snn, int32_t *tnn,
+                          void *stream) {
     BX_REQUIRE(a && b && keys && s_mids && t_mids && d_M, "bx_mutual_nn: null pointer");
     BX_REQUIRE(C == NN_C, "bx_mutual_nn: descriptor length must be %d", NN_C);
     BX_REQUIRE(Ka >= 0 && Kb >= 0, "bx_mutual_nn: negative size");
@@ -282,9 +301,9 @@ BX_API int bx_mutual_nn(const float *a, int Ka, const float *b, int Kb, int C, u
     nn_init_kernel<<<(Ka + Kb + 255) / 256, 256, 0, st>>>(keys, Ka + Kb);
     BX_LAUNCH_CHECK();
     dim3 grid((Ka + NN_TI - 1) / NN_TI, (Kb + NN_TJ - 1) / NN_TJ);
-    nn_tile_kernel<<<grid, 256, 0, st>>>(a, Ka, b, Kb, keys, keys + Ka);
+    nn_tile_kernel<<<grid, 256, 0, st>>>(a, Ka, b, Kb, keys, keys + Ka, d_Ka, d_Kb);
     BX_LAUNCH_CHECK();
-    nn_select_kernel<<<1, 1024, 0, st>>>(keys, keys + Ka, Ka, Kb, s_mids, t_mids, d_M, snn, tnn);
+    nn_select_kernel<<<1, 1024, 0, st>>>(keys, keys + Ka, Ka, Kb, s_mids, t_mids, d_M, snn, tnn, d_Ka, d_Kb);
     BX_LAUNCH_CHECK();
     return BX_OK;
 }

@@ -153,16 +153,22 @@ struct SpJobs {
     const float4 *pts4[SP_MAXJOBS];
     const float *kpts[SP_MAXJOBS];
     const float *d_radius[SP_MAXJOBS];
+    const int *d_K[SP_MAXJOBS];           // optional device key-point count of a job (NULL: K)
     int N[SP_MAXJOBS], K[SP_MAXJOBS], boff[SP_MAXJOBS + 1], koff[SP_MAXJOBS];
     int njobs;
 };
+
+// key-points of a job present this launch: min(*d_K, K), or K without a device count
+__device__ __forceinline__ int sp_count(const int *d_K, int K) { return d_K ? min(max(*d_K, 0), K) : K; }
 
 __global__ void __launch_bounds__(SP_WARPS * 32)
 select_patches_batched_kernel(const SpJobs jobs, int P, float *__restrict__ patches) {
     int j = 0;
     while (j + 1 < jobs.njobs && (int)blockIdx.x >= jobs.boff[j + 1]) ++j;
-    select_patches_body(jobs.pts4[j], jobs.N[j], jobs.kpts[j], jobs.K[j], 0.0f, jobs.d_radius[j], P, nullptr,
-                        patches + (size_t)jobs.koff[j] * P * 3, (int)blockIdx.x - jobs.boff[j]);
+    const int b = (int)blockIdx.x - jobs.boff[j], Kj = sp_count(jobs.d_K[j], jobs.K[j]);
+    if (b * SP_KP >= Kj) return;                          // the whole CTA: before any barrier
+    select_patches_body(jobs.pts4[j], jobs.N[j], jobs.kpts[j], Kj, 0.0f, jobs.d_radius[j], P, nullptr,
+                        patches + (size_t)jobs.koff[j] * P * 3, b);
 }
 
 // ---- hash-grid form of select_patches (large clouds: N >= ~50 k points) --------------------------------------------------
@@ -313,14 +319,17 @@ struct HgJobs {
     const float *d_radius[SP_MAXJOBS];
     float4 *sorted[SP_MAXJOBS];
     int *cnt[SP_MAXJOBS];                 // cnt, start = cnt + HG_CELLS, cursor = start + HG_CELLS + 4
+    const int *d_K[SP_MAXJOBS];           // optional device key-point count of a job: 0 skips every phase of the job
     int N[SP_MAXJOBS], koff[SP_MAXJOBS + 1];
     int njobs;
 };
 __global__ void hg_count_batched_kernel(const HgJobs J) {
     const int j = blockIdx.y;
+    if (J.d_K[j] && *J.d_K[j] <= 0) return;
     hg_count_body(J.pts4[j], J.N[j], J.d_radius[j], J.cnt[j], blockIdx.x * blockDim.x + threadIdx.x);
 }
 __global__ void __launch_bounds__(1024) hg_scan_batched_kernel(const HgJobs J) {
+    if (J.d_K[blockIdx.x] && *J.d_K[blockIdx.x] <= 0) return;
     int *cnt = J.cnt[blockIdx.x];
     hg_scan_body(cnt, cnt + HG_CELLS, cnt + 2 * HG_CELLS + 4);
 }
@@ -330,6 +339,7 @@ __global__ void __launch_bounds__(1024) hg_scan_batched_kernel(const HgJobs J) {
 constexpr int HG_CHUNK = 4096, HG_CHUNKS = HG_CELLS / HG_CHUNK, HG_SCAN_THREADS = 256;
 __global__ void __launch_bounds__(HG_SCAN_THREADS) hg_chunksum_batched_kernel(const HgJobs J) {
     __shared__ int sh[33];
+    if (J.d_K[blockIdx.y] && *J.d_K[blockIdx.y] <= 0) return;
     const int *cnt = J.cnt[blockIdx.y] + (size_t)blockIdx.x * HG_CHUNK;
     const int4 *c4 = reinterpret_cast<const int4 *>(cnt) + threadIdx.x * (HG_CHUNK / HG_SCAN_THREADS / 4);
     int local = 0;
@@ -341,6 +351,7 @@ __global__ void __launch_bounds__(HG_SCAN_THREADS) hg_chunksum_batched_kernel(co
 }
 __global__ void __launch_bounds__(HG_SCAN_THREADS) hg_chunkscan_batched_kernel(const HgJobs J) {
     __shared__ int sh[33];
+    if (J.d_K[blockIdx.y] && *J.d_K[blockIdx.y] <= 0) return;
     int *base = J.cnt[blockIdx.y];
     const int chunk = blockIdx.x;
     // sum of the totals of the chunks before this one (HG_CHUNKS = 32: one warp-wide sum, computed by every warp)
@@ -370,13 +381,16 @@ __global__ void __launch_bounds__(HG_SCAN_THREADS) hg_chunkscan_batched_kernel(c
 }
 __global__ void hg_scatter_batched_kernel(const HgJobs J) {
     const int j = blockIdx.y;
+    if (J.d_K[j] && *J.d_K[j] <= 0) return;
     hg_scatter_body(J.pts4[j], J.N[j], J.d_radius[j], J.cnt[j] + 2 * HG_CELLS + 4, J.sorted[j], blockIdx.x * blockDim.x + threadIdx.x);
 }
 __global__ void __launch_bounds__(HG_THREADS) hg_query_batched_kernel(const HgJobs J, int P, float *__restrict__ patches) {
     int j = 0;
     while (j + 1 < J.njobs && (int)blockIdx.x >= J.koff[j + 1]) ++j;
+    const int k = (int)blockIdx.x - J.koff[j];
+    if (J.d_K[j] && k >= *J.d_K[j]) return;               // the whole CTA: before any barrier
     hg_query_body(J.pts4[j], J.N[j], J.kpts[j], J.d_radius[j], P, J.cnt[j] + HG_CELLS, J.sorted[j], nullptr,
-                  patches + (size_t)J.koff[j] * P * 3, (int)blockIdx.x - J.koff[j]);
+                  patches + (size_t)J.koff[j] * P * 3, k);
 }
 
 // plain ordered ball query over a packed [n,3] cloud (pointnet2_ops.ball_query semantics)
@@ -442,11 +456,12 @@ constexpr int LRF_WARPS = 4;
 
 __global__ void __launch_bounds__(LRF_WARPS * 32)
 lrf_kernel(const float *__restrict__ patches, int K, int P, float des_r_v, const float *__restrict__ d_des_r, int flags,
-           float *__restrict__ delta, float *__restrict__ Rt, float *__restrict__ rand_axis, int r_group) {
+           float *__restrict__ delta, float *__restrict__ Rt, float *__restrict__ rand_axis, int r_group, const int *__restrict__ d_K) {
     const int aligned = flags & 1, stable = flags & 2;
     const int lane = threadIdx.x & 31;
     const int k = blockIdx.x * LRF_WARPS + (threadIdx.x >> 5);
     if (k >= K) return;
+    if (d_K && (r_group > 0 ? k % r_group >= d_K[k / r_group] : k >= *d_K)) return;     // beyond the group's device count
     const float des_r = d_des_r ? d_des_r[r_group > 0 ? k / r_group : 0] : des_r_v;     // batched call: one radius per r_group patches
     const float *pt = patches + (size_t)k * P * 3;
     float *dl = delta + (size_t)k * P * 3;
@@ -562,6 +577,11 @@ BX_API int bx_select_patches(const float *pts4, int N, const float *kpts, int K,
 
 BX_API int bx_select_patches_batched(int njobs, const void *const *pts4, const int32_t *N, const void *const *kpts, const int32_t *K,
                                      const void *const *d_radius, int P, float *patches, void *stream) {
+    return bx_select_patches_batched_n(njobs, pts4, N, kpts, K, d_radius, nullptr, P, patches, stream);
+}
+
+BX_API int bx_select_patches_batched_n(int njobs, const void *const *pts4, const int32_t *N, const void *const *kpts, const int32_t *K,
+                                       const void *const *d_radius, const void *const *d_K, int P, float *patches, void *stream) {
     BX_REQUIRE(pts4 && N && kpts && K && d_radius && patches, "bx_select_patches_batched: null pointer");
     BX_REQUIRE(njobs >= 1 && njobs <= SP_MAXJOBS && P >= 1, "bx_select_patches_batched: njobs=%d out of range [1,%d]", njobs, SP_MAXJOBS);
     SpJobs jobs = {};
@@ -573,6 +593,7 @@ BX_API int bx_select_patches_batched(int njobs, const void *const *pts4, const i
         jobs.pts4[j] = reinterpret_cast<const float4 *>(pts4[j]);
         jobs.kpts[j] = reinterpret_cast<const float *>(kpts[j]);
         jobs.d_radius[j] = reinterpret_cast<const float *>(d_radius[j]);
+        jobs.d_K[j] = d_K ? reinterpret_cast<const int *>(d_K[j]) : nullptr;
         jobs.N[j] = N[j]; jobs.K[j] = K[j];
         jobs.boff[j] = blocks; jobs.koff[j] = koff;
         blocks += (K[j] + SP_KP - 1) / SP_KP;
@@ -623,6 +644,12 @@ BX_API int bx_select_patches_grid(const float *pts4, int N, const float *kpts, i
 // bx_select_patches_grid_workspace_bytes(N[j]) bytes (16-byte aligned); patches: job after job like bx_select_patches_batched.
 BX_API int bx_select_patches_grid_batched(int njobs, const void *const *pts4, const int32_t *N, const void *const *kpts, const int32_t *K,
                                           const void *const *d_radius, int P, float *patches, void *workspace, void *stream) {
+    return bx_select_patches_grid_batched_n(njobs, pts4, N, kpts, K, d_radius, nullptr, P, patches, workspace, stream);
+}
+
+BX_API int bx_select_patches_grid_batched_n(int njobs, const void *const *pts4, const int32_t *N, const void *const *kpts, const int32_t *K,
+                                            const void *const *d_radius, const void *const *d_K, int P, float *patches, void *workspace,
+                                            void *stream) {
     BX_REQUIRE(pts4 && N && kpts && K && d_radius && patches && workspace, "bx_select_patches_grid_batched: null pointer");
     BX_REQUIRE(njobs >= 1 && njobs <= SP_MAXJOBS && P >= 1, "bx_select_patches_grid_batched: njobs=%d out of range [1,%d]", njobs, SP_MAXJOBS);
     BX_REQUIRE((reinterpret_cast<uintptr_t>(workspace) & 15) == 0, "bx_select_patches_grid_batched: workspace must be 16-byte aligned");
@@ -636,6 +663,7 @@ BX_API int bx_select_patches_grid_batched(int njobs, const void *const *pts4, co
         J.pts4[j] = reinterpret_cast<const float4 *>(pts4[j]);
         J.kpts[j] = reinterpret_cast<const float *>(kpts[j]);
         J.d_radius[j] = reinterpret_cast<const float *>(d_radius[j]);
+        J.d_K[j] = d_K ? reinterpret_cast<const int *>(d_K[j]) : nullptr;
         J.N[j] = N[j];
         J.sorted[j] = reinterpret_cast<float4 *>(ws);
         J.cnt[j] = reinterpret_cast<int *>(J.sorted[j] + N[j]);
@@ -685,11 +713,16 @@ BX_API int bx_lrf(const float *patches, int K, int P, float des_r, const float *
 
 BX_API int bx_lrf_batched(const float *patches, int K, int P, float des_r, const float *d_des_r, int r_group, int flags, float *delta,
                           float *Rt, float *rand_axis, void *stream) {
+    return bx_lrf_batched_n(patches, K, P, des_r, d_des_r, r_group, nullptr, flags, delta, Rt, rand_axis, stream);
+}
+
+BX_API int bx_lrf_batched_n(const float *patches, int K, int P, float des_r, const float *d_des_r, int r_group, const int32_t *d_K, int flags,
+                            float *delta, float *Rt, float *rand_axis, void *stream) {
     BX_REQUIRE(K >= 0 && P >= 1 && r_group >= 0, "bx_lrf: bad sizes");
     if (K == 0) return BX_OK;                 // an empty batch: torch hands empty tensors over as null pointers
     BX_REQUIRE(patches && delta && Rt && rand_axis, "bx_lrf: null pointer");
     lrf_kernel<<<(K + LRF_WARPS - 1) / LRF_WARPS, LRF_WARPS * 32, 0, bx_stream(stream)>>>(patches, K, P, des_r, d_des_r,
-                                                                                           flags, delta, Rt, rand_axis, r_group);
+                                                                                           flags, delta, Rt, rand_axis, r_group, d_K);
     BX_LAUNCH_CHECK();
     return BX_OK;
 }

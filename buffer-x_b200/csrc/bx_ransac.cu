@@ -432,7 +432,31 @@ refine_kernel(const float *__restrict__ ss, const float *__restrict__ tt, const 
     if (tid == 0 && d_rounds) *d_rounds = r;
 }
 
+// early-exit decision of the multi-scale pair (PoseEstimator.compute_confidence_score): the scale-0 RANSAC result decides on
+// the device whether the later scales run, so the pair is enqueued (and captured) without a host read
+constexpr int GATE_MAXN = 32;
+struct GateCaps { int cap[GATE_MAXN]; };
+__global__ void early_exit_gate_kernel(const RansacResult *__restrict__ res, int min_inliers, int n, GateCaps caps,
+                                       int *__restrict__ counts, int num_scales, double *__restrict__ scales_used) {
+    const bool stop = res->num_inliers >= min_inliers;
+    const int i = threadIdx.x;
+    if (i < n) counts[i] = stop ? 0 : caps.cap[i];
+    if (i == 0 && scales_used) *scales_used = stop ? 1.0 : (double)num_scales;
+}
+
 }  // namespace
+
+BX_API int bx_early_exit_gate(const void *result, int min_inliers, int n, const int32_t *h_caps, int32_t *d_counts, int num_scales,
+                              double *d_scales_used, void *stream) {
+    BX_REQUIRE(result && (n == 0 || (h_caps && d_counts)), "bx_early_exit_gate: null pointer");
+    BX_REQUIRE(n >= 0 && n <= GATE_MAXN && num_scales >= 1, "bx_early_exit_gate: 0 <= n <= %d counts, num_scales >= 1", GATE_MAXN);
+    GateCaps caps = {};
+    for (int i = 0; i < n; ++i) caps.cap[i] = h_caps[i];
+    early_exit_gate_kernel<<<1, 32, 0, bx_stream(stream)>>>(static_cast<const RansacResult *>(result), min_inliers, n, caps, d_counts,
+                                                           num_scales, d_scales_used);
+    BX_LAUNCH_CHECK();
+    return BX_OK;
+}
 
 BX_API int64_t bx_ransac_workspace_bytes(int max_iter) {
     (void)max_iter;

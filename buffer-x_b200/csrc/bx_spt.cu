@@ -41,8 +41,11 @@ __global__ void __launch_bounds__(SPT_THREADS)
 spt_pnt_kernel(const float *__restrict__ delta, int K, int P, const float *__restrict__ voxels, int V, int azi_n,
                const float *__restrict__ rot, float voxel_r, int nv, const float *__restrict__ w,
                const float *__restrict__ b, float *__restrict__ feat, int *__restrict__ dbg_vidx,
-               float *__restrict__ dbg_inv, long long sd_rows, int *__restrict__ sd_flag) {
+               float *__restrict__ dbg_inv, long long sd_rows, int *__restrict__ sd_flag, const int *__restrict__ d_K) {
     extern __shared__ float smem[];
+    // optional device-side count: patches at or beyond it are not touched (the whole CTA leaves before any barrier)
+    const int Kn = d_K ? min(max(*d_K, 0), K) : K;
+    if ((int)blockIdx.x >= Kn) return;
     const int NW = (P + 31) >> 5;
     float *px = smem;                                   // P
     float *py = px + P;                                 // P
@@ -275,7 +278,7 @@ spt_pnt_kernel(const float *__restrict__ delta, int K, int P, const float *__res
         for (int t = tid; t < 12 * 22; t += SPT_THREADS) {
             const int im = t / 22, xp = t - im * 22;
             img[(size_t)im * sd_rows + (size_t)k * 176 + xp] = z4;
-            if (k == K - 1) img[(size_t)im * sd_rows + (size_t)K * 176 + xp] = z4;
+            if (k == Kn - 1) img[(size_t)im * sd_rows + (size_t)Kn * 176 + xp] = z4;
         }
         if (!(omax < 65000.0f) && sd_flag) atomicOr(sd_flag, 1);
         return;
@@ -337,7 +340,7 @@ BX_API int bx_spt_pnt(const float *delta, int K, int P, const float *voxels, int
     if (bx_needs_attr(attr, smem))
         BX_CUDA(cudaFuncSetAttribute(spt_pnt_kernel<0>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     spt_pnt_kernel<0><<<K, SPT_THREADS, smem, bx_stream(stream)>>>(delta, K, P, voxels, V, azi_n, rot, voxel_r, nv, w, b,
-                                                                feat, dbg_vidx, dbg_inv, 0, nullptr);
+                                                                feat, dbg_vidx, dbg_inv, 0, nullptr, nullptr);
     BX_LAUNCH_CHECK();
     return BX_OK;
 }
@@ -345,6 +348,12 @@ BX_API int bx_spt_pnt(const float *delta, int K, int P, const float *voxels, int
 BX_API int bx_spt_pnt_sd(const float *delta, int K, int P, const float *voxels, int V, int azi_n, const float *rot,
                          float voxel_r, int nv, const float *w, const float *b, void *feat_sd, long long rows, int32_t *d_flag,
                          void *stream) {
+    return bx_spt_pnt_sd_n(delta, K, P, voxels, V, azi_n, rot, voxel_r, nv, w, b, feat_sd, rows, d_flag, nullptr, stream);
+}
+
+BX_API int bx_spt_pnt_sd_n(const float *delta, int K, int P, const float *voxels, int V, int azi_n, const float *rot,
+                           float voxel_r, int nv, const float *w, const float *b, void *feat_sd, long long rows, int32_t *d_flag,
+                           const int32_t *d_K, void *stream) {
     BX_REQUIRE(delta && voxels && rot && w && b && feat_sd, "bx_spt_pnt_sd: null pointer");
     BX_REQUIRE(K >= 0 && P >= 1 && P <= 65535 && nv >= 1 && nv <= MAX_NV, "bx_spt_pnt_sd: bad sizes");
     BX_REQUIRE(V == 420 && azi_n == 20, "bx_spt_pnt_sd: the presplit raster is 3 radial x 7 elevation x 20 azimuth voxels");
@@ -356,7 +365,7 @@ BX_API int bx_spt_pnt_sd(const float *delta, int K, int P, const float *voxels, 
     if (bx_needs_attr(attr, smem))
         BX_CUDA(cudaFuncSetAttribute(spt_pnt_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     spt_pnt_kernel<1><<<K, SPT_THREADS, smem, bx_stream(stream)>>>(delta, K, P, voxels, V, azi_n, rot, voxel_r, nv, w, b,
-                                                                reinterpret_cast<float *>(feat_sd), nullptr, nullptr, rows, d_flag);
+                                                                reinterpret_cast<float *>(feat_sd), nullptr, nullptr, rows, d_flag, d_K);
     BX_LAUNCH_CHECK();
     return BX_OK;
 }

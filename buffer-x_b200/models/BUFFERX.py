@@ -9,13 +9,16 @@ scales_used)``.  Differences that do not change results:
     per-scale calls return the same indices and FPS(k) is a prefix of FPS(k') (SURVEY 8.1 item 8);
   * the radius histogram is built once and serves every scale's bisection, on the device;
   * data-dependent sizes stay in device counters, so the whole pair is enqueued without a host round
-    trip; the host reads one small result block at the end (early-exit mode adds one read after scale 0).
+    trip; the host reads one small result block at the end (early-exit mode in ``forward`` adds one read after scale 0;
+    ``forward_async`` decides early exit on the device).
 
 Throughput API on top of the reference surface (CUDA streams + graphs instead of a tracing compiler):
   * ``enable_cuda_graphs(True)``: the enqueue of a pair is captured once per (Ns, Nt, aligned) shape and
     replayed -- one graph launch instead of ~150 kernel launches;
   * ``forward_async(data_source) -> handle`` / ``handle.result()``: several pairs in flight on separate
     streams (FPS is a latency-bound 16-SM kernel; a second pair's convolutions fill the other SMs).
+    With ``cfg.match.enable_early_exit`` the scale-0 RANSAC result gates the later scales on the device
+    (``_enqueue_device_exit``), so early-exit pairs are captured and replayed too.
 """
 import os
 
@@ -82,7 +85,7 @@ class _Timer:
 
 
 class _PairSlot:
-    """Static buffers + (optionally) a captured CUDA graph for one (Ns, Nt, aligned) shape on its own stream."""
+    """Static buffers + (optionally) a captured CUDA graph for one (Ns, Nt, aligned, early-exit setting) on its own stream."""
 
     def __init__(self, model, Ns, Nt, aligned, use_graph):
         cfg = model.config
@@ -122,7 +125,7 @@ class _PairSlot:
 
     def _enqueue(self):
         perms = [(self.perm_s[i], self.perm_t[i]) for i in range(self.perm_s.shape[0])]
-        return self.model._enqueue(self.src, self.tgt, self.aligned, perms, None, False)[0]
+        return self.model._enqueue(self.src, self.tgt, self.aligned, perms, None, False, device_exit=True)[0]
 
     def launch(self, data_source, perms):
         """H2D of the inputs (pinned staging when they arrive as host arrays), the pair, D2H of the result."""
@@ -258,13 +261,21 @@ class BufferX(nn.Module):
         return self
 
     def _graphable(self):
+        """Whether ``forward`` may route through the slots.  Early exit stays on the host decision in ``forward``: only that
+        reproduces the reference's NumPy draw order (scales 1..S-1 draw their permutations only when the pair does not exit),
+        the drop-in contract of ``forward``.  ``forward_async`` draws all 2*S permutations at launch and decides on the device."""
         cfg = self.config
         return not cfg.match.get("enable_early_exit", True) and not cfg.test.get("enable_timing", False)
+
+    def _exit_key(self):
+        m = self.config.match
+        return (True, int(m.get("early_exit_min_inliers", 15))) if m.get("enable_early_exit", True) else (False, None)
 
     MAX_GRAPH_SHAPES = 8      # graphs are per (Ns, Nt, aligned) shape; least recently used shapes are dropped beyond this
 
     def _slot(self, Ns, Nt, aligned):
-        key = (Ns, Nt, bool(aligned))
+        # the early-exit threshold is baked into a captured gate launch: a graph is never replayed under another setting
+        key = (Ns, Nt, bool(aligned)) + self._exit_key()
         if key not in self._slots and len(self._slots) >= self.MAX_GRAPH_SHAPES:
             # datasets with a different size for every pair would otherwise pin one set of graph pools per pair; for
             # those, run eager (`enable_cuda_graphs(False)`) or pad/bucket the clouds upstream
@@ -293,17 +304,18 @@ class BufferX(nn.Module):
         return slot
 
     def forward_async(self, data_source, perms=None):
-        """Enqueue one pair on a slot stream; returns a handle whose ``result()`` is the forward tuple."""
-        if not self._graphable():
-            raise ops.BufferXError("forward_async needs early exit and timing disabled (they require host round trips)")
+        """Enqueue one pair on a slot stream; returns a handle whose ``result()`` is the forward tuple.  Without ``perms`` the
+        2*S permutations are drawn from NumPy's global RNG at launch, also when early exit stops the pair after scale 0."""
+        if self.config.test.get("enable_timing", False):
+            raise ops.BufferXError("forward_async needs timing disabled (the per-stage timers require host round trips)")
         Ns = int(np.prod(data_source["src_fds_pcd"].shape[:-1]))
         Nt = int(np.prod(data_source["tgt_fds_pcd"].shape[:-1]))
         return self._slot(Ns, Nt, bool(data_source["is_aligned_to_global_z"])).launch(data_source, perms)
 
     # ------------------------------------------------------------------------------------------------
-    def _enqueue(self, src, tgt, aligned, perms, ransac_seed, debug, timers=None):
-        """Everything of one pair on the current stream, no host synchronisation unless early exit is on.
-        Returns (tail block on the device, debug dict)."""
+    def _enqueue(self, src, tgt, aligned, perms, ransac_seed, debug, timers=None, device_exit=False):
+        """Everything of one pair on the current stream, no host synchronisation unless early exit is on and the decision is
+        the host's (``device_exit`` False: ``forward``).  Returns (tail block on the device, debug dict)."""
         cfg = self.config
         dev = src.device
         Ns, Nt = src.shape[0], tgt.shape[0]
@@ -337,6 +349,9 @@ class BufferX(nn.Module):
         tt_acc = torch.empty((maxMc, 3), dtype=torch.float32, device=dev)
         offs = torch.zeros(S + 1, dtype=torch.int32, device=dev)
         dbg = dict(scales=[]) if debug else None
+        if enable_early_exit and device_exit and not debug:
+            tail = self._enqueue_device_exit(src, tgt, aligned, perms, ransac_seed, src_kpts, tgt_kpts, r_dev, R_acc, t_acc, ss_acc, tt_acc, offs)
+            return tail, None
 
         scales_used = 0
         should_exit = False
@@ -435,6 +450,72 @@ class BufferX(nn.Module):
         if debug:
             dbg.update(fps_idx=fidx, kpts=fk, des_r=r_dev, des_m=m_dev, ss=ss_acc, tt=tt_acc, R=R_acc, t=t_acc)
         return tail, dbg
+
+    def _enqueue_device_exit(self, src, tgt, aligned, perms, ransac_seed, src_kpts, tgt_kpts, r_dev, R_acc, t_acc, ss_acc, tt_acc, offs):
+        """Early exit decided on the device (forward_async / graphs): scale 0 on the batched route up to its RANSAC,
+        bx_early_exit_gate turns the result into the key-point counts of scales 1..S-1 (K to continue, 0 to exit), and those
+        scales' descriptors, matches, CostNet rows and hypotheses are sized by the counts and appended behind scale 0's.  On
+        exit offs[S] == offs[1], so the final consensus and RANSAC see exactly scale 0's inputs with the same seed and
+        reproduce its result; they are kept rather than skipped so that one captured graph serves both outcomes."""
+        cfg = self.config
+        dev = src.device
+        K, S, azi_n = cfg.patch.num_fps, cfg.patch.num_scales, cfg.patch.azi_n
+        G = S - 1
+        jobs = []
+        for i in range(S):
+            for pts_c, k_c, j in ((src, src_kpts, 0), (tgt, tgt_kpts, 1)):
+                pm = None if perms is None else perms[i][j]
+                if pm is None:
+                    pm = np.random.choice(pts_c.shape[0], pts_c.shape[0], replace=False)
+                if not isinstance(pm, torch.Tensor):
+                    pm = torch.from_numpy(np.ascontiguousarray(pm, dtype=np.int32))
+                if not pm.is_cuda or pm.dtype != torch.int32:
+                    pm = pm.to(dev, dtype=torch.int32, non_blocking=True)
+                jobs.append((pts_c, k_c, r_dev[i:i + 1], pm))
+        s_lists = torch.empty((S, K), dtype=torch.int32, device=dev)
+        t_lists = torch.empty((S, K), dtype=torch.int32, device=dev)
+        cnts = torch.zeros(S, dtype=torch.int32, device=dev)
+        # ---- scale 0: descriptors, matches, CostNet, hypotheses, consensus, RANSAC -------------------------------------
+        d0 = self.Desc.forward_multi(jobs[:2], aligned, radii=r_dev[0:1])
+        m0 = self.Desc.last_multi
+        ops.mutual_nn(d0[0]["desc"], d0[1]["desc"], out=(s_lists[0], t_lists[0], cnts[0:1]))
+        s0, t0 = ops.concat_matches(s_lists[:1], t_lists[:1], cnts[:1], [0], [K], offs[0:2])
+        logits = self.Pose.logits(m0["equi"], m0["equi"], s0, t0, cnts[0:1], K)
+        kp0 = torch.cat([src_kpts, tgt_kpts], dim=0)
+        ops.hypotheses(logits, azi_n, kp0, kp0, m0["R"], m0["R"], s0, t0, cnts[0:1], K, offs[0:1], offs[1:2], None,
+                       R_acc, t_acc, ss_acc, tt_acc)
+        inl, dI, _, _ = ops.consensus(ss_acc, tt_acc, R_acc, t_acc, offs[1:2], K, azi_n, cfg.match.inlier_th)
+        res0 = self.pose_estimator.enqueue(ss_acc, tt_acc, inl, dI, K, ransac_seed)
+        # ---- the decision: counts [key-points per job, patches per radius group (G), patches of the batch] -----------
+        counts = torch.empty(2 + G, dtype=torch.int32, device=dev)
+        su = torch.empty(1, dtype=torch.float64, device=dev)
+        ops.early_exit_gate(res0, cfg.match.get("early_exit_min_inliers", 15), [K] + [2 * K] * G + [2 * G * K], counts, S, su)
+        if G > 0:
+            # ---- scales 1..S-1, sized by the counts (nothing is computed on exit) ---------------------------------
+            d1 = self.Desc.forward_multi(jobs[2:], aligned, radii=r_dev[1:],
+                                         counts=dict(job=counts[0:1], group=counts[1:1 + G], total=counts[1 + G:2 + G]))
+            m1 = self.Desc.last_multi
+            for i in range(1, S):
+                ops.mutual_nn(d1[2 * i - 2]["desc"], d1[2 * i - 1]["desc"], out=(s_lists[i], t_lists[i], cnts[i:i + 1]),
+                              d_Ka=counts[0:1], d_Kb=counts[0:1])
+            offs_new = torch.empty(S, dtype=torch.int32, device=dev)
+            s1, t1 = ops.concat_matches(s_lists[1:], t_lists[1:], cnts[1:], [2 * j * K for j in range(G)],
+                                        [(2 * j + 1) * K for j in range(G)], offs_new)
+            torch.add(offs_new[1:], offs[1:2], out=offs[2:])          # offs[1 + i] = scale-0 matches + the new prefix sums
+            logits = self.Pose.logits(m1["equi"], m1["equi"], s1, t1, offs_new[G:G + 1], G * K)
+            kp1 = torch.cat([src_kpts, tgt_kpts] * G, dim=0)
+            ops.hypotheses(logits, azi_n, kp1, kp1, m1["R"], m1["R"], s1, t1, offs_new[G:G + 1], G * K, offs[1:2], offs[S:S + 1], None,
+                           R_acc, t_acc, ss_acc, tt_acc)
+        # ---- consensus over all appended rows, final RANSAC and refinement ------------------------------------------
+        d_Mc = offs[S:S + 1]
+        inl, dI, _, _ = ops.consensus(ss_acc, tt_acc, R_acc, t_acc, d_Mc, S * K, azi_n, cfg.match.inlier_th)
+        res_block = self.pose_estimator.enqueue(ss_acc, tt_acc, inl, dI, S * K, ransac_seed)
+        if cfg.test.pose_refine is True:
+            refined, _ = ops.refine(ss_acc, tt_acc, d_Mc, S * K, res_block[:16], cfg.match.dist_th)
+            refined = refined.double()
+        else:
+            refined = torch.zeros(16, dtype=torch.float64, device=dev)
+        return torch.cat([res_block, offs.double(), dI.double(), su, refined, self.Desc.conv_net.overflow_flag(dev).double()])
 
     def _decode(self, tail, times):
         cfg = self.config

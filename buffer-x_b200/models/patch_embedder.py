@@ -118,12 +118,16 @@ class MiniSpinNet(nn.Module):
                        x=ops.from_blocked(x).view(K, -1, self.ele_n, self.azi_n))
         return out
 
-    def forward_multi(self, jobs, is_aligned_to_global_z, radii=None):
+    def forward_multi(self, jobs, is_aligned_to_global_z, radii=None, counts=None):
         """Descriptors of several (cloud, key-points, radius, permutation) jobs in ONE pass through SPT, the
         convolution stack and the pooling layer (all CTA-per-patch kernels: batching the 2 x num_scales calls of a
         pair removes five of six launch tails and wave-quantisation losses).  Per-job results are views into the
         batched buffers; same arithmetic as ``forward`` per patch.  jobs: list of (pts [N,3], kpts [K,3], des_r
-        1-element CUDA tensor, perm int32 [N])."""
+        1-element CUDA tensor, perm int32 [N]).
+        ``counts`` (early-exit pairs: the later scales' work sized on the device, see BufferX._enqueue_device_exit): a dict of
+        int32 CUDA tensors, "job" [1] = key-points of every job, "group" [len(radii)] = patches of every radius group, "total" [1]
+        = patches of the batch (jobs of equal size, (src, tgt) per radius).  Patches beyond them are not computed and their
+        result rows are undefined."""
         dev = jobs[0][0].device
         prep = self.prepared(dev)
         P = self.patch_sample
@@ -139,6 +143,8 @@ class MiniSpinNet(nn.Module):
         # counts: the local reference frames of all jobs then run in ONE launch (patch k uses radii[k // (2 K)])
         one_lrf = radii is not None and len(set(Ks)) == 1 and len(jobs) == 2 * radii.numel()
         one_sel = len(jobs) <= 16 and all(isinstance(j[2], torch.Tensor) for j in jobs)   # all patch gatherings of the pair in one launch
+        if counts is not None and not (one_lrf and one_sel):
+            raise ops.BufferXError("forward_multi: device-side counts need equal-size (src, tgt) jobs per radius and device radii")
         sel = []
         for (pts, kpts, des_r, perm), K in zip(jobs, Ks):
             sel.append((ops.permute_cloud(pts.contiguous(), perm), kpts.contiguous(), des_r))
@@ -148,12 +154,15 @@ class MiniSpinNet(nn.Module):
         # small clouds: all jobs through the streaming scan in one launch; larger ones: all jobs through the hash grid, one launch
         # per phase; a mix of both (C5: 60 k vs 30 k points is above the threshold on both sides; 5 k vs 20 k would not be): job by job
         big = [pts4.shape[0] >= ops.GRID_MIN_POINTS for (pts4, _, _) in sel]
+        job_cnt = None if counts is None else [counts["job"]] * len(jobs)
         if one_sel and (all(big) or not any(big)):
-            ops.select_patches_batched(sel, P, patches, grid=all(big))
+            ops.select_patches_batched(sel, P, patches, grid=all(big), d_K=job_cnt)
         o = 0
         for j, ((pts4, kpts, des_r), K) in enumerate(zip(sel, Ks)):
             if not (one_sel and (all(big) or not any(big))):
-                if big[j] and isinstance(des_r, torch.Tensor):
+                if counts is not None:      # job by job, each with its device count
+                    ops.select_patches_batched([(pts4, kpts, des_r)], P, patches[o:o + K], grid=big[j], d_K=job_cnt[:1])
+                elif big[j] and isinstance(des_r, torch.Tensor):
                     ops.select_patches_grid(pts4, kpts, des_r, P, patches=patches[o:o + K])
                 else:
                     ops.select_patches(pts4, kpts, des_r, P, patches=patches[o:o + K])
@@ -161,17 +170,19 @@ class MiniSpinNet(nn.Module):
                 ops.lrf(patches[o:o + K], des_r, bool(is_aligned_to_global_z), delta=delta[o:o + K], Rt=R_all[o:o + K], ra=ra_all[o:o + K])
             o += K
         if one_lrf:
-            ops.lrf(patches, radii, bool(is_aligned_to_global_z), delta=delta, Rt=R_all, ra=ra_all, r_group=2 * Ks[0])
+            ops.lrf(patches, radii, bool(is_aligned_to_global_z), delta=delta, Rt=R_all, ra=ra_all, r_group=2 * Ks[0],
+                    d_K=None if counts is None else counts["group"])
         net = self.conv_net
         if not net.force_tf32 and self.rad_n * self.ele_n * self.azi_n == 420 and self.azi_n == 20:
             # production: features straight into the presplit fp16 format the first conv layer fetches with bulk copies
             feat = ops.spt_pnt_sd(delta, prep["voxels"], prep["rot"], self.delta / self.rad_n, self.voxel_sample, prep["w_pnt"],
-                                  prep["b_pnt"], self.azi_n, net.overflow_flag(dev))
+                                  prep["b_pnt"], self.azi_n, net.overflow_flag(dev), d_K=None if counts is None else counts["total"])
         else:
             feat = ops.spt_pnt(delta, prep["voxels"], prep["rot"], self.delta / self.rad_n, self.voxel_sample, prep["w_pnt"],
                                prep["b_pnt"], self.azi_n)
-        x, _ = self.conv_net(feat, K=Kt)
-        desc, equi = ops.pool_desc(x, prep["w1"], prep["b1"], prep["w2"], prep["b2"], channels_last=True)
+        total = None if counts is None else counts["total"]
+        x, _ = self.conv_net(feat, K=Kt, d_n=total)
+        desc, equi = ops.pool_desc(x, prep["w1"], prep["b1"], prep["w2"], prep["b2"], channels_last=True, d_K=total)
         outs, o = [], 0
         for K, R, ra in zip(Ks, Rs, axes):
             outs.append({"desc": desc[o:o + K], "equi": equi[o:o + K], "rand_axis": ra, "R": R, "patches": delta[o:o + K],

@@ -115,8 +115,9 @@ class Cylindrical_Net(_ConvStack):
             self._flag = torch.zeros(1, dtype=torch.int32, device=dev)
         return self._flag
 
-    def forward(self, x, K=None):
-        """x [K,4,420,4] channel-blocked (or the presplit image of K patches) -> (x_out [K,8,140,4], None)."""
+    def forward(self, x, K=None, d_n=None):
+        """x [K,4,420,4] channel-blocked (or the presplit image of K patches) -> (x_out [K,8,140,4], None).
+        d_n: optional int32[1] CUDA count: only the first min(d_n, K) samples are computed (the rest of x_out is undefined)."""
         presplit_in = x.dtype == torch.float16             # [3, 4, rows, 8] from bx_spt_pnt_sd: K is passed separately
         K = x.shape[0] if not presplit_in else int(K)
         dev = x.device
@@ -132,13 +133,13 @@ class Cylindrical_Net(_ConvStack):
             if use_sd:       # layer-to-layer activations in the presplit padded fp16 format; fp32 in at the first, fp32 out at the last layer
                 out = out if i == len(L) - 1 else ops.conv_sd_buffer(K, l["cout"], dev)
                 ops.conv_layer_sd(ops.GEOM_CYL3D if i == 0 else ops.GEOM_CYL2D, cur, l["w_sd"], l["b"], out, K, l["cin"], l["cout"], l["relu"], flag,
-                                  tile_ctr=None if ctrs is None else ctrs[2 * i:2 * i + 2])
+                                  d_n=d_n, tile_ctr=None if ctrs is None else ctrs[2 * i:2 * i + 2])
                 cur = out
                 continue
             if i == 0:
-                ops.conv_layer_tc(ops.GEOM_CYL3D, cur, l["w_tc"], l["b"], out, K, l["cin"], l["cout"], 3, 7, 20, 3, 3, 3, l["relu"])
+                ops.conv_layer_tc(ops.GEOM_CYL3D, cur, l["w_tc"], l["b"], out, K, l["cin"], l["cout"], 3, 7, 20, 3, 3, 3, l["relu"], d_n=d_n)
             else:
-                ops.conv_layer_tc(ops.GEOM_CYL2D, cur, l["w_tc"], l["b"], out, K, l["cin"], l["cout"], 1, 7, 20, 1, 3, 3, l["relu"])
+                ops.conv_layer_tc(ops.GEOM_CYL2D, cur, l["w_tc"], l["b"], out, K, l["cin"], l["cout"], 1, 7, 20, 1, 3, 3, l["relu"], d_n=d_n)
             cur = out
         return cur, None
 

@@ -25,6 +25,8 @@ SYMBOLS = [
     "bx_radius_neighbors", "bx_grid_subsample", "bx_costvol_ab", "bx_concat_matches",
     "bx_pca_analysis", "bx_project_range", "bx_voxel_down_sample", "bx_conv_layer_sd", "bx_conv_sd_rows", "bx_spt_pnt_sd", "bx_fps_set_sync_mode", "bx_conv_layer_sd_costab", "bx_lrf_batched", "bx_select_patches_batched", "bx_fps_ex", "bx_select_patches_grid", "bx_select_patches_grid_workspace_bytes", "bx_select_patches_grid_batched",
     "bx_gt_matches", "bx_so2_augment", "bx_equi_match", "bx_so2_gt",
+    "bx_select_patches_batched_n", "bx_select_patches_grid_batched_n", "bx_lrf_batched_n", "bx_spt_pnt_sd_n", "bx_pool_desc_n",
+    "bx_mutual_nn_n", "bx_early_exit_gate",
 ]
 
 GEOM_CYL3D, GEOM_CYL2D, GEOM_VALID3D, GEOM_COSTAB = 0, 1, 2, 4
@@ -64,10 +66,13 @@ def load_library():
     lib.bx_select_patches_grid.argtypes = [P, c_int, P, c_int, P, c_int, P, P, P, P]
     lib.bx_select_patches_grid_workspace_bytes.argtypes = [c_int]
     lib.bx_select_patches_grid_batched.argtypes = [c_int, P, P, P, P, P, c_int, P, P, P]
+    lib.bx_select_patches_batched_n.argtypes = [c_int, P, P, P, P, P, P, c_int, P, P]
+    lib.bx_select_patches_grid_batched_n.argtypes = [c_int, P, P, P, P, P, P, c_int, P, P, P]
     lib.bx_select_patches_grid_workspace_bytes.restype = c_int64
     lib.bx_ball_query.argtypes = [P, c_int, P, c_int, c_float, c_int, P, P]
     lib.bx_lrf.argtypes = [P, c_int, c_int, c_float, P, c_int, P, P, P, P]
     lib.bx_lrf_batched.argtypes = [P, c_int, c_int, c_float, P, c_int, c_int, P, P, P, P]
+    lib.bx_lrf_batched_n.argtypes = [P, c_int, c_int, c_float, P, c_int, P, c_int, P, P, P, P]
     lib.bx_spt_pnt.argtypes = [P, c_int, c_int, P, c_int, c_int, P, c_float, c_int, P, P, P, P, P, P]
     lib.bx_conv_layer_tc.argtypes = [c_int, P, P, P, P, c_int, P] + [c_int] * 9 + [P, P, P]
     lib.bx_conv_tc_ntile.argtypes = [c_int]
@@ -76,6 +81,7 @@ def load_library():
     lib.bx_conv_layer_sd_costab.argtypes = [P, P, P, P, P, c_int, c_int, P, c_int, P, P]
     lib.bx_fps_set_sync_mode.argtypes = [c_int]
     lib.bx_spt_pnt_sd.argtypes = [P, c_int, c_int, P, c_int, c_int, P, c_float, c_int, P, P, P, c_int64, P, P]
+    lib.bx_spt_pnt_sd_n.argtypes = [P, c_int, c_int, P, c_int, c_int, P, c_float, c_int, P, P, P, c_int64, P, P, P]
     lib.bx_conv_sd_rows.restype = c_int64
     lib.bx_costvol_ab.argtypes = [P, P, P, P, P, c_int, P, P, P, P, P, P]
     lib.bx_concat_matches.argtypes = [P, P, P, c_int, c_int, P, P, P, P, P, P]
@@ -83,7 +89,10 @@ def load_library():
     lib.bx_project_range.argtypes = [P, c_int, P, P, P, P]
     lib.bx_voxel_down_sample.argtypes = [P, c_int, ctypes.c_double, P, P, c_int, P, P, P, P, P, P]
     lib.bx_pool_desc.argtypes = [P, c_int, c_int, c_int, c_int, P, P, P, P, P, P, P]
+    lib.bx_pool_desc_n.argtypes = [P, c_int, c_int, c_int, c_int, P, P, P, P, P, P, P, P]
     lib.bx_mutual_nn.argtypes = [P, c_int, P, c_int, c_int, P, P, P, P, P, P, P]
+    lib.bx_mutual_nn_n.argtypes = [P, c_int, P, c_int, c_int, P, P, P, P, P, P, P, P, P]
+    lib.bx_early_exit_gate.argtypes = [P, c_int, c_int, P, P, c_int, P, P]
     lib.bx_hypotheses.argtypes = [P, c_int, P, P, P, P, P, P, P, c_int, P, P, P, P, P, P, P, P]
     lib.bx_consensus.argtypes = [P, P, P, P, P, c_int, c_int, c_float, P, P, P, P, P]
     lib.bx_ransac.argtypes = [P, P, P, P, c_int, c_double, c_double, c_double, c_int, c_uint64, P, P, P]
@@ -263,15 +272,17 @@ def select_patches_grid(pts4: torch.Tensor, kpts: torch.Tensor, radius: torch.Te
     return patches, idx
 
 
-def select_patches_batched(jobs, P: int, patches: torch.Tensor, grid=False):
+def select_patches_batched(jobs, P: int, patches: torch.Tensor, grid=False, d_K=None):
     """jobs: [(pts4 [N,4], kpts [K,3], radius 1-element CUDA tensor)]; patches [sum K, P, 3] is filled job after job by ONE launch
-    (grid=True: the hash-grid form, one launch per phase)."""
+    (grid=True: the hash-grid form, one launch per phase).  d_K: optional per-job 1-element int32 CUDA tensors (or None
+    entries): job j gathers only its first min(d_K[j], K_j) key-points."""
     import ctypes
     n = len(jobs)
     VP, I = ctypes.c_void_p * n, ctypes.c_int32 * n
     pts = VP(*[_dp(j[0], F32, "pts4") for j in jobs])
     kps = VP(*[_dp(j[1], F32, "kpts") for j in jobs])
     rad = VP(*[_dp(j[2], F32, "radius") for j in jobs])
+    cnt = None if d_K is None else VP(*[_dp(c, I32, "d_K") for c in d_K])
     Ns, Ks = I(*[int(j[0].shape[0]) for j in jobs]), I(*[int(j[1].shape[0]) for j in jobs])
     assert patches.shape[0] == sum(Ks) and patches.is_contiguous()
     lib = load_library()
@@ -280,9 +291,10 @@ def select_patches_batched(jobs, P: int, patches: torch.Tensor, grid=False):
         ws = torch.empty(sum(int(lib.bx_select_patches_grid_workspace_bytes(int(a))) for a in Ns) // 4, dtype=I32, device=patches.device)
     with _Span("select_patches", sum(16.0 * a + 12.0 * b + b * P * 12.0 for a, b in zip(Ns, Ks))):
         if grid:
-            _check(lib.bx_select_patches_grid_batched(n, pts, Ns, kps, Ks, rad, P, _dp(patches, F32, "patches"), _dp(ws), _stream()), "bx_select_patches_grid_batched")
+            _check(lib.bx_select_patches_grid_batched_n(n, pts, Ns, kps, Ks, rad, cnt, P, _dp(patches, F32, "patches"), _dp(ws), _stream()),
+                   "bx_select_patches_grid_batched")
         else:
-            _check(lib.bx_select_patches_batched(n, pts, Ns, kps, Ks, rad, P, _dp(patches, F32, "patches"), _stream()), "bx_select_patches_batched")
+            _check(lib.bx_select_patches_batched_n(n, pts, Ns, kps, Ks, rad, cnt, P, _dp(patches, F32, "patches"), _stream()), "bx_select_patches_batched")
     return patches
 
 
@@ -293,7 +305,8 @@ def ball_query(xyz: torch.Tensor, qry: torch.Tensor, radius: float, nsample: int
     return idx
 
 
-def lrf(patches: torch.Tensor, des_r, aligned: bool, delta=None, Rt=None, ra=None, r_group=0):
+def lrf(patches: torch.Tensor, des_r, aligned: bool, delta=None, Rt=None, ra=None, r_group=0, d_K=None):
+    """d_K: optional int32 CUDA counts, one per radius group (r_group > 0) or one in all: patches beyond a count are not touched."""
     K, P, _ = patches.shape
     dev = patches.device
     if delta is None:
@@ -305,18 +318,21 @@ def lrf(patches: torch.Tensor, des_r, aligned: bool, delta=None, Rt=None, ra=Non
     rv, rp = (0.0, _dp(des_r, F32, "des_r")) if isinstance(des_r, torch.Tensor) else (float(des_r), None)
     with _Span("lrf", 24.0 * K * P):
         flags = int(bool(aligned)) | (2 if os.environ.get("BX_LRF", "").lower() == "stable" else 0)
-        _check(load_library().bx_lrf_batched(_dp(patches, F32, "patches"), K, P, rv, rp, int(r_group), flags, _dp(delta), _dp(Rt), _dp(ra), _stream()), "bx_lrf")
+        _check(load_library().bx_lrf_batched_n(_dp(patches, F32, "patches"), K, P, rv, rp, int(r_group), _dp(d_K, I32, "d_K"), flags, _dp(delta), _dp(Rt),
+                                               _dp(ra), _stream()), "bx_lrf")
     return delta, Rt, ra
 
 
-def spt_pnt_sd(delta, voxels, rot, voxel_r: float, nv: int, w, b, azi_n: int, flag=None):
-    """SPT + point layer with the features in the presplit padded fp16 format: [3, 4, conv_sd_rows(K), 8] fp16."""
+def spt_pnt_sd(delta, voxels, rot, voxel_r: float, nv: int, w, b, azi_n: int, flag=None, d_K=None):
+    """SPT + point layer with the features in the presplit padded fp16 format: [3, 4, conv_sd_rows(K), 8] fp16.
+    d_K: optional int32[1] CUDA count: only the first min(d_K, K) patches are written."""
     K, P, _ = delta.shape
     V = voxels.shape[0]
     feat = conv_sd_buffer(K, 48, delta.device)
     with _Span("spt", 12.0 * K * P + 64.0 * K * V):
-        _check(load_library().bx_spt_pnt_sd(_dp(delta, F32, "delta"), K, P, _dp(voxels, F32), V, azi_n, _dp(rot, F32), float(voxel_r), nv,
-                                            _dp(w, F32), _dp(b, F32), _dp(feat), feat.shape[2], _dp(flag, I32, "flag"), _stream()), "bx_spt_pnt_sd")
+        _check(load_library().bx_spt_pnt_sd_n(_dp(delta, F32, "delta"), K, P, _dp(voxels, F32), V, azi_n, _dp(rot, F32), float(voxel_r), nv,
+                                              _dp(w, F32), _dp(b, F32), _dp(feat), feat.shape[2], _dp(flag, I32, "flag"), _dp(d_K, I32, "d_K"),
+                                              _stream()), "bx_spt_pnt_sd")
     return feat
 
 
@@ -523,8 +539,9 @@ def costvol_ab(equi_s, equi_t, s_mids, t_mids, d_M, maxM, wa, wb, bias, A=None, 
     return A, B
 
 
-def pool_desc(x, w1, b1, w2, b2, desc=None, equi=None, channels_last=False):
-    """x: [K,32,7,20] (channel-first) or channel-blocked [K,8,140,4] with channels_last=True.  equi is always [K,32,7,20]."""
+def pool_desc(x, w1, b1, w2, b2, desc=None, equi=None, channels_last=False, d_K=None):
+    """x: [K,32,7,20] (channel-first) or channel-blocked [K,8,140,4] with channels_last=True.  equi is always [K,32,7,20].
+    d_K: optional int32[1] CUDA count: rows at or beyond it are not written."""
     K, C = x.shape[0], 32
     S = x.numel() // max(K * C, 1) if K > 0 else 140
     dev = x.device
@@ -532,13 +549,14 @@ def pool_desc(x, w1, b1, w2, b2, desc=None, equi=None, channels_last=False):
         desc = torch.empty((K, C), dtype=F32, device=dev)
     if equi is None:
         equi = torch.empty((K, C, 7, 20) if S == 140 else (K, C, S), dtype=F32, device=dev)
-    _check(load_library().bx_pool_desc(_dp(x, F32, "x"), K, C, S, int(bool(channels_last)), _dp(w1, F32), _dp(b1, F32), _dp(w2, F32), _dp(b2, F32),
-                                       _dp(desc), _dp(equi), _stream()), "bx_pool_desc")
+    _check(load_library().bx_pool_desc_n(_dp(x, F32, "x"), K, C, S, int(bool(channels_last)), _dp(w1, F32), _dp(b1, F32), _dp(w2, F32), _dp(b2, F32),
+                                         _dp(desc), _dp(equi), _dp(d_K, I32, "d_K"), _stream()), "bx_pool_desc")
     return desc, equi
 
 
-def mutual_nn(a, b, want_nn=False, out=None):
-    """out: optional (s_mids [>=Ka], t_mids [>=Ka], dM [1]) int32 buffers to fill (dM must be zero on entry)."""
+def mutual_nn(a, b, want_nn=False, out=None, d_Ka=None, d_Kb=None):
+    """out: optional (s_mids [>=Ka], t_mids [>=Ka], dM [1]) int32 buffers to fill (dM must be zero on entry).
+    d_Ka / d_Kb: optional int32[1] CUDA counts: only the first rows of a / b take part (0 on either side: *dM = 0)."""
     Ka, Kb, C = a.shape[0], b.shape[0], a.shape[1]
     dev = a.device
     keys = torch.empty(Ka + Kb + 1, dtype=torch.int64, device=dev)
@@ -550,8 +568,8 @@ def mutual_nn(a, b, want_nn=False, out=None):
         dM = torch.zeros(1, dtype=I32, device=dev)
     snn = torch.empty(max(Ka, 1), dtype=I32, device=dev) if want_nn else None
     tnn = torch.empty(max(Kb, 1), dtype=I32, device=dev) if want_nn else None
-    _check(load_library().bx_mutual_nn(_dp(a, F32, "a"), Ka, _dp(b, F32, "b"), Kb, C, _dp(keys), _dp(s), _dp(t), _dp(dM), _dp(snn), _dp(tnn), _stream()),
-           "bx_mutual_nn")
+    _check(load_library().bx_mutual_nn_n(_dp(a, F32, "a"), Ka, _dp(b, F32, "b"), Kb, C, _dp(d_Ka, I32, "d_Ka"), _dp(d_Kb, I32, "d_Kb"), _dp(keys),
+                                         _dp(s), _dp(t), _dp(dM), _dp(snn), _dp(tnn), _stream()), "bx_mutual_nn")
     return s, t, dM, snn, tnn
 
 
@@ -609,6 +627,17 @@ def ransac(ss, tt, inlier_ind, d_I, maxI, dist_th, similar_th, confidence, max_i
     if ev:
         ev[1].record()
     return result
+
+
+def early_exit_gate(result, min_inliers: int, caps, counts, num_scales: int, scales_used=None):
+    """Early-exit decision on the device from a RANSAC result block: counts[i] = 0 when result's num_inliers >= min_inliers,
+    else caps[i] (host ints); scales_used (float64[1], optional) = 1 or num_scales."""
+    cp = np.ascontiguousarray(caps, dtype=np.int32)
+    assert counts.numel() >= len(cp)
+    _check(load_library().bx_early_exit_gate(_dp(result, torch.float64, "result"), int(min_inliers), len(cp), cp.ctypes.data_as(c_void_p),
+                                             _dp(counts, I32, "counts"), int(num_scales), _dp(scales_used, torch.float64, "scales_used"),
+                                             _stream()), "bx_early_exit_gate")
+    return counts
 
 
 def decode_ransac_result(result_cpu: torch.Tensor):

@@ -98,6 +98,15 @@ long long bx_select_patches_grid_workspace_bytes(int N);
  * workspace = the sum of bx_select_patches_grid_workspace_bytes(N[j]) bytes). */
 int bx_select_patches_grid_batched(int njobs, const void *const *pts4, const int32_t *N, const void *const *kpts, const int32_t *K,
                                    const void *const *d_radius, int P, float *patches, void *workspace, void *stream);
+/* Device-side key-point counts (early-exit pairs: the later scales' work is sized on the device).  d_K: host array of njobs
+ * device int32 pointers (an entry or the array may be NULL = no count).  Job j processes its first min(*d_K[j], K[j])
+ * key-points; the patch rows of the others are left untouched.  In the grid form a job whose count is 0 also skips its
+ * binning phases (count, scan, scatter).  Otherwise identical to the calls above (which pass NULL). */
+int bx_select_patches_batched_n(int njobs, const void *const *pts4, const int32_t *N, const void *const *kpts, const int32_t *K,
+                                const void *const *d_radius, const void *const *d_K, int P, float *patches, void *stream);
+int bx_select_patches_grid_batched_n(int njobs, const void *const *pts4, const int32_t *N, const void *const *kpts, const int32_t *K,
+                                     const void *const *d_radius, const void *const *d_K, int P, float *patches, void *workspace,
+                                     void *stream);
 
 /* Plain ordered ball query (pointnet2_ops.ball_query; utils/common.py:442): xyz [n,3] packed. */
 int bx_ball_query(const float *xyz, int n, const float *qry, int m, float radius, int nsample, int32_t *idx,
@@ -115,6 +124,10 @@ int bx_lrf(const float *patches, int K, int P, float des_r, const float *d_des_r
  * d_des_r[k / r_group] (r_group > 0; r_group == 0: d_des_r[0] / des_r like bx_lrf). */
 int bx_lrf_batched(const float *patches, int K, int P, float des_r, const float *d_des_r, int r_group, int flags, float *delta,
                    float *Rt, float *rand_axis, void *stream);
+/* With device-side counts: r_group > 0: d_K[g] per radius group g, patch k is processed iff k % r_group < d_K[k / r_group];
+ * r_group == 0: iff k < *d_K.  Rows of the other patches (delta, Rt, rand_axis) are left untouched.  d_K NULL = bx_lrf_batched. */
+int bx_lrf_batched_n(const float *patches, int K, int P, float des_r, const float *d_des_r, int r_group, const int32_t *d_K, int flags,
+                     float *delta, float *Rt, float *rand_axis, void *stream);
 
 /* ---- a6+a7: spherical-voxel transformer + point layer ---------------------------------------
  * Replaces MiniSpinNet.SPT (models/patch_embedder.py:150-165: get_voxel_coordinate,
@@ -133,6 +146,12 @@ int bx_spt_pnt(const float *delta, int K, int P, const float *voxels, int V, int
 int bx_spt_pnt_sd(const float *delta, int K, int P, const float *voxels, int V, int azi_n, const float *rot,
                   float voxel_r, int nv, const float *w, const float *b, void *feat_sd, long long rows, int32_t *d_flag,
                   void *stream);
+/* With a device-side count (d_K NULL = bx_spt_pnt_sd): the first n = min(*d_K, K) patches are written, with the zero row
+ * that follows patch n - 1 (as bx_conv_layer_sd writes the zero row of sample s + 1 for a live sample s); the rows of the
+ * later patches are left untouched. */
+int bx_spt_pnt_sd_n(const float *delta, int K, int P, const float *voxels, int V, int azi_n, const float *rot,
+                    float voxel_r, int nv, const float *w, const float *b, void *feat_sd, long long rows, int32_t *d_flag,
+                    const int32_t *d_K, void *stream);
 
 /* ---- a8/a11: convolution stacks -------------------------------------------------------------
  * Every conv layer of Cylindrical_Net (models/patchnet.py:16-84, circular-azimuth / zero-elevation padding of
@@ -208,6 +227,9 @@ int bx_costvol_ab(const float *equi_s, const float *equi_t, const int32_t *s_mid
  * b1 [16], w2 [16], b2 [1] (BatchNorm folded); desc: [K,32]; equi: [K,32,S] (always channel-first). */
 int bx_pool_desc(const float *x, int K, int C, int S, int channels_last, const float *w1, const float *b1,
                  const float *w2, const float *b2, float *desc, float *equi, void *stream);
+/* With a device-side count (d_K NULL = bx_pool_desc): rows k < min(*d_K, K) are written, the others left untouched. */
+int bx_pool_desc_n(const float *x, int K, int C, int S, int channels_last, const float *w1, const float *b1,
+                   const float *w2, const float *b2, float *desc, float *equi, const int32_t *d_K, void *stream);
 
 /* ---- a10: mutual nearest-neighbour matching -------------------------------------------------
  * Replaces BufferX.mutual_matching (models/BUFFERX.py:469-496) -> knn_cuda.KNN(k=1) both ways.
@@ -215,6 +237,12 @@ int bx_pool_desc(const float *x, int K, int C, int S, int channels_last, const f
  * snn [Ka] / tnn [Kb] optional. */
 int bx_mutual_nn(const float *a, int Ka, const float *b, int Kb, int C, unsigned long long *keys, int32_t *s_mids,
                  int32_t *t_mids, int32_t *d_M, int32_t *snn, int32_t *tnn, void *stream);
+/* With device-side counts on either side (NULL = no count; both NULL = bx_mutual_nn): matches the first min(*d_Ka, Ka)
+ * rows of a against the first min(*d_Kb, Kb) rows of b, exactly as bx_mutual_nn on those rows.  A count of 0 on either
+ * side writes *d_M = 0 and nothing else. */
+int bx_mutual_nn_n(const float *a, int Ka, const float *b, int Kb, int C, const int32_t *d_Ka, const int32_t *d_Kb,
+                   unsigned long long *keys, int32_t *s_mids, int32_t *t_mids, int32_t *d_M, int32_t *snn, int32_t *tnn,
+                   void *stream);
 
 /* Concatenate the S per-scale match lists (s_lists/t_lists: [S][stride] int32, counts d_counts[S] on the device)
  * into one list in scale order, adding the per-scale row offsets h_s_off/h_t_off[S] (host arrays) so the entries
@@ -252,6 +280,12 @@ int64_t bx_ransac_workspace_bytes(int max_iter);
 int bx_ransac(const float *ss, const float *tt, const int32_t *inlier_ind, const int32_t *d_I, int maxI,
               double dist_th, double similar_th, double confidence, int max_iter, uint64_t seed, void *workspace,
               void *result, void *stream);
+/* Early-exit decision of a multi-scale pair (models/pose_estimator.py compute_confidence_score) on the device: the pair
+ * stops after scale 0 when result->num_inliers >= min_inliers.  Writes d_counts[i] = 0 (stop) or h_caps[i] (continue) for
+ * i < n (n <= 32; h_caps is a host array: the capacities the later scales' launches were sized for), and, if
+ * d_scales_used != NULL, *d_scales_used = 1 (stop) or num_scales. */
+int bx_early_exit_gate(const void *result, int min_inliers, int n, const int32_t *h_caps, int32_t *d_counts, int num_scales,
+                       double *d_scales_used, void *stream);
 
 /* ---- a15: post refinement -------------------------------------------------------------------
  * Replaces BufferX.post_refinement + rigid_transform_3d (models/BUFFERX.py:522-603).
