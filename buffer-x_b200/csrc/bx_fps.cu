@@ -92,7 +92,7 @@ __device__ __forceinline__ void fps_wait_cluster(uint32_t bar, uint32_t parity) 
 template <int THREADS, int PPT>
 __global__ void __launch_bounds__(THREADS, 1)
 fps_cluster_kernel(const float *__restrict__ xyz_all, const FpsOffsets offsets, int npoint,
-                   int *__restrict__ idx_out, float *__restrict__ kpts_out, int sync_mode) {
+                   int *__restrict__ idx_out, float *__restrict__ kpts_out, int sync_mode, const int *__restrict__ d_counts) {
     constexpr int NW = THREADS / 32;
     cg::cluster_group cluster = cg::this_cluster();
     const int CL = (int)cluster.num_blocks();
@@ -101,7 +101,9 @@ fps_cluster_kernel(const float *__restrict__ xyz_all, const FpsOffsets offsets, 
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
 
     const int start = offsets.v[cloud];
-    const int N = offsets.v[cloud + 1] - start;
+    const int cap = offsets.v[cloud + 1] - start;
+    // device count (size-class slots): the points of the cloud present this launch, clamped to [1, capacity]
+    const int N = d_counts ? min(max(d_counts[cloud], 1), cap) : cap;
     const float *xyz = xyz_all + 3 * (size_t)start;
     int *idx = idx_out + (size_t)cloud * npoint;
     float *kp = kpts_out ? kpts_out + 3 * (size_t)cloud * npoint : nullptr;
@@ -245,7 +247,8 @@ fps_cluster_kernel(const float *__restrict__ xyz_all, const FpsOffsets offsets, 
 int g_fps_sync_override = -1;
 
 template <int THREADS, int PPT>
-int launch_fps(const float *xyz, const FpsOffsets off, int B, int CL, int npoint, int *idx, float *kpts, cudaStream_t st) {
+int launch_fps(const float *xyz, const FpsOffsets off, int B, int CL, int npoint, int *idx, float *kpts, const int *d_counts,
+               cudaStream_t st) {
     auto kern = fps_cluster_kernel<THREADS, PPT>;
     if (CL > 8) BX_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeNonPortableClusterSizeAllowed, 1));
     cudaLaunchConfig_t cfg = {};
@@ -263,9 +266,44 @@ int launch_fps(const float *xyz, const FpsOffsets off, int B, int CL, int npoint
     static int sync_mode = -1;     // BX_FPS_SYNC: 0 = st.async exchange (production), 1 = cluster.sync() (racecheck-clean reference form),
     if (sync_mode < 0) { const char *e = getenv("BX_FPS_SYNC"); sync_mode = e ? atoi(e) : 0; }   // 2 = remote stores + mbarrier arrive / acquire wait (round 1)
     if (g_fps_sync_override >= 0) sync_mode = g_fps_sync_override;
-    BX_CUDA(cudaLaunchKernelEx(&cfg, kern, xyz, off, npoint, idx, kpts, sync_mode));
+    BX_CUDA(cudaLaunchKernelEx(&cfg, kern, xyz, off, npoint, idx, kpts, sync_mode, d_counts));
     ++g_bx_launches;
     return BX_OK;
+}
+
+
+// Launch configuration of a cloud of n points (the largest cloud of the call): register tier = (threads, points per thread,
+// CTAs per cloud).  Also returns, in *hi, the largest n that gets the same configuration -- the cloud's size class.
+enum FpsTier { T256x2, T256x4, T1024x4c, T1024x6c, T1024x10c, T1024x12c, T1024x1c16, T1024x2c16, T1024x2, T1024x3, T1024x4,
+               T1024x8, T1024x8c16, T512x32, T512x64 };
+
+FpsTier fps_tier(int n, int max_cluster, int *hi) {
+    if (n <= 4096) { *hi = 4096; return T256x2; }
+    if (n <= 8192) { *hi = 8192; return T256x4; }
+    // larger clouds: 1024 threads per CTA and few points per thread -- the per-iteration register scan is a dependent
+    // chain per thread, so its latency scales with the points per thread, while the reductions / cluster exchange
+    // do not depend on the thread count
+    if (max_cluster > 0 && n <= 49152) {
+        const int cl = max_cluster >= 4 ? 4 : 2;
+        const int per_cta = (n + cl - 1) / cl;          // points per CTA of 1024 threads
+        if (per_cta <= 4096) { *hi = min(4096 * cl, 49152); return T1024x4c; }
+        if (per_cta <= 6144) { *hi = min(6144 * cl, 49152); return T1024x6c; }
+        if (per_cta <= 10240) { *hi = min(10240 * cl, 49152); return T1024x10c; }
+        if (per_cta <= 12288) { *hi = min(12288 * cl, 49152); return T1024x12c; }
+    }
+    { static int cl16 = -1; if (cl16 < 0) { const char *e = getenv("BX_FPS_CL16"); cl16 = e ? atoi(e) : 0; }     // experiment: 16-CTA clusters, fewer points per thread
+      if (cl16 && n <= 16384) { *hi = 16384; return T1024x1c16; }
+      if (cl16 && n <= 32768) { *hi = 32768; return T1024x2c16; } }
+    if (n <= 16384) { *hi = 16384; return T1024x2; }
+    if (n <= 24576) { *hi = 24576; return T1024x3; }
+    if (n <= 32768) { *hi = 32768; return T1024x4; }
+    if (n <= 65536) { *hi = 65536; return T1024x8; }
+    if (n <= 131072) { *hi = 131072; return T1024x8c16; }
+    // beyond 128 K points per cloud (raw LiDAR sweeps before voxel down-sampling): 512-thread CTAs leave 128 registers per
+    // thread, enough for 32 / 64 points each -- slower per iteration, same result contract
+    if (n <= 262144) { *hi = 262144; return T512x32; }
+    *hi = 524288;
+    return T512x64;
 }
 
 }  // namespace
@@ -281,7 +319,7 @@ BX_API int bx_fps_set_sync_mode(int mode) {
 
 BX_API int bx_fps(const float *xyz, const int32_t *h_offsets, int B, int npoint, int32_t *idx, float *kpts,
                   void *stream) {
-    return bx_fps_ex(xyz, h_offsets, B, npoint, idx, kpts, 0, stream);
+    return bx_fps_n(xyz, h_offsets, B, npoint, idx, kpts, 0, nullptr, stream);
 }
 
 // max_cluster > 0: THROUGHPUT form -- at most that many CTAs per cloud (2 or 4), more points per thread.  An iteration is a
@@ -291,6 +329,13 @@ BX_API int bx_fps(const float *xyz, const int32_t *h_offsets, int B, int npoint,
 // quarter of the SMs.  Same indices in every form (the tie rank does not depend on the layout).
 BX_API int bx_fps_ex(const float *xyz, const int32_t *h_offsets, int B, int npoint, int32_t *idx, float *kpts, int max_cluster,
                      void *stream) {
+    return bx_fps_n(xyz, h_offsets, B, npoint, idx, kpts, max_cluster, nullptr, stream);
+}
+
+// d_counts (optional, device, B ints): cloud b holds min(max(d_counts[b], 1), h_offsets[b+1] - h_offsets[b]) points at
+// h_offsets[b]; the launch is sized by the capacities, so one captured launch serves every count up to them.
+BX_API int bx_fps_n(const float *xyz, const int32_t *h_offsets, int B, int npoint, int32_t *idx, float *kpts, int max_cluster,
+                    const int32_t *d_counts, void *stream) {
     BX_REQUIRE(xyz && h_offsets && idx, "bx_fps: null pointer");
     BX_REQUIRE(B >= 1 && B <= kMaxClouds, "bx_fps: B=%d out of range [1,%d]", B, kMaxClouds);
     BX_REQUIRE(npoint >= 0, "bx_fps: npoint < 0");
@@ -305,29 +350,33 @@ BX_API int bx_fps_ex(const float *xyz, const int32_t *h_offsets, int B, int npoi
     cudaStream_t st = bx_stream(stream);
     FpsOffsets d_off;
     for (int b = 0; b <= kMaxClouds; ++b) d_off.v[b] = h_offsets[b <= B ? b : B];
-    if (maxN <= 4096) return launch_fps<256, 2>(xyz, d_off, B, 8, npoint, idx, kpts, st);
-    if (maxN <= 8192) return launch_fps<256, 4>(xyz, d_off, B, 8, npoint, idx, kpts, st);
-    // larger clouds: 1024 threads per CTA and few points per thread -- the per-iteration register scan is a dependent
-    // chain per thread, so its latency scales with the points per thread, while the reductions / cluster exchange
-    // do not depend on the thread count
-    if (max_cluster > 0 && maxN <= 49152) {
-        const int cl = max_cluster >= 4 ? 4 : 2;
-        const int per_cta = (maxN + cl - 1) / cl;          // points per CTA of 1024 threads
-        if (per_cta <= 4096) return launch_fps<1024, 4>(xyz, d_off, B, cl, npoint, idx, kpts, st);
-        if (per_cta <= 6144) return launch_fps<1024, 6>(xyz, d_off, B, cl, npoint, idx, kpts, st);
-        if (per_cta <= 10240) return launch_fps<1024, 10>(xyz, d_off, B, cl, npoint, idx, kpts, st);
-        if (per_cta <= 12288) return launch_fps<1024, 12>(xyz, d_off, B, cl, npoint, idx, kpts, st);
+    const int *dc = d_counts;
+    int hi;
+    switch (fps_tier(maxN, max_cluster, &hi)) {
+        case T256x2: return launch_fps<256, 2>(xyz, d_off, B, 8, npoint, idx, kpts, dc, st);
+        case T256x4: return launch_fps<256, 4>(xyz, d_off, B, 8, npoint, idx, kpts, dc, st);
+        case T1024x4c: return launch_fps<1024, 4>(xyz, d_off, B, max_cluster >= 4 ? 4 : 2, npoint, idx, kpts, dc, st);
+        case T1024x6c: return launch_fps<1024, 6>(xyz, d_off, B, max_cluster >= 4 ? 4 : 2, npoint, idx, kpts, dc, st);
+        case T1024x10c: return launch_fps<1024, 10>(xyz, d_off, B, max_cluster >= 4 ? 4 : 2, npoint, idx, kpts, dc, st);
+        case T1024x12c: return launch_fps<1024, 12>(xyz, d_off, B, max_cluster >= 4 ? 4 : 2, npoint, idx, kpts, dc, st);
+        case T1024x1c16: return launch_fps<1024, 1>(xyz, d_off, B, 16, npoint, idx, kpts, dc, st);
+        case T1024x2c16: return launch_fps<1024, 2>(xyz, d_off, B, 16, npoint, idx, kpts, dc, st);
+        case T1024x2: return launch_fps<1024, 2>(xyz, d_off, B, 8, npoint, idx, kpts, dc, st);
+        case T1024x3: return launch_fps<1024, 3>(xyz, d_off, B, 8, npoint, idx, kpts, dc, st);
+        case T1024x4: return launch_fps<1024, 4>(xyz, d_off, B, 8, npoint, idx, kpts, dc, st);
+        case T1024x8: return launch_fps<1024, 8>(xyz, d_off, B, 8, npoint, idx, kpts, dc, st);
+        case T1024x8c16: return launch_fps<1024, 8>(xyz, d_off, B, 16, npoint, idx, kpts, dc, st);
+        case T512x32: return launch_fps<512, 32>(xyz, d_off, B, 16, npoint, idx, kpts, dc, st);
+        default: return launch_fps<512, 64>(xyz, d_off, B, 16, npoint, idx, kpts, dc, st);
     }
-    { static int cl16 = -1; if (cl16 < 0) { const char *e = getenv("BX_FPS_CL16"); cl16 = e ? atoi(e) : 0; }     // experiment: 16-CTA clusters, fewer points per thread
-      if (cl16 && maxN <= 16384) return launch_fps<1024, 1>(xyz, d_off, B, 16, npoint, idx, kpts, st);
-      if (cl16 && maxN <= 32768) return launch_fps<1024, 2>(xyz, d_off, B, 16, npoint, idx, kpts, st); }
-    if (maxN <= 16384) return launch_fps<1024, 2>(xyz, d_off, B, 8, npoint, idx, kpts, st);
-    if (maxN <= 24576) return launch_fps<1024, 3>(xyz, d_off, B, 8, npoint, idx, kpts, st);
-    if (maxN <= 32768) return launch_fps<1024, 4>(xyz, d_off, B, 8, npoint, idx, kpts, st);
-    if (maxN <= 65536) return launch_fps<1024, 8>(xyz, d_off, B, 8, npoint, idx, kpts, st);
-    if (maxN <= 131072) return launch_fps<1024, 8>(xyz, d_off, B, 16, npoint, idx, kpts, st);
-    // beyond 128 K points per cloud (raw LiDAR sweeps before voxel down-sampling): 512-thread CTAs leave 128 registers per
-    // thread, enough for 32 / 64 points each -- slower per iteration, same result contract
-    if (maxN <= 262144) return launch_fps<512, 32>(xyz, d_off, B, 16, npoint, idx, kpts, st);
-    return launch_fps<512, 64>(xyz, d_off, B, 16, npoint, idx, kpts, st);
+}
+
+// Size class of a cloud of n points: the largest point count whose launch gets the same configuration as n (n <= 0: 0;
+// n > 524288: -1, no launch exists).  Capacity buffers of this size keep the kernel on n's register tier.
+BX_API int bx_fps_size_class(int n, int max_cluster) {
+    if (n <= 0) return 0;
+    if (n > 524288) return -1;
+    int hi;
+    fps_tier(n, max_cluster, &hi);
+    return hi;
 }

@@ -19,9 +19,9 @@
 namespace {
 
 __global__ void permute_cloud_kernel(const float *__restrict__ pts, const int *__restrict__ perm, int N,
-                                     float4 *__restrict__ out) {
+                                     float4 *__restrict__ out, const int *__restrict__ d_N) {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= N) return;
+    if (i >= (d_N ? min(max(*d_N, 0), N) : N)) return;
     const int s = perm ? perm[i] : i;
     out[i] = make_float4(pts[3 * (size_t)s], pts[3 * (size_t)s + 1], pts[3 * (size_t)s + 2], 0.0f);
 }
@@ -154,12 +154,15 @@ struct SpJobs {
     const float *kpts[SP_MAXJOBS];
     const float *d_radius[SP_MAXJOBS];
     const int *d_K[SP_MAXJOBS];           // optional device key-point count of a job (NULL: K)
+    const int *d_N[SP_MAXJOBS];           // optional device point count of a job (NULL: N = the capacity)
     int N[SP_MAXJOBS], K[SP_MAXJOBS], boff[SP_MAXJOBS + 1], koff[SP_MAXJOBS];
     int njobs;
 };
 
 // key-points of a job present this launch: min(*d_K, K), or K without a device count
 __device__ __forceinline__ int sp_count(const int *d_K, int K) { return d_K ? min(max(*d_K, 0), K) : K; }
+// points of a job's permuted cloud present this launch: min(*d_N, N) (at least 1), or N without a device count
+__device__ __forceinline__ int sp_points(const int *d_N, int N) { return d_N ? min(max(*d_N, 1), N) : N; }
 
 __global__ void __launch_bounds__(SP_WARPS * 32)
 select_patches_batched_kernel(const SpJobs jobs, int P, float *__restrict__ patches) {
@@ -167,7 +170,7 @@ select_patches_batched_kernel(const SpJobs jobs, int P, float *__restrict__ patc
     while (j + 1 < jobs.njobs && (int)blockIdx.x >= jobs.boff[j + 1]) ++j;
     const int b = (int)blockIdx.x - jobs.boff[j], Kj = sp_count(jobs.d_K[j], jobs.K[j]);
     if (b * SP_KP >= Kj) return;                          // the whole CTA: before any barrier
-    select_patches_body(jobs.pts4[j], jobs.N[j], jobs.kpts[j], Kj, 0.0f, jobs.d_radius[j], P, nullptr,
+    select_patches_body(jobs.pts4[j], sp_points(jobs.d_N[j], jobs.N[j]), jobs.kpts[j], Kj, 0.0f, jobs.d_radius[j], P, nullptr,
                         patches + (size_t)jobs.koff[j] * P * 3, b);
 }
 
@@ -320,13 +323,14 @@ struct HgJobs {
     float4 *sorted[SP_MAXJOBS];
     int *cnt[SP_MAXJOBS];                 // cnt, start = cnt + HG_CELLS, cursor = start + HG_CELLS + 4
     const int *d_K[SP_MAXJOBS];           // optional device key-point count of a job: 0 skips every phase of the job
+    const int *d_N[SP_MAXJOBS];           // optional device point count of a job (NULL: N = the capacity the workspace is laid out for)
     int N[SP_MAXJOBS], koff[SP_MAXJOBS + 1];
     int njobs;
 };
 __global__ void hg_count_batched_kernel(const HgJobs J) {
     const int j = blockIdx.y;
     if (J.d_K[j] && *J.d_K[j] <= 0) return;
-    hg_count_body(J.pts4[j], J.N[j], J.d_radius[j], J.cnt[j], blockIdx.x * blockDim.x + threadIdx.x);
+    hg_count_body(J.pts4[j], sp_points(J.d_N[j], J.N[j]), J.d_radius[j], J.cnt[j], blockIdx.x * blockDim.x + threadIdx.x);
 }
 __global__ void __launch_bounds__(1024) hg_scan_batched_kernel(const HgJobs J) {
     if (J.d_K[blockIdx.x] && *J.d_K[blockIdx.x] <= 0) return;
@@ -382,14 +386,15 @@ __global__ void __launch_bounds__(HG_SCAN_THREADS) hg_chunkscan_batched_kernel(c
 __global__ void hg_scatter_batched_kernel(const HgJobs J) {
     const int j = blockIdx.y;
     if (J.d_K[j] && *J.d_K[j] <= 0) return;
-    hg_scatter_body(J.pts4[j], J.N[j], J.d_radius[j], J.cnt[j] + 2 * HG_CELLS + 4, J.sorted[j], blockIdx.x * blockDim.x + threadIdx.x);
+    hg_scatter_body(J.pts4[j], sp_points(J.d_N[j], J.N[j]), J.d_radius[j], J.cnt[j] + 2 * HG_CELLS + 4, J.sorted[j],
+                    blockIdx.x * blockDim.x + threadIdx.x);
 }
 __global__ void __launch_bounds__(HG_THREADS) hg_query_batched_kernel(const HgJobs J, int P, float *__restrict__ patches) {
     int j = 0;
     while (j + 1 < J.njobs && (int)blockIdx.x >= J.koff[j + 1]) ++j;
     const int k = (int)blockIdx.x - J.koff[j];
     if (J.d_K[j] && k >= *J.d_K[j]) return;               // the whole CTA: before any barrier
-    hg_query_body(J.pts4[j], J.N[j], J.kpts[j], J.d_radius[j], P, J.cnt[j] + HG_CELLS, J.sorted[j], nullptr,
+    hg_query_body(J.pts4[j], sp_points(J.d_N[j], J.N[j]), J.kpts[j], J.d_radius[j], P, J.cnt[j] + HG_CELLS, J.sorted[j], nullptr,
                   patches + (size_t)J.koff[j] * P * 3, k);
 }
 
@@ -556,9 +561,13 @@ lrf_kernel(const float *__restrict__ patches, int K, int P, float des_r_v, const
 }  // namespace
 
 BX_API int bx_permute_cloud(const float *pts, const int32_t *perm, int N, float *out4, void *stream) {
+    return bx_permute_cloud_n(pts, perm, N, nullptr, out4, stream);
+}
+
+BX_API int bx_permute_cloud_n(const float *pts, const int32_t *perm, int N, const int32_t *d_N, float *out4, void *stream) {
     BX_REQUIRE(pts && out4 && N >= 1, "bx_permute_cloud: bad arguments");
     BX_REQUIRE((reinterpret_cast<uintptr_t>(out4) & 15) == 0, "bx_permute_cloud: out4 must be 16-byte aligned");
-    permute_cloud_kernel<<<(N + 255) / 256, 256, 0, bx_stream(stream)>>>(pts, perm, N, reinterpret_cast<float4 *>(out4));
+    permute_cloud_kernel<<<(N + 255) / 256, 256, 0, bx_stream(stream)>>>(pts, perm, N, reinterpret_cast<float4 *>(out4), d_N);
     BX_LAUNCH_CHECK();
     return BX_OK;
 }
@@ -582,6 +591,12 @@ BX_API int bx_select_patches_batched(int njobs, const void *const *pts4, const i
 
 BX_API int bx_select_patches_batched_n(int njobs, const void *const *pts4, const int32_t *N, const void *const *kpts, const int32_t *K,
                                        const void *const *d_radius, const void *const *d_K, int P, float *patches, void *stream) {
+    return bx_select_patches_batched_counts(njobs, pts4, N, nullptr, kpts, K, d_radius, d_K, P, patches, stream);
+}
+
+BX_API int bx_select_patches_batched_counts(int njobs, const void *const *pts4, const int32_t *N, const void *const *d_N, const void *const *kpts,
+                                            const int32_t *K, const void *const *d_radius, const void *const *d_K, int P, float *patches,
+                                            void *stream) {
     BX_REQUIRE(pts4 && N && kpts && K && d_radius && patches, "bx_select_patches_batched: null pointer");
     BX_REQUIRE(njobs >= 1 && njobs <= SP_MAXJOBS && P >= 1, "bx_select_patches_batched: njobs=%d out of range [1,%d]", njobs, SP_MAXJOBS);
     SpJobs jobs = {};
@@ -594,6 +609,7 @@ BX_API int bx_select_patches_batched_n(int njobs, const void *const *pts4, const
         jobs.kpts[j] = reinterpret_cast<const float *>(kpts[j]);
         jobs.d_radius[j] = reinterpret_cast<const float *>(d_radius[j]);
         jobs.d_K[j] = d_K ? reinterpret_cast<const int *>(d_K[j]) : nullptr;
+        jobs.d_N[j] = d_N ? reinterpret_cast<const int *>(d_N[j]) : nullptr;
         jobs.N[j] = N[j]; jobs.K[j] = K[j];
         jobs.boff[j] = blocks; jobs.koff[j] = koff;
         blocks += (K[j] + SP_KP - 1) / SP_KP;
@@ -650,6 +666,14 @@ BX_API int bx_select_patches_grid_batched(int njobs, const void *const *pts4, co
 BX_API int bx_select_patches_grid_batched_n(int njobs, const void *const *pts4, const int32_t *N, const void *const *kpts, const int32_t *K,
                                             const void *const *d_radius, const void *const *d_K, int P, float *patches, void *workspace,
                                             void *stream) {
+    return bx_select_patches_grid_batched_counts(njobs, pts4, N, nullptr, kpts, K, d_radius, d_K, P, patches, workspace, stream);
+}
+
+// d_N: the device point counts of the jobs (see bx_select_patches_batched_counts).  The workspace, the bitmap and the grids of the
+// point-parallel phases are sized by the capacities N[j]; every phase stops at the count.
+BX_API int bx_select_patches_grid_batched_counts(int njobs, const void *const *pts4, const int32_t *N, const void *const *d_N,
+                                                 const void *const *kpts, const int32_t *K, const void *const *d_radius,
+                                                 const void *const *d_K, int P, float *patches, void *workspace, void *stream) {
     BX_REQUIRE(pts4 && N && kpts && K && d_radius && patches && workspace, "bx_select_patches_grid_batched: null pointer");
     BX_REQUIRE(njobs >= 1 && njobs <= SP_MAXJOBS && P >= 1, "bx_select_patches_grid_batched: njobs=%d out of range [1,%d]", njobs, SP_MAXJOBS);
     BX_REQUIRE((reinterpret_cast<uintptr_t>(workspace) & 15) == 0, "bx_select_patches_grid_batched: workspace must be 16-byte aligned");
@@ -664,6 +688,7 @@ BX_API int bx_select_patches_grid_batched_n(int njobs, const void *const *pts4, 
         J.kpts[j] = reinterpret_cast<const float *>(kpts[j]);
         J.d_radius[j] = reinterpret_cast<const float *>(d_radius[j]);
         J.d_K[j] = d_K ? reinterpret_cast<const int *>(d_K[j]) : nullptr;
+        J.d_N[j] = d_N ? reinterpret_cast<const int *>(d_N[j]) : nullptr;
         J.N[j] = N[j];
         J.sorted[j] = reinterpret_cast<float4 *>(ws);
         J.cnt[j] = reinterpret_cast<int *>(J.sorted[j] + N[j]);

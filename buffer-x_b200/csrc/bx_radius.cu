@@ -21,7 +21,16 @@ constexpr int KT = 500;             // key-points per smem tile (float4 each)
 // hist[m] (m in 0..NB+1) = #{d2 : smallest m with d2 < thr[m]}, bin NB+1 = "d2 == 25".
 __global__ void __launch_bounds__(HT)
 radius_hist_kernel(const float *__restrict__ kpts, int Kr, const float *__restrict__ pts, int N,
-                   uint32_t *__restrict__ hist) {
+                   uint32_t *__restrict__ hist, const float *__restrict__ kpts_t, const float *__restrict__ pts_t, int N_t,
+                   const int *__restrict__ d_counts) {
+    if (d_counts) {     // pair form: the larger cloud by the reference's rule (source iff Ns > Nt), counts clamped to the capacities
+        const int ns = min(max(d_counts[0], 0), N), nt = min(max(d_counts[1], 0), N_t);
+        if (ns > nt) {
+            N = ns;
+        } else {
+            kpts = kpts_t; pts = pts_t; N = nt;
+        }
+    }
     extern __shared__ unsigned char smem_raw[];
     float *thr = reinterpret_cast<float *>(smem_raw);                 // NB+1
     uint32_t *sh = reinterpret_cast<uint32_t *>(thr + (NB + 1));      // NB+2
@@ -75,7 +84,11 @@ struct Thresholds {
 __global__ void __launch_bounds__(1024)
 radius_bisect_kernel(uint32_t *__restrict__ hist, long long denom, const Thresholds thresholds, int n_thr,
                      double tolerance, const float *__restrict__ round_table, float *__restrict__ out_r,
-                     int *__restrict__ out_m) {
+                     int *__restrict__ out_m, const int *__restrict__ d_counts, int cap_s, int cap_t, int Kr) {
+    if (d_counts) {     // pair form: denom = N * Kr of the cloud the histogram was built on
+        const int ns = min(max(d_counts[0], 0), cap_s), nt = min(max(d_counts[1], 0), cap_t);
+        denom = (long long)(ns > nt ? ns : nt) * (long long)Kr;
+    }
     __shared__ uint32_t part[1024];
     const int b0 = threadIdx.x * 9;  // 9 consecutive bins per thread (9*1024 >= NB+1)
     uint32_t loc[9];
@@ -132,12 +145,11 @@ radius_bisect_kernel(uint32_t *__restrict__ hist, long long denom, const Thresho
 
 }  // namespace
 
-BX_API int bx_radius_estimate(const float *kpts, int Kr, const float *pts, int N, int64_t denom,
-                              const double *h_thresholds, int n_thr, double tolerance, const float *round_table,
-                              uint32_t *hist, float *out_r, int32_t *out_m, void *stream) {
-    BX_REQUIRE(kpts && pts && h_thresholds && round_table && hist && out_r, "bx_radius_estimate: null pointer");
-    BX_REQUIRE(Kr >= 1 && N >= 1 && n_thr >= 1 && n_thr <= 16, "bx_radius_estimate: bad sizes Kr=%d N=%d n_thr=%d", Kr, N, n_thr);
-    BX_REQUIRE((int64_t)Kr * (int64_t)N < ((int64_t)1 << 32), "bx_radius_estimate: Kr*N must be < 2^32");
+namespace {
+
+int radius_launch(const float *kpts, int Kr, const float *pts, int N, int64_t denom, const float *kpts_t, const float *pts_t, int N_t,
+                  const int32_t *d_counts, const double *h_thresholds, int n_thr, double tolerance, const float *round_table,
+                  uint32_t *hist, float *out_r, int32_t *out_m, void *stream) {
     cudaStream_t st = bx_stream(stream);
     BX_CUDA(cudaMemsetAsync(hist, 0, sizeof(uint32_t) * (NB + 2), st));
     const size_t smem = sizeof(float) * (NB + 1) + sizeof(uint32_t) * (NB + 3) + sizeof(float4) * KT;
@@ -147,15 +159,42 @@ BX_API int bx_radius_estimate(const float *kpts, int Kr, const float *pts, int N
     int sms = bx_device_sm_count();
     if (sms <= 0) sms = 132;
     const int gy = (Kr + KT - 1) / KT;
-    int gx = (N + HT - 1) / HT;
+    int gx = ((N > N_t ? N : N_t) + HT - 1) / HT;
     const int cap = (4 * sms + gy - 1) / gy;  // ~4 CTAs per SM overall; beyond that grid-stride
     if (gx > cap) gx = cap;
     if (gx < 1) gx = 1;
-    radius_hist_kernel<<<dim3(gx, gy), HT, smem, st>>>(kpts, Kr, pts, N, hist);
+    radius_hist_kernel<<<dim3(gx, gy), HT, smem, st>>>(kpts, Kr, pts, N, hist, kpts_t, pts_t, N_t, d_counts);
     BX_LAUNCH_CHECK();
     Thresholds thr;
     for (int i = 0; i < 16; ++i) thr.v[i] = h_thresholds[i < n_thr ? i : 0];
-    radius_bisect_kernel<<<1, 1024, 0, st>>>(hist, (long long)denom, thr, n_thr, tolerance, round_table, out_r, out_m);
+    radius_bisect_kernel<<<1, 1024, 0, st>>>(hist, (long long)denom, thr, n_thr, tolerance, round_table, out_r, out_m, d_counts, N, N_t, Kr);
     BX_LAUNCH_CHECK();
     return BX_OK;
+}
+
+}  // namespace
+
+BX_API int bx_radius_estimate(const float *kpts, int Kr, const float *pts, int N, int64_t denom,
+                              const double *h_thresholds, int n_thr, double tolerance, const float *round_table,
+                              uint32_t *hist, float *out_r, int32_t *out_m, void *stream) {
+    BX_REQUIRE(kpts && pts && h_thresholds && round_table && hist && out_r, "bx_radius_estimate: null pointer");
+    BX_REQUIRE(Kr >= 1 && N >= 1 && n_thr >= 1 && n_thr <= 16, "bx_radius_estimate: bad sizes Kr=%d N=%d n_thr=%d", Kr, N, n_thr);
+    BX_REQUIRE((int64_t)Kr * (int64_t)N < ((int64_t)1 << 32), "bx_radius_estimate: Kr*N must be < 2^32");
+    return radius_launch(kpts, Kr, pts, N, denom, nullptr, nullptr, 0, nullptr, h_thresholds, n_thr, tolerance, round_table, hist, out_r,
+                         out_m, stream);
+}
+
+// Pair form with device point counts: the histogram is built on the source cloud iff ns > nt (ns, nt = d_counts clamped to the
+// capacities cap_s, cap_t), with denom = N * Kr of that cloud.  The grid is sized by the larger capacity; the counts are
+// integer atomics, so the histogram does not depend on how the points are spread over the CTAs.
+BX_API int bx_radius_estimate_n(const float *kpts_s, const float *pts_s, int cap_s, const float *kpts_t, const float *pts_t, int cap_t,
+                                int Kr, const int32_t *d_counts, const double *h_thresholds, int n_thr, double tolerance,
+                                const float *round_table, uint32_t *hist, float *out_r, int32_t *out_m, void *stream) {
+    BX_REQUIRE(kpts_s && pts_s && kpts_t && pts_t && d_counts && h_thresholds && round_table && hist && out_r,
+               "bx_radius_estimate_n: null pointer");
+    BX_REQUIRE(Kr >= 1 && cap_s >= 1 && cap_t >= 1 && n_thr >= 1 && n_thr <= 16, "bx_radius_estimate_n: bad sizes Kr=%d N=%d/%d n_thr=%d",
+               Kr, cap_s, cap_t, n_thr);
+    BX_REQUIRE((int64_t)Kr * (int64_t)(cap_s > cap_t ? cap_s : cap_t) < ((int64_t)1 << 32), "bx_radius_estimate_n: Kr*N must be < 2^32");
+    return radius_launch(kpts_s, Kr, pts_s, cap_s, 0, kpts_t, pts_t, cap_t, d_counts, h_thresholds, n_thr, tolerance, round_table, hist,
+                         out_r, out_m, stream);
 }

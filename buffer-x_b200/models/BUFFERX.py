@@ -14,7 +14,9 @@ scales_used)``.  Differences that do not change results:
 
 Throughput API on top of the reference surface (CUDA streams + graphs instead of a tracing compiler):
   * ``enable_cuda_graphs(True)``: the enqueue of a pair is captured once per (Ns, Nt, aligned) shape and
-    replayed -- one graph launch instead of ~150 kernel launches;
+    replayed -- one graph launch instead of ~150 kernel launches; with ``size_classes=True`` once per
+    (C_src, C_tgt, aligned) capacity, the true point counts read by the N-dependent kernels from the device, so
+    a stream of pairs of every size replays a handful of graphs;
   * ``forward_async(data_source) -> handle`` / ``handle.result()``: several pairs in flight on separate
     streams (FPS is a latency-bound 16-SM kernel; a second pair's convolutions fill the other SMs).
     With ``cfg.match.enable_early_exit`` the scale-0 RANSAC result gates the later scales on the device
@@ -85,23 +87,30 @@ class _Timer:
 
 
 class _PairSlot:
-    """Static buffers + (optionally) a captured CUDA graph for one (Ns, Nt, aligned, early-exit setting) on its own stream."""
+    """Static buffers + (optionally) a captured CUDA graph for one (C_src, C_tgt, aligned, early-exit setting) on its own
+    stream.  C_src / C_tgt are the capacities of the cloud buffers.  An exact-shape slot (``counted`` False) serves the pairs
+    of exactly that shape and runs the kernels without point counts; a size-class slot (``counted`` True) serves every pair
+    whose clouds fit the capacities: the true counts are copied to the device before each replay and the N-dependent
+    kernels (FPS, radius histogram, permutation, patch gathering) stop at them, so the padding rows are never read."""
 
-    def __init__(self, model, Ns, Nt, aligned, use_graph):
+    def __init__(self, model, Cs, Ct, aligned, use_graph, counted=False):
         cfg = model.config
-        self.model, self.Ns, self.Nt, self.aligned = model, Ns, Nt, aligned
+        self.model, self.Cs, self.Ct, self.aligned, self.counted = model, Cs, Ct, aligned, counted
+        self.n_s, self.n_t = Cs, Ct
         dev = next(model.parameters()).device
         self.dev = dev
         S = cfg.patch.num_scales
         self.stream = torch.cuda.Stream(device=dev)
-        self.src = torch.empty((Ns, 3), dtype=torch.float32, device=dev)
-        self.tgt = torch.empty((Nt, 3), dtype=torch.float32, device=dev)
-        self.perm_s = torch.empty((S, Ns), dtype=torch.int32, device=dev)
-        self.perm_t = torch.empty((S, Nt), dtype=torch.int32, device=dev)
-        self.h_perm_s = torch.empty((S, Ns), dtype=torch.int32).pin_memory()
-        self.h_perm_t = torch.empty((S, Nt), dtype=torch.int32).pin_memory()
-        self.h_src = torch.empty((Ns, 3), dtype=torch.float32).pin_memory()
-        self.h_tgt = torch.empty((Nt, 3), dtype=torch.float32).pin_memory()
+        self.xyz = torch.empty((Cs + Ct, 3), dtype=torch.float32, device=dev)      # both clouds back to back: the FPS input
+        self.src, self.tgt = self.xyz[:Cs], self.xyz[Cs:]
+        self.perm_s = torch.empty((S, Cs), dtype=torch.int32, device=dev)
+        self.perm_t = torch.empty((S, Ct), dtype=torch.int32, device=dev)
+        self.h_perm_s = torch.empty((S, Cs), dtype=torch.int32).pin_memory()
+        self.h_perm_t = torch.empty((S, Ct), dtype=torch.int32).pin_memory()
+        self.h_src = torch.empty((Cs, 3), dtype=torch.float32).pin_memory()
+        self.h_tgt = torch.empty((Ct, 3), dtype=torch.float32).pin_memory()
+        self.counts = torch.tensor([Cs, Ct], dtype=torch.int32, device=dev) if counted else None
+        self.h_counts = torch.empty(2, dtype=torch.int32).pin_memory() if counted else None
         self.h_tail = None
         self.done = torch.cuda.Event()
         self.graph = None
@@ -109,11 +118,11 @@ class _PairSlot:
         self.busy = False
         if use_graph:
             with torch.cuda.device(dev), torch.cuda.stream(self.stream):
-                self.src.zero_(); self.tgt.zero_()
-                base = torch.arange(max(Ns, Nt), dtype=torch.int32, device=dev)
-                self.perm_s.copy_(base[:Ns].expand(S, Ns)); self.perm_t.copy_(base[:Nt].expand(S, Nt))
-                self.src[:, 0] = torch.linspace(1, 2, Ns, device=dev)      # any valid cloud: warm-up sets kernel attributes
-                self.tgt[:, 0] = torch.linspace(1, 2, Nt, device=dev)
+                self.xyz.zero_()
+                base = torch.arange(max(Cs, Ct), dtype=torch.int32, device=dev)
+                self.perm_s.copy_(base[:Cs].expand(S, Cs)); self.perm_t.copy_(base[:Ct].expand(S, Ct))
+                self.src[:, 0] = torch.linspace(1, 2, Cs, device=dev)      # any valid cloud: warm-up sets kernel attributes
+                self.tgt[:, 0] = torch.linspace(1, 2, Ct, device=dev)
                 self._enqueue()                                            # eager warm-up on this stream
             self.stream.synchronize()
             self.graph = torch.cuda.CUDAGraph()
@@ -125,41 +134,56 @@ class _PairSlot:
 
     def _enqueue(self):
         perms = [(self.perm_s[i], self.perm_t[i]) for i in range(self.perm_s.shape[0])]
-        return self.model._enqueue(self.src, self.tgt, self.aligned, perms, None, False, device_exit=True)[0]
+        return self.model._enqueue(self.src, self.tgt, self.aligned, perms, None, False, device_exit=True, counts=self.counts,
+                                   xyz=self.xyz)[0]
 
     def launch(self, data_source, perms):
         """H2D of the inputs (pinned staging when they arrive as host arrays), the pair, D2H of the result."""
+        xs, xt = torch.as_tensor(data_source["src_fds_pcd"]).reshape(-1, 3), torch.as_tensor(data_source["tgt_fds_pcd"]).reshape(-1, 3)
+        n_s, n_t = xs.shape[0], xt.shape[0]
+        if n_s > self.Cs or n_t > self.Ct or (not self.counted and (n_s, n_t) != (self.Cs, self.Ct)):
+            raise ops.BufferXError(f"forward_async: a ({n_s}, {n_t})-point pair does not fit a slot of capacity ({self.Cs}, {self.Ct})")
+        self.n_s, self.n_t = n_s, n_t
         # CUDA inputs may still be in flight on the caller's stream (`.cuda(non_blocking=True)`, a voxel_down_sample
         # kernel): the slot stream starts after everything the caller has enqueued so far, and the caching allocator is
         # told that the slot stream reads them (so the memory is not handed out again before the copy has run).
         self.stream.wait_stream(torch.cuda.current_stream(self.dev))
         with torch.cuda.device(self.dev), torch.cuda.stream(self.stream):
-            for dst, hbuf, x in ((self.src, self.h_src, data_source["src_fds_pcd"]), (self.tgt, self.h_tgt, data_source["tgt_fds_pcd"])):
-                x = torch.as_tensor(x)
+            # only the first n rows are written: the padding of a size-class buffer keeps whatever the last pair left there
+            for dst, hbuf, x in ((self.src[:n_s], self.h_src[:n_s], xs), (self.tgt[:n_t], self.h_tgt[:n_t], xt)):
                 if x.is_cuda:
                     x.record_stream(self.stream)
-                    dst.copy_(x.reshape(-1, 3), non_blocking=True)
+                    dst.copy_(x, non_blocking=True)
                 else:
                     if x.is_pinned():
-                        dst.copy_(x.reshape(-1, 3), non_blocking=True)
+                        dst.copy_(x, non_blocking=True)
                     else:
-                        hbuf.copy_(x.reshape(-1, 3))
+                        hbuf.copy_(x)
                         dst.copy_(hbuf, non_blocking=True)
             S = self.perm_s.shape[0]
+            on_device = perms is not None and isinstance(perms[0][0], torch.Tensor) and perms[0][0].is_cuda
             for i in range(S):
                 if perms is None:   # the reference's host draws, in its order (src then tgt, per scale)
-                    self.h_perm_s[i].copy_(torch.from_numpy(np.random.choice(self.Ns, self.Ns, replace=False).astype(np.int32)))
-                    self.h_perm_t[i].copy_(torch.from_numpy(np.random.choice(self.Nt, self.Nt, replace=False).astype(np.int32)))
+                    self.h_perm_s[i, :n_s].copy_(torch.from_numpy(np.random.choice(n_s, n_s, replace=False).astype(np.int32)))
+                    self.h_perm_t[i, :n_t].copy_(torch.from_numpy(np.random.choice(n_t, n_t, replace=False).astype(np.int32)))
                 else:
                     ps, pt = perms[i]
-                    if isinstance(ps, torch.Tensor) and ps.is_cuda:
+                    if on_device:
                         ps.record_stream(self.stream); pt.record_stream(self.stream)
-                        self.perm_s[i].copy_(ps, non_blocking=True); self.perm_t[i].copy_(pt, non_blocking=True)
+                        self.perm_s[i, :n_s].copy_(ps, non_blocking=True); self.perm_t[i, :n_t].copy_(pt, non_blocking=True)
                         continue
-                    self.h_perm_s[i].copy_(torch.as_tensor(ps, dtype=torch.int32)); self.h_perm_t[i].copy_(torch.as_tensor(pt, dtype=torch.int32))
-            if perms is None or not (isinstance(perms[0][0], torch.Tensor) and perms[0][0].is_cuda):
-                self.perm_s.copy_(self.h_perm_s, non_blocking=True)
-                self.perm_t.copy_(self.h_perm_t, non_blocking=True)
+                    self.h_perm_s[i, :n_s].copy_(torch.as_tensor(ps, dtype=torch.int32)); self.h_perm_t[i, :n_t].copy_(torch.as_tensor(pt, dtype=torch.int32))
+            if not on_device:
+                if (n_s, n_t) == (self.Cs, self.Ct):
+                    self.perm_s.copy_(self.h_perm_s, non_blocking=True)
+                    self.perm_t.copy_(self.h_perm_t, non_blocking=True)
+                else:           # rows of a capacity buffer: the first n entries of each
+                    for i in range(S):
+                        self.perm_s[i, :n_s].copy_(self.h_perm_s[i, :n_s], non_blocking=True)
+                        self.perm_t[i, :n_t].copy_(self.h_perm_t[i, :n_t], non_blocking=True)
+            if self.counted:
+                self.h_counts[0], self.h_counts[1] = n_s, n_t
+                self.counts.copy_(self.h_counts, non_blocking=True)
             if self.graph is not None:
                 self.graph.replay()
                 tail = self.tail
@@ -175,8 +199,9 @@ class _PairSlot:
         self.busy = False
         out = self.model._decode(self.h_tail.clone(), [0.0, 0.0, 0.0])
         if self.model._overflow:            # an activation left fp16 range: this pair is recomputed on the TF32 kernel
-            return self.model._rerun_tf32(dict(src_fds_pcd=self.src.clone(), tgt_fds_pcd=self.tgt.clone(), is_aligned_to_global_z=self.aligned),
-                                          [(self.perm_s[i].clone(), self.perm_t[i].clone()) for i in range(self.perm_s.shape[0])], None)
+            n_s, n_t = self.n_s, self.n_t   # the exact clouds and permutations, not the capacity buffers
+            return self.model._rerun_tf32(dict(src_fds_pcd=self.src[:n_s].clone(), tgt_fds_pcd=self.tgt[:n_t].clone(), is_aligned_to_global_z=self.aligned),
+                                          [(self.perm_s[i, :n_s].clone(), self.perm_t[i, :n_t].clone()) for i in range(self.perm_s.shape[0])], None)
         return out
 
 
@@ -194,6 +219,7 @@ class BufferX(nn.Module):
         self._use_graphs = False
         self._slots = {}
         self._slots_per_shape = 2
+        self._size_classes = False
         self._fps_cluster = 0        # > 0: throughput form of the FPS kernel (ops.fps max_cluster), chosen by enable_cuda_graphs
         self._rr = {}
 
@@ -246,10 +272,21 @@ class BufferX(nn.Module):
         return T.view(1, 4, 4)
 
     # ------------------------------------------------------------------------------------------------
-    def enable_cuda_graphs(self, flag=True, slots_per_shape=2):
-        """Capture the per-pair enqueue once per (Ns, Nt, aligned) shape and replay it (no effect on results)."""
+    def enable_cuda_graphs(self, flag=True, slots_per_shape=2, size_classes=False):
+        """Capture the per-pair enqueue once per slot key and replay it (no effect on results); ``forward`` then runs through
+        the same slots as ``forward_async`` (unless early exit, timing or debug is on).
+
+        ``size_classes=False``: slots are keyed by the exact (Ns, Nt, aligned) shape (plus the early-exit setting), so a stream
+        whose pairs all differ in size captures a graph for almost every pair.  ``size_classes=True``: each cloud is given a
+        capacity, its size class (``ops.fps_size_class``: the largest point count with the same FPS launch configuration),
+        slots are keyed by (C_src, C_tgt, aligned) and every pair whose clouds fit replays the class graph with its true
+        point counts on the device -- results bit-identical to the exact-shape route.  A pair whose larger cloud has more
+        than 200000 points keeps an exact-shape slot (the reference sub-samples such a cloud with a draw sized by N).
+        ``slots_per_shape`` slots (pairs in flight) are kept per key.  These options also apply to ``forward_async``
+        without graphs."""
         self._use_graphs = bool(flag)
         self._slots_per_shape = int(slots_per_shape)
+        self._size_classes = bool(size_classes)
         # three or more pairs in flight: the key-point sampling of a pair runs beside the other pairs' convolutions; bx_fps_ex offers
         # a 2- / 4-CTA-per-cloud form (fewer SMs, longer)
         # (what the other streams lose is governed by how LONG the sampling holds its SMs, not by how many, so the default stays
@@ -271,22 +308,38 @@ class BufferX(nn.Module):
         m = self.config.match
         return (True, int(m.get("early_exit_min_inliers", 15))) if m.get("enable_early_exit", True) else (False, None)
 
-    MAX_GRAPH_SHAPES = 8      # graphs are per (Ns, Nt, aligned) shape; least recently used shapes are dropped beyond this
+    MAX_GRAPH_SHAPES = 8      # graphs are per slot key; least recently used keys are dropped beyond this
+    MAX_CLASS_POINTS = 200000  # larger clouds are sub-sampled by a draw sized by N (reference BUFFERX.py:664-665): exact slots
+
+    def _slot_key(self, Ns, Nt, aligned):
+        """(slot key, capacities, counted) of a pair.  The early-exit threshold is baked into a captured gate launch: a
+        graph is never replayed under another setting."""
+        if self._size_classes and max(Ns, Nt) <= self.MAX_CLASS_POINTS:
+            Cs, Ct = ops.fps_size_class(Ns, self._fps_cluster), ops.fps_size_class(Nt, self._fps_cluster)
+            return (Cs, Ct, bool(aligned)) + self._exit_key(), Cs, Ct, True
+        return (Ns, Nt, bool(aligned)) + self._exit_key(), Ns, Nt, False
+
+    def _evict(self, key):
+        pe = getattr(self, "pose_estimator", None)
+        for sl in self._slots[key]:
+            if pe is not None and hasattr(pe, "_ws"):
+                pe._ws.pop((str(sl.dev), sl.stream.cuda_stream), None)
+        del self._slots[key]
+        self._rr.pop(key, None)
 
     def _slot(self, Ns, Nt, aligned):
-        # the early-exit threshold is baked into a captured gate launch: a graph is never replayed under another setting
-        key = (Ns, Nt, bool(aligned)) + self._exit_key()
+        key, Cs, Ct, counted = self._slot_key(Ns, Nt, aligned)
+        if key in self._slots and any(sl.counted != counted for sl in self._slots[key]):
+            # an exact shape above MAX_CLASS_POINTS that equals a size class: the two kinds of slot never share a key
+            if any(sl.busy for sl in self._slots[key]):
+                raise ops.BufferXError("forward_async: collect the pending results before launching this pair")
+            self._evict(key)
         if key not in self._slots and len(self._slots) >= self.MAX_GRAPH_SHAPES:
             # datasets with a different size for every pair would otherwise pin one set of graph pools per pair; for
-            # those, run eager (`enable_cuda_graphs(False)`) or pad/bucket the clouds upstream
+            # those, use size classes (`enable_cuda_graphs(True, size_classes=True)`)
             for old in list(self._slots):
                 if all(not sl.busy for sl in self._slots[old]):
-                    pe = getattr(self, "pose_estimator", None)
-                    for sl in self._slots[old]:
-                        if pe is not None and hasattr(pe, "_ws"):
-                            pe._ws.pop((str(sl.dev), sl.stream.cuda_stream), None)
-                    del self._slots[old]
-                    self._rr.pop(old, None)
+                    self._evict(old)
                     break
         else:
             if key in self._slots:          # keep insertion order = recency order
@@ -294,7 +347,7 @@ class BufferX(nn.Module):
         lst = self._slots.setdefault(key, [])
         i = self._rr.get(key, 0)
         if len(lst) < self._slots_per_shape:
-            lst.append(_PairSlot(self, Ns, Nt, aligned, self._use_graphs))
+            lst.append(_PairSlot(self, Cs, Ct, aligned, self._use_graphs, counted))
             slot = lst[-1]
         else:
             slot = lst[i % len(lst)]
@@ -305,7 +358,10 @@ class BufferX(nn.Module):
 
     def forward_async(self, data_source, perms=None):
         """Enqueue one pair on a slot stream; returns a handle whose ``result()`` is the forward tuple.  Without ``perms`` the
-        2*S permutations are drawn from NumPy's global RNG at launch, also when early exit stops the pair after scale 0."""
+        2*S permutations are drawn from NumPy's global RNG at launch, also when early exit stops the pair after scale 0.
+        The slot is chosen by the pair's shape, or by its clouds' size classes after
+        ``enable_cuda_graphs(..., size_classes=True)``; either way the result is that of eager ``forward`` with the same
+        ``perms``."""
         if self.config.test.get("enable_timing", False):
             raise ops.BufferXError("forward_async needs timing disabled (the per-stage timers require host round trips)")
         Ns = int(np.prod(data_source["src_fds_pcd"].shape[:-1]))
@@ -313,9 +369,12 @@ class BufferX(nn.Module):
         return self._slot(Ns, Nt, bool(data_source["is_aligned_to_global_z"])).launch(data_source, perms)
 
     # ------------------------------------------------------------------------------------------------
-    def _enqueue(self, src, tgt, aligned, perms, ransac_seed, debug, timers=None, device_exit=False):
+    def _enqueue(self, src, tgt, aligned, perms, ransac_seed, debug, timers=None, device_exit=False, counts=None, xyz=None):
         """Everything of one pair on the current stream, no host synchronisation unless early exit is on and the decision is
-        the host's (``device_exit`` False: ``forward``).  Returns (tail block on the device, debug dict)."""
+        the host's (``device_exit`` False: ``forward``).  Returns (tail block on the device, debug dict).
+        ``counts`` (size-class slots): [2] int32 CUDA point counts; src / tgt are then capacity buffers whose first counts
+        rows are the clouds, and ``perms`` rows likewise (clouds of at most MAX_CLASS_POINTS points).  ``xyz``: src and tgt
+        back to back, when the caller holds them so (saves the concatenation before FPS)."""
         cfg = self.config
         dev = src.device
         Ns, Nt = src.shape[0], tgt.shape[0]
@@ -327,19 +386,26 @@ class BufferX(nn.Module):
         azi_n = cfg.patch.azi_n
         desc_t, pose_t, opt_t = timers if timers is not None else (_Timer(False), _Timer(False), _Timer(False))
 
+        assert counts is None or not debug
+        npts = None if counts is None else [counts[0:1], counts[1:2]] * S      # per descriptor job: (src, tgt) per scale
+
         desc_t.tic()
         # ---- key-points: one FPS per cloud, both clouds in one launch --------------------------------
-        xyz = torch.cat([src, tgt], dim=0)
+        if xyz is None:
+            xyz = torch.cat([src, tgt], dim=0)
         nfps = max(Kr, K)
-        fidx, fk = ops.fps(xyz, [0, Ns, Ns + Nt], nfps, max_cluster=self._fps_cluster)
+        fidx, fk = ops.fps(xyz, [0, Ns, Ns + Nt], nfps, max_cluster=self._fps_cluster, d_counts=counts)
         kpts1, kpts2 = fk[0, :Kr].contiguous(), fk[1, :Kr].contiguous()
         src_kpts, tgt_kpts = fk[0, :K].contiguous(), fk[1, :K].contiguous()
         # ---- density-aware radii of every scale from one histogram ------------------------------------
-        pts_r, kpts_r = (src, kpts1) if Ns > Nt else (tgt, kpts2)
-        denom = pts_r.shape[0] * Kr
-        if pts_r.shape[0] > 200000:  # reference BUFFERX.py:664-665 (denominator keeps the original size)
-            pts_r = pts_r[torch.randint(0, pts_r.shape[0], (200000,), device=dev)].contiguous()
-        r_dev, m_dev, _ = ops.radius_estimate(kpts_r, pts_r, thresholds, denom=denom)
+        if counts is not None:      # the device picks the larger cloud from the counts (clouds of at most 200000 points)
+            r_dev, m_dev, _ = ops.radius_estimate_pair(kpts1, src, kpts2, tgt, thresholds, counts)
+        else:
+            pts_r, kpts_r = (src, kpts1) if Ns > Nt else (tgt, kpts2)
+            denom = pts_r.shape[0] * Kr
+            if pts_r.shape[0] > 200000:  # reference BUFFERX.py:664-665 (denominator keeps the original size)
+                pts_r = pts_r[torch.randint(0, pts_r.shape[0], (200000,), device=dev)].contiguous()
+            r_dev, m_dev, _ = ops.radius_estimate(kpts_r, pts_r, thresholds, denom=denom)
         desc_t.toc()
 
         maxMc = S * K
@@ -350,7 +416,8 @@ class BufferX(nn.Module):
         offs = torch.zeros(S + 1, dtype=torch.int32, device=dev)
         dbg = dict(scales=[]) if debug else None
         if enable_early_exit and device_exit and not debug:
-            tail = self._enqueue_device_exit(src, tgt, aligned, perms, ransac_seed, src_kpts, tgt_kpts, r_dev, R_acc, t_acc, ss_acc, tt_acc, offs)
+            tail = self._enqueue_device_exit(src, tgt, aligned, perms, ransac_seed, src_kpts, tgt_kpts, r_dev, R_acc, t_acc, ss_acc, tt_acc, offs,
+                                             npts)
             return tail, None
 
         scales_used = 0
@@ -374,7 +441,7 @@ class BufferX(nn.Module):
                     if not pm.is_cuda or pm.dtype != torch.int32:
                         pm = pm.to(dev, dtype=torch.int32, non_blocking=True)
                     jobs.append((pts_c, k_c, r_dev[i:i + 1], pm))
-            batched = self.Desc.forward_multi(jobs, aligned, radii=r_dev)
+            batched = self.Desc.forward_multi(jobs, aligned, radii=r_dev, npts=npts)
             desc_t.toc()
         if batched is not None and S <= 8:
             # all scales at once: per-scale mutual matching into rows of one [S,K] buffer, one concatenation kernel
@@ -451,7 +518,8 @@ class BufferX(nn.Module):
             dbg.update(fps_idx=fidx, kpts=fk, des_r=r_dev, des_m=m_dev, ss=ss_acc, tt=tt_acc, R=R_acc, t=t_acc)
         return tail, dbg
 
-    def _enqueue_device_exit(self, src, tgt, aligned, perms, ransac_seed, src_kpts, tgt_kpts, r_dev, R_acc, t_acc, ss_acc, tt_acc, offs):
+    def _enqueue_device_exit(self, src, tgt, aligned, perms, ransac_seed, src_kpts, tgt_kpts, r_dev, R_acc, t_acc, ss_acc, tt_acc, offs,
+                             npts=None):
         """Early exit decided on the device (forward_async / graphs): scale 0 on the batched route up to its RANSAC,
         bx_early_exit_gate turns the result into the key-point counts of scales 1..S-1 (K to continue, 0 to exit), and those
         scales' descriptors, matches, CostNet rows and hypotheses are sized by the counts and appended behind scale 0's.  On
@@ -476,7 +544,7 @@ class BufferX(nn.Module):
         t_lists = torch.empty((S, K), dtype=torch.int32, device=dev)
         cnts = torch.zeros(S, dtype=torch.int32, device=dev)
         # ---- scale 0: descriptors, matches, CostNet, hypotheses, consensus, RANSAC -------------------------------------
-        d0 = self.Desc.forward_multi(jobs[:2], aligned, radii=r_dev[0:1])
+        d0 = self.Desc.forward_multi(jobs[:2], aligned, radii=r_dev[0:1], npts=None if npts is None else npts[:2])
         m0 = self.Desc.last_multi
         ops.mutual_nn(d0[0]["desc"], d0[1]["desc"], out=(s_lists[0], t_lists[0], cnts[0:1]))
         s0, t0 = ops.concat_matches(s_lists[:1], t_lists[:1], cnts[:1], [0], [K], offs[0:2])
@@ -493,7 +561,8 @@ class BufferX(nn.Module):
         if G > 0:
             # ---- scales 1..S-1, sized by the counts (nothing is computed on exit) ---------------------------------
             d1 = self.Desc.forward_multi(jobs[2:], aligned, radii=r_dev[1:],
-                                         counts=dict(job=counts[0:1], group=counts[1:1 + G], total=counts[1 + G:2 + G]))
+                                         counts=dict(job=counts[0:1], group=counts[1:1 + G], total=counts[1 + G:2 + G]),
+                                         npts=None if npts is None else npts[2:])
             m1 = self.Desc.last_multi
             for i in range(1, S):
                 ops.mutual_nn(d1[2 * i - 2]["desc"], d1[2 * i - 1]["desc"], out=(s_lists[i], t_lists[i], cnts[i:i + 1]),

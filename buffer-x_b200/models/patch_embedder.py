@@ -118,7 +118,7 @@ class MiniSpinNet(nn.Module):
                        x=ops.from_blocked(x).view(K, -1, self.ele_n, self.azi_n))
         return out
 
-    def forward_multi(self, jobs, is_aligned_to_global_z, radii=None, counts=None):
+    def forward_multi(self, jobs, is_aligned_to_global_z, radii=None, counts=None, npts=None):
         """Descriptors of several (cloud, key-points, radius, permutation) jobs in ONE pass through SPT, the
         convolution stack and the pooling layer (all CTA-per-patch kernels: batching the 2 x num_scales calls of a
         pair removes five of six launch tails and wave-quantisation losses).  Per-job results are views into the
@@ -127,7 +127,10 @@ class MiniSpinNet(nn.Module):
         ``counts`` (early-exit pairs: the later scales' work sized on the device, see BufferX._enqueue_device_exit): a dict of
         int32 CUDA tensors, "job" [1] = key-points of every job, "group" [len(radii)] = patches of every radius group, "total" [1]
         = patches of the batch (jobs of equal size, (src, tgt) per radius).  Patches beyond them are not computed and their
-        result rows are undefined."""
+        result rows are undefined.
+        ``npts`` (size-class slots, see BufferX.enable_cuda_graphs): one 1-element int32 CUDA tensor per job, the points of its
+        cloud; pts and perm are then capacity buffers whose first npts[j] entries hold the cloud and its permutation, and the
+        scan / hash-grid choice follows the capacity.  Results are those of the exact clouds."""
         dev = jobs[0][0].device
         prep = self.prepared(dev)
         P = self.patch_sample
@@ -145,9 +148,11 @@ class MiniSpinNet(nn.Module):
         one_sel = len(jobs) <= 16 and all(isinstance(j[2], torch.Tensor) for j in jobs)   # all patch gatherings of the pair in one launch
         if counts is not None and not (one_lrf and one_sel):
             raise ops.BufferXError("forward_multi: device-side counts need equal-size (src, tgt) jobs per radius and device radii")
+        if npts is not None and not one_sel:
+            raise ops.BufferXError("forward_multi: device-side point counts need device radii and at most 16 jobs")
         sel = []
-        for (pts, kpts, des_r, perm), K in zip(jobs, Ks):
-            sel.append((ops.permute_cloud(pts.contiguous(), perm), kpts.contiguous(), des_r))
+        for j, ((pts, kpts, des_r, perm), K) in enumerate(zip(jobs, Ks)):
+            sel.append((ops.permute_cloud(pts.contiguous(), perm, d_N=None if npts is None else npts[j]), kpts.contiguous(), des_r))
             Rs.append(R_all[o:o + K])
             axes.append(ra_all[o:o + K])
             o += K
@@ -156,12 +161,13 @@ class MiniSpinNet(nn.Module):
         big = [pts4.shape[0] >= ops.GRID_MIN_POINTS for (pts4, _, _) in sel]
         job_cnt = None if counts is None else [counts["job"]] * len(jobs)
         if one_sel and (all(big) or not any(big)):
-            ops.select_patches_batched(sel, P, patches, grid=all(big), d_K=job_cnt)
+            ops.select_patches_batched(sel, P, patches, grid=all(big), d_K=job_cnt, d_N=npts)
         o = 0
         for j, ((pts4, kpts, des_r), K) in enumerate(zip(sel, Ks)):
             if not (one_sel and (all(big) or not any(big))):
-                if counts is not None:      # job by job, each with its device count
-                    ops.select_patches_batched([(pts4, kpts, des_r)], P, patches[o:o + K], grid=big[j], d_K=job_cnt[:1])
+                if counts is not None or npts is not None:      # job by job, each with its device counts
+                    ops.select_patches_batched([(pts4, kpts, des_r)], P, patches[o:o + K], grid=big[j],
+                                               d_K=None if job_cnt is None else job_cnt[:1], d_N=None if npts is None else npts[j:j + 1])
                 elif big[j] and isinstance(des_r, torch.Tensor):
                     ops.select_patches_grid(pts4, kpts, des_r, P, patches=patches[o:o + K])
                 else:

@@ -27,6 +27,8 @@ SYMBOLS = [
     "bx_gt_matches", "bx_so2_augment", "bx_equi_match", "bx_so2_gt",
     "bx_select_patches_batched_n", "bx_select_patches_grid_batched_n", "bx_lrf_batched_n", "bx_spt_pnt_sd_n", "bx_pool_desc_n",
     "bx_mutual_nn_n", "bx_early_exit_gate",
+    "bx_fps_n", "bx_fps_size_class", "bx_radius_estimate_n", "bx_permute_cloud_n", "bx_select_patches_batched_counts",
+    "bx_select_patches_grid_batched_counts",
 ]
 
 GEOM_CYL3D, GEOM_CYL2D, GEOM_VALID3D, GEOM_COSTAB = 0, 1, 2, 4
@@ -59,6 +61,12 @@ def load_library():
     P = c_void_p
     lib.bx_fps.argtypes = [P, P, c_int, c_int, P, P, P]
     lib.bx_fps_ex.argtypes = [P, P, c_int, c_int, P, P, c_int, P]
+    lib.bx_fps_n.argtypes = [P, P, c_int, c_int, P, P, c_int, P, P]
+    lib.bx_fps_size_class.argtypes = [c_int, c_int]
+    lib.bx_radius_estimate_n.argtypes = [P, P, c_int, P, P, c_int, c_int, P, P, c_int, c_double, P, P, P, P, P]
+    lib.bx_permute_cloud_n.argtypes = [P, P, c_int, P, P, P]
+    lib.bx_select_patches_batched_counts.argtypes = [c_int, P, P, P, P, P, P, P, c_int, P, P]
+    lib.bx_select_patches_grid_batched_counts.argtypes = [c_int, P, P, P, P, P, P, P, c_int, P, P, P]
     lib.bx_radius_estimate.argtypes = [P, c_int, P, c_int, c_int64, P, c_int, c_double, P, P, P, P, P]
     lib.bx_permute_cloud.argtypes = [P, P, c_int, P, P]
     lib.bx_select_patches.argtypes = [P, c_int, P, c_int, c_float, P, c_int, P, P, P]
@@ -186,17 +194,28 @@ class _Span:
         return False
 
 
-def fps(xyz: torch.Tensor, offsets, npoint: int, want_kpts=True, max_cluster=0):
+def fps(xyz: torch.Tensor, offsets, npoint: int, want_kpts=True, max_cluster=0, d_counts=None):
     """xyz [sumN,3] f32 cuda; offsets: host sequence of B+1 ints.  Returns idx [B,npoint] i32, kpts [B,npoint,3].
-    max_cluster 2 / 4: throughput form (fewer SMs per cloud, same indices)."""
+    max_cluster 2 / 4: throughput form (fewer SMs per cloud, same indices).  d_counts: optional [B] int32 CUDA tensor of
+    point counts; the offsets then give each cloud's capacity and cloud b is its first min(d_counts[b], capacity) points."""
     lib = load_library()
     off = np.ascontiguousarray(offsets, dtype=np.int32)
     B = len(off) - 1
     idx = torch.empty((B, npoint), dtype=I32, device=xyz.device)
     kp = torch.empty((B, npoint, 3), dtype=F32, device=xyz.device) if want_kpts else None
     with _Span("fps"):
-        _check(lib.bx_fps_ex(_dp(xyz, F32, "xyz"), off.ctypes.data_as(c_void_p), B, npoint, _dp(idx), _dp(kp), int(max_cluster), _stream()), "bx_fps")
+        if d_counts is None:
+            _check(lib.bx_fps_ex(_dp(xyz, F32, "xyz"), off.ctypes.data_as(c_void_p), B, npoint, _dp(idx), _dp(kp), int(max_cluster), _stream()), "bx_fps")
+        else:
+            assert d_counts.numel() >= B
+            _check(lib.bx_fps_n(_dp(xyz, F32, "xyz"), off.ctypes.data_as(c_void_p), B, npoint, _dp(idx), _dp(kp), int(max_cluster),
+                                _dp(d_counts, I32, "d_counts"), _stream()), "bx_fps_n")
     return idx, kp
+
+
+def fps_size_class(n: int, max_cluster=0) -> int:
+    """The largest point count that gets the same FPS launch configuration as an n-point cloud (-1 above the FPS limit)."""
+    return int(load_library().bx_fps_size_class(int(n), int(max_cluster)))
 
 
 _round_tables = {}
@@ -227,11 +246,35 @@ def radius_estimate(kpts: torch.Tensor, pts: torch.Tensor, thresholds, denom=Non
     return out_r, out_m, hist
 
 
-def permute_cloud(pts: torch.Tensor, perm: torch.Tensor | None, out4: torch.Tensor | None = None):
+def radius_estimate_pair(kpts_s, pts_s, kpts_t, pts_t, thresholds, d_counts, tolerance=0.01, hist=None):
+    """Both clouds (capacity buffers) and their [Kr,3] key-points, d_counts [2] int32 CUDA = (ns, nt): the device picks the
+    larger cloud (source iff ns > nt) and denom = N * Kr.  Returns (r, m, hist) like radius_estimate."""
+    lib = load_library()
+    th = np.ascontiguousarray(thresholds, dtype=np.float64)
+    Kr = kpts_s.shape[0]
+    assert kpts_t.shape[0] == Kr
+    dev = pts_s.device
+    if hist is None:
+        hist = torch.empty(RADIUS_BINS + 2, dtype=I32, device=dev)
+    out_r = torch.empty(len(th), dtype=F32, device=dev)
+    out_m = torch.empty(len(th), dtype=I32, device=dev)
+    _check(lib.bx_radius_estimate_n(_dp(kpts_s, F32, "kpts_s"), _dp(pts_s, F32, "pts_s"), pts_s.shape[0], _dp(kpts_t, F32, "kpts_t"),
+                                    _dp(pts_t, F32, "pts_t"), pts_t.shape[0], Kr, _dp(d_counts, I32, "d_counts"), th.ctypes.data_as(c_void_p),
+                                    len(th), float(tolerance), _dp(radius_round_table(dev)), _dp(hist), _dp(out_r), _dp(out_m), _stream()),
+           "bx_radius_estimate_n")
+    return out_r, out_m, hist
+
+
+def permute_cloud(pts: torch.Tensor, perm: torch.Tensor | None, out4: torch.Tensor | None = None, d_N=None):
+    """d_N: optional 1-element int32 CUDA point count; rows of out4 from the count on are left untouched."""
     N = pts.shape[0]
     if out4 is None:
         out4 = torch.empty((N, 4), dtype=F32, device=pts.device)
-    _check(load_library().bx_permute_cloud(_dp(pts, F32, "pts"), _dp(perm, I32, "perm"), N, _dp(out4), _stream()), "bx_permute_cloud")
+    if d_N is None:
+        _check(load_library().bx_permute_cloud(_dp(pts, F32, "pts"), _dp(perm, I32, "perm"), N, _dp(out4), _stream()), "bx_permute_cloud")
+    else:
+        _check(load_library().bx_permute_cloud_n(_dp(pts, F32, "pts"), _dp(perm, I32, "perm"), N, _dp(d_N, I32, "d_N"), _dp(out4), _stream()),
+               "bx_permute_cloud_n")
     return out4
 
 
@@ -272,10 +315,11 @@ def select_patches_grid(pts4: torch.Tensor, kpts: torch.Tensor, radius: torch.Te
     return patches, idx
 
 
-def select_patches_batched(jobs, P: int, patches: torch.Tensor, grid=False, d_K=None):
+def select_patches_batched(jobs, P: int, patches: torch.Tensor, grid=False, d_K=None, d_N=None):
     """jobs: [(pts4 [N,4], kpts [K,3], radius 1-element CUDA tensor)]; patches [sum K, P, 3] is filled job after job by ONE launch
     (grid=True: the hash-grid form, one launch per phase).  d_K: optional per-job 1-element int32 CUDA tensors (or None
-    entries): job j gathers only its first min(d_K[j], K_j) key-points."""
+    entries): job j gathers only its first min(d_K[j], K_j) key-points.  d_N: the same for points: pts4 of job j is then a
+    capacity buffer whose first min(d_N[j], N_j) rows are the permuted cloud."""
     import ctypes
     n = len(jobs)
     VP, I = ctypes.c_void_p * n, ctypes.c_int32 * n
@@ -283,6 +327,7 @@ def select_patches_batched(jobs, P: int, patches: torch.Tensor, grid=False, d_K=
     kps = VP(*[_dp(j[1], F32, "kpts") for j in jobs])
     rad = VP(*[_dp(j[2], F32, "radius") for j in jobs])
     cnt = None if d_K is None else VP(*[_dp(c, I32, "d_K") for c in d_K])
+    npt = None if d_N is None else VP(*[_dp(c, I32, "d_N") for c in d_N])
     Ns, Ks = I(*[int(j[0].shape[0]) for j in jobs]), I(*[int(j[1].shape[0]) for j in jobs])
     assert patches.shape[0] == sum(Ks) and patches.is_contiguous()
     lib = load_library()
@@ -290,9 +335,15 @@ def select_patches_batched(jobs, P: int, patches: torch.Tensor, grid=False, d_K=
     if grid:
         ws = torch.empty(sum(int(lib.bx_select_patches_grid_workspace_bytes(int(a))) for a in Ns) // 4, dtype=I32, device=patches.device)
     with _Span("select_patches", sum(16.0 * a + 12.0 * b + b * P * 12.0 for a, b in zip(Ns, Ks))):
-        if grid:
+        if grid and npt is not None:
+            _check(lib.bx_select_patches_grid_batched_counts(n, pts, Ns, npt, kps, Ks, rad, cnt, P, _dp(patches, F32, "patches"), _dp(ws),
+                                                             _stream()), "bx_select_patches_grid_batched_counts")
+        elif grid:
             _check(lib.bx_select_patches_grid_batched_n(n, pts, Ns, kps, Ks, rad, cnt, P, _dp(patches, F32, "patches"), _dp(ws), _stream()),
                    "bx_select_patches_grid_batched")
+        elif npt is not None:
+            _check(lib.bx_select_patches_batched_counts(n, pts, Ns, npt, kps, Ks, rad, cnt, P, _dp(patches, F32, "patches"), _stream()),
+                   "bx_select_patches_batched_counts")
         else:
             _check(lib.bx_select_patches_batched_n(n, pts, Ns, kps, Ks, rad, cnt, P, _dp(patches, F32, "patches"), _stream()), "bx_select_patches_batched")
     return patches

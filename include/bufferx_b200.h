@@ -54,6 +54,17 @@ int bx_fps(const float *xyz, const int32_t *h_offsets, int B, int npoint, int32_
  * pairs in flight (0 = bx_fps).  Identical indices. */
 int bx_fps_ex(const float *xyz, const int32_t *h_offsets, int B, int npoint, int32_t *idx, float *kpts, int max_cluster,
               void *stream);
+/* With device-side point counts (size-class buffers: one captured launch serves every cloud up to a capacity).  h_offsets
+ * give each cloud's first point and its CAPACITY (h_offsets[b+1] - h_offsets[b]); cloud b holds its first
+ * n_b = min(max(d_counts[b], 1), capacity) points, and points beyond n_b are never read.  The launch configuration and
+ * the grid follow the capacities; indices and key-points are those of bx_fps_ex on the n_b-point clouds (the tie rule's
+ * block size bs is derived from n_b).  d_counts NULL = bx_fps_ex. */
+int bx_fps_n(const float *xyz, const int32_t *h_offsets, int B, int npoint, int32_t *idx, float *kpts, int max_cluster,
+             const int32_t *d_counts, void *stream);
+/* Size class of an n-point cloud: the largest point count that gets the same FPS launch configuration (register tier,
+ * CTAs per cloud) as n under this max_cluster -- the capacity whose buffers keep the kernel on n's tier.  0 for n <= 0,
+ * -1 above the 524288-point limit. */
+int bx_fps_size_class(int n, int max_cluster);
 /* Switch for the FPS cluster exchange: 0 = st.async + transaction-count mbarrier (production), 1 = cluster.sync() per iteration
  * (racecheck-clean reference form), 2 = remote stores + remote mbarrier arrive / acquire wait (round 1), -1 = BX_FPS_SYNC
  * environment variable.  Same results in every mode.  Returns the old value. */
@@ -70,6 +81,14 @@ int bx_fps_set_sync_mode(int mode);
 int bx_radius_estimate(const float *kpts, int Kr, const float *pts, int N, int64_t denom,
                        const double *h_thresholds, int n_thr, double tolerance, const float *round_table,
                        uint32_t *hist, float *out_r, int32_t *out_m, void *stream);
+/* Pair form with device-side point counts: both clouds (capacities cap_s, cap_t) and both key-point sets ([Kr,3] each);
+ * d_counts [2] (device, required) = (ns, nt), clamped to the capacities.  The device picks the source iff ns > nt (the
+ * reference's rule, models/BUFFERX.py:654) and uses denom = N * Kr of the chosen cloud; points beyond a count are never
+ * read.  Same radii and m as bx_radius_estimate on the chosen exact cloud.  No sub-sampling: the reference draws 200000
+ * points of a larger cloud, which needs N on the host (callers keep such clouds on bx_radius_estimate). */
+int bx_radius_estimate_n(const float *kpts_s, const float *pts_s, int cap_s, const float *kpts_t, const float *pts_t, int cap_t,
+                         int Kr, const int32_t *d_counts, const double *h_thresholds, int n_thr, double tolerance,
+                         const float *round_table, uint32_t *hist, float *out_r, int32_t *out_m, void *stream);
 
 /* ---- a3: order-preserving radius-neighbour patch gathering ----------------------------------
  * Replaces MiniSpinNet.select_patches (models/patch_embedder.py:92-120) =
@@ -80,6 +99,9 @@ int bx_radius_estimate(const float *kpts, int Kr, const float *pts, int N, int64
  * with d2 < r*r; r = *d_radius if d_radius != NULL else `radius`.
  * idx: [K,P] int32 raw ball-query indices (may be NULL); patches: [K,P,3]. */
 int bx_permute_cloud(const float *pts, const int32_t *perm, int N, float *out4, void *stream);
+/* With a device-side point count (d_N NULL = bx_permute_cloud): rows i < min(*d_N, N) are written, the others left
+ * untouched; perm entries beyond the count are never read.  The grid is sized by the capacity N. */
+int bx_permute_cloud_n(const float *pts, const int32_t *perm, int N, const int32_t *d_N, float *out4, void *stream);
 int bx_select_patches(const float *pts4, int N, const float *kpts, int K, float radius, const float *d_radius,
                       int P, int32_t *idx, float *patches, void *stream);
 /* The same for several (permuted cloud, key-point set, device radius) jobs in ONE launch (all 2 x num_scales jobs of a pair):
@@ -107,6 +129,17 @@ int bx_select_patches_batched_n(int njobs, const void *const *pts4, const int32_
 int bx_select_patches_grid_batched_n(int njobs, const void *const *pts4, const int32_t *N, const void *const *kpts, const int32_t *K,
                                      const void *const *d_radius, const void *const *d_K, int P, float *patches, void *workspace,
                                      void *stream);
+/* Device-side point counts as well (size-class buffers).  N[j] is job j's CAPACITY; d_N: host array of njobs device int32
+ * pointers (an entry or the array may be NULL = no count): job j's permuted cloud holds min(max(*d_N[j], 1), N[j]) points
+ * and points beyond that are never read.  Grids, the grid form's workspace (bx_select_patches_grid_workspace_bytes(N[j])
+ * per job) and its shared-memory bitmap are sized by the capacities.  Output is bit-identical to the calls above on the
+ * exact clouds; d_N NULL = the _n calls above. */
+int bx_select_patches_batched_counts(int njobs, const void *const *pts4, const int32_t *N, const void *const *d_N, const void *const *kpts,
+                                     const int32_t *K, const void *const *d_radius, const void *const *d_K, int P, float *patches,
+                                     void *stream);
+int bx_select_patches_grid_batched_counts(int njobs, const void *const *pts4, const int32_t *N, const void *const *d_N,
+                                          const void *const *kpts, const int32_t *K, const void *const *d_radius,
+                                          const void *const *d_K, int P, float *patches, void *workspace, void *stream);
 
 /* Plain ordered ball query (pointnet2_ops.ball_query; utils/common.py:442): xyz [n,3] packed. */
 int bx_ball_query(const float *xyz, int n, const float *qry, int m, float radius, int nsample, int32_t *idx,
