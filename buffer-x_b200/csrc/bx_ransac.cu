@@ -13,7 +13,8 @@
 //      ties by rmse; confidence-driven est_k; stop when itr >= est_k).
 // Later chunks see est_k in device memory and turn into no-ops once itr >= est_k.
 // a15 replaces post_refinement + rigid_transform_3d (/root/reference/models/BUFFERX.py:522-603; builds
-// an I x I diag matrix for a 3x3 result): one CTA, <= 20 rounds, weighted Horn fit from 16 block sums.
+// an I x I diag matrix for a 3x3 result): one CTA, <= 20 rounds, weighted Horn fit from 16 block sums taken about the
+// first correspondence, with the reference's centroids over (sum w + 1e-6).
 // Compiled with -fmad=false (bit contract with the oracle's fp64 arithmetic).
 #include "bx_common.cuh"
 
@@ -354,6 +355,11 @@ refine_kernel(const float *__restrict__ ss, const float *__restrict__ tt, const 
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     if (tid < 16) sT[tid] = (float)T_in[tid];
     __syncthreads();
+    // the sums are taken about a pivot (the first correspondence): differences of fp32 values are exact in fp64, so the
+    // cross-covariance does not cancel |offset|^2 far from the origin
+    double pa[3] = {0, 0, 0}, pb[3] = {0, 0, 0};
+    if (n > 0)
+        for (int e = 0; e < 3; ++e) { pa[e] = (double)ss[e]; pb[e] = (double)tt[e]; }
     int prev = 0, r = 0;
     for (r = 0; r < 20; ++r) {
         float T[12];
@@ -375,7 +381,8 @@ refine_kernel(const float *__restrict__ ss, const float *__restrict__ tt, const 
                 ++cnt;
                 const float q = d / dist_th;
                 const double w = (double)(1.0f / (1.0f + (q * q)));
-                const double a[3] = {(double)x, (double)y, (double)z}, b[3] = {(double)gx, (double)gy, (double)gz};
+                const double a[3] = {(double)x - pa[0], (double)y - pa[1], (double)z - pa[2]};
+                const double b[3] = {(double)gx - pb[0], (double)gy - pb[1], (double)gz - pb[2]};
                 acc[0] += w;
 #pragma unroll
                 for (int e = 0; e < 3; ++e) {
@@ -415,12 +422,19 @@ refine_kernel(const float *__restrict__ ss, const float *__restrict__ tt, const 
                 for (int w = 0; w < 8; ++w) v += red[w][e];
                 sum[e] = v;
             }
-            const double sw = sum[0];
-            double ca[3], cb[3], S[3][3];
-            for (int e = 0; e < 3; ++e) { ca[e] = sum[1 + e] / sw; cb[e] = sum[4 + e] / sw; }
-            // S = sum w (a-ca)(b-cb)^T = sum w a b^T - sw ca cb^T
+            const double sw = sum[0], den = sw + 1e-6;
+            double ma[3], mb[3], ca[3], cb[3], ea[3], eb[3], S[3][3];
+            for (int e = 0; e < 3; ++e) {
+                ma[e] = sum[1 + e] / sw;                       // weighted mean, relative to the pivot
+                mb[e] = sum[4 + e] / sw;
+                ca[e] = ((sw * pa[e]) + sum[1 + e]) / den;     // rigid_transform_3d's centroids over (sum w + 1e-6)
+                cb[e] = ((sw * pb[e]) + sum[4 + e]) / den;
+                ea[e] = (ca[e] * 1e-6) / sw;                   // mean - centroid
+                eb[e] = (cb[e] * 1e-6) / sw;
+            }
+            // S = sum w (a-ca)(b-cb)^T = sum w (a-p)(b-q)^T - sw ma mb^T + sw (mean_a-ca)(mean_b-cb)^T
             for (int e = 0; e < 3; ++e)
-                for (int f = 0; f < 3; ++f) S[e][f] = sum[7 + 3 * e + f] - (sw * ca[e]) * cb[f];
+                for (int f = 0; f < 3; ++f) S[e][f] = (sum[7 + 3 * e + f] - (sw * ma[e]) * mb[f]) + (sw * ea[e]) * eb[f];
             double Td[16];
             horn_from_S(S, ca, cb, Td);
             for (int e = 0; e < 16; ++e) sT[e] = (float)Td[e];

@@ -636,9 +636,10 @@ static void jacobi4_max_eigvec(double A[4][4], double q[4]) {
 }
 
 /* rigid fit of n weighted pairs (fp64); T row-major 4x4.  w == NULL -> unit weights.
- * Frozen order: centroids = (sum_i w_i p_i) / (sum_i w_i); S = sum_i w_i (a_i - ca)(b_i - cb)^T
- * accumulated sequentially in i. */
-static void horn_fit(const double *a, const double *b, const double *w, int n, double T[16]) {
+ * Frozen order: centroids = (sum_i w_i p_i) / (sum_i w_i + eps); S = sum_i w_i (a_i - ca)(b_i - cb)^T
+ * accumulated sequentially in i; t = cb - R ca.  eps = 1e-6 restates rigid_transform_3d (BUFFERX.py:582-587),
+ * 0 gives Open3D's unit-weight fit (RANSAC). */
+static void horn_fit(const double *a, const double *b, const double *w, int n, double eps, double T[16]) {
     double ca[3] = {0, 0, 0}, cb[3] = {0, 0, 0}, sw = 0.0;
     for (int i = 0; i < n; ++i) {
         const double wi = w ? w[i] : 1.0;
@@ -648,7 +649,7 @@ static void horn_fit(const double *a, const double *b, const double *w, int n, d
             cb[c] = cb[c] + (wi * b[3 * i + c]);
         }
     }
-    for (int c = 0; c < 3; ++c) { ca[c] = ca[c] / sw; cb[c] = cb[c] / sw; }
+    for (int c = 0; c < 3; ++c) { ca[c] = ca[c] / (sw + eps); cb[c] = cb[c] / (sw + eps); }
     double S[3][3] = {{0, 0, 0}, {0, 0, 0}, {0, 0, 0}};
     for (int i = 0; i < n; ++i) {
         const double wi = w ? w[i] : 1.0;
@@ -691,7 +692,9 @@ static void horn_fit(const double *a, const double *b, const double *w, int n, d
     T[12] = 0.0; T[13] = 0.0; T[14] = 0.0; T[15] = 1.0;
 }
 
-BX_EXPORT void bxo_horn_fit(const double *a, const double *b, const double *w, int n, double *T) { horn_fit(a, b, w, n, T); }
+BX_EXPORT void bxo_horn_fit(const double *a, const double *b, const double *w, int n, double eps, double *T) {
+    horn_fit(a, b, w, n, eps, T);
+}
 
 static inline void xform(const double T[16], const double p[3], double o[3]) {
     for (int r = 0; r < 3; ++r) o[r] = (((T[4 * r] * p[0]) + (T[4 * r + 1] * p[1])) + (T[4 * r + 2] * p[2])) + T[4 * r + 3];
@@ -751,7 +754,7 @@ BX_EXPORT int bxo_ransac(const float *src, const float *tgt, const int32_t *inli
             }
         if (!ok) continue;
         double T[16];
-        horn_fit(a, b, NULL, 3, T);
+        horn_fit(a, b, NULL, 3, 0.0, T);
         for (int j = 0; j < 3 && ok; ++j) {
             double o[3];
             xform(T, a + 3 * j, o);
@@ -795,7 +798,8 @@ BX_EXPORT int bxo_ransac(const float *src, const float *tgt, const int32_t *inli
  * :562-603).  Up to 20 rounds over ALL matches: inliers = |T s - t| < dist_th; stop when the
  * inlier count equals the previous round's; weights 1/(1+(d/th)^2); weighted rigid fit.
  * The reference runs this in fp32 with torch.svd; this restatement evaluates distances in fp32
- * (the inlier decision) and the fit in fp64 (Horn).  ref_check.py pins it against the
+ * (the inlier decision) and the fit in fp64 (Horn), with the reference's centroids over (sum w + 1e-6).
+ * ref_check.py pins it against the
  * reference's own function within 1e-4.
  * ------------------------------------------------------------------------------------------ */
 BX_EXPORT int bxo_refine(const float *src, const float *tgt, int n, const float *T_in /*16*/, float dist_th,
@@ -826,7 +830,7 @@ BX_EXPORT int bxo_refine(const float *src, const float *tgt, int n, const float 
         prev = cnt;
         if (cnt == 0) break;
         double Td[16];
-        horn_fit(a, b, w, cnt, Td);
+        horn_fit(a, b, w, cnt, 1e-6, Td);
         for (int i = 0; i < 16; ++i) T[i] = (float)Td[i];
     }
     memcpy(T_out, T, sizeof(T));

@@ -74,7 +74,7 @@ def lib():
         _lib.bxo_spt.argtypes = [c_void_p, c_int, c_int, c_void_p, c_int, c_int, c_void_p, c_float, c_int, c_void_p, c_void_p]
         _lib.bxo_consensus.argtypes = [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_float, c_void_p, c_void_p, c_void_p]
         _lib.bxo_refine.argtypes = [c_void_p, c_void_p, c_int, c_void_p, c_float, c_void_p, c_void_p]
-        _lib.bxo_horn_fit.argtypes = [c_void_p, c_void_p, c_void_p, c_int, c_void_p]
+        _lib.bxo_horn_fit.argtypes = [c_void_p, c_void_p, c_void_p, c_int, c_double, c_void_p]
         _lib.bxo_fps.argtypes = [c_void_p, c_int, c_int, c_void_p]
         _lib.bxo_mutual_nn.argtypes = [c_void_p, c_int, c_void_p, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p]
         _lib.bxo_radius_hist.argtypes = [c_void_p, c_int, c_void_p, c_int, c_void_p]
@@ -308,13 +308,271 @@ def refine(src, tgt, T_in, dist_th):
     return Tout.reshape(4, 4).copy(), int(rounds[0])
 
 
-def horn_fit(a, b, w=None):
+def horn_fit(a, b, w=None, eps=0.0):
+    """The C restatement's rigid fit; ``eps`` is added to the weight sum of the centroids (refinement: 1e-6)."""
     a = np.ascontiguousarray(a, dtype=np.float64)
     b = np.ascontiguousarray(b, dtype=np.float64)
     w = None if w is None else np.ascontiguousarray(w, dtype=np.float64)
     T = np.zeros(16, dtype=np.float64)
-    lib().bxo_horn_fit(_p(a), _p(b), _p(w), a.shape[0], _p(T))
+    lib().bxo_horn_fit(_p(a), _p(b), _p(w), a.shape[0], c_double(eps), _p(T))
     return T.reshape(4, 4)
+
+
+# --------------------------------------------------------------------------- #
+# a10, a13-a15 evaluated in float64 from the reference's formulas (tests/test_pose_fp64_*.py)
+# --------------------------------------------------------------------------- #
+def mutual_nn_fp64(a, b):
+    """knn_cuda KNN(k=1) both ways on the fp32 descriptors, distances sum (a - b)^2 in float64 -> dict(D [Ka,Kb], and per
+    row (r_*) and per column (c_*): the best and second-best distance and the best's index (first minimum))."""
+    a = np.asarray(a, np.float32).astype(np.float64)
+    b = np.asarray(b, np.float32).astype(np.float64)
+    D = ((a[:, None, :] - b[None, :, :]) ** 2).sum(-1) if a.size and b.size else np.zeros((len(a), len(b)))
+    out = dict(D=D)
+    for side, M in (("r", D), ("c", D.T)):
+        n = M.shape[1]
+        srt = np.sort(M, axis=1) if n else np.zeros((M.shape[0], 0))
+        out[side + "_idx"] = M.argmin(1) if n else np.zeros(M.shape[0], np.int64)
+        out[side + "_best"] = srt[:, 0] if n else np.full(M.shape[0], np.inf)
+        out[side + "_second"] = srt[:, 1] if n > 1 else np.full(M.shape[0], np.inf)
+    return out
+
+
+def consensus_fp64(ss, tt, R, t, azi_n, inlier_th):
+    """BUFFERX.py:404-417 literally, in float64 on the fp32 inputs: diffs [Mc,Mc] (hypothesis j, correspondence i),
+    thr [Mc], sign = diffs < thr, counts, best = first arg-max."""
+    ss, tt, R, t = (torch.from_numpy(np.asarray(x, np.float32).astype(np.float64)) for x in (ss, tt, R, t))
+    tss = ss[None] @ R.transpose(-1, -2) + t[:, None]
+    diffs = torch.sqrt(torch.sum((tss - tt[None]) ** 2, dim=-1))
+    thr = torch.sqrt(torch.sum(ss ** 2, dim=-1)) * np.pi / azi_n * float(np.float32(inlier_th))
+    sign = diffs < thr[None]
+    counts = torch.sum(sign, dim=-1)
+    best = int(torch.argmax(counts)) if len(counts) else 0
+    return dict(diffs=diffs.numpy(), thr=thr.numpy(), sign=sign.numpy(), counts=counts.numpy(), best=best)
+
+
+def umeyama_fp64(a, b, w=None):
+    """Rigid fit without scale (Umeyama / Open3D TransformationEstimationPointToPoint(False)) in float64: weighted
+    centroids, H = sum w (a - ca)(b - cb)^T, H = U S V^T, d = sign det(V U^T), R = V diag(1, 1, d) U^T, t = cb - R ca.
+    -> dict(R, t, ca, cb, sv (singular values, descending), d)."""
+    a = np.asarray(a, np.float64).reshape(-1, 3)
+    b = np.asarray(b, np.float64).reshape(-1, 3)
+    w = np.ones(len(a)) if w is None else np.asarray(w, np.float64)
+    sw = w.sum()
+    ca, cb = (w[:, None] * a).sum(0) / sw, (w[:, None] * b).sum(0) / sw
+    H = (w[:, None] * (a - ca)).T @ (b - cb)
+    U, S, Vt = np.linalg.svd(H)
+    d = 1.0 if np.linalg.det(Vt.T @ U.T) >= 0 else -1.0
+    R = Vt.T @ np.diag([1.0, 1.0, d]) @ U.T
+    return dict(R=R, t=cb - R @ ca, ca=ca, cb=cb, sv=S, d=d)
+
+
+def philox4x32_10_np(ctr, key):
+    """Philox4x32-10 (Salmon et al., SC'11) in NumPy: ctr [n,4] / key [2] uint32 -> [n,4] uint32."""
+    c = [np.asarray(ctr, np.uint64)[:, i].copy() for i in range(4)]
+    k0, k1 = np.uint64(int(key[0]) & 0xFFFFFFFF), np.uint64(int(key[1]) & 0xFFFFFFFF)
+    m32 = np.uint64(0xFFFFFFFF)
+    for _ in range(10):
+        p0 = np.uint64(0xD2511F53) * c[0]
+        p1 = np.uint64(0xCD9E8D57) * c[2]
+        c = [(p1 >> np.uint64(32)) ^ c[1] ^ k0, p1 & m32, (p0 >> np.uint64(32)) ^ c[3] ^ k1, p0 & m32]
+        k0 = (k0 + np.uint64(0x9E3779B9)) & m32
+        k1 = (k1 + np.uint64(0xBB67AE85)) & m32
+    return np.stack(c, axis=1).astype(np.uint32)
+
+
+def ransac_draws(seed, I, n):
+    """The three correspondence draws of iterations 0..n-1: counter (itr, 0, 0, 0), key (seed lo, seed hi),
+    sel = (rnd * I) >> 32 -> [n,3] int64."""
+    ctr = np.zeros((n, 4), np.uint64)
+    ctr[:, 0] = np.arange(n, dtype=np.uint64)
+    rnd = philox4x32_10_np(ctr, (seed & 0xFFFFFFFF, (seed >> 32) & 0xFFFFFFFF))[:, :3].astype(np.uint64)
+    return ((rnd * np.uint64(I)) >> np.uint64(32)).astype(np.int64)
+
+
+def refine_fp64(src, tgt, T_in, dist_th):
+    """post_refinement + rigid_transform_3d (BUFFERX.py:522-603) literally, in torch float64 on the fp32 inputs: 20 rounds
+    at dist_th, stop when |inliers - previous| < 1, weights 1 / (1 + (d / th)^2), centroids over (sum w + 1e-6), torch.svd
+    and the det correction.  -> dict(T (final), rounds, per round: T used, d [n], mask, and the fit's (w, R, t))."""
+    src = torch.from_numpy(np.asarray(src, np.float32).astype(np.float64))[None]
+    tgt = torch.from_numpy(np.asarray(tgt, np.float32).astype(np.float64))[None]
+    tr = torch.from_numpy(np.asarray(T_in, np.float32).astype(np.float64).reshape(4, 4))[None]
+    th = float(np.float32(dist_th))
+    prev, hist, r = 0, [], 0
+    while r < 20:
+        L2 =torch.norm((tr[:, :3, :3] @ src.permute(0, 2, 1) + tr[:, :3, 3:4]).permute(0, 2, 1) - tgt, dim=-1)
+        pred = (L2 < th)[0]
+        n = int(pred.sum())
+        step = dict(T=tr[0].numpy().copy(), d=L2[0].numpy().copy(), mask=pred.numpy().copy())
+        hist.append(step)
+        if abs(n - prev) < 1:
+            break
+        prev = n
+        A, B, wt = src[:, pred], tgt[:, pred], (1 / (1 + (L2 / th) ** 2))[:, pred]
+        cA = (A * wt[:, :, None]).sum(1, keepdim=True) / (wt.sum(1, keepdim=True)[:, :, None] + 1e-6)
+        cB = (B * wt[:, :, None]).sum(1, keepdim=True) / (wt.sum(1, keepdim=True)[:, :, None] + 1e-6)
+        H = (A - cA).permute(0, 2, 1) @ torch.diag_embed(wt) @ (B - cB)
+        U, S, V = torch.svd(H)
+        eye = torch.eye(3, dtype=torch.float64)[None].clone()
+        eye[:, -1, -1] = torch.det(V @ U.permute(0, 2, 1))
+        R = V @ eye @ U.permute(0, 2, 1)
+        tr = torch.eye(4, dtype=torch.float64)[None].clone()
+        tr[:, :3, :3], tr[:, :3, 3:4] = R, cB.permute(0, 2, 1) - R @ cA.permute(0, 2, 1)
+        step.update(w=wt[0].numpy().copy(), R=R[0].numpy().copy(), t=tr[0, :3, 3].numpy().copy(), sv=S[0].numpy().copy(),
+                    cA=cA[0, 0].numpy().copy(), cB=cB[0, 0].numpy().copy())
+        r += 1
+    return dict(T=tr[0].numpy().copy(), rounds=r, hist=hist)
+
+
+U53 = 2.0 ** -53
+
+
+def fit_bounds(a, b, kf=16.0):
+    """Umeyama on one triple (or any set) and what bounds a float64 fit of it: bR (largest entry of R - R64, from
+    |dH| <= kf u53 sum |a - ca| |b - cb| over the gap sigma_2 + d sigma_3), or inf when the fit is degenerate (bR > 1e-6:
+    duplicate, collinear or coincident points, where the rotation about the line is free); the line (unit u through ca,
+    v through cb) and the largest off-line distance of the points for that case."""
+    f = umeyama_fp64(a, b)
+    a = np.asarray(a, np.float64).reshape(-1, 3)
+    b = np.asarray(b, np.float64).reshape(-1, 3)
+    da, db = a - f["ca"], b - f["cb"]
+    dH = kf * U53 * (np.linalg.norm(da, axis=1) * np.linalg.norm(db, axis=1)).sum()
+    gap = f["sv"][1] + f["d"] * f["sv"][2]
+    bR = 2.0 * dH / gap if gap > 0 else np.inf
+    f["bR"] = bR if bR <= 1e-6 else np.inf
+    U, _, Vt = np.linalg.svd(da.T @ db)
+    u, v = U[:, 0], Vt[0]
+    f["line"] = (u, v, f["sv"][0] > 0)
+    f["off"] = max(np.linalg.norm(da - np.outer(da @ u, u), axis=1).max(), np.linalg.norm(db - np.outer(db @ v, v), axis=1).max())
+    return f
+
+
+def _fit_dist(f, x, g, kf=16.0):
+    """|T64 x - g| and its margin for a fit of bound f["bR"]: a rotation error bR per entry moves x by <= 3 bR |x - ca|,
+    plus kf u53 of the magnitudes (centroids, evaluation)."""
+    x, g = np.asarray(x, np.float64).reshape(-1, 3), np.asarray(g, np.float64).reshape(-1, 3)
+    e = np.linalg.norm(x @ f["R"].T + f["t"] - g, axis=1)
+    m = 3 * f["bR"] * np.linalg.norm(x - f["ca"], axis=1) + kf * U53 * (np.abs(f["ca"]).sum() + np.abs(f["cb"]).sum()
+                                                                        + 3 * np.abs(x).sum(1) + np.abs(g).sum(1) + e)
+    return e, m
+
+
+def _line_dist(f, x, g):
+    """Smallest |T x - g| over every rigid T that maps the fit's line onto its target line and ca onto cb (the free
+    rotation of a degenerate triple): the cylinder coordinates (h, rho) of x about (ca, u) and of g about (cb, v); for a
+    coincident triple (no line), | |x - ca| - |g - cb| |."""
+    x, g = np.asarray(x, np.float64).reshape(-1, 3), np.asarray(g, np.float64).reshape(-1, 3)
+    u, v, has_line = f["line"]
+    dx, dg = x - f["ca"], g - f["cb"]
+    if not has_line:
+        return np.abs(np.linalg.norm(dx, axis=1) - np.linalg.norm(dg, axis=1))
+    hx, hg = dx @ u, dg @ v
+    rx, rg = np.linalg.norm(dx - np.outer(hx, u), axis=1), np.linalg.norm(dg - np.outer(hg, v), axis=1)
+    return np.hypot(hx - hg, rx - rg)
+
+
+def ransac_fp64(src, tgt, inlier_ind, dist_th, similar_th, confidence, max_iter, seed, ke=8.0, kf=16.0, recs=None):
+    """RegistrationRANSACBasedOnCorrespondence replayed in float64 on the kernel's draws (``ransac_draws``): per
+    iteration the EdgeLength checker, the Umeyama fit of the triple, the Distance checker, the inlier count and rmse; then
+    Open3D's sequential bookkeeping (more inliers wins, then lower rmse; est_k = ceil(log(1 - conf) / log(1 - r^3))).
+    Every decision within its rounding margin is flagged: the checkers (ke u53 of the edge lengths; the fit margin of
+    ``_fit_dist``), each inlier test (-> a count interval [lo, hi]), the rmse tie-break and est_k near an integer.  A
+    degenerate triple (``fit_bounds``) has a free rotation about its line: its Distance checker is decided only for
+    points on that line and its count lies in [0, hi] with hi from ``_line_dist``; it cannot win once hi < best.  With
+    ``recs`` (an implementation's per-iteration records) a degenerate iteration takes the recorded count and rmse -- its
+    own choice among the equally good rotations -- once that count is shown to lie in [0, hi].
+    -> dict(num_inliers, best_itr, iters, first_marginal (itr or None), recs (per iteration), fits (itr -> fit))."""
+    S = np.asarray(src, np.float32).astype(np.float64)
+    D = np.asarray(tgt, np.float32).astype(np.float64)
+    ind = np.asarray(inlier_ind, np.int64)
+    I = len(ind)
+    out = dict(num_inliers=0, best_itr=-1, iters=0, first_marginal=None, recs=[], fits={})
+    if I < 3 or max_iter <= 0:
+        return out
+    s, g = S[ind], D[ind]
+    sel_all = ransac_draws(seed, I, max_iter)
+    th = float(dist_th)
+    best_good, best_rmse, best_itr, best_sel, best_dr, est_k = 0, 0.0, -1, None, 0.0, max_iter
+    first_marg = None
+
+    def marg(itr):
+        nonlocal first_marg
+        if first_marg is None:
+            first_marg = itr
+
+    itr = 0
+    while itr < max_iter and itr < est_k:
+        sel = sel_all[itr]
+        a, b = s[sel], g[sel]
+        rec = dict(itr=itr, sel=tuple(sel), passed=False, marginal=False, deg=False, lo=0, hi=0, rmse=0.0)
+        out["recs"].append(rec)
+        ok = True
+        for i in range(3):
+            for j in range(i + 1, 3):
+                ds, dt = np.linalg.norm(a[i] - a[j]), np.linalg.norm(b[i] - b[j])
+                m = ke * U53 * (ds + dt)
+                if abs(ds - dt * similar_th) < m or abs(dt - ds * similar_th) < m:
+                    rec["marginal"] = True
+                if ds < dt * similar_th or dt < ds * similar_th:
+                    ok = False
+        if ok:
+            f = fit_bounds(a, b, kf)
+            out["fits"][itr] = f
+            rec["deg"] = deg = not np.isfinite(f["bR"])
+            if deg:
+                e = np.linalg.norm(a @ f["R"].T + f["t"] - b, axis=1)
+                m = 2 * f["off"] + kf * U53 * (np.abs(a).sum(1) + np.abs(b).sum(1) + 1)
+            else:
+                e, m = _fit_dist(f, a, b, kf)
+            if (np.abs(e - th) <= m).any():
+                rec["marginal"] = True
+            ok = not (e > th).any()
+        rec["passed"] = ok
+        if rec["marginal"]:
+            marg(itr)
+        if not ok:
+            itr += 1
+            continue
+        if deg:
+            ld = _line_dist(f, s, g)
+            rec["hi"] = hi = int((ld < th + 2 * f["off"] + kf * U53 * (np.abs(s).sum(1) + np.abs(g).sum(1))).sum())
+            if recs is not None and itr < len(recs) and recs["pass"][itr]:
+                good, rmse, dr = int(recs["good"][itr]), float(recs["rmse"][itr]), 0.0
+                assert good <= hi, f"itr {itr}: a degenerate triple counted {good} inliers, more than the {hi} its line allows"
+                rec["lo"] = rec["hi"] = good
+                rec["rmse"] = rmse
+            else:
+                if not (hi < best_good or (hi == 0 and best_good == 0)):
+                    marg(itr)
+                    rec["marginal"] = True
+                itr += 1
+                continue
+        else:
+            e, m = _fit_dist(f, s, g, kf)
+            inl = e < th
+            mg = np.abs(e - th) <= m
+            rec["lo"], rec["hi"] = lo, hi = int((inl & ~mg).sum()), int((inl | mg).sum())
+            good = int(inl.sum())
+            rmse = float(np.sqrt((e[inl] ** 2).sum() / good)) if good else 0.0
+            dr = float(m.max()) if good else 0.0
+            rec["rmse"] = rmse
+            if lo != hi and hi >= best_good:
+                marg(itr)
+                rec["marginal"] = True
+        better = good > best_good or (good == best_good and rmse < best_rmse)
+        if good == best_good and good > 0 and tuple(sel) != best_sel and abs(rmse - best_rmse) <= dr + best_dr:
+            marg(itr)
+            rec["marginal"] = True
+        if better:
+            best_good, best_rmse, best_itr, best_sel, best_dr = good, rmse, itr, tuple(sel), dr
+            with np.errstate(divide="ignore", invalid="ignore"):
+                est = float(np.log(np.float64(1.0 - confidence)) / np.log(np.float64(1.0 - (good / I) ** 3)))
+            if np.isfinite(est) and abs(est - round(est)) <= 1e-9 * abs(est) and est != 0:
+                marg(itr)
+            if est < est_k:
+                est_k = int(math.ceil(est))
+        itr += 1
+    out.update(num_inliers=best_good, best_itr=best_itr, iters=itr, first_marginal=first_marg)
+    return out
 
 
 # --------------------------------------------------------------------------- #
