@@ -22,6 +22,12 @@ constexpr int NN_C = 32;    // descriptor length (fixed by the network)
 // rows present this launch: min(*d_n, n), or n without a device count
 __device__ __forceinline__ int nn_count(const int *d_n, int n) { return d_n ? min(max(*d_n, 0), n) : n; }
 
+// one step of the squared distance, summed over the feature dimension in order from +0 (the arithmetic of bxo_mutual_nn)
+__device__ __forceinline__ float nn_acc(float acc, float x, float y) {
+    const float t = x - y;
+    return acc + (t * t);
+}
+
 __global__ void nn_init_kernel(unsigned long long *keys, int n) {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i < n) keys[i] = ~0ull;
@@ -57,10 +63,7 @@ nn_tile_kernel(const float *__restrict__ a, int Ka, const float *__restrict__ b,
             if (gj >= Kb) break;
             float acc = 0.0f;
 #pragma unroll
-            for (int c = 0; c < NN_C; ++c) {
-                const float t = sa[ti][c] - sb[jj][c];
-                acc = acc + (t * t);
-            }
+            for (int c = 0; c < NN_C; ++c) acc = nn_acc(acc, sa[ti][c], sb[jj][c]);
             const unsigned long long kd = (unsigned long long)__float_as_uint(acc) << 32;
             const unsigned long long rk = kd | (unsigned)gj;
             if (rk < rbest) rbest = rk;
@@ -112,6 +115,63 @@ nn_select_kernel(const unsigned long long *__restrict__ row_keys, const unsigned
     if (tnn)
         for (int j = threadIdx.x; j < Kb; j += 1024) tnn[j] = (int)(col_keys[j] & 0xffffffffull);
     if (threadIdx.x == 0) *d_M = run;
+}
+
+// k = 1 nearest neighbour of every query row among the ref rows, any feature length D, B independent problems
+// (knn_cuda.KNN(k=1, transpose_mode=True)).  The tile and key scheme of nn_tile_kernel, rows only: grid (ceil(Nq/64),
+// ceil(Nr/64), B), 256 threads, thread (row tid/4, columns tid%4 + 4u); the features are staged NN_C at a time and each
+// thread carries its 16 partial sums across the stages, so every distance is summed over D in order.
+constexpr int KNN_COLS = NN_TJ / 4;
+
+__global__ void __launch_bounds__(256)
+knn1_tile_kernel(const float *__restrict__ ref, int Nr, const float *__restrict__ qry, int Nq, int D,
+                 unsigned long long *__restrict__ keys) {
+    __shared__ float sq[NN_TI][NN_C + 1];
+    __shared__ float sr[NN_TJ][NN_C + 1];
+    const size_t b = blockIdx.z;
+    const int i0 = blockIdx.x * NN_TI, j0 = blockIdx.y * NN_TJ;
+    ref += b * Nr * D;
+    qry += b * Nq * D;
+    const int tid = threadIdx.x, ti = tid >> 2, tj = tid & 3;
+    float acc[KNN_COLS];
+#pragma unroll
+    for (int u = 0; u < KNN_COLS; ++u) acc[u] = 0.0f;
+    for (int c0 = 0; c0 < D; c0 += NN_C) {
+        const int dc = min(NN_C, D - c0);
+        for (int e = tid; e < NN_TI * NN_C; e += 256) {
+            const int r = e / NN_C, c = e % NN_C;
+            sq[r][c] = (i0 + r < Nq && c < dc) ? qry[(size_t)(i0 + r) * D + c0 + c] : 0.0f;
+            sr[r][c] = (j0 + r < Nr && c < dc) ? ref[(size_t)(j0 + r) * D + c0 + c] : 0.0f;
+        }
+        __syncthreads();
+        for (int c = 0; c < dc; ++c) {
+            const float x = sq[ti][c];
+#pragma unroll
+            for (int u = 0; u < KNN_COLS; ++u) acc[u] = nn_acc(acc[u], x, sr[tj + 4 * u][c]);
+        }
+        __syncthreads();
+    }
+    unsigned long long best = ~0ull;
+#pragma unroll
+    for (int u = 0; u < KNN_COLS; ++u) {
+        const int gj = j0 + tj + 4 * u;
+        const unsigned long long k = ((unsigned long long)__float_as_uint(acc[u]) << 32) | (unsigned)gj;
+        if (gj < Nr && k < best) best = k;
+    }
+    unsigned long long o = __shfl_xor_sync(BX_FULL, best, 1);
+    if (o < best) best = o;
+    o = __shfl_xor_sync(BX_FULL, best, 2);
+    if (o < best) best = o;
+    if (tj == 0 && i0 + ti < Nq) atomicMin(&keys[b * Nq + i0 + ti], best);
+}
+
+__global__ void knn1_finish_kernel(const unsigned long long *__restrict__ keys, size_t n, float *__restrict__ dist,
+                                   long long *__restrict__ idx) {
+    const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    const unsigned long long k = keys[i];
+    dist[i] = sqrtf(__uint_as_float((unsigned)(k >> 32)));
+    idx[i] = (long long)(k & 0xffffffffull);
 }
 
 // ---- a11 tail + a12 ---------------------------------------------------------------------------------
@@ -304,6 +364,26 @@ BX_API int bx_mutual_nn_n(const float *a, int Ka, const float *b, int Kb, int C,
     nn_tile_kernel<<<grid, 256, 0, st>>>(a, Ka, b, Kb, keys, keys + Ka, d_Ka, d_Kb);
     BX_LAUNCH_CHECK();
     nn_select_kernel<<<1, 1024, 0, st>>>(keys, keys + Ka, Ka, Kb, s_mids, t_mids, d_M, snn, tnn, d_Ka, d_Kb);
+    BX_LAUNCH_CHECK();
+    return BX_OK;
+}
+
+BX_API int bx_knn1(const float *ref, int Nr, const float *qry, int Nq, int D, int B, unsigned long long *keys, float *dist,
+                   int64_t *idx, void *stream) {
+    BX_REQUIRE(ref && qry && keys && dist && idx, "bx_knn1: null pointer");
+    BX_REQUIRE(B >= 1 && B <= 65535 && Nr >= 1 && Nq >= 0 && D >= 1,
+               "bx_knn1: bad sizes (B=%d in [1,65535], Nr=%d >= 1, Nq=%d >= 0, D=%d >= 1)", B, Nr, Nq, D);
+    BX_REQUIRE((long long)B * Nq < (1ll << 31), "bx_knn1: B*Nq=%lld query rows exceed 2^31", (long long)B * Nq);
+    BX_REQUIRE(Nr <= 65535 * NN_TJ, "bx_knn1: Nr=%d exceeds %d ref rows", Nr, 65535 * NN_TJ);
+    if (Nq == 0) return BX_OK;
+    cudaStream_t st = bx_stream(stream);
+    const int n = B * Nq;
+    nn_init_kernel<<<(n + 255) / 256, 256, 0, st>>>(keys, n);
+    BX_LAUNCH_CHECK();
+    knn1_tile_kernel<<<dim3((unsigned)((Nq + NN_TI - 1) / NN_TI), (unsigned)((Nr + NN_TJ - 1) / NN_TJ), (unsigned)B), 256, 0, st>>>(
+        ref, Nr, qry, Nq, D, keys);
+    BX_LAUNCH_CHECK();
+    knn1_finish_kernel<<<(n + 255) / 256, 256, 0, st>>>(keys, (size_t)n, dist, reinterpret_cast<long long *>(idx));
     BX_LAUNCH_CHECK();
     return BX_OK;
 }

@@ -38,6 +38,9 @@ constexpr int SP_CH = 2048;
 constexpr int SP_SUB = SP_CH / SP_SPLIT;      // points of a chunk scanned by one warp
 constexpr int SP_STEPS = SP_SUB / 32;         // ballots per warp and chunk
 constexpr int BQ_WARPS = 8;
+// bx_ball_query_batched stages a cloud of up to this many points in shared memory (48 KB, no opt-in attribute needed)
+constexpr int BQ_SMEM_MAX_N = 4096;
+constexpr int BQ_SMEM_TARGET_CTAS = 8 * 132;  // about eight resident CTAs per SM of an H100 SXM
 
 __device__ __forceinline__ void select_patches_body(const float4 *__restrict__ pts4, int N, const float *__restrict__ kpts, int K, float radius,
                                                     const float *__restrict__ d_radius, int P, int *__restrict__ idx, float *__restrict__ patches,
@@ -398,16 +401,11 @@ __global__ void __launch_bounds__(HG_THREADS) hg_query_batched_kernel(const HgJo
                   patches + (size_t)J.koff[j] * P * 3, k);
 }
 
-// plain ordered ball query over a packed [n,3] cloud (pointnet2_ops.ball_query semantics)
-__global__ void __launch_bounds__(BQ_WARPS * 32)
-ball_query_kernel(const float *__restrict__ xyz, int n, const float *__restrict__ qry, int m, float radius, int nsample,
-                  int *__restrict__ idx) {
-    const int lane = threadIdx.x & 31;
-    const int j = blockIdx.x * BQ_WARPS + (threadIdx.x >> 5);
-    if (j >= m) return;
-    const float r2 = radius * radius;
-    const float qx = qry[3 * (size_t)j], qy = qry[3 * (size_t)j + 1], qz = qry[3 * (size_t)j + 2];
-    int *row = idx + (size_t)j * nsample;
+// plain ordered ball query of one query point over a packed [n,3] cloud (pointnet2_ops.ball_query semantics), one warp:
+// the first nsample hits in index order, padded with the first hit (0 when there is none).  xyz may be global or shared.
+__device__ __forceinline__ void ball_query_row(const float *xyz, int n, const float *q, float r2, int nsample, int *row,
+                                               int lane) {
+    const float qx = q[0], qy = q[1], qz = q[2];
     int cnt = 0, first = 0;
     for (int base = 0; base < n && cnt < nsample; base += 32) {
         const int i = base + lane;
@@ -426,6 +424,32 @@ ball_query_kernel(const float *__restrict__ xyz, int n, const float *__restrict_
     }
     if (cnt > nsample) cnt = nsample;
     for (int s = cnt + lane; s < nsample; s += 32) row[s] = first;
+}
+
+// one warp per query, the cloud read through L1/L2 (large clouds); grid.y = batch element
+__global__ void __launch_bounds__(BQ_WARPS * 32)
+ball_query_kernel(const float *__restrict__ xyz, int n, const float *__restrict__ qry, int m, float radius, int nsample,
+                  int *__restrict__ idx) {
+    const int j = blockIdx.x * BQ_WARPS + (threadIdx.x >> 5);
+    if (j >= m) return;
+    const size_t b = blockIdx.y;
+    ball_query_row(xyz + b * n * 3, n, qry + (b * m + j) * 3, radius * radius, nsample, idx + (b * m + j) * nsample,
+                   threadIdx.x & 31);
+}
+
+// many small clouds (sphere_query: 1500 patches x 420 voxel centres): grid (split, B), the CTA stages cloud b in shared
+// memory and its warps take queries blockIdx.x * BQ_WARPS + w, stepping by split * BQ_WARPS.
+__global__ void __launch_bounds__(BQ_WARPS * 32)
+ball_query_smem_kernel(const float *__restrict__ xyz, int n, const float *__restrict__ qry, int m, float radius, int nsample,
+                       int *__restrict__ idx) {
+    extern __shared__ float s_xyz[];
+    const size_t b = blockIdx.y;
+    const float *src = xyz + b * n * 3;
+    for (int e = threadIdx.x; e < 3 * n; e += BQ_WARPS * 32) s_xyz[e] = src[e];
+    __syncthreads();
+    const float r2 = radius * radius;
+    for (int j = blockIdx.x * BQ_WARPS + (threadIdx.x >> 5); j < m; j += gridDim.x * BQ_WARPS)
+        ball_query_row(s_xyz, n, qry + (b * m + j) * 3, r2, nsample, idx + (b * m + j) * nsample, threadIdx.x & 31);
 }
 
 // ---- LRF ------------------------------------------------------------------------------------------
@@ -727,6 +751,28 @@ BX_API int bx_ball_query(const float *xyz, int n, const float *qry, int m, float
     if (m == 0) return BX_OK;
     ball_query_kernel<<<(m + BQ_WARPS - 1) / BQ_WARPS, BQ_WARPS * 32, 0, bx_stream(stream)>>>(xyz, n, qry, m, radius,
                                                                                                 nsample, idx);
+    BX_LAUNCH_CHECK();
+    return BX_OK;
+}
+
+BX_API int bx_ball_query_batched(const float *xyz, int B, int n, const float *qry, int m, float radius, int nsample, int32_t *idx,
+                                 void *stream) {
+    BX_REQUIRE(xyz && qry && idx, "bx_ball_query_batched: null pointer");
+    BX_REQUIRE(B >= 1 && B <= 65535 && n >= 1 && m >= 0 && nsample >= 1,
+               "bx_ball_query_batched: bad sizes (B=%d in [1,65535], n=%d >= 1, m=%d >= 0, nsample=%d >= 1)", B, n, m, nsample);
+    if (m == 0) return BX_OK;
+    cudaStream_t st = bx_stream(stream);
+    if (n <= BQ_SMEM_MAX_N) {
+        // enough CTAs per cloud to fill the GPU when B is small; one CTA per cloud (the cloud staged once) when B is large
+        const int per_cloud = (m + BQ_WARPS - 1) / BQ_WARPS;
+        const int want = (BQ_SMEM_TARGET_CTAS + B - 1) / B;
+        const int split = want < per_cloud ? want : per_cloud;
+        ball_query_smem_kernel<<<dim3((unsigned)split, (unsigned)B), BQ_WARPS * 32, (size_t)n * 3 * sizeof(float), st>>>(
+            xyz, n, qry, m, radius, nsample, idx);
+    } else {
+        ball_query_kernel<<<dim3((unsigned)((m + BQ_WARPS - 1) / BQ_WARPS), (unsigned)B), BQ_WARPS * 32, 0, st>>>(
+            xyz, n, qry, m, radius, nsample, idx);
+    }
     BX_LAUNCH_CHECK();
     return BX_OK;
 }

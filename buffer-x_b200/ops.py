@@ -29,6 +29,7 @@ SYMBOLS = [
     "bx_mutual_nn_n", "bx_early_exit_gate",
     "bx_fps_n", "bx_fps_size_class", "bx_radius_estimate_n", "bx_permute_cloud_n", "bx_select_patches_batched_counts",
     "bx_select_patches_grid_batched_counts",
+    "bx_ball_query_batched", "bx_gather_channels", "bx_knn1", "bx_svd3",
 ]
 
 GEOM_CYL3D, GEOM_CYL2D, GEOM_VALID3D, GEOM_COSTAB = 0, 1, 2, 4
@@ -78,6 +79,10 @@ def load_library():
     lib.bx_select_patches_grid_batched_n.argtypes = [c_int, P, P, P, P, P, P, c_int, P, P, P]
     lib.bx_select_patches_grid_workspace_bytes.restype = c_int64
     lib.bx_ball_query.argtypes = [P, c_int, P, c_int, c_float, c_int, P, P]
+    lib.bx_ball_query_batched.argtypes = [P, c_int, c_int, P, c_int, c_float, c_int, P, P]
+    lib.bx_gather_channels.argtypes = [P, c_int, c_int, c_int, P, c_int, P, P]
+    lib.bx_knn1.argtypes = [P, c_int, P, c_int, c_int, c_int, P, P, P, P]
+    lib.bx_svd3.argtypes = [P, c_int, P, P, P, P]
     lib.bx_lrf.argtypes = [P, c_int, c_int, c_float, P, c_int, P, P, P, P]
     lib.bx_lrf_batched.argtypes = [P, c_int, c_int, c_float, P, c_int, c_int, P, P, P, P]
     lib.bx_lrf_batched_n.argtypes = [P, c_int, c_int, c_float, P, c_int, P, c_int, P, P, P, P]
@@ -354,6 +359,73 @@ def ball_query(xyz: torch.Tensor, qry: torch.Tensor, radius: float, nsample: int
     _check(load_library().bx_ball_query(_dp(xyz, F32, "xyz"), xyz.shape[0], _dp(qry, F32, "qry"), qry.shape[0], float(radius), nsample,
                                         _dp(idx), _stream()), "bx_ball_query")
     return idx
+
+
+def dropin_tensor(t, name: str, shape: str, dtype=F32):
+    """Argument check of the drop-in modules under dropin/: a CUDA tensor of `dtype` with as many dims as `shape` names
+    (e.g. "[B,N,3]"), returned contiguous.  Inputs that require grad raise NotImplementedError (no backward is built)."""
+    if not isinstance(t, torch.Tensor):
+        raise TypeError(f"{name}: expected a torch.Tensor {shape}, got {type(t).__name__}")
+    if t.requires_grad:
+        raise NotImplementedError(f"{name}: inputs that require grad are not supported (forward only; no backward is built)")
+    if not t.is_cuda:
+        raise BufferXError(f"{name}: expected a CUDA tensor (bufferx_b200 has no CPU path)")
+    if t.dim() != shape.count(",") + 1:
+        raise BufferXError(f"{name}: expected shape {shape}, got {tuple(t.shape)}")
+    if t.dtype != dtype:
+        raise NotImplementedError(f"{name}: only {dtype} {shape} is supported, got {t.dtype}")
+    return t.contiguous()
+
+
+def ball_query_batched(xyz: torch.Tensor, qry: torch.Tensor, radius: float, nsample: int):
+    """xyz [B,N,3], qry [B,M,3] f32 -> idx [B,M,nsample] int32: per cloud, the first nsample points (index order) with
+    d2 < radius^2, padded with the first hit, all zero when nothing is hit."""
+    B, N, M = xyz.shape[0], xyz.shape[1], qry.shape[1]
+    idx = torch.empty((B, M, nsample), dtype=I32, device=xyz.device)
+    if B == 0 or M == 0:
+        return idx
+    _check(load_library().bx_ball_query_batched(_dp(xyz, F32, "xyz"), B, N, _dp(qry, F32, "qry"), M, float(radius), int(nsample), _dp(idx),
+                                                _stream()), "bx_ball_query_batched")
+    return idx
+
+
+def gather_channels(features: torch.Tensor, idx: torch.Tensor):
+    """features [B,C,N] f32, idx [B,...] int32 -> [B,C,...]: out[b,c,k] = features[b,c,idx[b,k]] (NaN for an index outside
+    [0,N))."""
+    B, C, N = features.shape
+    out = torch.empty((B, C) + tuple(idx.shape[1:]), dtype=F32, device=features.device)
+    if out.numel() == 0:
+        return out
+    K = idx[0].numel()
+    _check(load_library().bx_gather_channels(_dp(features, F32, "features"), B, C, N, _dp(idx, I32, "idx"), K, _dp(out), _stream()),
+           "bx_gather_channels")
+    return out
+
+
+def knn1(ref: torch.Tensor, qry: torch.Tensor):
+    """ref [B,Nr,D], qry [B,Nq,D] f32 -> (dist [B,Nq] f32 = sqrtf(d2), idx [B,Nq] int64): the first nearest ref row of each
+    query row, d2 summed over D in order without FMA."""
+    B, Nr, D = ref.shape
+    Nq = qry.shape[1]
+    dist = torch.empty((B, Nq), dtype=F32, device=ref.device)
+    idx = torch.empty((B, Nq), dtype=torch.int64, device=ref.device)
+    if B == 0 or Nq == 0:
+        return dist, idx
+    keys = torch.empty(B * Nq, dtype=torch.int64, device=ref.device)
+    _check(load_library().bx_knn1(_dp(ref, F32, "ref"), Nr, _dp(qry, F32, "qry"), Nq, D, B, _dp(keys), _dp(dist), _dp(idx), _stream()),
+           "bx_knn1")
+    return dist, idx
+
+
+def svd3(A: torch.Tensor):
+    """A [B,3,3] f32 -> (U [B,3,3], S [B,3] descending, V [B,3,3]) with A = U diag(S) V^T (fp64 one-sided Jacobi)."""
+    B = A.shape[0]
+    U = torch.empty((B, 3, 3), dtype=F32, device=A.device)
+    S = torch.empty((B, 3), dtype=F32, device=A.device)
+    V = torch.empty((B, 3, 3), dtype=F32, device=A.device)
+    if B:
+        _check(load_library().bx_svd3(_dp(A, F32, "A"), B, _dp(U), _dp(S), _dp(V), _stream()), "bx_svd3")
+    return U, S, V
 
 
 def lrf(patches: torch.Tensor, des_r, aligned: bool, delta=None, Rt=None, ra=None, r_group=0, d_K=None):

@@ -144,6 +144,34 @@ int bx_select_patches_grid_batched_counts(int njobs, const void *const *pts4, co
 /* Plain ordered ball query (pointnet2_ops.ball_query; utils/common.py:442): xyz [n,3] packed. */
 int bx_ball_query(const float *xyz, int n, const float *qry, int m, float radius, int nsample, int32_t *idx,
                   void *stream);
+/* The same over B clouds of n points each (pointnet2_ops.ball_query as the reference calls it: models/patch_embedder.py:99
+ * with B = 1 and one large cloud, utils/common.py:62,442 sphere_query with B = K patches of 512 points): xyz [B,n,3],
+ * qry [B,m,3], idx [B,m,nsample]; row j of cloud b holds the first nsample indices i (index order) with
+ * ((dx*dx)+(dy*dy))+(dz*dz) < radius*radius, padded with the first hit, all zero when nothing is hit.  Clouds of up to
+ * 4096 points are staged in shared memory (one CTA per cloud when B is large, several when B is small); larger clouds are
+ * scanned by one warp per query like bx_ball_query.  B <= 65535. */
+int bx_ball_query_batched(const float *xyz, int B, int n, const float *qry, int m, float radius, int nsample, int32_t *idx,
+                          void *stream);
+
+/* ---- pointnet2 channel-first gathers ---------------------------------------------------------
+ * Replace pointnet2_ops gather_operation (models/BUFFERX.py:289-290, 342-345) and grouping_operation
+ * (models/patch_embedder.py:101, utils/common.py:64,453): out[b][c][k] = features[b][c][idx[b][k]], features [B,C,N],
+ * idx [B,K] int32 (grouping: idx [B,M,S] with K = M*S, out [B,C,M,S]).  An index outside [0,N) gives NaN. */
+int bx_gather_channels(const float *features, int B, int C, int N, const int32_t *idx, int K, float *out, void *stream);
+
+/* ---- k = 1 nearest neighbour ----------------------------------------------------------------
+ * Replaces knn_cuda.KNN(k=1, transpose_mode=True)(ref, query) (models/BUFFERX.py:481,486,511): for each of B problems,
+ * every query row [Nq,D] finds the ref row [Nr,D] with the smallest d2 = sum over D in order, without FMA, of (q - r)^2
+ * (the arithmetic of bx_mutual_nn); the first minimum in ref order wins.  ref [B,Nr,D], qry [B,Nq,D]; keys [B*Nq] uint64
+ * workspace; dist [B,Nq] = sqrtf(d2), idx [B,Nq] int64.  Nr >= 1. */
+int bx_knn1(const float *ref, int Nr, const float *qry, int Nq, int D, int B, unsigned long long *keys, float *dist,
+            int64_t *idx, void *stream);
+
+/* ---- batched 3x3 SVD ------------------------------------------------------------------------
+ * Replaces torch_batch_svd.svd (utils/common.py:715, cal_Z_axis): A [B,3,3] -> U [B,3,3], S [B,3] descending,
+ * V [B,3,3] with A = U diag(S) V^T.  One thread per matrix, fp64 one-sided Jacobi; general (non-symmetric, singular)
+ * matrices; U and V orthonormal; singular-vector signs unspecified. */
+int bx_svd3(const float *A, int B, float *U, float *S, float *V, void *stream);
 
 /* ---- a4+a5: local reference frame + normalisation -------------------------------------------
  * Replaces MiniSpinNet.axis_align / normalize (models/patch_embedder.py:122-148, 167-170),
