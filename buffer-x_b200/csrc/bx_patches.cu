@@ -181,8 +181,8 @@ select_patches_batched_kernel(const SpJobs jobs, int P, float *__restrict__ patc
 // The streaming kernel reads the permuted cloud front to back until a key-point has its P hits: fine when a ball holds a
 // few per cent of the cloud (C2: 20 k points), wasteful for a LiDAR-sized cloud (C3: 120 k points, a ball holds < 2 %).
 // Here the cloud is binned into a spatial hash of cubic cells of edge >= radius (classic three-prime hash of the integer
-// cell coordinates, 2^17 buckets: no bounding box needed, aliases only add candidates), and a key-point looks at the 27
-// cells around it only.  The ORDER contract (first P hits in permuted-index order, patch_embedder.py:92-120) does not
+// cell coordinates, 2^17 buckets: no bounding box needed, aliases only add candidates), and a key-point looks at the cells
+// around it only (27, up to 64 far from the origin: hg_window).  The ORDER contract (first P hits in permuted-index order, patch_embedder.py:92-120) does not
 // need a sort: hits set bits in a per-key-point bitmap over the point indices (N / 8 bytes of shared memory), and the
 // bitmap is read back front to back -- counts per thread range, a block scan, then every thread emits the hits of its
 // range at their ordered slots.  Membership is the same exact test d2 < r*r as everywhere, so index rows and patches are
@@ -194,9 +194,23 @@ __device__ __forceinline__ int hg_coord(float v, float inv_cell) { return (int)f
 __device__ __forceinline__ unsigned hg_hash(int ix, int iy, int iz) {
     return ((unsigned)ix * 73856093u ^ (unsigned)iy * 19349663u ^ (unsigned)iz * 83492791u) & (unsigned)(HG_CELLS - 1);
 }
-// cell edge = radius * (1 + 1e-3): two points closer than the radius then differ by less than one cell in exact arithmetic
-// with 1e-3 of slack for the fp32 rounding of v * inv_cell (|v| / cell < 2^13 cells keeps that error below 1e-3)
+// cell edge = radius * (1 + 1e-3): two points closer than the radius differ by less than one cell in exact arithmetic, but the
+// fp32 cell value fl(v * inv_cell) carries an error of u |v * inv_cell| that outgrows the 1e-3 of slack beyond ~2^13 cells, and
+// where the value crosses a power of two a hit can land two cells away.  So the query does not take the key point's cell +-1:
+// it takes the cells of the window a -+ w, w = 0.9993 + 2^-22 |a|, a = fl(q * inv_cell), per axis (hg_window).
 __device__ __forceinline__ float hg_inv_cell(float r) { return 1.0f / (r * 1.001f); }
+// Window proof (u = 2^-24, -fmad=false).  A hit has d2 = ((dx*dx)+(dy*dy))+(dz*dz) < fl(r*r) with non-negative terms, so each
+// |q_x - p_x| < r (1 + 3.1u); r * inv_cell < 0.99901.  The point's b = fl(p_x * inv_cell) then lies within
+// 0.99901 (1 + 4.1u) + 2.0001u |a| of a, and fl(a -+ w) (one more rounding, u(|a| + w)) still encloses it, with 2e-4 to spare.
+// floorf is monotone, so floor(b), the cell the point was binned in, lies in [floorf(fl(a - w)), floorf(fl(a + w))]: at most
+// floor(2w) + 1 cells per axis -- 3, the classic query's 27 buckets, while |a| < 2900 cells; 4 up to |a| < 2^21 (w < 1.5).
+// Beyond that (and for a NaN key point) the key point scans the whole cloud; a radius of 0 (or NaN) admits no hit at all.
+constexpr float HG_WINDOW_MAX = 2097152.0f;     // 2^21 cells from the origin
+__device__ __forceinline__ void hg_window(float a, int &lo, int &n) {
+    const float w = 0.9993f + 2.384185791015625e-07f * fabsf(a);       // 0.9993 + 2^-22 |a|
+    lo = (int)floorf(a - w);
+    n = (int)floorf(a + w) - lo + 1;                                    // 2 to 4
+}
 
 __device__ __forceinline__ void hg_count_body(const float4 *__restrict__ pts4, int N, const float *__restrict__ d_radius, int *__restrict__ cnt, int i) {
     if (i >= N) return;
@@ -260,16 +274,32 @@ __device__ __forceinline__ void hg_query_body(const float4 *__restrict__ pts4, i
     for (int w = tid; w < W; w += HG_THREADS) hg_bits[w] = 0u;
     if (tid == 0) s_first = 0x7fffffff;
     __syncthreads();
-    const int cx = hg_coord(qx, ic), cy = hg_coord(qy, ic), cz = hg_coord(qz, ic);
-    for (int c = warp; c < 27; c += HG_THREADS / 32) {
-        const unsigned h = hg_hash(cx + c % 3 - 1, cy + (c / 3) % 3 - 1, cz + c / 9 - 1);
-        const int s = start[h], e = start[h + 1];
-        for (int j = s + lane; j < e; j += 32) {
-            const float4 p = sorted[j];
-            if (bx_d2(qx - p.x, qy - p.y, qz - p.z) < r2) {
-                const int i = __float_as_int(p.w);
-                atomicOr(&hg_bits[i >> 5], 1u << (i & 31));
+    const float ax = qx * ic, ay = qy * ic, az = qz * ic;
+    if (!(r2 > 0.0f)) {
+        // no point has d2 < 0: an empty ball (and no cell arithmetic on an infinite inverse cell)
+    } else if (fabsf(ax) < HG_WINDOW_MAX && fabsf(ay) < HG_WINDOW_MAX && fabsf(az) < HG_WINDOW_MAX) {
+        int lx, nx, ly, ny, lz, nz;
+        hg_window(ax, lx, nx);
+        hg_window(ay, ly, ny);
+        hg_window(az, lz, nz);
+        for (int c = warp; c < 64; c += HG_THREADS / 32) {
+            const int ix = c & 3, iy = (c >> 2) & 3, iz = c >> 4;
+            if (ix >= nx || iy >= ny || iz >= nz) continue;
+            const unsigned h = hg_hash(lx + ix, ly + iy, lz + iz);
+            const int s = start[h], e = start[h + 1];
+            for (int j = s + lane; j < e; j += 32) {
+                const float4 p = sorted[j];
+                if (bx_d2(qx - p.x, qy - p.y, qz - p.z) < r2) {
+                    const int i = __float_as_int(p.w);
+                    atomicOr(&hg_bits[i >> 5], 1u << (i & 31));
+                }
             }
+        }
+    } else {
+        // beyond 2^21 cells from the origin the window could need more than 4 cells per axis: the whole cloud
+        for (int i = tid; i < N; i += HG_THREADS) {
+            const float4 p = pts4[i];
+            if (bx_d2(qx - p.x, qy - p.y, qz - p.z) < r2) atomicOr(&hg_bits[i >> 5], 1u << (i & 31));
         }
     }
     __syncthreads();

@@ -273,8 +273,10 @@ class BufferX(nn.Module):
 
     # ------------------------------------------------------------------------------------------------
     def enable_cuda_graphs(self, flag=True, slots_per_shape=2, size_classes=False):
-        """Capture the per-pair enqueue once per slot key and replay it (no effect on results); ``forward`` then runs through
-        the same slots as ``forward_async`` (unless early exit, timing or debug is on).
+        """Capture the per-pair enqueue once per slot key and replay it (no effect on results, except for a pair whose larger
+        cloud has more than 200000 points: the capture draws its radius sub-sample on the device, not from torch's CPU generator
+        as eager ``forward`` and the reference do); ``forward`` then runs through the same slots as ``forward_async`` (unless
+        early exit, timing or debug is on).
 
         ``size_classes=False``: slots are keyed by the exact (Ns, Nt, aligned) shape (plus the early-exit setting), so a stream
         whose pairs all differ in size captures a graph for almost every pair.  ``size_classes=True``: each cloud is given a
@@ -361,7 +363,8 @@ class BufferX(nn.Module):
         2*S permutations are drawn from NumPy's global RNG at launch, also when early exit stops the pair after scale 0.
         The slot is chosen by the pair's shape, or by its clouds' size classes after
         ``enable_cuda_graphs(..., size_classes=True)``; either way the result is that of eager ``forward`` with the same
-        ``perms``."""
+        ``perms``, except on a captured slot for a pair whose larger cloud has more than 200000 points, whose radius
+        sub-sample the capture draws on the device."""
         if self.config.test.get("enable_timing", False):
             raise ops.BufferXError("forward_async needs timing disabled (the per-stage timers require host round trips)")
         Ns = int(np.prod(data_source["src_fds_pcd"].shape[:-1]))
@@ -404,7 +407,13 @@ class BufferX(nn.Module):
             pts_r, kpts_r = (src, kpts1) if Ns > Nt else (tgt, kpts2)
             denom = pts_r.shape[0] * Kr
             if pts_r.shape[0] > 200000:  # reference BUFFERX.py:664-665 (denominator keeps the original size)
-                pts_r = pts_r[torch.randint(0, pts_r.shape[0], (200000,), device=dev)].contiguous()
+                # eager: the reference's draw from the CPU generator (same indices under torch.manual_seed); under CUDA-graph
+                # capture a host draw would be frozen into the graph, so the capture draws on the device (DESIGN.md section 2)
+                if torch.cuda.is_current_stream_capturing():
+                    sub = torch.randint(0, pts_r.shape[0], (200000,), device=dev)
+                else:
+                    sub = torch.randint(0, pts_r.shape[0], (200000,)).to(dev, non_blocking=True)
+                pts_r = pts_r[sub].contiguous()
             r_dev, m_dev, _ = ops.radius_estimate(kpts_r, pts_r, thresholds, denom=denom)
         desc_t.toc()
 

@@ -110,7 +110,8 @@ int bx_select_patches(const float *pts4, int N, const float *kpts, int K, float 
 int bx_select_patches_batched(int njobs, const void *const *pts4, const int32_t *N, const void *const *kpts, const int32_t *K,
                               const void *const *d_radius, int P, float *patches, void *stream);
 /* Hash-grid form for large clouds (N >= ~50 k points): the permuted cloud is binned into a spatial hash of cells of edge >=
- * radius, a key-point tests the 27 cells around it only, hits set bits in a per-key-point bitmap over the point indices that
+ * radius, a key-point tests the cells around it only (27; up to 64 beyond ~2900 cells from the origin, the whole cloud
+ * beyond 2^21 cells, so that fp32 rounding of the cell coordinates never loses a neighbour), hits set bits in a per-key-point bitmap over the point indices that
  * is read back in index order -- same contract and bit-identical output as bx_select_patches (device-side radius required).
  * workspace: bx_select_patches_grid_workspace_bytes(N) bytes, 16-byte aligned. */
 int bx_select_patches_grid(const float *pts4, int N, const float *kpts, int K, const float *d_radius, int P, int32_t *idx,

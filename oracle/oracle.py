@@ -247,18 +247,21 @@ def radius_hist(kpts, pts) -> np.ndarray:
     return cum
 
 
-def radius_estimation(src_pts, src_kpts, tgt_pts, tgt_kpts, thresholds, tolerance=0.01, cum=None):
+def radius_estimation(src_pts, src_kpts, tgt_pts, tgt_kpts, thresholds, tolerance=0.01, cum=None, sub_idx=None):
     """``density_aware_radius_estimation`` (models/BUFFERX.py:627-696): the larger cloud wins
-    (strict >, else target); returns the list of 2-decimal radii."""
+    (strict >, else target); returns the list of 2-decimal radii.  Above 200000 points the reference histograms
+    ``pts[sub_idx]`` (its ``torch.randint`` draw, passed in here) and keeps the original size in the denominator."""
     if src_pts.shape[0] > tgt_pts.shape[0]:
         pts, kpts = src_pts, src_kpts
     else:
         pts, kpts = tgt_pts, tgt_kpts
+    denom = int(pts.shape[0]) * int(kpts.shape[0])
     if pts.shape[0] > 200000:
-        raise NotImplementedError("random 200k sub-sampling (BUFFERX.py:664-665) needs explicit indices")
+        if sub_idx is None:
+            raise NotImplementedError("random 200k sub-sampling (BUFFERX.py:664-665) needs explicit indices")
+        pts = np.asarray(pts)[np.asarray(sub_idx)]
     if cum is None:
         cum = radius_hist(kpts, pts)
-    denom = int(pts.shape[0]) * int(kpts.shape[0])
     out = []
     for th in thresholds:
         m = lib().bxo_radius_bisect(_p(cum), c_int64(denom), float(th), float(tolerance))
@@ -316,6 +319,204 @@ def horn_fit(a, b, w=None, eps=0.0):
     T = np.zeros(16, dtype=np.float64)
     lib().bxo_horn_fit(_p(a), _p(b), _p(w), a.shape[0], c_double(eps), _p(T))
     return T.reshape(4, 4)
+
+
+# --------------------------------------------------------------------------- #
+# a1-a3 evaluated in float64 from the reference's formulas (tests/test_frontend_fp64_*.py).  Torch on whichever device
+# the inputs live on; the fp32 inputs are widened exactly.  Margins use U = 2^-24; the bounds are derived in
+# tests/test_frontend_fp64_cpu.py.
+# --------------------------------------------------------------------------- #
+U24 = 2.0 ** -24
+RADIUS_MAX = 5.0
+RADIUS_BINS = 8192
+
+
+def _t64(a, device=None):
+    t = a if isinstance(a, torch.Tensor) else torch.from_numpy(np.ascontiguousarray(a, dtype=np.float32))
+    return t.to(device=device if device is not None else t.device, dtype=torch.float32).to(torch.float64)
+
+
+def _fits32(v):
+    """v (float64) is an fp32 value: the fp32 operation that produced it was exact."""
+    return v.to(torch.float32).to(torch.float64) == v
+
+
+def fps_fp64(xyz, idx, ks=4.0, kd=12.0):
+    """pointnet2 ``furthest_point_sample`` in float64 on the fp32 coordinates, teacher-forced on the picks ``idx``.
+
+    A point is skipped when mag = x*x+y*y+z*z <= 1e-3 (double literal); the skip is decided outside ks*u*1e-3 of it, or
+    exactly when every fp32 partial sum of mag is exact.  temp = running minimum of the float64 distances to the earlier
+    picks (from 1e10).  At step j the candidates are the points not decided-skipped; vmax = the largest temp of the
+    decided-valid ones, margin = kd*u*vmax.  Returns per step j >= 1 (index j-1): vmax, the pick's temp, the largest
+    decided-valid temp strictly below vmax (-1 if none), whether the pick is a candidate, whether the step is decided
+    (vmax - second > margin and no undecided-skip point within the margin of vmax or above), and the number of
+    decided-valid points."""
+    x = _t64(xyz)
+    idx = torch.as_tensor(np.asarray(idx) if not isinstance(idx, torch.Tensor) else idx).to(x.device).long()
+    n, m = x.shape[0], idx.shape[0]
+    sq = x * x
+    s1 = sq[:, 0] + sq[:, 1]
+    mag = s1 + sq[:, 2]
+    exact = _fits32(sq).all(1) & _fits32(s1) & _fits32(mag)
+    lo_m, hi_m = 1e-3 * (1 - ks * U24), 1e-3 * (1 + ks * U24)
+    valid = torch.where(exact, mag > 1e-3, mag > hi_m)
+    skip = torch.where(exact, mag <= 1e-3, mag < lo_m)
+    cand = ~skip
+    n_valid = int(valid.sum())
+    temp = torch.full((n,), 1e10, dtype=torch.float64, device=x.device)
+    steps = max(m - 1, 0)
+    vmax = torch.zeros(steps, dtype=torch.float64, device=x.device)
+    vpick, vsec = torch.zeros_like(vmax), torch.zeros_like(vmax)
+    pick_ok = torch.zeros(steps, dtype=torch.bool, device=x.device)
+    decided = torch.zeros_like(pick_ok)
+    neg = torch.tensor(-1.0, dtype=torch.float64, device=x.device)
+    for j in range(1, m):
+        d = ((x - x[idx[j - 1]]) ** 2).sum(1)
+        temp = torch.minimum(temp, d)
+        t = torch.where(valid, temp, neg)
+        mx = t.max()
+        below = torch.where(t == mx, neg, t).max()
+        und = torch.where(cand & ~valid, temp, neg).max()
+        k = idx[j]
+        vmax[j - 1], vsec[j - 1] = mx, below
+        vpick[j - 1] = torch.where(cand[k], temp[k], neg)
+        pick_ok[j - 1] = cand[k] | ((k == 0) & (n_valid == 0))
+        marg = kd * U24 * mx
+        decided[j - 1] = (mx - below > marg) & (und < mx - marg)
+    return dict(vmax=vmax, vpick=vpick, vsecond=vsec, pick_ok=pick_ok, decided=decided, n_valid=n_valid,
+                n_skip=int(skip.sum()), n_undecided_skip=int((~valid & ~skip).sum()))
+
+
+def radius_count_bounds(kpts, pts, kc=9.0, chunk=1 << 23):
+    """squared_cdist (BUFFERX.py:610-624) as count intervals over the 8193 probed radii r_m = 5 m / 8192.
+
+    d64 = |k - p|^2; the reference's (|k|^2 + |p|^2) - 2 k.p in fp32 (any order, FMA or not) lies within
+    e = kc*u*(|k|^2 + |p|^2) of it -- and equals it when every coordinate is a multiple of 2^-13 and (|k| + |p|)^2 < 1/4
+    (every partial sum is then a multiple of 2^-26 below 2^-2: exact in fp32).  The filter d2 <= max_r^2 keeps every d2
+    below a probed threshold, so it never changes a count.  Returns (lo, hi) int64 [8193]:
+    lo[m] = #{d64 + e < thr_m} <= count(m) <= hi[m] = #{d64 - e < thr_m}, thr_m = fl32(r_m^2)."""
+    k, p = _t64(kpts), _t64(pts)
+    dev = k.device
+    m = torch.arange(RADIUS_BINS + 1, dtype=torch.float64, device=dev)
+    thr = ((RADIUS_MAX * m / RADIUS_BINS) ** 2).to(torch.float32).to(torch.float64)
+    lo = torch.zeros(RADIUS_BINS + 2, dtype=torch.int64, device=dev)
+    hi = torch.zeros_like(lo)
+    k2, p2 = (k * k).sum(1), (p * p).sum(1)
+    kq = ((k * 8192.0) == torch.round(k * 8192.0)).all(1)
+    pq = ((p * 8192.0) == torch.round(p * 8192.0)).all(1)
+    kn, pn = k2.sqrt(), p2.sqrt()
+    step = max(1, chunk // max(p.shape[0], 1))
+    for a in range(0, k.shape[0], step):
+        kk = k[a:a + step]
+        d = ((kk[:, None, :] - p[None, :, :]) ** 2).sum(-1)
+        e = kc * U24 * (k2[a:a + step, None] + p2[None, :])
+        ex = kq[a:a + step, None] & pq[None, :] & ((kn[a:a + step, None] + pn[None, :]) ** 2 < 0.25)
+        e = torch.where(ex, torch.zeros_like(e), e)
+        # bin b = first m with x < thr_m (RADIUS_BINS + 1: none); cumulative counts follow
+        lo += torch.bincount(torch.searchsorted(thr, (d + e).reshape(-1), right=True), minlength=RADIUS_BINS + 2)
+        hi += torch.bincount(torch.searchsorted(thr, (d - e).reshape(-1), right=True), minlength=RADIUS_BINS + 2)
+    return lo.cumsum(0)[:RADIUS_BINS + 1].cpu().numpy(), hi.cumsum(0)[:RADIUS_BINS + 1].cpu().numpy()
+
+
+def _pct32(count, denom):
+    """points_within_radius.sum().float() / (num_pts * num_kpts) * 100 in fp32 (BUFFERX.py:682-684)."""
+    return float(np.float32(np.float32(count) / np.float32(denom)) * np.float32(100.0))
+
+
+def radius_fp64(lo, hi, denom, threshold, tolerance=0.01):
+    """The bisection of BUFFERX.py:675-694 on count intervals [lo[m], hi[m]].  pct is monotone in the count, so a
+    decision is decided when the pct of both ends falls on the same side; an undecided one follows every outcome.
+    Returns (the set of reachable m, the number of undecided decisions met, the rounded radius of each reachable m)."""
+    reach, und = set(), 0
+    stack = [(0, RADIUS_BINS, 0)]
+    while stack:
+        lo_i, hi_i, m = stack.pop()
+        if not RADIUS_MAX * hi_i / RADIUS_BINS - RADIUS_MAX * lo_i / RADIUS_BINS > 1e-3:
+            reach.add(m)
+            continue
+        m = (lo_i + hi_i) // 2
+        outs = set()
+        for c in (lo[m], hi[m]):
+            p = _pct32(c, denom)
+            outs.add(0 if p < threshold - tolerance else 2 if p > threshold + tolerance else 1)
+        if outs == {0, 2}:
+            outs.add(1)
+        und += len(outs) > 1
+        for o in outs:
+            if o == 0:
+                stack.append((m, hi_i, m))
+            elif o == 2:
+                stack.append((lo_i, m, m))
+            else:
+                reach.add(m)
+    return reach, und, {mm: np.float32(round(RADIUS_MAX * mm / RADIUS_BINS, 2)) for mm in reach}
+
+
+def radius_replay(cum, denom, threshold, tolerance=0.01, max_r=5.0):
+    """The reference loop literally (BUFFERX.py:674-694) on a cumulative histogram cum[m] = #{d2 < fl32(r_m^2)}: Python
+    float64 bisection, torch fp32 percentage, round(des_r, 2).  Returns (m, float32 radius)."""
+    low, high, des_r = 0.0, max_r, 0.0
+    while high - low > 1e-3:
+        des_r = (low + high) / 2.0
+        m = int(round(des_r * RADIUS_BINS / max_r))
+        assert max_r * m / RADIUS_BINS == des_r
+        percentage = (torch.tensor(int(cum[m]), dtype=torch.int64).float() / int(denom) * 100).item()
+        if percentage < threshold - tolerance:
+            low = des_r
+        elif percentage > threshold + tolerance:
+            high = des_r
+        else:
+            break
+    return int(round(des_r * RADIUS_BINS / max_r)), np.float32(round(des_r, 2))
+
+
+def radius_estimation_fp64(src_pts, src_kpts, tgt_pts, tgt_kpts, thresholds, tolerance=0.01, sub_idx=None):
+    """density_aware_radius_estimation (BUFFERX.py:627-696) on count intervals: the source only when it has strictly
+    more points, pts[sub_idx] above 200000 points with the original N in the denominator.  Returns dict(lo, hi, denom,
+    and per threshold (reach, undecided, radii))."""
+    if src_pts.shape[0] > tgt_pts.shape[0]:
+        pts, kpts = src_pts, src_kpts
+    else:
+        pts, kpts = tgt_pts, tgt_kpts
+    denom = int(pts.shape[0]) * int(kpts.shape[0])
+    if pts.shape[0] > 200000:
+        pts = pts[sub_idx]
+    lo, hi = radius_count_bounds(kpts, pts)
+    return dict(lo=lo, hi=hi, denom=denom, per=[radius_fp64(lo, hi, denom, th, tolerance) for th in thresholds])
+
+
+def ball_query_fp64(xyz, qry, radius, kb=7.0):
+    """pointnet2 ``ball_query`` hit test d2 < radius^2 in float64: radius^2 the fp32 product, d64 = sum (q - p)^2.  The
+    fp32 d2 = ((dx*dx)+(dy*dy))+(dz*dz), dx = fl(q - p), is within 5u d64 and equals it when every fp32 intermediate is
+    exact.  Returns status [Q,N] int8: 1 decided hit, 0 decided miss, 2 undecided."""
+    p, q = _t64(xyz), _t64(qry)
+    r = np.float32(radius)
+    r2 = float(np.float32(r * r))
+    dd = q[:, None, :] - p[None, :, :]
+    sq = dd * dd
+    s1 = sq[..., 0] + sq[..., 1]
+    d = s1 + sq[..., 2]
+    exact = _fits32(dd).all(-1) & _fits32(sq).all(-1) & _fits32(s1) & _fits32(d)
+    hit = torch.where(exact, d < r2, d * (1 + kb * U24) < r2)
+    miss = torch.where(exact, d >= r2, d * (1 - kb * U24) >= r2)
+    st = torch.full(d.shape, 2, dtype=torch.int8, device=d.device)
+    st[hit] = 1
+    st[miss] = 0
+    return st
+
+
+def select_patches_fp64(pts_perm, kpts, idx):
+    """patch_embedder.py:99-111 after the ball query, in float64 on an index row [K,P]: the gathered points, with every
+    slot s > 0 whose index equals slot 0's and always slot P-1 replaced by the key point (mask formula)."""
+    p, k = _t64(pts_perm), _t64(kpts)
+    idx = torch.as_tensor(idx).to(p.device).long()
+    P = idx.shape[1]
+    new_points = p[idx]
+    mask = (idx == idx[:, :1].repeat(1, P)).to(torch.float64)
+    mask[:, 0] = 0
+    mask[:, P - 1] = 1
+    mask = mask.unsqueeze(2)
+    return new_points * (1 - mask) + k.unsqueeze(1) * mask
 
 
 # --------------------------------------------------------------------------- #
