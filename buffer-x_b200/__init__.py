@@ -32,7 +32,7 @@ _alias()
 from . import models  # noqa: E402,F401
 from .models import patchnet, patch_embedder, pose_estimator, BUFFERX  # noqa: E402,F401
 from .models.BUFFERX import BufferX  # noqa: E402,F401
-from . import driver, bootstrap, evaluation  # noqa: E402,F401
+from . import driver, bootstrap, evaluation, registration  # noqa: E402,F401
 _alias()
 
 __version__ = "0.2.0"

@@ -18,12 +18,13 @@ import torch
 from bufferx_b200 import ops
 
 
-def _cloud(x, device):
+def _cloud(x, device, dtype=torch.float32):
+    """An Open3D-like cloud (``.points``), array or tensor -> contiguous [N,3] `dtype` tensor on `device`."""
     if hasattr(x, "points"):
         x = np.asarray(x.points)
     if not isinstance(x, torch.Tensor):
-        x = torch.from_numpy(np.ascontiguousarray(np.asarray(x), dtype=np.float32))
-    return x.to(device=device, dtype=torch.float32).reshape(-1, 3).contiguous()
+        x = torch.from_numpy(np.ascontiguousarray(np.asarray(x), dtype=torch.empty((), dtype=dtype).numpy().dtype))
+    return x.to(device=device, dtype=dtype).reshape(-1, 3).contiguous()
 
 
 def compute_pca_alignment(pts: torch.Tensor, sample_idx=None):

@@ -5,7 +5,7 @@
 Two groups of translation units:
   EXACT  compiled with -fmad=false: every kernel whose result feeds an integer / index decision
          that must be bit-identical to the oracle (FPS, radius histogram, ball query, LRF, SPT,
-         matching, consensus, RANSAC).
+         matching, consensus, RANSAC, ICP).
   FAST   compiled with FMA contraction: the convolution stacks (tolerance parity).
 The shared object lands next to the package (buffer-x_b200/libbufferx_b200.so); it is git-ignored.
 """
@@ -20,7 +20,7 @@ OUT = os.path.join(PKG, "libbufferx_b200.so")
 OBJ = os.path.join(HERE, "_obj")
 
 EXACT = ["bx_api.cu", "bx_fps.cu", "bx_radius.cu", "bx_patches.cu", "bx_spt.cu", "bx_match.cu", "bx_ransac.cu", "bx_neighbors.cu",
-         "bx_bootstrap.cu", "bx_train.cu", "bx_group.cu", "bx_svd.cu"]
+         "bx_bootstrap.cu", "bx_train.cu", "bx_group.cu", "bx_svd.cu", "bx_icp.cu"]
 FAST = ["bx_conv.cu", "bx_conv_tc.cu", "bx_conv_sd.cu"]
 ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 COMMON = ["-O3", "-lineinfo", "-std=c++17", "-Xcompiler", "-fPIC,-fvisibility=hidden", "--expt-relaxed-constexpr"]

@@ -15,6 +15,7 @@
 //
 // Bit contract: oracle/c/bx_oracle.c::bxo_ball_query / bxo_select_patches / bxo_lrf.  -fmad=false.
 #include "bx_common.cuh"
+#include "bx_hashgrid.cuh"
 
 namespace {
 
@@ -187,18 +188,13 @@ select_patches_batched_kernel(const SpJobs jobs, int P, float *__restrict__ patc
 // bitmap is read back front to back -- counts per thread range, a block scan, then every thread emits the hits of its
 // range at their ordered slots.  Membership is the same exact test d2 < r*r as everywhere, so index rows and patches are
 // bit-identical to the streaming kernel (tests/test_gpu_parity.py::test_select_patches_grid_equals_scan).
-constexpr int HG_BITS = 17, HG_CELLS = 1 << HG_BITS;
+// The binning phases (hg_count_body, hg_scan_body, hg_scatter_body) live in bx_hashgrid.cuh.
 constexpr int HG_THREADS = 128;
 
-__device__ __forceinline__ int hg_coord(float v, float inv_cell) { return (int)floorf(v * inv_cell); }
-__device__ __forceinline__ unsigned hg_hash(int ix, int iy, int iz) {
-    return ((unsigned)ix * 73856093u ^ (unsigned)iy * 19349663u ^ (unsigned)iz * 83492791u) & (unsigned)(HG_CELLS - 1);
-}
-// cell edge = radius * (1 + 1e-3): two points closer than the radius differ by less than one cell in exact arithmetic, but the
+// cell edge = radius * (1 + 1e-3) (hg_inv_cell): two points closer than the radius differ by less than one cell in exact arithmetic, but the
 // fp32 cell value fl(v * inv_cell) carries an error of u |v * inv_cell| that outgrows the 1e-3 of slack beyond ~2^13 cells, and
 // where the value crosses a power of two a hit can land two cells away.  So the query does not take the key point's cell +-1:
 // it takes the cells of the window a -+ w, w = 0.9993 + 2^-22 |a|, a = fl(q * inv_cell), per axis (hg_window).
-__device__ __forceinline__ float hg_inv_cell(float r) { return 1.0f / (r * 1.001f); }
 // Window proof (u = 2^-24, -fmad=false).  A hit has d2 = ((dx*dx)+(dy*dy))+(dz*dz) < fl(r*r) with non-negative terms, so each
 // |q_x - p_x| < r (1 + 3.1u); r * inv_cell < 0.99901.  The point's b = fl(p_x * inv_cell) then lies within
 // 0.99901 (1 + 4.1u) + 2.0001u |a| of a, and fl(a -+ w) (one more rounding, u(|a| + w)) still encloses it, with 2e-4 to spare.
@@ -212,50 +208,12 @@ __device__ __forceinline__ void hg_window(float a, int &lo, int &n) {
     n = (int)floorf(a + w) - lo + 1;                                    // 2 to 4
 }
 
-__device__ __forceinline__ void hg_count_body(const float4 *__restrict__ pts4, int N, const float *__restrict__ d_radius, int *__restrict__ cnt, int i) {
-    if (i >= N) return;
-    const float ic = hg_inv_cell(*d_radius);
-    const float4 p = pts4[i];
-    atomicAdd(cnt + hg_hash(hg_coord(p.x, ic), hg_coord(p.y, ic), hg_coord(p.z, ic)), 1);
-}
 __global__ void hg_count_kernel(const float4 *__restrict__ pts4, int N, const float *__restrict__ d_radius, int *__restrict__ cnt) {
     hg_count_body(pts4, N, d_radius, cnt, blockIdx.x * blockDim.x + threadIdx.x);
 }
 
-// exclusive scan of the HG_CELLS bucket counts (one CTA of 1024 threads, 128 consecutive buckets per thread, 16-byte accesses);
-// cursor = start
-__device__ __forceinline__ void hg_scan_body(const int *__restrict__ cnt, int *__restrict__ start, int *__restrict__ cursor) {
-    __shared__ int sh[33];
-    constexpr int PER4 = HG_CELLS / 1024 / 4;
-    const int t = threadIdx.x;
-    const int4 *c4 = reinterpret_cast<const int4 *>(cnt) + (size_t)t * PER4;
-    int local = 0;
-#pragma unroll 8
-    for (int j = 0; j < PER4; ++j) { const int4 v = c4[j]; local += (v.x + v.y) + (v.z + v.w); }
-    int total;
-    int run = bx_block_exscan(local, sh, &total);
-    int4 *s4 = reinterpret_cast<int4 *>(start) + (size_t)t * PER4, *u4 = reinterpret_cast<int4 *>(cursor) + (size_t)t * PER4;
-#pragma unroll 8
-    for (int j = 0; j < PER4; ++j) {
-        const int4 v = c4[j];
-        int4 o;
-        o.x = run; o.y = o.x + v.x; o.z = o.y + v.y; o.w = o.z + v.z;
-        run = o.w + v.w;
-        s4[j] = o;
-        u4[j] = o;
-    }
-    if (t == 1023) start[HG_CELLS] = run;
-}
 __global__ void __launch_bounds__(1024) hg_scan_kernel(const int *__restrict__ cnt, int *__restrict__ start, int *__restrict__ cursor) { hg_scan_body(cnt, start, cursor); }
 
-__device__ __forceinline__ void hg_scatter_body(const float4 *__restrict__ pts4, int N, const float *__restrict__ d_radius, int *__restrict__ cursor,
-                                                float4 *__restrict__ sorted, int i) {
-    if (i >= N) return;
-    const float ic = hg_inv_cell(*d_radius);
-    const float4 p = pts4[i];
-    const int pos = atomicAdd(cursor + hg_hash(hg_coord(p.x, ic), hg_coord(p.y, ic), hg_coord(p.z, ic)), 1);
-    sorted[pos] = make_float4(p.x, p.y, p.z, __int_as_float(i));        // the order inside a bucket does not matter (bitmap)
-}
 __global__ void hg_scatter_kernel(const float4 *__restrict__ pts4, int N, const float *__restrict__ d_radius, int *__restrict__ cursor,
                                   float4 *__restrict__ sorted) {
     hg_scatter_body(pts4, N, d_radius, cursor, sorted, blockIdx.x * blockDim.x + threadIdx.x);

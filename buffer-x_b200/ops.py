@@ -29,7 +29,7 @@ SYMBOLS = [
     "bx_mutual_nn_n", "bx_early_exit_gate",
     "bx_fps_n", "bx_fps_size_class", "bx_radius_estimate_n", "bx_permute_cloud_n", "bx_select_patches_batched_counts",
     "bx_select_patches_grid_batched_counts",
-    "bx_ball_query_batched", "bx_gather_channels", "bx_knn1", "bx_svd3",
+    "bx_ball_query_batched", "bx_gather_channels", "bx_knn1", "bx_svd3", "bx_icp_workspace_bytes", "bx_icp",
 ]
 
 GEOM_CYL3D, GEOM_CYL2D, GEOM_VALID3D, GEOM_COSTAB = 0, 1, 2, 4
@@ -116,6 +116,9 @@ def load_library():
     lib.bx_so2_augment.argtypes = [P, c_int, c_int, P, P, P, P]
     lib.bx_equi_match.argtypes = [P, P, c_int, c_int, c_int, c_int, P, P]
     lib.bx_so2_gt.argtypes = [P, P, P, P, P, c_int, c_int, P, P, P]
+    lib.bx_icp_workspace_bytes.argtypes = [c_int, c_int]
+    lib.bx_icp_workspace_bytes.restype = c_int64
+    lib.bx_icp.argtypes = [P, c_int, P, c_int, c_double, P, c_double, c_double, c_int, P, P, P, P]
     _lib = lib
     return lib
 
@@ -918,3 +921,34 @@ def so2_gt(s_rand_axis, s_R, t_R, T, azi_n: int, integer: bool, aug_R=None):
     _check(load_library().bx_so2_gt(_dp(s_rand_axis, F32, "s_rand_axis"), _dp(s_R, F32, "s_R"), _dp(t_R, F32, "t_R"), _dp(T, F32, "T"),
                                     _dp(aug_R, F32, "aug_R"), P, int(azi_n), li, lf, _stream()), "bx_so2_gt")
     return out
+
+
+def icp(src: torch.Tensor, tgt: torch.Tensor, max_correspondence_distance: float, init: torch.Tensor, relative_fitness: float,
+        relative_rmse: float, max_iteration: int):
+    """Point-to-point ICP (bx_icp): src [Ns,3], tgt [Nt,3], init [4,4] float64 CUDA tensors.  Returns (result float64 [20] =
+    T (16) + fitness + inlier_rmse + int32 {num_correspondences, iterations, converged, 0}, corr int32 [Ns]: each source
+    point's target index or -1), both on the device; nothing is read back."""
+    for t, name in ((src, "src"), (tgt, "tgt")):
+        if t.dim() != 2 or t.shape[1] != 3 or t.shape[0] < 1:
+            raise BufferXError(f"icp: {name} must be [N,3] with N >= 1, got {tuple(t.shape)}")
+    if init.numel() != 16:
+        raise BufferXError(f"icp: init must hold a 4x4 matrix (16 doubles), got {tuple(init.shape)}")
+    lib = load_library()
+    Ns, Nt = src.shape[0], tgt.shape[0]
+    dev = src.device
+    ws = torch.empty((int(lib.bx_icp_workspace_bytes(Ns, Nt)) + 255) // 8 + 32, dtype=torch.float64, device=dev)
+    off = (-ws.data_ptr()) % 256 // 8                                    # the workspace must be 256-byte aligned
+    result = torch.empty(20, dtype=F64, device=dev)
+    corr = torch.empty(max(Ns, 1), dtype=I32, device=dev)
+    with _Span("icp"):
+        _check(lib.bx_icp(_dp(src, F64, "src"), Ns, _dp(tgt, F64, "tgt"), Nt, float(max_correspondence_distance),
+                          _dp(init, F64, "init"), float(relative_fitness), float(relative_rmse), int(max_iteration), _dp(corr),
+                          _dp(result), ws[off:].data_ptr(), _stream()), "bx_icp")
+    return result, corr
+
+
+def decode_icp_result(result_cpu: torch.Tensor):
+    """-> (T [4,4] float64, fitness, inlier_rmse, num_correspondences, iterations, converged)."""
+    T = result_cpu[:16].reshape(4, 4).numpy().copy()
+    ints = result_cpu[18:20].numpy().view(np.int32)
+    return T, float(result_cpu[16]), float(result_cpu[17]), int(ints[0]), int(ints[1]), bool(ints[2])

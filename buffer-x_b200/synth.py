@@ -328,3 +328,19 @@ def init_synthetic_weights(model, seed: int = 123, logit_gain: float = 4.0, trai
         if hasattr(m, "invalidate"):
             m.invalidate()
     return model
+
+
+def kitti_icp_pair(seed: int = 0, n: int | None = None):
+    """The KITTI loader's ground-truth ICP input (dataset/kitti.py:95-102) on a C3-sized synthetic scan pair: the source scan
+    (float32 values) pre-aligned by its ground truth perturbed by 0.5 deg and 5 cm, as the loader pre-aligns by the odometry
+    poses.  -> (source [N,3], target [N,3]) float64; the call is r = 0.20, init = I, max_iteration = 200."""
+    d = make_pair("C3", seed, n_src=n, n_tgt=n)
+    rng = np.random.default_rng(seed + 77)
+    ax = rng.normal(size=3)
+    ax /= np.linalg.norm(ax)
+    K = np.array([[0, -ax[2], ax[1]], [ax[2], 0, -ax[0]], [-ax[1], ax[0], 0]])
+    t = math.radians(0.5)
+    P = _se3(np.eye(3) + math.sin(t) * K + (1 - math.cos(t)) * (K @ K), rng.normal(size=3) * 0.05 / math.sqrt(3))
+    M = P @ np.asarray(d["relt_pose"], np.float64)
+    src = (d["src_fds_pcd"].astype(np.float64) @ M[:3, :3].T + M[:3, 3]).astype(np.float32).astype(np.float64)
+    return src, d["tgt_fds_pcd"].astype(np.float64)

@@ -416,6 +416,25 @@ int bx_equi_match(const float *D1, const float *D2, int B, int C, int K, int L, 
 int bx_so2_gt(const float *s_rand_axis, const float *s_R, const float *t_R, const float *T, const float *aug_R, int P,
               int azi_n, long long *label_int, float *label_float, void *stream);
 
+/* ---- loader-side ground truth: point-to-point ICP ---------------------------------------------------
+ * Replaces open3d.pipelines.registration.registration_icp(source, target, r, init, TransformationEstimationPointToPoint(),
+ * ICPConvergenceCriteria(...)) (Open3D 0.18), which the KITTI loader runs on the CPU to refine every pair's ground-truth
+ * pose (dataset/kitti.py:95-102: the two raw scans, r = 0.20, init = I, max_iteration = 200).  Open3D's loop: evaluate
+ * (nearest target with float64 d2 < r*r per source point; fitness = correspondences / n_src, inlier_rmse = sqrt(sum d2 /
+ * correspondences), 0 without any), then up to max_iteration times: Umeyama update (with_scaling = false; the identity
+ * without correspondences), transformation = update * transformation, source copy transformed by the update, re-evaluate,
+ * stop when |d fitness| < relative_fitness and |d rmse| < relative_rmse.  Assumptions where Open3D defers to FLANN: the
+ * radius test is strict and ties between equidistant targets go to the lowest target index.
+ * src [n_src,3], tgt [n_tgt,3] and init [16] (row-major 4x4) are float64; n_src, n_tgt >= 1; r > 0 and finite.
+ * corr [n_src] int32: each source point's target of the final evaluation, or -1.  result (8-byte aligned): 16 doubles T,
+ * double fitness, double inlier_rmse, int32 {num_correspondences, iterations (updates applied), converged, reserved} =
+ * 160 bytes.  workspace: bx_icp_workspace_bytes(n_src, n_tgt) bytes, 256-byte aligned.  All max_iteration steps are
+ * enqueued at once; the steps after the stop return at once on the device. */
+int64_t bx_icp_workspace_bytes(int n_src, int n_tgt);
+int bx_icp(const double *src, int n_src, const double *tgt, int n_tgt, double max_correspondence_distance, const double *init,
+           double relative_fitness, double relative_rmse, int max_iteration, int32_t *corr, void *result, void *workspace,
+           void *stream);
+
 #ifdef __cplusplus
 }
 #endif
