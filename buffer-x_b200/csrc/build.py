@@ -19,7 +19,7 @@ PKG = os.path.dirname(HERE)
 OUT = os.path.join(PKG, "libbufferx_b200.so")
 OBJ = os.path.join(HERE, "_obj")
 
-EXACT = ["bx_api.cu", "bx_fps.cu", "bx_radius.cu", "bx_patches.cu", "bx_spt.cu", "bx_match.cu", "bx_ransac.cu", "bx_neighbors.cu",
+EXACT = ["bx_api.cu", "bx_fps.cu", "bx_fps_large.cu", "bx_radius.cu", "bx_patches.cu", "bx_spt.cu", "bx_match.cu", "bx_ransac.cu", "bx_neighbors.cu",
          "bx_bootstrap.cu", "bx_train.cu", "bx_group.cu", "bx_svd.cu", "bx_icp.cu"]
 FAST = ["bx_conv.cu", "bx_conv_tc.cu", "bx_conv_sd.cu"]
 ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]

@@ -358,6 +358,17 @@ class BufferX(nn.Module):
         self._rr[key] = i + 1
         return slot
 
+    @staticmethod
+    def _cloud_sizes(data_source):
+        """(Ns, Nt) of a pair; refuses, before anything is launched, a cloud larger than the patch gatherer's shared-memory
+        bitmap holds (ops.FPS_LARGE_MAX_POINTS points)."""
+        sizes = tuple(int(np.prod(np.shape(data_source[k])[:-1])) for k in ("src_fds_pcd", "tgt_fds_pcd"))
+        for name, n in zip(("source", "target"), sizes):
+            if n > ops.FPS_LARGE_MAX_POINTS:
+                raise ops.BufferXError(f"BufferX: the {name} cloud has {n} points; clouds of up to {ops.FPS_LARGE_MAX_POINTS} "
+                                       "points are supported (the patch gatherer's shared-memory bitmap holds one bit per point)")
+        return sizes
+
     def forward_async(self, data_source, perms=None):
         """Enqueue one pair on a slot stream; returns a handle whose ``result()`` is the forward tuple.  Without ``perms`` the
         2*S permutations are drawn from NumPy's global RNG at launch, also when early exit stops the pair after scale 0.
@@ -367,8 +378,7 @@ class BufferX(nn.Module):
         sub-sample the capture draws on the device."""
         if self.config.test.get("enable_timing", False):
             raise ops.BufferXError("forward_async needs timing disabled (the per-stage timers require host round trips)")
-        Ns = int(np.prod(data_source["src_fds_pcd"].shape[:-1]))
-        Nt = int(np.prod(data_source["tgt_fds_pcd"].shape[:-1]))
+        Ns, Nt = self._cloud_sizes(data_source)
         return self._slot(Ns, Nt, bool(data_source["is_aligned_to_global_z"])).launch(data_source, perms)
 
     # ------------------------------------------------------------------------------------------------
@@ -397,7 +407,13 @@ class BufferX(nn.Module):
         if xyz is None:
             xyz = torch.cat([src, tgt], dim=0)
         nfps = max(Kr, K)
-        fidx, fk = ops.fps(xyz, [0, Ns, Ns + Nt], nfps, max_cluster=self._fps_cluster, d_counts=counts)
+        if max(Ns, Nt) <= ops.FPS_MAX_POINTS:
+            fidx, fk = ops.fps(xyz, [0, Ns, Ns + Nt], nfps, max_cluster=self._fps_cluster, d_counts=counts)
+        else:   # beyond one cluster's registers: that cloud on the grid-wide kernel (exact-shape pairs only, counts is None)
+            per = [ops.fps_large(c, nfps) if c.shape[0] > ops.FPS_MAX_POINTS
+                   else ops.fps(c, [0, c.shape[0]], nfps, max_cluster=self._fps_cluster) for c in (src, tgt)]
+            fidx = torch.stack([i.reshape(nfps) for i, _ in per])
+            fk = torch.stack([k.reshape(nfps, 3) for _, k in per])
         kpts1, kpts2 = fk[0, :Kr].contiguous(), fk[1, :Kr].contiguous()
         src_kpts, tgt_kpts = fk[0, :K].contiguous(), fk[1, :K].contiguous()
         # ---- density-aware radii of every scale from one histogram ------------------------------------
@@ -726,6 +742,7 @@ class BufferX(nn.Module):
         dev = next(self.parameters()).device
         if dev.type != "cuda":
             raise ops.BufferXError("BufferX.forward needs the model on a CUDA device: there is no CPU path")
+        self._cloud_sizes(data_source)
         if self._use_graphs and not debug and ransac_seed is None and self._graphable():
             return self.forward_async(data_source, perms).result()
 

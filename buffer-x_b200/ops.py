@@ -30,6 +30,7 @@ SYMBOLS = [
     "bx_fps_n", "bx_fps_size_class", "bx_radius_estimate_n", "bx_permute_cloud_n", "bx_select_patches_batched_counts",
     "bx_select_patches_grid_batched_counts",
     "bx_ball_query_batched", "bx_gather_channels", "bx_knn1", "bx_svd3", "bx_icp_workspace_bytes", "bx_icp",
+    "bx_fps_large", "bx_fps_large_workspace_bytes",
 ]
 
 GEOM_CYL3D, GEOM_CYL2D, GEOM_VALID3D, GEOM_COSTAB = 0, 1, 2, 4
@@ -64,6 +65,9 @@ def load_library():
     lib.bx_fps_ex.argtypes = [P, P, c_int, c_int, P, P, c_int, P]
     lib.bx_fps_n.argtypes = [P, P, c_int, c_int, P, P, c_int, P, P]
     lib.bx_fps_size_class.argtypes = [c_int, c_int]
+    lib.bx_fps_large.argtypes = [P, c_int, c_int, P, P, P, P]
+    lib.bx_fps_large_workspace_bytes.argtypes = [c_int]
+    lib.bx_fps_large_workspace_bytes.restype = c_int64
     lib.bx_radius_estimate_n.argtypes = [P, P, c_int, P, P, c_int, c_int, P, P, c_int, c_double, P, P, P, P, P]
     lib.bx_permute_cloud_n.argtypes = [P, P, c_int, P, P, P]
     lib.bx_select_patches_batched_counts.argtypes = [c_int, P, P, P, P, P, P, P, c_int, P, P]
@@ -218,6 +222,25 @@ def fps(xyz: torch.Tensor, offsets, npoint: int, want_kpts=True, max_cluster=0, 
             assert d_counts.numel() >= B
             _check(lib.bx_fps_n(_dp(xyz, F32, "xyz"), off.ctypes.data_as(c_void_p), B, npoint, _dp(idx), _dp(kp), int(max_cluster),
                                 _dp(d_counts, I32, "d_counts"), _stream()), "bx_fps_n")
+    return idx, kp
+
+
+FPS_MAX_POINTS = 524288          # bx_fps: one 16-CTA cluster's registers
+FPS_LARGE_MAX_POINTS = 1638400   # bx_fps_large: the patch gatherer's shared-memory bitmap bounds every cloud of a pair
+
+
+def fps_large(xyz: torch.Tensor, npoint: int, want_kpts=True):
+    """One cloud xyz [N,3] f32 cuda, 1 <= N <= FPS_LARGE_MAX_POINTS, on the grid-wide kernel (bx_fps_large).  Returns idx
+    [npoint] i32, kpts [npoint,3] (None unless want_kpts): for any N the indices ops.fps gives where it accepts N."""
+    if xyz.dim() != 2 or xyz.shape[1] != 3 or xyz.shape[0] < 1:
+        raise BufferXError(f"fps_large: xyz must be [N,3] with N >= 1, got {tuple(xyz.shape)}")
+    lib = load_library()
+    N = xyz.shape[0]
+    idx = torch.empty(npoint, dtype=I32, device=xyz.device)
+    kp = torch.empty((npoint, 3), dtype=F32, device=xyz.device) if want_kpts else None
+    ws = torch.empty(int(lib.bx_fps_large_workspace_bytes(N)), dtype=torch.uint8, device=xyz.device)
+    with _Span("fps_large"):
+        _check(lib.bx_fps_large(_dp(xyz, F32, "xyz"), N, int(npoint), _dp(idx), _dp(kp), _dp(ws), _stream()), "bx_fps_large")
     return idx, kp
 
 

@@ -69,6 +69,15 @@ int bx_fps_size_class(int n, int max_cluster);
  * (racecheck-clean reference form), 2 = remote stores + remote mbarrier arrive / acquire wait (round 1), -1 = BX_FPS_SYNC
  * environment variable.  Same results in every mode.  Returns the old value. */
 int bx_fps_set_sync_mode(int mode);
+/* One cloud of any size up to 1638400 points (models/BUFFERX.py:286-290 on the first-downsampled clouds of dense sensors,
+ * which bx_fps refuses above 524288 points): xyz [n,3], idx [npoint] int32, kpts [npoint,3] (may be NULL).  Same result
+ * contract as bx_fps, so any n gives bx_fps's indices.  The cloud is spread over ceil(n / 18432) SMs of one cooperative
+ * grid (coordinates in shared memory, running distances in registers) that exchanges one candidate per SM and iteration
+ * through global memory; capturable into a CUDA graph.  workspace: bx_fps_large_workspace_bytes(n) bytes, 16-byte aligned,
+ * not shared with a launch in flight.  1638400 is the limit of the patch gatherer's shared-memory bitmap
+ * (bx_select_patches_grid): a larger n is refused. */
+int bx_fps_large(const float *xyz, int n, int npoint, int32_t *idx, float *kpts, void *workspace, void *stream);
+long long bx_fps_large_workspace_bytes(int n);
 
 /* ---- a2: density-aware radius estimation ----------------------------------------------------
  * Replaces density_aware_radius_estimation + squared_cdist (models/BUFFERX.py:610-696) without
