@@ -193,8 +193,9 @@ __global__ void so2_gt_kernel(const float *__restrict__ s_ra, const float *__res
 
 BX_API int bx_gt_matches(const float *src, int N, const float *tgt, int M, const float *T, float voxel, int32_t *nn_ws,
                          int32_t *pairs, int32_t *d_count, void *stream) {
-    BX_REQUIRE(src && (tgt || M == 0) && T && nn_ws && pairs && d_count, "bx_gt_matches: null pointer");
+    // an empty tensor has no storage: src / tgt may be null when N / M is 0
     BX_REQUIRE(N >= 0 && M >= 0, "bx_gt_matches: negative size");
+    BX_REQUIRE((src || N == 0) && (tgt || M == 0) && T && nn_ws && pairs && d_count, "bx_gt_matches: null pointer");
     cudaStream_t st = bx_stream(stream);
     if (N == 0) {
         BX_CUDA(cudaMemsetAsync(d_count, 0, sizeof(int), st));
@@ -208,20 +209,20 @@ BX_API int bx_gt_matches(const float *src, int N, const float *tgt, int M, const
 }
 
 BX_API int bx_so2_augment(float *delta, int K, int P, float *rand_axis, const float *angles, float *aug_R, void *stream) {
-    BX_REQUIRE(delta && rand_axis && angles, "bx_so2_augment: null pointer");
     BX_REQUIRE(K >= 0 && P >= 1, "bx_so2_augment: bad sizes");
-    if (K == 0) return BX_OK;
+    if (K == 0) return BX_OK;                       // no patches: the (empty) tensors may have no storage
+    BX_REQUIRE(delta && rand_axis && angles, "bx_so2_augment: null pointer");
     so2_augment_kernel<<<K, 256, 0, bx_stream(stream)>>>(delta, P, rand_axis, angles, aug_R);
     BX_LAUNCH_CHECK();
     return BX_OK;
 }
 
 BX_API int bx_equi_match(const float *D1, const float *D2, int B, int C, int K, int L, float *cor, void *stream) {
-    BX_REQUIRE(D1 && D2 && cor, "bx_equi_match: null pointer");
     BX_REQUIRE(B >= 0 && C >= 1 && K >= 1 && L >= 1 && L <= 32, "bx_equi_match: bad sizes (1 <= L <= 32)");
     const size_t smem = 2 * (size_t)C * K * L * sizeof(float);
     BX_REQUIRE(smem <= 48 * 1024, "bx_equi_match: maps of %d x %d x %d do not fit in shared memory", C, K, L);
-    if (B == 0) return BX_OK;
+    if (B == 0) return BX_OK;                       // no patches: the (empty) tensors may have no storage
+    BX_REQUIRE(D1 && D2 && cor, "bx_equi_match: null pointer");
     equi_match_kernel<<<B, 32 * L, smem, bx_stream(stream)>>>(D1, D2, C, K, L, cor);
     BX_LAUNCH_CHECK();
     return BX_OK;
@@ -229,10 +230,10 @@ BX_API int bx_equi_match(const float *D1, const float *D2, int B, int C, int K, 
 
 BX_API int bx_so2_gt(const float *s_rand_axis, const float *s_R, const float *t_R, const float *T, const float *aug_R, int P,
                      int azi_n, long long *label_int, float *label_float, void *stream) {
+    BX_REQUIRE(P >= 0 && azi_n >= 1, "bx_so2_gt: bad sizes");
+    if (P == 0) return BX_OK;                       // no patches: the (empty) tensors may have no storage
     BX_REQUIRE(s_rand_axis && s_R && t_R && T, "bx_so2_gt: null pointer");
     BX_REQUIRE((label_int != nullptr) != (label_float != nullptr), "bx_so2_gt: exactly one of label_int / label_float");
-    BX_REQUIRE(P >= 0 && azi_n >= 1, "bx_so2_gt: bad sizes");
-    if (P == 0) return BX_OK;
     so2_gt_kernel<<<(P + 127) / 128, 128, 0, bx_stream(stream)>>>(s_rand_axis, s_R, t_R, T, aug_R, P, azi_n, label_int,
                                                                   label_float);
     BX_LAUNCH_CHECK();

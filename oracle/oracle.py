@@ -936,16 +936,32 @@ def soft_argmax(logits: torch.Tensor) -> torch.Tensor:
     return torch.sum(prob * torch.arange(lg.shape[-1], dtype=torch.float64)[None], dim=-1)
 
 
-def azimuth_rotation(angle: torch.Tensor) -> torch.Tensor:
-    """kornia ``axis_angle_to_rotation_matrix`` for the axis-angle (0,0,angle) (BUFFERX.py:383-386)."""
+def soft_argmax_bound(l64: torch.Tensor, l32: torch.Tensor):
+    """The a11 bound on a soft arg-max bin against float64 logits ``l64``, given the fp32 oracle's logits ``l32`` of the same
+    rows -> (ind64, bound, s, ind32_err).  1e-4 (about 10x the fp32 oracle's error on a single peak), scaled by
+    s = sum p_k |k - ind| (d ind / d logit_k = p_k (k - ind), so a row whose mass sits at both ends of the bin range turns
+    the same fp32-grade logit error into a larger bin error; s <= 1 on a single peak), at least 1.5 x the fp32 oracle's own
+    error on the row, never beyond 2e-4."""
+    ind64 = soft_argmax(l64)
+    ind32_err = (soft_argmax(l32) - ind64).abs()
+    p = torch.softmax(l64, dim=1)
+    s = (p * (torch.arange(l64.shape[1], dtype=torch.float64)[None] - ind64[:, None]).abs()).sum(dim=1)
+    bound = torch.clamp(torch.maximum(1e-4 * s.clamp(min=1.0), 1.5 * ind32_err), max=2e-4)
+    return ind64, bound, s, ind32_err
+
+
+def azimuth_rotation(angle: torch.Tensor, _mutations=()) -> torch.Tensor:
+    """kornia ``axis_angle_to_rotation_matrix`` for the axis-angle (0,0,angle) (BUFFERX.py:383-386).  ``_mutations``
+    (tests/test_train_fp64_cpu.py only): "no_eps" drops the + 1e-6 of the axis, "ge_threshold" takes the full form at
+    theta^2 >= 1e-6."""
     theta2 = angle * angle
     theta = torch.sqrt(theta2)
-    wz = angle / (theta + 1e-6)
+    wz = angle / theta if "no_eps" in _mutations else angle / (theta + 1e-6)
     c, s = torch.cos(theta), torch.sin(theta)
     one, zero = torch.ones_like(c), torch.zeros_like(c)
     Rn = torch.stack([c, -wz * s, zero, wz * s, c, zero, zero, zero, c + wz * wz * (one - c)], dim=1).view(-1, 3, 3)
     Rt = torch.stack([one, -angle, zero, angle, one, zero, zero, zero, one], dim=1).view(-1, 3, 3)
-    mask = (theta2 > 1e-6).view(-1, 1, 1)
+    mask = ((theta2 >= 1e-6) if "ge_threshold" in _mutations else (theta2 > 1e-6)).view(-1, 1, 1)
     return torch.where(mask, Rn, Rt)
 
 

@@ -34,9 +34,15 @@ def transform(pts, T):
     return np.stack([(((T[j, 0] * x) + (T[j, 1] * y)) + (T[j, 2] * z)) + T[j, 3] for j in range(3)], axis=1)
 
 
-def matching_indices(src, tgt, T, voxel, chunk=512):
+def matching_indices(src, tgt, T, voxel, chunk=512, _mutations=()):
     """[C,2] int64 ([i, nn(i)] in source order): nearest target point of every transformed source point (first minimum
-    in target order wins), kept where sqrt(((dx*dx) + (dy*dy)) + (dz*dz)) < voxel."""
+    in target order wins), kept where sqrt(((dx*dx) + (dy*dy)) + (dz*dz)) < voxel.  ``_mutations``
+    (tests/test_train_fp64_cpu.py only): "le" keeps at <= voxel, "last_tie" lets the last minimum win, "T_transposed"
+    applies R^T."""
+    T = _f32(T)
+    if "T_transposed" in _mutations:
+        T = T.copy()
+        T[:3, :3] = T[:3, :3].T
     q = transform(src, T)
     t = _f32(tgt)
     v = F32(voxel)
@@ -51,11 +57,38 @@ def matching_indices(src, tgt, T, voxel, chunk=512):
         dy = q[a:b, 1, None] - t[None, :, 1]
         dz = q[a:b, 2, None] - t[None, :, 2]
         d2 = ((dx * dx) + (dy * dy)) + (dz * dz)
-        j = np.argmin(d2, axis=1)
+        j = (d2.shape[1] - 1 - np.argmin(d2[:, ::-1], axis=1)) if "last_tie" in _mutations else np.argmin(d2, axis=1)
         nn[a:b] = j
-        keep[a:b] = np.sqrt(d2[np.arange(b - a), j]) < v
+        d = np.sqrt(d2[np.arange(b - a), j])
+        keep[a:b] = (d <= v) if "le" in _mutations else (d < v)
     i = np.flatnonzero(keep)
     return np.stack([i, nn[i]], axis=1).astype(np.int64)
+
+
+def matching_indices_fp64(src, tgt, T, voxel, rows=None, chunk=256):
+    """get_matching_indices (BUFFERX.py:498-520) in float64 on the fp32 inputs: q = R p + t, the nearest target (the
+    lowest index wins a tie, knn_cuda's rule) and the strict keep test d < voxel, voxel the fp32 value the kernel
+    receives.  ``rows``: evaluate only these source rows.  -> dict(q, best, second, arg (-1 without targets), keep,
+    qmag = sum_k |R_jk| |p_k| + |t_j| per coordinate, voxel)."""
+    p = _f32(src).astype(np.float64).reshape(-1, 3)
+    if rows is not None:
+        p = p[np.asarray(rows)]
+    t = _f32(tgt).astype(np.float64).reshape(-1, 3)
+    T64 = _f32(T).astype(np.float64)
+    q = p @ T64[:3, :3].T + T64[:3, 3]
+    N, M = len(q), len(t)
+    best, second = np.full(N, np.inf), np.full(N, np.inf)
+    arg = np.full(N, -1, dtype=np.int64)
+    for a in range(0, N if M else 0, chunk):
+        b = min(N, a + chunk)
+        d = np.sqrt(((q[a:b, None, :] - t[None]) ** 2).sum(-1))
+        arg[a:b] = np.argmin(d, axis=1)
+        best[a:b] = d[np.arange(b - a), arg[a:b]]
+        if M > 1:
+            second[a:b] = np.partition(d, 1, axis=1)[:, 1]
+    v = float(F32(voxel))
+    return dict(q=q, best=best, second=second, arg=arg, keep=best < v, voxel=v,
+                qmag=np.abs(p) @ np.abs(T64[:3, :3]).T + np.abs(T64[:3, 3]))
 
 
 def _rotate_rows(v, R):
@@ -64,15 +97,41 @@ def _rotate_rows(v, R):
     return np.stack([((x * R[..., j, 0]) + (y * R[..., j, 1])) + (z * R[..., j, 2]) for j in range(3)], axis=-1)
 
 
-def aug_rotations(angles):
+def aug_rotations(angles, _mutations=()):
     """[K] fp32 angles -> [K,3,3] fp32 (kornia axis_angle_to_rotation_matrix of (0, 0, angle))."""
-    return O.azimuth_rotation(torch.from_numpy(_f32(angles))).numpy()
+    return O.azimuth_rotation(torch.from_numpy(_f32(angles)), _mutations).numpy()
 
 
-def so2_augment(delta, rand_axis, angles):
-    """-> (delta [K,P,3], rand_axis [K,3], aug_R [K,3,3]) rotated patch by patch."""
-    R = aug_rotations(angles)
-    return _rotate_rows(_f32(delta), R[:, None]).astype(F32), _rotate_rows(_f32(rand_axis), R).astype(F32), R
+def so2_augment(delta, rand_axis, angles, _mutations=()):
+    """-> (delta [K,P,3], rand_axis [K,3], aug_R [K,3,3]) rotated patch by patch.  ``_mutations``: those of
+    oracle.azimuth_rotation, and "transposed" rotates by R^T (rows @ R)."""
+    R = aug_rotations(angles, _mutations)
+    A = np.ascontiguousarray(np.swapaxes(R, -1, -2)) if "transposed" in _mutations else R
+    return _rotate_rows(_f32(delta), A[:, None]).astype(F32), _rotate_rows(_f32(rand_axis), A).astype(F32), R
+
+
+AUG_THRESHOLD = float(F32(1e-6))        # kornia's theta^2 > 1e-6 on an fp32 tensor: the scalar is fp32(1e-6)
+
+
+def so2_augment_fp64(delta, rand_axis, angles):
+    """kornia's axis_angle_to_rotation_matrix for (0, 0, a) in float64 on the fp32 angles, literally: theta = |a|, the axis
+    a / (theta + 1e-6) (not a unit axis for small theta), the first-order form where theta^2 <= fp32(1e-6).  theta^2 is
+    compared in float64; ``decided`` is False where fl32(a * a) (within u a^2) could fall on the other side.
+    -> dict(R (the float64 branch), R_full, R_taylor, full (bool [K]), decided, delta, rand_axis: the rows @ R^T)."""
+    a = _f32(angles).astype(np.float64).reshape(-1)
+    th2 = a * a
+    th = np.abs(a)
+    wz = a / (th + AUG_THRESHOLD)
+    c, s = np.cos(th), np.sin(th)
+    z, o = np.zeros_like(a), np.ones_like(a)
+    Rf = np.stack([c, -wz * s, z, wz * s, c, z, z, z, c + wz * wz * (1 - c)], axis=1).reshape(-1, 3, 3)
+    Rt = np.stack([o, -a, z, a, o, z, z, z, o], axis=1).reshape(-1, 3, 3)
+    full = th2 > AUG_THRESHOLD
+    decided = np.abs(th2 - AUG_THRESHOLD) > 2.0 ** -23 * th2
+    R = np.where(full[:, None, None], Rf, Rt)
+    d = _f32(delta).astype(np.float64)
+    return dict(R=R, R_full=Rf, R_taylor=Rt, full=full, decided=decided, delta=np.einsum("kpj,kij->kpi", d, R),
+                rand_axis=np.einsum("kj,kij->ki", _f32(rand_axis).astype(np.float64), R))
 
 
 def draw_aug_angles(rng, K):
@@ -80,40 +139,79 @@ def draw_aug_angles(rng, K):
     return (rng.random([K, 1]) * 2 * np.pi)[:, 0].astype(F32)
 
 
-def equi_match(d1: torch.Tensor, d2: torch.Tensor) -> torch.Tensor:
-    """cor[b,a] = sum_{c,k,l} d1[b,c,k,(l-a) mod L] * d2[b,c,k,l] in the reference's einsum form."""
+def equi_match(d1: torch.Tensor, d2: torch.Tensor, _mutations=()) -> torch.Tensor:
+    """cor[b,a] = sum_{c,k,l} d1[b,c,k,(l-a) mod L] * d2[b,c,k,l] in the reference's einsum form, in the dtype of the
+    inputs (float64 inputs give the float64 evaluation).  ``_mutations``: "shift_plus" takes (l + a) mod L."""
     B, C, K, L = d1.shape
     l = torch.arange(L)
-    idx = (l[None, :] - l[:, None]) % L
+    idx = ((l[None, :] + l[:, None]) if "shift_plus" in _mutations else (l[None, :] - l[:, None])) % L
     x = d1[:, :, :, idx.reshape(-1)].reshape(B, C, K, L, L).permute(0, 1, 3, 2, 4).reshape(B, C, L, K * L)
     return torch.einsum("bfag,bfg->ba", x, d2.reshape(B, C, K * L))
 
 
-def so2_gt(s_rand_axis, s_R, t_R, T, azi_n, integer=True, aug_R=None):
-    """cal_so2_gt in torch CPU fp32, literally: the rand axis through both LRFs (and the augmentation), projection onto the
+def so2_gt(s_rand_axis, s_R, t_R, T, azi_n, integer=True, aug_R=None, device="cpu", _mutations=()):
+    """cal_so2_gt in torch fp32, literally: the rand axis through both LRFs (and the augmentation), projection onto the
     xy plane, acos of the cosine similarity, sign from the cross product, 2 pi - angle.  int64 labels (rounded half to
-    even, azi_n -> 0) or fp32 labels."""
-    s = torch.from_numpy(_f32(s_rand_axis))[:, None]
-    G = torch.from_numpy(_f32(T)[:3, :3])
+    even, azi_n -> 0) or fp32 labels.  ``device``: where torch evaluates it (on "cuda" the reference's own device
+    arithmetic: cuBLAS matmuls and CUDA's division by a scalar).  ``_mutations`` (tests/test_train_fp64_cpu.py only):
+    "sign_inverted" takes 2 pi - angle where the cross product is positive, "no_wrap" keeps the label azi_n,
+    "aug_untransposed" applies aug_R instead of aug_R^T."""
+    dt = lambda x: torch.from_numpy(_f32(x)).to(device)
+    s = dt(s_rand_axis)[:, None]
+    G = dt(_f32(T)[:3, :3])
     t = torch.matmul(s, G.transpose(-1, -2))
-    s = torch.matmul(s, torch.from_numpy(_f32(s_R)))
-    t = torch.matmul(t, torch.from_numpy(_f32(t_R)))
+    s = torch.matmul(s, dt(s_R))
+    t = torch.matmul(t, dt(t_R))
     if aug_R is not None:
-        t = t @ torch.from_numpy(_f32(aug_R)).transpose(-1, -2)
+        A = dt(aug_R)
+        t = t @ (A if "aug_untransposed" in _mutations else A.transpose(-1, -2))
     z = torch.zeros_like(t)
     z[:, :, -1] = 1
     proj = F.normalize(t - torch.sum(t * z, dim=-1, keepdim=True) * z, p=2, dim=-1)
     s, proj, z = s[:, 0], proj[:, 0], z[:, 0]
     ang = torch.acos(F.cosine_similarity(s, proj).clamp(min=-1, max=1))
-    neg = torch.sum(torch.linalg.cross(s, proj, dim=-1) * z, dim=-1) < 0
+    cz = torch.sum(torch.linalg.cross(s, proj, dim=-1) * z, dim=-1)
+    neg = (cz > 0) if "sign_inverted" in _mutations else (cz < 0)
     ang[neg] = 2 * np.pi - ang[neg]
     lab = ang * azi_n / (2 * np.pi)
     if integer:
         lab = torch.round(lab)
+        if "no_wrap" not in _mutations:
+            lab[lab == azi_n] = 0
+        return lab.to(torch.int64).cpu().numpy()
+    if "no_wrap" not in _mutations:
         lab[lab == azi_n] = 0
-        return lab.to(torch.int64).numpy()
-    lab[lab == azi_n] = 0
-    return lab.numpy()
+    return lab.cpu().numpy()
+
+
+def so2_gt_fp64(s_rand_axis, s_R, t_R, T, azi_n, aug_R=None):
+    """cal_so2_gt (BUFFERX.py:86-126) in float64 on the fp32 inputs: u = s @ s_R, v = (s @ gtR^T) @ t_R (@ aug_R^T), the
+    angle between u and the xy projection of v, 2 pi - angle where (u x p)_z < 0, label = angle azi_n / 2 pi (azi_n -> 0).
+    -> dict(lab, u, v, p (the unit projection; 0 where |v_xy| = 0), cs, unorm, vnorm, vxy = |v_xy|, sin_th, cz (the cross
+    product's z), half (distance of the label to the nearest half-integer, modulo azi_n)); the intermediate t for the
+    error bounds."""
+    f = lambda x: _f32(x).astype(np.float64)
+    s = f(s_rand_axis).reshape(-1, 3)
+    t = s @ f(T)[:3, :3].T
+    u = np.einsum("pk,pkj->pj", s, f(s_R).reshape(-1, 3, 3))
+    v = np.einsum("pk,pkj->pj", t, f(t_R).reshape(-1, 3, 3))
+    v0 = v
+    if aug_R is not None:
+        v = np.einsum("pk,pjk->pj", v, f(aug_R).reshape(-1, 3, 3))
+    vxy = np.hypot(v[:, 0], v[:, 1])
+    p = np.zeros_like(v)
+    nz = vxy > 0
+    p[nz, :2] = v[nz, :2] / vxy[nz, None]
+    unorm = np.linalg.norm(u, axis=1)
+    cs = np.clip((u * p).sum(1) / unorm, -1.0, 1.0)
+    th = np.arccos(cs)
+    cz = u[:, 0] * p[:, 1] - u[:, 1] * p[:, 0]
+    ang = np.where(cz < 0, 2 * np.pi - th, th)
+    lab = ang * azi_n / (2 * np.pi)
+    lab = np.where(lab == azi_n, 0.0, lab)
+    half = np.abs(np.mod(lab, 1.0) - 0.5)
+    return dict(lab=lab, u=u, v=v, v_pre_aug=v0, t=t, p=p, cs=cs, th=th, unorm=unorm, vnorm=np.linalg.norm(v, axis=1),
+                vxy=vxy, sin_th=np.sin(th), cz=cz, half=half)
 
 
 def draw_des_r(cfg, rng):

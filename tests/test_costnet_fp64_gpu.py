@@ -397,15 +397,9 @@ def test_forward_matches_every_route_vs_fp64(dev, nets, oracle, c2_runs, monkeyp
         l32, _ = oracle._cost_net(d1, d2, sd, 20, "Pose.conv.")
     err32 = (l32.double() - l64).abs().max(dim=1).values
     bound = 1.5 * err32 + 2e-5 * l64.abs().max(dim=1).values
-    ind64 = oracle.soft_argmax(l64)
-    # soft arg-max: 1e-4 (about 10x the fp32 oracle's error on a single peak).  d ind / d logit_k = p_k (k - ind), so a row
-    # whose mass sits at both ends of the bin range turns the same fp32-grade logit error into a larger bin error: the bound
-    # scales with s = sum p_k |k - ind| (<= 1 on a single peak) and is at least 1.5 x the fp32 oracle's own error; never
-    # beyond 2e-4
-    ind32_err = (oracle.soft_argmax(l32) - ind64).abs()
-    p = torch.softmax(l64, dim=1)
-    s = (p * (torch.arange(20, dtype=torch.float64)[None] - ind64[:, None]).abs()).sum(dim=1)
-    ind_bound = torch.clamp(torch.maximum(1e-4 * s.clamp(min=1.0), 1.5 * ind32_err), max=2e-4)
+    # soft arg-max: 1e-4 scaled by s = sum p_k |k - ind|, at least 1.5 x the fp32 oracle's own error, never beyond 2e-4
+    # (oracle.soft_argmax_bound)
+    ind64, ind_bound, s, ind32_err = oracle.soft_argmax_bound(l64, l32)
 
     def worst_row(dind):
         r = int((dind - ind_bound).argmax())

@@ -161,7 +161,9 @@ def _compare_forward(oracle, TS, sd, cfg, stage, out, ref, what):
         assert _rel_rows(es, oe).max() < 1e-3      # on maps that already differ by the descriptor stack's fp32 rounding
     else:
         assert out["pred_ind"].shape == ref["pred_ind"].shape and out["gt_ind"].dtype == torch.float32
-        assert np.abs(out["pred_ind"].cpu().numpy() - ref["pred_ind"].numpy()).max() < 2e-3     # soft arg-max bound
+        # a loose cross-check only: the two sides' maps differ by the descriptor stack's rounding.  The kernel's bound is
+        # the a11 bound against float64 on its own recorded maps, test_train_fp64_gpu.py::test_production_route_vs_fp64
+        assert np.abs(out["pred_ind"].cpu().numpy() - ref["pred_ind"].numpy()).max() < 2e-3
         # float labels: 1e-4 bins, plus the conditioning of acos where the cosine is next to +-1 (an fp32 cosine that is
         # a few ulps apart moves the angle by up to sqrt(2 * eps))
         g, e = out["gt_ind"].cpu().numpy(), ref["gt_ind"].numpy()
