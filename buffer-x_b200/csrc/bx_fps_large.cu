@@ -19,6 +19,10 @@
 // without a second exchange.  Slots are double-buffered: a CTA can only be one iteration ahead of the slowest (its next
 // wait needs everybody's next arrival, which follows their read of the current slots).
 //
+// Count form (bx_fps_large_n, size-class slots): the grid is sized for a capacity and the kernel reads the point count
+// from the device.  The layout argument above holds for any G, so the indices are still those of bx_fps for every N; the
+// points of a CTA whose range lies beyond N start (and stay) skipped, so it posts the "none" candidate each iteration.
+//
 // The grid waits on itself, so it must be co-resident: the launch is cooperative (cudaLaunchAttributeCooperative), which
 // the driver schedules all at once or not at once, whatever other streams have in flight, and which stream capture turns
 // into a cooperative graph node.
@@ -65,9 +69,11 @@ __device__ __forceinline__ unsigned load_acquire(const unsigned *ctr) {
     return v;
 }
 
+// kCount: the grid is sized for a capacity N and the cloud is its first clamp(*d_n, 1, N) points (a size-class slot).
+template <bool kCount>
 __global__ void __launch_bounds__(kThreads, 1)
 fps_grid_kernel(const float *__restrict__ xyz, int N, int npoint, int *__restrict__ idx, float *__restrict__ kp,
-                unsigned char *__restrict__ ws) {
+                unsigned char *__restrict__ ws, const int *__restrict__ d_n) {
     extern __shared__ float s_xyz[];                    // [3][kPerCta]
     __shared__ uint4 w_a[32];
     __shared__ float w_z[32];
@@ -77,6 +83,7 @@ fps_grid_kernel(const float *__restrict__ xyz, int N, int npoint, int *__restric
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     unsigned *ctr = reinterpret_cast<unsigned *>(ws);
     uint4 *slots = reinterpret_cast<uint4 *>(ws + kSlotsOffset);      // [2][G][2]
+    if constexpr (kCount) N = min(max(*d_n, 1), N);                   // CTAs whose range is empty post "none"
 
     int log2bs = 0;
     while ((2 << log2bs) <= N && log2bs < 9) ++log2bs;  // bs = min(512, 2^floor(log2 N))
@@ -184,29 +191,28 @@ fps_grid_kernel(const float *__restrict__ xyz, int N, int npoint, int *__restric
 
 int grid_ctas(int n) { return (n + kPerCta - 1) / kPerCta; }
 
-}  // namespace
+// Size classes above 524288 points: CTA counts on a ladder where each capacity is at most 1.25x the smallest cloud of its
+// class (the first one at most 1.25x 524289), then the 1638400-point limit.
+constexpr int kClassCtas[] = {35, 43, 53, 66, 82};
 
-BX_API long long bx_fps_large_workspace_bytes(int n) {
-    if (n < 1) n = 1;
-    return (long long)kSlotsOffset + 2LL * grid_ctas(n < kMaxN ? n : kMaxN) * 32;
-}
-
-BX_API int bx_fps_large(const float *xyz, int n, int npoint, int32_t *idx, float *kpts, void *workspace, void *stream) {
-    BX_REQUIRE(xyz && idx && workspace, "bx_fps_large: null pointer");
-    BX_REQUIRE(n >= 1, "bx_fps_large: the cloud is empty");
-    BX_REQUIRE(n <= kMaxN, "bx_fps_large: N=%d exceeds the %d-point limit (the patch gatherer's shared-memory bitmap)", n, kMaxN);
-    BX_REQUIRE(npoint >= 0, "bx_fps_large: npoint < 0");
-    BX_REQUIRE(((uintptr_t)workspace & 15) == 0, "bx_fps_large: workspace must be 16-byte aligned");
+template <bool kCount>
+int launch(const char *name, const float *xyz, int n, const int32_t *d_n, int npoint, int32_t *idx, float *kpts, void *workspace,
+           void *stream) {
+    BX_REQUIRE(xyz && idx && workspace && (!kCount || d_n), "%s: null pointer", name);
+    BX_REQUIRE(n >= 1, "%s: the cloud is empty", name);
+    BX_REQUIRE(n <= kMaxN, "%s: N=%d exceeds the %d-point limit (the patch gatherer's shared-memory bitmap)", name, n, kMaxN);
+    BX_REQUIRE(npoint >= 0, "%s: npoint < 0", name);
+    BX_REQUIRE(((uintptr_t)workspace & 15) == 0, "%s: workspace must be 16-byte aligned", name);
     if (npoint == 0) return BX_OK;
     const int G = grid_ctas(n);
     static_assert(kMaxCtas <= 96, "the candidate reduction takes at most three slots per lane");
     const int sms = bx_device_sm_count();
-    BX_REQUIRE(sms > 0, "bx_fps_large: no CUDA device");
-    BX_REQUIRE(G <= sms, "bx_fps_large: N=%d needs %d co-resident CTAs, the device has %d SMs", n, G, sms);
+    BX_REQUIRE(sms > 0, "%s: no CUDA device", name);
+    BX_REQUIRE(G <= sms, "%s: N=%d needs %d co-resident CTAs, the device has %d SMs", name, n, G, sms);
     cudaStream_t st = bx_stream(stream);
     static BxPerDevice attr = {};
     if (bx_needs_attr(attr))
-        BX_CUDA(cudaFuncSetAttribute(fps_grid_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemBytes));
+        BX_CUDA(cudaFuncSetAttribute(fps_grid_kernel<kCount>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemBytes));
     BX_CUDA(cudaMemsetAsync(workspace, 0, sizeof(unsigned), st));      // the arrival counter
     cudaLaunchConfig_t cfg = {};
     cfg.gridDim = dim3((unsigned)G);
@@ -218,7 +224,32 @@ BX_API int bx_fps_large(const float *xyz, int n, int npoint, int32_t *idx, float
     at[0].val.cooperative = 1;
     cfg.attrs = at;
     cfg.numAttrs = 1;
-    BX_CUDA(cudaLaunchKernelEx(&cfg, fps_grid_kernel, xyz, n, npoint, (int *)idx, kpts, (unsigned char *)workspace));
+    BX_CUDA(cudaLaunchKernelEx(&cfg, fps_grid_kernel<kCount>, xyz, n, npoint, (int *)idx, kpts, (unsigned char *)workspace,
+                               (const int *)d_n));
     ++g_bx_launches;
     return BX_OK;
+}
+
+}  // namespace
+
+BX_API long long bx_fps_large_workspace_bytes(int n) {
+    if (n < 1) n = 1;
+    return (long long)kSlotsOffset + 2LL * grid_ctas(n < kMaxN ? n : kMaxN) * 32;
+}
+
+BX_API int bx_fps_large(const float *xyz, int n, int npoint, int32_t *idx, float *kpts, void *workspace, void *stream) {
+    return launch<false>("bx_fps_large", xyz, n, nullptr, npoint, idx, kpts, workspace, stream);
+}
+
+BX_API int bx_fps_large_n(const float *xyz, int cap, const int32_t *d_n, int npoint, int32_t *idx, float *kpts, void *workspace,
+                          void *stream) {
+    return launch<true>("bx_fps_large_n", xyz, cap, d_n, npoint, idx, kpts, workspace, stream);
+}
+
+BX_API int bx_fps_large_size_class(int n, int max_cluster) {
+    if (n <= 524288) return bx_fps_size_class(n, max_cluster);
+    if (n > kMaxN) return -1;
+    for (const int g : kClassCtas)
+        if (n <= g * kPerCta) return g * kPerCta;
+    return kMaxN;
 }

@@ -18,11 +18,15 @@ constexpr int NB = BX_RADIUS_BINS;  // 8192
 constexpr int HT = 256;             // threads
 constexpr int KT = 500;             // key-points per smem tile (float4 each)
 
+constexpr int kSub = BX_RADIUS_SUBSAMPLE;  // 200000
+
 // hist[m] (m in 0..NB+1) = #{d2 : smallest m with d2 < thr[m]}, bin NB+1 = "d2 == 25".
+// kSubsampled (pair form only): a chosen cloud of more than kSub points is read through the kSub indices d_sub.
+template <bool kSubsampled>
 __global__ void __launch_bounds__(HT)
 radius_hist_kernel(const float *__restrict__ kpts, int Kr, const float *__restrict__ pts, int N,
                    uint32_t *__restrict__ hist, const float *__restrict__ kpts_t, const float *__restrict__ pts_t, int N_t,
-                   const int *__restrict__ d_counts) {
+                   const int *__restrict__ d_counts, const int *__restrict__ d_sub) {
     if (d_counts) {     // pair form: the larger cloud by the reference's rule (source iff Ns > Nt), counts clamped to the capacities
         const int ns = min(max(d_counts[0], 0), N), nt = min(max(d_counts[1], 0), N_t);
         if (ns > nt) {
@@ -30,6 +34,11 @@ radius_hist_kernel(const float *__restrict__ kpts, int Kr, const float *__restri
         } else {
             kpts = kpts_t; pts = pts_t; N = nt;
         }
+    }
+    [[maybe_unused]] const int n_full = N;  // kSubsampled: the chosen cloud's size (indices are clamped to it), N the sample size
+    if constexpr (kSubsampled) {
+        if (N > kSub) N = kSub;
+        else d_sub = nullptr;
     }
     extern __shared__ unsigned char smem_raw[];
     float *thr = reinterpret_cast<float *>(smem_raw);                 // NB+1
@@ -52,7 +61,11 @@ radius_hist_kernel(const float *__restrict__ kpts, int Kr, const float *__restri
         }
         __syncthreads();
         for (int p = blockIdx.x * HT + threadIdx.x; p < N; p += gridDim.x * HT) {
-            const float px = pts[3 * (size_t)p], py = pts[3 * (size_t)p + 1], pz = pts[3 * (size_t)p + 2];
+            int pi = p;
+            if constexpr (kSubsampled) {
+                if (d_sub) pi = min(max(d_sub[p], 0), n_full - 1);
+            }
+            const float px = pts[3 * (size_t)pi], py = pts[3 * (size_t)pi + 1], pz = pts[3 * (size_t)pi + 2];
             const float p2 = ((px * px) + (py * py)) + (pz * pz);
             for (int i = 0; i < kn; ++i) {
                 const float4 q = kq[i];
@@ -148,14 +161,16 @@ radius_bisect_kernel(uint32_t *__restrict__ hist, long long denom, const Thresho
 namespace {
 
 int radius_launch(const float *kpts, int Kr, const float *pts, int N, int64_t denom, const float *kpts_t, const float *pts_t, int N_t,
-                  const int32_t *d_counts, const double *h_thresholds, int n_thr, double tolerance, const float *round_table,
+                  const int32_t *d_counts, const int32_t *d_sub, const double *h_thresholds, int n_thr, double tolerance, const float *round_table,
                   uint32_t *hist, float *out_r, int32_t *out_m, void *stream) {
     cudaStream_t st = bx_stream(stream);
     BX_CUDA(cudaMemsetAsync(hist, 0, sizeof(uint32_t) * (NB + 2), st));
     const size_t smem = sizeof(float) * (NB + 1) + sizeof(uint32_t) * (NB + 3) + sizeof(float4) * KT;
-    static BxPerDevice attr_done = {};
+    static BxPerDevice attr_done = {}, attr_sub_done = {};
     if (bx_needs_attr(attr_done))
-        BX_CUDA(cudaFuncSetAttribute(radius_hist_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        BX_CUDA(cudaFuncSetAttribute(radius_hist_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    if (d_sub && bx_needs_attr(attr_sub_done))
+        BX_CUDA(cudaFuncSetAttribute(radius_hist_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     int sms = bx_device_sm_count();
     if (sms <= 0) sms = 132;
     const int gy = (Kr + KT - 1) / KT;
@@ -163,7 +178,10 @@ int radius_launch(const float *kpts, int Kr, const float *pts, int N, int64_t de
     const int cap = (4 * sms + gy - 1) / gy;  // ~4 CTAs per SM overall; beyond that grid-stride
     if (gx > cap) gx = cap;
     if (gx < 1) gx = 1;
-    radius_hist_kernel<<<dim3(gx, gy), HT, smem, st>>>(kpts, Kr, pts, N, hist, kpts_t, pts_t, N_t, d_counts);
+    if (d_sub)
+        radius_hist_kernel<true><<<dim3(gx, gy), HT, smem, st>>>(kpts, Kr, pts, N, hist, kpts_t, pts_t, N_t, d_counts, d_sub);
+    else
+        radius_hist_kernel<false><<<dim3(gx, gy), HT, smem, st>>>(kpts, Kr, pts, N, hist, kpts_t, pts_t, N_t, d_counts, nullptr);
     BX_LAUNCH_CHECK();
     Thresholds thr;
     for (int i = 0; i < 16; ++i) thr.v[i] = h_thresholds[i < n_thr ? i : 0];
@@ -180,7 +198,7 @@ BX_API int bx_radius_estimate(const float *kpts, int Kr, const float *pts, int N
     BX_REQUIRE(kpts && pts && h_thresholds && round_table && hist && out_r, "bx_radius_estimate: null pointer");
     BX_REQUIRE(Kr >= 1 && N >= 1 && n_thr >= 1 && n_thr <= 16, "bx_radius_estimate: bad sizes Kr=%d N=%d n_thr=%d", Kr, N, n_thr);
     BX_REQUIRE((int64_t)Kr * (int64_t)N < ((int64_t)1 << 32), "bx_radius_estimate: Kr*N must be < 2^32");
-    return radius_launch(kpts, Kr, pts, N, denom, nullptr, nullptr, 0, nullptr, h_thresholds, n_thr, tolerance, round_table, hist, out_r,
+    return radius_launch(kpts, Kr, pts, N, denom, nullptr, nullptr, 0, nullptr, nullptr, h_thresholds, n_thr, tolerance, round_table, hist, out_r,
                          out_m, stream);
 }
 
@@ -195,6 +213,22 @@ BX_API int bx_radius_estimate_n(const float *kpts_s, const float *pts_s, int cap
     BX_REQUIRE(Kr >= 1 && cap_s >= 1 && cap_t >= 1 && n_thr >= 1 && n_thr <= 16, "bx_radius_estimate_n: bad sizes Kr=%d N=%d/%d n_thr=%d",
                Kr, cap_s, cap_t, n_thr);
     BX_REQUIRE((int64_t)Kr * (int64_t)(cap_s > cap_t ? cap_s : cap_t) < ((int64_t)1 << 32), "bx_radius_estimate_n: Kr*N must be < 2^32");
-    return radius_launch(kpts_s, Kr, pts_s, cap_s, 0, kpts_t, pts_t, cap_t, d_counts, h_thresholds, n_thr, tolerance, round_table, hist,
-                         out_r, out_m, stream);
+    return radius_launch(kpts_s, Kr, pts_s, cap_s, 0, kpts_t, pts_t, cap_t, d_counts, nullptr, h_thresholds, n_thr, tolerance, round_table,
+                         hist, out_r, out_m, stream);
+}
+
+// Sub-sampled pair form: as bx_radius_estimate_n, and when the chosen cloud has more than BX_RADIUS_SUBSAMPLE points the
+// histogram runs over its points d_sub[0..BX_RADIUS_SUBSAMPLE) (the reference's draw, made by the caller), denom still N * Kr.
+// The counts are integer atomics: the same histogram, radii and m as bx_radius_estimate on the gathered cloud.
+BX_API int bx_radius_estimate_n_sub(const float *kpts_s, const float *pts_s, int cap_s, const float *kpts_t, const float *pts_t, int cap_t,
+                                    int Kr, const int32_t *d_counts, const int32_t *d_sub, const double *h_thresholds, int n_thr,
+                                    double tolerance, const float *round_table, uint32_t *hist, float *out_r, int32_t *out_m, void *stream) {
+    BX_REQUIRE(kpts_s && pts_s && kpts_t && pts_t && d_counts && d_sub && h_thresholds && round_table && hist && out_r,
+               "bx_radius_estimate_n_sub: null pointer");
+    BX_REQUIRE(Kr >= 1 && cap_s >= 1 && cap_t >= 1 && n_thr >= 1 && n_thr <= 16,
+               "bx_radius_estimate_n_sub: bad sizes Kr=%d N=%d/%d n_thr=%d", Kr, cap_s, cap_t, n_thr);
+    const int cap = cap_s > cap_t ? cap_s : cap_t;
+    BX_REQUIRE((int64_t)Kr * (int64_t)(cap < kSub ? cap : kSub) < ((int64_t)1 << 32), "bx_radius_estimate_n_sub: Kr*min(N, %d) must be < 2^32", kSub);
+    return radius_launch(kpts_s, Kr, pts_s, cap_s, 0, kpts_t, pts_t, cap_t, d_counts, d_sub, h_thresholds, n_thr, tolerance, round_table,
+                         hist, out_r, out_m, stream);
 }

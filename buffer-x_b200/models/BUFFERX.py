@@ -16,7 +16,8 @@ Throughput API on top of the reference surface (CUDA streams + graphs instead of
   * ``enable_cuda_graphs(True)``: the enqueue of a pair is captured once per (Ns, Nt, aligned) shape and
     replayed -- one graph launch instead of ~150 kernel launches; with ``size_classes=True`` once per
     (C_src, C_tgt, aligned) capacity, the true point counts read by the N-dependent kernels from the device, so
-    a stream of pairs of every size replays a handful of graphs;
+    a stream of pairs of every size replays a handful of graphs (``large_classes=True`` extends this to clouds of more
+    than 200000 points, their radius sub-sample drawn on the host at launch);
   * ``forward_async(data_source) -> handle`` / ``handle.result()``: several pairs in flight on separate
     streams (FPS is a latency-bound 16-SM kernel; a second pair's convolutions fill the other SMs).
     With ``cfg.match.enable_early_exit`` the scale-0 RANSAC result gates the later scales on the device
@@ -91,9 +92,11 @@ class _PairSlot:
     stream.  C_src / C_tgt are the capacities of the cloud buffers.  An exact-shape slot (``counted`` False) serves the pairs
     of exactly that shape and runs the kernels without point counts; a size-class slot (``counted`` True) serves every pair
     whose clouds fit the capacities: the true counts are copied to the device before each replay and the N-dependent
-    kernels (FPS, radius histogram, permutation, patch gathering) stop at them, so the padding rows are never read."""
+    kernels (FPS, radius histogram, permutation, patch gathering) stop at them, so the padding rows are never read.
+    A large-class slot (``subsample`` True: a size-class slot whose larger capacity exceeds MAX_CLASS_POINTS) also holds the
+    reference's 200000-index radius sub-sample, drawn at launch from torch's CPU generator as eager ``forward`` draws it."""
 
-    def __init__(self, model, Cs, Ct, aligned, use_graph, counted=False):
+    def __init__(self, model, Cs, Ct, aligned, use_graph, counted=False, subsample=False):
         cfg = model.config
         self.model, self.Cs, self.Ct, self.aligned, self.counted = model, Cs, Ct, aligned, counted
         self.n_s, self.n_t = Cs, Ct
@@ -111,6 +114,9 @@ class _PairSlot:
         self.h_tgt = torch.empty((Ct, 3), dtype=torch.float32).pin_memory()
         self.counts = torch.tensor([Cs, Ct], dtype=torch.int32, device=dev) if counted else None
         self.h_counts = torch.empty(2, dtype=torch.int32).pin_memory() if counted else None
+        # index 0 is valid in any cloud: the warm-up and the capture read it before the first launch draws
+        self.sub = torch.zeros(ops.RADIUS_SUBSAMPLE, dtype=torch.int32, device=dev) if subsample else None
+        self.h_sub = torch.empty(ops.RADIUS_SUBSAMPLE, dtype=torch.int32).pin_memory() if subsample else None
         self.h_tail = None
         self.done = torch.cuda.Event()
         self.graph = None
@@ -135,7 +141,7 @@ class _PairSlot:
     def _enqueue(self):
         perms = [(self.perm_s[i], self.perm_t[i]) for i in range(self.perm_s.shape[0])]
         return self.model._enqueue(self.src, self.tgt, self.aligned, perms, None, False, device_exit=True, counts=self.counts,
-                                   xyz=self.xyz)[0]
+                                   xyz=self.xyz, sub=self.sub)[0]
 
     def launch(self, data_source, perms):
         """H2D of the inputs (pinned staging when they arrive as host arrays), the pair, D2H of the result."""
@@ -184,6 +190,10 @@ class _PairSlot:
             if self.counted:
                 self.h_counts[0], self.h_counts[1] = n_s, n_t
                 self.counts.copy_(self.h_counts, non_blocking=True)
+            if self.sub is not None and max(n_s, n_t) > ops.RADIUS_SUBSAMPLE:
+                # eager forward's draw (reference BUFFERX.py:664-665) on the cloud it picks: the source iff n_s > n_t
+                self.h_sub.copy_(torch.randint(0, n_s if n_s > n_t else n_t, (ops.RADIUS_SUBSAMPLE,)))
+                self.sub.copy_(self.h_sub, non_blocking=True)
             if self.graph is not None:
                 self.graph.replay()
                 tail = self.tail
@@ -220,6 +230,7 @@ class BufferX(nn.Module):
         self._slots = {}
         self._slots_per_shape = 2
         self._size_classes = False
+        self._large_classes = False
         self._fps_cluster = 0        # > 0: throughput form of the FPS kernel (ops.fps max_cluster), chosen by enable_cuda_graphs
         self._rr = {}
 
@@ -272,23 +283,30 @@ class BufferX(nn.Module):
         return T.view(1, 4, 4)
 
     # ------------------------------------------------------------------------------------------------
-    def enable_cuda_graphs(self, flag=True, slots_per_shape=2, size_classes=False):
+    def enable_cuda_graphs(self, flag=True, slots_per_shape=2, size_classes=False, large_classes=False):
         """Capture the per-pair enqueue once per slot key and replay it (no effect on results, except for a pair whose larger
-        cloud has more than 200000 points: the capture draws its radius sub-sample on the device, not from torch's CPU generator
-        as eager ``forward`` and the reference do); ``forward`` then runs through the same slots as ``forward_async`` (unless
-        early exit, timing or debug is on).
+        cloud has more than 200000 points on an exact-shape slot: the capture draws its radius sub-sample on the device, not
+        from torch's CPU generator as eager ``forward`` and the reference do); ``forward`` then runs through the same slots as
+        ``forward_async`` (unless early exit, timing or debug is on).
 
         ``size_classes=False``: slots are keyed by the exact (Ns, Nt, aligned) shape (plus the early-exit setting), so a stream
         whose pairs all differ in size captures a graph for almost every pair.  ``size_classes=True``: each cloud is given a
         capacity, its size class (``ops.fps_size_class``: the largest point count with the same FPS launch configuration),
         slots are keyed by (C_src, C_tgt, aligned) and every pair whose clouds fit replays the class graph with its true
         point counts on the device -- results bit-identical to the exact-shape route.  A pair whose larger cloud has more
-        than 200000 points keeps an exact-shape slot (the reference sub-samples such a cloud with a draw sized by N).
+        than 200000 points keeps an exact-shape slot (the reference sub-samples such a cloud with a draw sized by N), unless
+        ``large_classes=True``: such pairs then get size-class slots too (``ops.fps_large_size_class``: above 524288 points,
+        capacities at most 1.25x the cloud, up to 1638400 points), and each launch draws the 200000-index sub-sample on the
+        host from torch's CPU generator and uploads it with the counts -- results byte-identical to eager ``forward`` with
+        the same ``perms`` and the same generator state, graphs on or off.
         ``slots_per_shape`` slots (pairs in flight) are kept per key.  These options also apply to ``forward_async``
         without graphs."""
+        if large_classes and not size_classes:
+            raise ValueError("enable_cuda_graphs: large_classes=True extends size_classes=True; set both")
         self._use_graphs = bool(flag)
         self._slots_per_shape = int(slots_per_shape)
         self._size_classes = bool(size_classes)
+        self._large_classes = bool(large_classes)
         # three or more pairs in flight: the key-point sampling of a pair runs beside the other pairs' convolutions; bx_fps_ex offers
         # a 2- / 4-CTA-per-cloud form (fewer SMs, longer)
         # (what the other streams lose is governed by how LONG the sampling holds its SMs, not by how many, so the default stays
@@ -311,11 +329,15 @@ class BufferX(nn.Module):
         return (True, int(m.get("early_exit_min_inliers", 15))) if m.get("enable_early_exit", True) else (False, None)
 
     MAX_GRAPH_SHAPES = 8      # graphs are per slot key; least recently used keys are dropped beyond this
-    MAX_CLASS_POINTS = 200000  # larger clouds are sub-sampled by a draw sized by N (reference BUFFERX.py:664-665): exact slots
+    # larger clouds are sub-sampled by a draw sized by N (reference BUFFERX.py:664-665): exact slots, unless large_classes
+    MAX_CLASS_POINTS = 200000
 
     def _slot_key(self, Ns, Nt, aligned):
         """(slot key, capacities, counted) of a pair.  The early-exit threshold is baked into a captured gate launch: a
         graph is never replayed under another setting."""
+        if self._size_classes and self._large_classes:
+            Cs, Ct = ops.fps_large_size_class(Ns, self._fps_cluster), ops.fps_large_size_class(Nt, self._fps_cluster)
+            return (Cs, Ct, bool(aligned)) + self._exit_key(), Cs, Ct, True
         if self._size_classes and max(Ns, Nt) <= self.MAX_CLASS_POINTS:
             Cs, Ct = ops.fps_size_class(Ns, self._fps_cluster), ops.fps_size_class(Nt, self._fps_cluster)
             return (Cs, Ct, bool(aligned)) + self._exit_key(), Cs, Ct, True
@@ -349,7 +371,8 @@ class BufferX(nn.Module):
         lst = self._slots.setdefault(key, [])
         i = self._rr.get(key, 0)
         if len(lst) < self._slots_per_shape:
-            lst.append(_PairSlot(self, Cs, Ct, aligned, self._use_graphs, counted))
+            subsample = counted and self._large_classes and max(Cs, Ct) > self.MAX_CLASS_POINTS
+            lst.append(_PairSlot(self, Cs, Ct, aligned, self._use_graphs, counted, subsample))
             slot = lst[-1]
         else:
             slot = lst[i % len(lst)]
@@ -374,20 +397,23 @@ class BufferX(nn.Module):
         2*S permutations are drawn from NumPy's global RNG at launch, also when early exit stops the pair after scale 0.
         The slot is chosen by the pair's shape, or by its clouds' size classes after
         ``enable_cuda_graphs(..., size_classes=True)``; either way the result is that of eager ``forward`` with the same
-        ``perms``, except on a captured slot for a pair whose larger cloud has more than 200000 points, whose radius
-        sub-sample the capture draws on the device."""
+        ``perms``, except on a captured exact-shape slot for a pair whose larger cloud has more than 200000 points, whose
+        radius sub-sample the capture draws on the device.  A large-class slot (``large_classes=True``) draws it at launch
+        from torch's CPU generator, as eager ``forward`` does."""
         if self.config.test.get("enable_timing", False):
             raise ops.BufferXError("forward_async needs timing disabled (the per-stage timers require host round trips)")
         Ns, Nt = self._cloud_sizes(data_source)
         return self._slot(Ns, Nt, bool(data_source["is_aligned_to_global_z"])).launch(data_source, perms)
 
     # ------------------------------------------------------------------------------------------------
-    def _enqueue(self, src, tgt, aligned, perms, ransac_seed, debug, timers=None, device_exit=False, counts=None, xyz=None):
+    def _enqueue(self, src, tgt, aligned, perms, ransac_seed, debug, timers=None, device_exit=False, counts=None, xyz=None, sub=None):
         """Everything of one pair on the current stream, no host synchronisation unless early exit is on and the decision is
         the host's (``device_exit`` False: ``forward``).  Returns (tail block on the device, debug dict).
         ``counts`` (size-class slots): [2] int32 CUDA point counts; src / tgt are then capacity buffers whose first counts
-        rows are the clouds, and ``perms`` rows likewise (clouds of at most MAX_CLASS_POINTS points).  ``xyz``: src and tgt
-        back to back, when the caller holds them so (saves the concatenation before FPS)."""
+        rows are the clouds, and ``perms`` rows likewise.  ``sub`` (large-class slots, with ``counts``): [200000] int32 CUDA
+        radius sub-sample, read when the larger cloud has more than 200000 points; without it the counted clouds have at most
+        MAX_CLASS_POINTS points.  ``xyz``: src and tgt back to back, when the caller holds them so (saves the concatenation
+        before FPS)."""
         cfg = self.config
         dev = src.device
         Ns, Nt = src.shape[0], tgt.shape[0]
@@ -409,16 +435,17 @@ class BufferX(nn.Module):
         nfps = max(Kr, K)
         if max(Ns, Nt) <= ops.FPS_MAX_POINTS:
             fidx, fk = ops.fps(xyz, [0, Ns, Ns + Nt], nfps, max_cluster=self._fps_cluster, d_counts=counts)
-        else:   # beyond one cluster's registers: that cloud on the grid-wide kernel (exact-shape pairs only, counts is None)
-            per = [ops.fps_large(c, nfps) if c.shape[0] > ops.FPS_MAX_POINTS
-                   else ops.fps(c, [0, c.shape[0]], nfps, max_cluster=self._fps_cluster) for c in (src, tgt)]
+        else:   # beyond one cluster's registers: that cloud on the grid-wide kernel (a capacity above it holds such a cloud)
+            per = [ops.fps_large(c, nfps, d_count=None if counts is None else counts[j:j + 1]) if c.shape[0] > ops.FPS_MAX_POINTS
+                   else ops.fps(c, [0, c.shape[0]], nfps, max_cluster=self._fps_cluster, d_counts=None if counts is None else counts[j:j + 1])
+                   for j, c in enumerate((src, tgt))]
             fidx = torch.stack([i.reshape(nfps) for i, _ in per])
             fk = torch.stack([k.reshape(nfps, 3) for _, k in per])
         kpts1, kpts2 = fk[0, :Kr].contiguous(), fk[1, :Kr].contiguous()
         src_kpts, tgt_kpts = fk[0, :K].contiguous(), fk[1, :K].contiguous()
         # ---- density-aware radii of every scale from one histogram ------------------------------------
-        if counts is not None:      # the device picks the larger cloud from the counts (clouds of at most 200000 points)
-            r_dev, m_dev, _ = ops.radius_estimate_pair(kpts1, src, kpts2, tgt, thresholds, counts)
+        if counts is not None:      # the device picks the larger cloud from the counts (and sub-samples it through ``sub``)
+            r_dev, m_dev, _ = ops.radius_estimate_pair(kpts1, src, kpts2, tgt, thresholds, counts, d_sub=sub)
         else:
             pts_r, kpts_r = (src, kpts1) if Ns > Nt else (tgt, kpts2)
             denom = pts_r.shape[0] * Kr

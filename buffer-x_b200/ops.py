@@ -30,7 +30,7 @@ SYMBOLS = [
     "bx_fps_n", "bx_fps_size_class", "bx_radius_estimate_n", "bx_permute_cloud_n", "bx_select_patches_batched_counts",
     "bx_select_patches_grid_batched_counts",
     "bx_ball_query_batched", "bx_gather_channels", "bx_knn1", "bx_svd3", "bx_icp_workspace_bytes", "bx_icp",
-    "bx_fps_large", "bx_fps_large_workspace_bytes",
+    "bx_fps_large", "bx_fps_large_workspace_bytes", "bx_fps_large_n", "bx_fps_large_size_class", "bx_radius_estimate_n_sub",
 ]
 
 GEOM_CYL3D, GEOM_CYL2D, GEOM_VALID3D, GEOM_COSTAB = 0, 1, 2, 4
@@ -68,6 +68,9 @@ def load_library():
     lib.bx_fps_large.argtypes = [P, c_int, c_int, P, P, P, P]
     lib.bx_fps_large_workspace_bytes.argtypes = [c_int]
     lib.bx_fps_large_workspace_bytes.restype = c_int64
+    lib.bx_fps_large_n.argtypes = [P, c_int, P, c_int, P, P, P, P]
+    lib.bx_fps_large_size_class.argtypes = [c_int, c_int]
+    lib.bx_radius_estimate_n_sub.argtypes = [P, P, c_int, P, P, c_int, c_int, P, P, P, c_int, c_double, P, P, P, P, P]
     lib.bx_radius_estimate_n.argtypes = [P, P, c_int, P, P, c_int, c_int, P, P, c_int, c_double, P, P, P, P, P]
     lib.bx_permute_cloud_n.argtypes = [P, P, c_int, P, P, P]
     lib.bx_select_patches_batched_counts.argtypes = [c_int, P, P, P, P, P, P, P, c_int, P, P]
@@ -229,24 +232,39 @@ FPS_MAX_POINTS = 524288          # bx_fps: one 16-CTA cluster's registers
 FPS_LARGE_MAX_POINTS = 1638400   # bx_fps_large: the patch gatherer's shared-memory bitmap bounds every cloud of a pair
 
 
-def fps_large(xyz: torch.Tensor, npoint: int, want_kpts=True):
+def fps_large(xyz: torch.Tensor, npoint: int, want_kpts=True, d_count=None):
     """One cloud xyz [N,3] f32 cuda, 1 <= N <= FPS_LARGE_MAX_POINTS, on the grid-wide kernel (bx_fps_large).  Returns idx
-    [npoint] i32, kpts [npoint,3] (None unless want_kpts): for any N the indices ops.fps gives where it accepts N."""
+    [npoint] i32, kpts [npoint,3] (None unless want_kpts): for any N the indices ops.fps gives where it accepts N.
+    d_count: optional 1-element int32 CUDA point count (bx_fps_large_n); xyz is then a capacity buffer, the grid is sized
+    for its N rows and the cloud is its first min(max(d_count, 1), N) points."""
     if xyz.dim() != 2 or xyz.shape[1] != 3 or xyz.shape[0] < 1:
         raise BufferXError(f"fps_large: xyz must be [N,3] with N >= 1, got {tuple(xyz.shape)}")
+    if d_count is not None and d_count.numel() != 1:
+        raise BufferXError(f"fps_large: d_count must hold one point count, got {d_count.numel()} elements")
     lib = load_library()
     N = xyz.shape[0]
     idx = torch.empty(npoint, dtype=I32, device=xyz.device)
     kp = torch.empty((npoint, 3), dtype=F32, device=xyz.device) if want_kpts else None
     ws = torch.empty(int(lib.bx_fps_large_workspace_bytes(N)), dtype=torch.uint8, device=xyz.device)
     with _Span("fps_large"):
-        _check(lib.bx_fps_large(_dp(xyz, F32, "xyz"), N, int(npoint), _dp(idx), _dp(kp), _dp(ws), _stream()), "bx_fps_large")
+        if d_count is None:
+            _check(lib.bx_fps_large(_dp(xyz, F32, "xyz"), N, int(npoint), _dp(idx), _dp(kp), _dp(ws), _stream()), "bx_fps_large")
+        else:
+            _check(lib.bx_fps_large_n(_dp(xyz, F32, "xyz"), N, _dp(d_count, I32, "d_count"), int(npoint), _dp(idx), _dp(kp), _dp(ws),
+                                      _stream()), "bx_fps_large_n")
     return idx, kp
 
 
 def fps_size_class(n: int, max_cluster=0) -> int:
     """The largest point count that gets the same FPS launch configuration as an n-point cloud (-1 above the FPS limit)."""
     return int(load_library().bx_fps_size_class(int(n), int(max_cluster)))
+
+
+def fps_large_size_class(n: int, max_cluster=0) -> int:
+    """Capacity of an n-point cloud's size class up to FPS_LARGE_MAX_POINTS: fps_size_class(n, max_cluster) up to
+    FPS_MAX_POINTS; above, multiples of 18432 points (bx_fps_large_n's CTAs) each at most 1.25x the smallest cloud of its
+    class, then FPS_LARGE_MAX_POINTS.  -1 above FPS_LARGE_MAX_POINTS."""
+    return int(load_library().bx_fps_large_size_class(int(n), int(max_cluster)))
 
 
 _round_tables = {}
@@ -277,22 +295,35 @@ def radius_estimate(kpts: torch.Tensor, pts: torch.Tensor, thresholds, denom=Non
     return out_r, out_m, hist
 
 
-def radius_estimate_pair(kpts_s, pts_s, kpts_t, pts_t, thresholds, d_counts, tolerance=0.01, hist=None):
+RADIUS_SUBSAMPLE = 200000       # the reference's sub-sample of a larger cloud (BUFFERX.py:664-665)
+
+
+def radius_estimate_pair(kpts_s, pts_s, kpts_t, pts_t, thresholds, d_counts, tolerance=0.01, hist=None, d_sub=None):
     """Both clouds (capacity buffers) and their [Kr,3] key-points, d_counts [2] int32 CUDA = (ns, nt): the device picks the
-    larger cloud (source iff ns > nt) and denom = N * Kr.  Returns (r, m, hist) like radius_estimate."""
+    larger cloud (source iff ns > nt) and denom = N * Kr.  Returns (r, m, hist) like radius_estimate.
+    d_sub: optional [RADIUS_SUBSAMPLE] int32 CUDA indices (bx_radius_estimate_n_sub): when the chosen cloud has more than
+    RADIUS_SUBSAMPLE points, the histogram runs over its points d_sub, as radius_estimate(kpts, pts[d_sub], denom=N * Kr)."""
     lib = load_library()
     th = np.ascontiguousarray(thresholds, dtype=np.float64)
     Kr = kpts_s.shape[0]
     assert kpts_t.shape[0] == Kr
+    if d_sub is not None and tuple(d_sub.shape) != (RADIUS_SUBSAMPLE,):
+        raise BufferXError(f"radius_estimate_pair: d_sub must be [{RADIUS_SUBSAMPLE}], got {tuple(d_sub.shape)}")
     dev = pts_s.device
     if hist is None:
         hist = torch.empty(RADIUS_BINS + 2, dtype=I32, device=dev)
     out_r = torch.empty(len(th), dtype=F32, device=dev)
     out_m = torch.empty(len(th), dtype=I32, device=dev)
-    _check(lib.bx_radius_estimate_n(_dp(kpts_s, F32, "kpts_s"), _dp(pts_s, F32, "pts_s"), pts_s.shape[0], _dp(kpts_t, F32, "kpts_t"),
-                                    _dp(pts_t, F32, "pts_t"), pts_t.shape[0], Kr, _dp(d_counts, I32, "d_counts"), th.ctypes.data_as(c_void_p),
-                                    len(th), float(tolerance), _dp(radius_round_table(dev)), _dp(hist), _dp(out_r), _dp(out_m), _stream()),
-           "bx_radius_estimate_n")
+    if d_sub is None:
+        _check(lib.bx_radius_estimate_n(_dp(kpts_s, F32, "kpts_s"), _dp(pts_s, F32, "pts_s"), pts_s.shape[0], _dp(kpts_t, F32, "kpts_t"),
+                                        _dp(pts_t, F32, "pts_t"), pts_t.shape[0], Kr, _dp(d_counts, I32, "d_counts"), th.ctypes.data_as(c_void_p),
+                                        len(th), float(tolerance), _dp(radius_round_table(dev)), _dp(hist), _dp(out_r), _dp(out_m), _stream()),
+               "bx_radius_estimate_n")
+    else:
+        _check(lib.bx_radius_estimate_n_sub(_dp(kpts_s, F32, "kpts_s"), _dp(pts_s, F32, "pts_s"), pts_s.shape[0], _dp(kpts_t, F32, "kpts_t"),
+                                            _dp(pts_t, F32, "pts_t"), pts_t.shape[0], Kr, _dp(d_counts, I32, "d_counts"), _dp(d_sub, I32, "d_sub"),
+                                            th.ctypes.data_as(c_void_p), len(th), float(tolerance), _dp(radius_round_table(dev)), _dp(hist),
+                                            _dp(out_r), _dp(out_m), _stream()), "bx_radius_estimate_n_sub")
     return out_r, out_m, hist
 
 

@@ -34,6 +34,7 @@ extern "C" {
 #define BX_ERR_UNSUPPORTED (-3)
 
 #define BX_RADIUS_BINS 8192 /* candidate radii r_m = 5*m/8192 probed by the reference's bisection */
+#define BX_RADIUS_SUBSAMPLE 200000 /* a larger cloud is histogrammed on this many drawn points (models/BUFFERX.py:664-665) */
 
 /* ---- library ------------------------------------------------------------------------------ */
 const char *bx_last_error(void);
@@ -78,6 +79,15 @@ int bx_fps_set_sync_mode(int mode);
  * (bx_select_patches_grid): a larger n is refused. */
 int bx_fps_large(const float *xyz, int n, int npoint, int32_t *idx, float *kpts, void *workspace, void *stream);
 long long bx_fps_large_workspace_bytes(int n);
+/* Count form (size-class buffers): the grid is sized for the capacity cap (ceil(cap / 18432) CTAs) and the cloud is the first
+ * n = min(max(*d_n, 1), cap) points of xyz; points beyond n are never read.  Indices and key-points are those of
+ * bx_fps_large on the n-point cloud.  workspace: bx_fps_large_workspace_bytes(cap) bytes. */
+int bx_fps_large_n(const float *xyz, int cap, const int32_t *d_n, int npoint, int32_t *idx, float *kpts, void *workspace,
+                   void *stream);
+/* Size class of an n-point cloud up to 1638400 points: bx_fps_size_class(n, max_cluster) up to 524288 points; above, the
+ * capacities 18432 * {35, 43, 53, 66, 82} and 1638400 (bx_fps_large_n's grid), each at most 1.25x the smallest cloud of its
+ * class.  0 for n <= 0, -1 above 1638400. */
+int bx_fps_large_size_class(int n, int max_cluster);
 
 /* ---- a2: density-aware radius estimation ----------------------------------------------------
  * Replaces density_aware_radius_estimation + squared_cdist (models/BUFFERX.py:610-696) without
@@ -93,11 +103,19 @@ int bx_radius_estimate(const float *kpts, int Kr, const float *pts, int N, int64
 /* Pair form with device-side point counts: both clouds (capacities cap_s, cap_t) and both key-point sets ([Kr,3] each);
  * d_counts [2] (device, required) = (ns, nt), clamped to the capacities.  The device picks the source iff ns > nt (the
  * reference's rule, models/BUFFERX.py:654) and uses denom = N * Kr of the chosen cloud; points beyond a count are never
- * read.  Same radii and m as bx_radius_estimate on the chosen exact cloud.  No sub-sampling: the reference draws 200000
- * points of a larger cloud, which needs N on the host (callers keep such clouds on bx_radius_estimate). */
+ * read.  Same radii and m as bx_radius_estimate on the chosen exact cloud.  No sub-sampling: for a chosen cloud of more
+ * than BX_RADIUS_SUBSAMPLE points use bx_radius_estimate_n_sub. */
 int bx_radius_estimate_n(const float *kpts_s, const float *pts_s, int cap_s, const float *kpts_t, const float *pts_t, int cap_t,
                          int Kr, const int32_t *d_counts, const double *h_thresholds, int n_thr, double tolerance,
                          const float *round_table, uint32_t *hist, float *out_r, int32_t *out_m, void *stream);
+/* The same with the reference's sub-sample: when the chosen cloud has N > BX_RADIUS_SUBSAMPLE points, the histogram runs
+ * over its points d_sub[i], i < BX_RADIUS_SUBSAMPLE (device int32 indices, clamped to [0, N)), with denom = N * Kr; otherwise
+ * d_sub is not read.  The draw sizes itself by N, which the caller knows on the host when it uploads the counts, so it is made
+ * there (torch.randint(0, N, (200000,)) on torch's CPU generator, as the reference) and uploaded with them.  Same histogram,
+ * radii and m as bx_radius_estimate on the gathered cloud pts[d_sub] with that denom. */
+int bx_radius_estimate_n_sub(const float *kpts_s, const float *pts_s, int cap_s, const float *kpts_t, const float *pts_t, int cap_t,
+                             int Kr, const int32_t *d_counts, const int32_t *d_sub, const double *h_thresholds, int n_thr,
+                             double tolerance, const float *round_table, uint32_t *hist, float *out_r, int32_t *out_m, void *stream);
 
 /* ---- a3: order-preserving radius-neighbour patch gathering ----------------------------------
  * Replaces MiniSpinNet.select_patches (models/patch_embedder.py:92-120) =
