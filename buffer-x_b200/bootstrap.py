@@ -37,6 +37,9 @@ def compute_pca_alignment(pts: torch.Tensor, sample_idx=None):
     if not isinstance(sample_idx, torch.Tensor):
         sample_idx = torch.from_numpy(np.ascontiguousarray(sample_idx, dtype=np.int32))
     sample_idx = sample_idx.to(device=pts.device, dtype=torch.int32).contiguous()
+    if sample_idx.shape[0] < 3:        # what sklearn's PCA(n_components=3).fit raises: a cloud of fewer than 30 points
+        raise ValueError(f"n_components=3 must be between 0 and min(n_samples, n_features)={sample_idx.shape[0]} "
+                         f"(PCA of {sample_idx.shape[0]} sampled points)")
     mean, var, comps = ops.pca_analysis(pts, sample_idx)
     h = torch.cat([var, comps[2]]).cpu().numpy()          # one small read: the decisions below are host decisions
     sphericity = float(h[2] / h[0])

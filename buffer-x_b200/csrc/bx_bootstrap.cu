@@ -170,7 +170,8 @@ __global__ void vds_insert_kernel(const float *__restrict__ pts, int n, double v
         p[c] = (double)pts[3 * (size_t)i + c];
         iv[c] = (long long)floor((p[c] - vmb) / voxel);
     }
-    // 21 bits per axis: ample for any cloud / voxel ratio of the reference's datasets (checked on the host side)
+    // 21 bits per axis: distinct keys below 2^21 voxels per axis.  Not checked here; the host reads minmax6 with d_m
+    // and refuses a wider cloud (ops.voxel_down_sample).
     const unsigned long long key = ((unsigned long long)iv[0] & 0x1FFFFFull) | (((unsigned long long)iv[1] & 0x1FFFFFull) << 21) |
                                    (((unsigned long long)iv[2] & 0x1FFFFFull) << 42);
     const unsigned long long h = key * 0x9E3779B97F4A7C15ull;
@@ -213,7 +214,8 @@ int grid_blocks(int n) {
 BX_API int bx_pca_analysis(const float *pts, int n, const int32_t *sample_idx, int n_sample, double *acc9, double *out15,
                            void *stream) {
     BX_REQUIRE(pts && acc9 && out15, "bx_pca_analysis: null pointer");
-    BX_REQUIRE(n >= 2 && n_sample >= 2 && (sample_idx || n_sample == n), "bx_pca_analysis: need at least two samples (n=%d, n_sample=%d)", n, n_sample);
+    BX_REQUIRE(n >= 2 && n_sample >= 3 && (sample_idx || n_sample == n),
+               "bx_pca_analysis: PCA(n_components=3) needs at least three samples (n=%d, n_sample=%d)", n, n_sample);
     cudaStream_t st = bx_stream(stream);
     BX_CUDA(cudaMemsetAsync(acc9, 0, 9 * sizeof(double), st));
     pca_accum_kernel<<<grid_blocks(n_sample), 256, 0, st>>>(pts, sample_idx, n_sample, 0, acc9);

@@ -3,17 +3,19 @@
 // a17 bx_radius_neighbors replaces radius_neighbors.batch_query
 //     (/root/reference/cpp_wrappers/cpp_neighbors/wrapper.cpp:58-239 ->
 //      neighbors/neighbors.cpp:334-480 batch_nanoflanntbb_neighbors): for every query ALL supports of its cloud
-//     with d < r*r (fp64 distance from the fp32 coordinates, strict), sorted by distance, rows padded with the
-//     total support count.  Query batch b searches support cloud (b % 2) exactly like the reference, which
-//     only builds kd-trees for s_batches[0] and s_batches[1].  One CTA per query: ballot-free brute scan with a
+//     with d < r*r (fp64 distance from the fp32 coordinates, strict), sorted by (distance, index), rows padded with
+//     the total support count.  The reference sorts with std::sort, which leaves equal distances in no set order:
+//     its rows share our distance sequence and the index set of every equal-distance run, not the order inside one.
+//     Query batch b searches support cloud (b % 2) exactly like the reference, which only builds kd-trees for
+//     s_batches[0] and s_batches[1].  One CTA per query: ballot-free brute scan with a
 //     shared-memory append, then an in-CTA bitonic sort of (distance, index) -- two double kd-trees and a TBB
 //     reduction in the reference.
 // a18 bx_grid_subsample replaces grid_subsampling.subsample
 //     (/root/reference/cpp_wrappers/cpp_subsampling/wrapper.cpp:631-859 -> grid_subsampling.cpp:5-106):
 //     voxel barycentres through a device hash grid keyed by the reference's cell id
 //     iX + NX*iY + NX*NY*iZ (origin = floor(min/dl)*dl), instead of a serial unordered_map.
-// Bit contract: oracle bxo_radius_neighbors (exact) / bxo_grid_subsample (cell keys and counts exact, barycentres
-// to fp32 summation order).  Compiled with -fmad=false.
+// Bit contract: oracle bxo_radius_neighbors (exact, ties by index) / bxo_grid_subsample (cell keys and counts exact,
+// barycentres to fp32 summation order).  Compiled with -fmad=false.
 #include "bx_common.cuh"
 
 namespace {
@@ -120,6 +122,11 @@ radius_neighbors_kernel(const float *__restrict__ queries, int nq, const float *
 }
 
 // ---- a18 --------------------------------------------------------------------------------------------------
+// Empty-slot marker of the cell table.  Keys wrap modulo 2^64 (a cell index of -1 gives keys just below 2^64, 2^64-1
+// itself included), so ~0 cannot mark an empty slot; 0x8080... (a memset byte) is reached only by a grid of more
+// than 9e18 cells.
+constexpr unsigned long long GRID_EMPTY = 0x8080808080808080ull;
+
 struct GridGeom {
     float org[3];
     float dl;
@@ -178,18 +185,23 @@ __global__ void grid_insert_kernel(const float *__restrict__ pts, int n, float d
     for (int c = 0; c < 3; ++c) org[c] = floorf(decode_ordered(mi[c]) * inv) * dl;
     mx[0] = decode_ordered(mi[3]);
     mx[1] = decode_ordered(mi[4]);
-    const unsigned long long NX = (unsigned long long)floorf((mx[0] - org[0]) / dl) + 1ull;
-    const unsigned long long NY = (unsigned long long)floorf((mx[1] - org[1]) / dl) + 1ull;
+    // The grid dimensions wrap the same way: a flat axis whose origin rounded above it gives floor = -1, hence NX = 0
+    // (or NY = 0) in the reference, and every point of the cloud shares its aliased keys.
+    const unsigned long long NX = (unsigned long long)(long long)floorf((mx[0] - org[0]) / dl) + 1ull;
+    const unsigned long long NY = (unsigned long long)(long long)floorf((mx[1] - org[1]) / dl) + 1ull;
     const float x = pts[3 * (size_t)i], y = pts[3 * (size_t)i + 1], z = pts[3 * (size_t)i + 2];
-    const unsigned long long ix = (unsigned long long)floorf((x - org[0]) / dl), iy = (unsigned long long)floorf((y - org[1]) / dl),
-                             iz = (unsigned long long)floorf((z - org[2]) / dl);
+    // The fp32 origin can round above the minimum (dl = 0.025, min 40.6f: origin 40.600002), giving a cell index of -1.
+    // The reference's (size_t)floor(-1.f) is 2^64-1 on x86 (cvttss2si), so its key aliases cell (NX-1, iY-1, iZ); a
+    // direct float -> u64 cvt clamps to 0 instead.  Going through long long wraps like the reference.
+    const unsigned long long ix = (unsigned long long)(long long)floorf((x - org[0]) / dl),
+                             iy = (unsigned long long)(long long)floorf((y - org[1]) / dl),
+                             iz = (unsigned long long)(long long)floorf((z - org[2]) / dl);
     const unsigned long long key = ix + NX * iy + NX * NY * iz;
     unsigned long long h = key * 0x9E3779B97F4A7C15ull;
     unsigned slot = (unsigned)(h >> 32) & (unsigned)(tcap - 1);
-    const unsigned long long EMPTY = ~0ull;
     while (true) {
-        const unsigned long long prev = atomicCAS(&tkeys[slot], EMPTY, key);
-        if (prev == EMPTY || prev == key) break;
+        const unsigned long long prev = atomicCAS(&tkeys[slot], GRID_EMPTY, key);
+        if (prev == GRID_EMPTY || prev == key) break;
         slot = (slot + 1) & (unsigned)(tcap - 1);
     }
     atomicAdd(&tacc[4 * (size_t)slot], x);
@@ -204,7 +216,7 @@ __global__ void grid_emit_kernel(const unsigned long long *__restrict__ tkeys, c
     const int s = blockIdx.x * blockDim.x + threadIdx.x;
     if (s >= tcap) return;
     const unsigned long long k = tkeys[s];
-    if (k == ~0ull) return;
+    if (k == GRID_EMPTY) return;
     const int c = *reinterpret_cast<const int *>(&tacc[4 * (size_t)s + 3]);
     const int o = atomicAdd(d_m, 1);
     const float a = (float)(1.0 / (double)c);
@@ -253,7 +265,7 @@ BX_API int bx_grid_subsample(const float *pts, int n, float dl, unsigned long lo
     BX_REQUIRE(n >= 1 && dl > 0.0f, "bx_grid_subsample: bad arguments");
     BX_REQUIRE(table_cap >= 2 * n && (table_cap & (table_cap - 1)) == 0, "bx_grid_subsample: table_cap must be a power of two >= 2n");
     cudaStream_t st = bx_stream(stream);
-    BX_CUDA(cudaMemsetAsync(table_keys, 0xFF, sizeof(unsigned long long) * (size_t)table_cap, st));
+    BX_CUDA(cudaMemsetAsync(table_keys, 0x80, sizeof(unsigned long long) * (size_t)table_cap, st));   // GRID_EMPTY
     BX_CUDA(cudaMemsetAsync(table_acc, 0, sizeof(float) * 4 * (size_t)table_cap, st));
     BX_CUDA(cudaMemsetAsync(d_m, 0, sizeof(int), st));
     // min -> +inf (0x7f800000), max -> -inf encoded: ordered-int(-inf) = 0xff800000 ^ 0x7fffffff = 0x807fffff

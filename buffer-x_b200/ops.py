@@ -8,6 +8,7 @@ CUDA device the call raises.
 from __future__ import annotations
 
 import ctypes
+import math
 import os
 from ctypes import c_double, c_float, c_int, c_int64, c_uint64, c_void_p
 
@@ -908,24 +909,49 @@ def project_range(points: torch.Tensor, mean: torch.Tensor, axis: torch.Tensor):
     return out
 
 
+VOXEL_AXIS_CELLS = 1 << 21          # voxel keys hold 21 bits per axis
+
+
+def _dec_ordered(e):
+    """bx_bootstrap.cu's order-preserving u64 encoding of doubles, decoded on the host: int64 array -> float64 array."""
+    u = e.view(np.uint64)
+    neg = (u >> np.uint64(63)) == 0
+    return np.where(neg, ~u, u & np.uint64(0x7FFFFFFFFFFFFFFF)).view(np.float64)
+
+
 def voxel_down_sample(points: torch.Tensor, voxel: float):
-    """Open3D voxel_down_sample: returns (keys [m] int64 = ix | iy << 21 | iz << 42, xyz [m,3] f32, counts [m]), hash order."""
+    """Open3D voxel_down_sample: returns (keys [m] int64 = ix | iy << 21 | iz << 42, xyz [m,3] f32, counts [m]), hash order.
+    A cloud spanning 2^21 voxels or more on an axis is refused (its keys would alias); the extent is read from the
+    kernel's min / max in the same transfer as the voxel count.  So is a cloud whose extent is not finite (an infinite
+    coordinate, or an axis without one finite value): it has no voxel grid.  The min / max skip NaN coordinates."""
     lib = load_library()
     n = points.shape[0]
     dev = points.device
+    voxel = float(voxel)
     cap = 1
     while cap < 2 * n:
         cap <<= 1
     tkeys = torch.empty(cap, dtype=torch.int64, device=dev)
     tacc = torch.empty((cap, 4), dtype=F64, device=dev)
-    mm = torch.empty(6, dtype=torch.int64, device=dev)
+    mm_dm = torch.empty(7, dtype=torch.int64, device=dev)         # minmax6, then the voxel count in the low half of [6]
+    mm, dm = mm_dm[:6], mm_dm[6:].view(I32)
     keys = torch.empty(n, dtype=torch.int64, device=dev)
     xyz = torch.empty((n, 3), dtype=F32, device=dev)
     cnt = torch.empty(n, dtype=I32, device=dev)
-    dm = torch.zeros(1, dtype=I32, device=dev)
-    _check(lib.bx_voxel_down_sample(_dp(points, F32, "points"), n, float(voxel), _dp(tkeys), _dp(tacc), cap, _dp(mm), _dp(keys), _dp(xyz),
+    _check(lib.bx_voxel_down_sample(_dp(points, F32, "points"), n, voxel, _dp(tkeys), _dp(tacc), cap, _dp(mm), _dp(keys), _dp(xyz),
                                     _dp(cnt), _dp(dm), _stream()), "bx_voxel_down_sample")
-    m = int(dm.item())
+    h = mm_dm.cpu().numpy()
+    m = int(h[6:7].view(np.int32)[0])
+    lo, hi = _dec_ordered(h[0:3]), _dec_ordered(h[3:6])
+    for c in range(3):
+        t = (float(hi[c]) - (float(lo[c]) - voxel * 0.5)) / voxel                    # the kernel's index of the largest point
+        if not math.isfinite(t):
+            raise BufferXError(f"bx_voxel_down_sample: axis {'xyz'[c]} has no finite extent (min {lo[c]}, max {hi[c]}); "
+                               "voxel_down_sample needs finite coordinates")
+        top = math.floor(t)
+        if top >= VOXEL_AXIS_CELLS:
+            raise BufferXError(f"bx_voxel_down_sample: the cloud spans {top + 1} voxels of {voxel} on axis {'xyz'[c]}; "
+                               f"voxel keys hold fewer than 2^21 = {VOXEL_AXIS_CELLS} per axis")
     return keys[:m], xyz[:m], cnt[:m]
 
 

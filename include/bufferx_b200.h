@@ -386,8 +386,10 @@ int bx_refine(const float *ss, const float *tt, const int32_t *d_n, int maxn, co
  * Replaces radius_neighbors.batch_query (cpp_wrappers/cpp_neighbors/wrapper.cpp:58-239 ->
  * neighbors/neighbors.cpp:334-480 batch_nanoflanntbb_neighbors).  h_q_batches / h_s_batches: HOST arrays
  * (1..8 query batches, 1..2 support clouds; query batch b searches support cloud b % 2 like the reference).
- * out == NULL: counting pass (only *d_max_count is written).  Otherwise out is [nq, cap] int32, rows sorted by distance
- * and padded with ns; *d_max_count = largest true neighbour count.  Balls of up to 4096 neighbours are sorted in shared
+ * out == NULL: counting pass (only *d_max_count is written).  Otherwise out is [nq, cap] int32, rows sorted by
+ * (fp64 distance, index) and padded with ns; *d_max_count = largest true neighbour count.  The reference orders equal
+ * distances by std::sort, which is not stable: its rows have the same distance sequence and, within each run of equal
+ * distances, the same index set, but not necessarily the same order.  Balls of up to 4096 neighbours are sorted in shared
  * memory; cap > 4096 needs scratch_d [nq, cap] doubles + scratch_i [nq, cap] int32 (global rank sort of the large balls;
  * both may be NULL when cap <= 4096). */
 int bx_radius_neighbors(const float *queries, int nq, const float *supports, int ns, const int32_t *h_q_batches, int nqb,
@@ -398,7 +400,10 @@ int bx_radius_neighbors(const float *queries, int nq, const float *supports, int
  * Replaces grid_subsampling.subsample (cpp_wrappers/cpp_subsampling/wrapper.cpp:631-859 ->
  * grid_subsampling/grid_subsampling.cpp:5-106, points only).  table_keys [table_cap] u64 and table_acc
  * [table_cap,4] f32 are workspaces (table_cap = power of two >= 2n), minmax6 a 6-float workspace.
- * keys_out [n] (reference cell id iX + NX*iY + NX*NY*iZ), xyz_out [n,3], cnt_out [n] (may be NULL), *d_m = cells.
+ * keys_out [n] (reference cell id iX + NX*iY + NX*NY*iZ, u64 arithmetic), xyz_out [n,3], cnt_out [n] (may be NULL),
+ * *d_m = cells.  The fp32 origin floor(min/dl)*dl can round above the minimum; the cell index -1 then wraps to 2^64-1
+ * as in the reference's x86 build, so such points share the reference's (aliased) cell; NX and NY wrap the same way
+ * (a flat axis below its rounded-up origin gives NX or NY = 0).
  * Cells are emitted in hash-table order (the reference emits in unordered_map order). */
 int bx_grid_subsample(const float *pts, int n, float dl, unsigned long long *table_keys, float *table_acc, int table_cap,
                       float *minmax6, unsigned long long *keys_out, float *xyz_out, int32_t *cnt_out, int32_t *d_m,
@@ -406,7 +411,8 @@ int bx_grid_subsample(const float *pts, int n, float dl, unsigned long long *tab
 
 /* ---- SURVEY 8(f) row 1: loader-side geometric bootstrapping ---------------------------------------
  * bx_pca_analysis replaces compute_pca_alignment (utils/tools.py:132-149) = sklearn PCA(n_components=3) of the
- * sampled points pts[sample_idx[0..n_sample)] (sample_idx NULL: all n points), fp64.  acc9: 9-double workspace.
+ * sampled points pts[sample_idx[0..n_sample)] (sample_idx NULL: all n points), fp64; n_sample >= 3, as sklearn
+ * refuses fewer samples than components.  acc9: 9-double workspace.
  * out15: mean[3], explained variance[3] (descending), components[3][3] (rows; largest-magnitude entry positive).
  * bx_project_range: min / max over the whole cloud of (p - mean) . axis (mean_axis6 = mean[3], axis[3], on the
  * device) = the z-range of pca.transform (utils/tools.py:181-182).  work2: 2 x u64 workspace, out2: {min, max}.
@@ -414,7 +420,9 @@ int bx_grid_subsample(const float *pts, int n, float dl, unsigned long long *tab
  * 218-219): voxel_min_bound = min - voxel/2, index = floor((p - voxel_min_bound)/voxel) in fp64, output = mean of the
  * points of a voxel.  table_keys [table_cap] u64, table_acc [table_cap,4] f64 (table_cap = power of two >= 2n) and
  * minmax6 [6] u64 are workspaces; keys_out [n] = ix | iy << 21 | iz << 42, xyz_out [n,3], cnt_out [n] (may be NULL),
- * *d_m = voxels.  Emitted in hash-table order (Open3D: unordered_map order). */
+ * *d_m = voxels.  Emitted in hash-table order (Open3D: unordered_map order).  Keys are distinct only while every
+ * axis spans fewer than 2^21 voxels: the caller reads minmax6 (min xyz, max xyz, order-preserving u64 encoding of
+ * the doubles) with *d_m and refuses floor((max - voxel_min_bound)/voxel) >= 2^21, as ops.voxel_down_sample does. */
 int bx_pca_analysis(const float *pts, int n, const int32_t *sample_idx, int n_sample, double *acc9, double *out15,
                     void *stream);
 int bx_project_range(const float *pts, int n, const double *mean_axis6, unsigned long long *work2, double *out2,

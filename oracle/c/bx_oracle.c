@@ -921,8 +921,8 @@ BX_EXPORT void bxo_free(void *p) { free(p); }
 /* ------------------------------------------------------------------------------------------
  * a18. Voxel-grid barycentre sub-sampling (baseline semantics):
  * /root/reference/cpp_wrappers/cpp_subsampling/grid_subsampling/grid_subsampling.cpp:5-106 (points only).
- *   origin = floor(min * (1/dl)) * dl (fp32, :27); NX, NY = floor((max - origin)/dl) + 1 (:30-31);
- *   cell = floor((p - origin)/dl) per axis (:53-55), key = iX + NX*iY + NX*NY*iZ (:56); per cell the points are
+ *   origin = floor(min * (1/dl)) * dl (fp32, :27); NX, NY = floor((max - origin)/dl) + 1 (:30-31; -1 wraps, so 0);
+ *   cell = floor((p - origin)/dl) per axis (:53-55; -1 wraps to 2^64-1), key = iX + NX*iY + NX*NY*iZ (:56, modulo 2^64); per cell the points are
  *   summed in INPUT order in fp32 (SampledData::update_points, grid_subsampling.h:93-98) and the barycentre is
  *   sum * float(1.0/count) (:87).  The reference emits cells in unordered_map iteration order; here ascending key.
  * keys_out / xyz_out / cnt_out need capacity n.  Returns the number of occupied cells.
@@ -946,11 +946,14 @@ BX_EXPORT int bxo_grid_subsample(const float *pts, int n, float dl, uint64_t *ke
     const float inv = 1 / dl;
     float org[3];
     for (int c = 0; c < 3; ++c) org[c] = floorf(mn[c] * inv) * dl;
-    const uint64_t NX = (uint64_t)floorf((mx[0] - org[0]) / dl) + 1, NY = (uint64_t)floorf((mx[1] - org[1]) / dl) + 1;
+    /* through int64_t like the cell indices: a flat axis below its rounded-up origin gives floor = -1, NX (NY) = 0 */
+    const uint64_t NX = (uint64_t)(int64_t)floorf((mx[0] - org[0]) / dl) + 1, NY = (uint64_t)(int64_t)floorf((mx[1] - org[1]) / dl) + 1;
     bxo_ki *ki = (bxo_ki *)malloc(sizeof(bxo_ki) * (size_t)n);
     for (int i = 0; i < n; ++i) {
-        const uint64_t ix = (uint64_t)floorf((pts[3 * i] - org[0]) / dl), iy = (uint64_t)floorf((pts[3 * i + 1] - org[1]) / dl),
-                       iz = (uint64_t)floorf((pts[3 * i + 2] - org[2]) / dl);
+        /* through int64_t: a cell index of -1 (origin rounded above the minimum) wraps to 2^64-1 like the reference's
+         * x86 build, with defined behaviour */
+        const uint64_t ix = (uint64_t)(int64_t)floorf((pts[3 * i] - org[0]) / dl), iy = (uint64_t)(int64_t)floorf((pts[3 * i + 1] - org[1]) / dl),
+                       iz = (uint64_t)(int64_t)floorf((pts[3 * i + 2] - org[2]) / dl);
         ki[i].key = ix + NX * iy + NX * NY * iz;
         ki[i].idx = i;
     }

@@ -1191,6 +1191,8 @@ def pca_alignment(pts, sample_idx):
     largest magnitude is positive (sklearn >= 1.5: svd_flip(u_based_decision=False)).  Pinned against sklearn itself in
     tests/test_oracle_cpu.py.  Returns (sphericity, is_aligned, mean, variance[3], components[3,3])."""
     X = np.asarray(pts, dtype=np.float64)[np.asarray(sample_idx)]
+    if X.shape[0] < 3:                 # sklearn's PCA(n_components=3) refuses fewer samples than components
+        raise ValueError(f"n_components=3 must be between 0 and min(n_samples, n_features)={X.shape[0]}")
     mean = X.mean(axis=0)
     Xc = X - mean
     C = (Xc.T @ Xc) / (X.shape[0] - 1)
@@ -1229,10 +1231,16 @@ def voxel_down_sample(pts, voxel: float):
     not under /root/reference -- restated from the published algorithm, anchored on the call sites dataset/*.py and
     utils/tools.py:218-219): voxel_min_bound = min_bound - voxel*0.5; index = floor((p - voxel_min_bound)/voxel);
     output = mean of the points of a voxel (double accumulation).  Returns (keys [m] = ix | iy<<21 | iz<<42 sorted
-    ascending, means [m,3] float64, counts [m]) -- Open3D's own output order is that of an unordered_map."""
+    ascending, means [m,3] float64, counts [m]) -- Open3D's own output order is that of an unordered_map.  Like
+    ops.voxel_down_sample it refuses a cloud spanning 2^21 voxels or more on an axis, where those keys would alias."""
     P = np.asarray(pts, dtype=np.float64)
+    if not np.isfinite(P).all():
+        raise ValueError("voxel_down_sample: needs finite coordinates")
     vmb = P.min(axis=0) - voxel * 0.5
     iv = np.floor((P - vmb) / voxel).astype(np.int64)
+    if iv.max() >= 1 << 21:
+        raise ValueError(f"voxel_down_sample: the cloud spans {iv.max() + 1} voxels of {voxel} on an axis; keys hold "
+                         f"fewer than 2^21 = {1 << 21} per axis")
     keys = (iv[:, 0] & 0x1FFFFF) | ((iv[:, 1] & 0x1FFFFF) << 21) | ((iv[:, 2] & 0x1FFFFF) << 42)
     uk, inv, cnt = np.unique(keys, return_inverse=True, return_counts=True)
     sums = np.zeros((len(uk), 3))
