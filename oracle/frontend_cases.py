@@ -250,19 +250,31 @@ PATCH_KINDS = ("uniform", "exact", "cells", "counts", "empty", "big")
 def check_ball_query(xyz, qry, radius, idx, chunk=1 << 24):
     """Each row: strictly increasing listed prefix of hits or undecided points; no decided hit skipped below the last
     listed entry; when fewer than P are listed, no decided hit missing; the rest padded with the first index; an empty
-    ball all zeros."""
+    ball all zeros.  Batched form: xyz [B,N,3], qry [B,Q,3], idx [B,Q,P], every cloud's rows to its own points."""
     idx = torch.as_tensor(np.asarray(idx) if not isinstance(idx, torch.Tensor) else idx).long()
     q = qry if isinstance(qry, torch.Tensor) else torch.from_numpy(np.ascontiguousarray(qry))
     p = xyz if isinstance(xyz, torch.Tensor) else torch.from_numpy(np.ascontiguousarray(xyz))
     dev = p.device
     idx = idx.to(dev)
+    if p.dim() == 3:
+        out = {}
+        step = max(1, chunk // max(1, q.shape[1] * p.shape[1]))
+        for b in range(0, p.shape[0], step):
+            merge(out, _check_ball_query_rows(lambda a, s: O.ball_query_fp64(p[b:b + step], q[b:b + step], radius).reshape(-1, p.shape[1]),
+                                              idx[b:b + step].reshape(-1, idx.shape[-1]), p.shape[1], 1 << 62))
+        return out
+    return _check_ball_query_rows(lambda a, s: O.ball_query_fp64(p, q[a:a + s], radius), idx, p.shape[0], chunk)
+
+
+def _check_ball_query_rows(status, idx, N, chunk):
+    """check_ball_query on index rows [Q,P] whose float64 statuses [rows, N] status(a, step) gives for rows a..a+step."""
+    dev = idx.device
     Q, P = idx.shape
-    N = p.shape[0]
     out = dict(bq_rows=Q, bq_undecided_pairs=0, bq_undecided_listed=0, bq_empty=0, bq_full=0)
     step = max(1, chunk // N)
     ar = torch.arange(N, device=dev)
     for a in range(0, Q, step):
-        st = O.ball_query_fp64(p, q[a:a + step], radius)
+        st = status(a, step)
         row = idx[a:a + step]
         inc = row[:, 1:] > row[:, :-1]
         c = 1 + torch.cumprod(inc.to(torch.int64), 1).sum(1)

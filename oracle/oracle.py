@@ -488,11 +488,12 @@ def radius_estimation_fp64(src_pts, src_kpts, tgt_pts, tgt_kpts, thresholds, tol
 def ball_query_fp64(xyz, qry, radius, kb=7.0):
     """pointnet2 ``ball_query`` hit test d2 < radius^2 in float64: radius^2 the fp32 product, d64 = sum (q - p)^2.  The
     fp32 d2 = ((dx*dx)+(dy*dy))+(dz*dz), dx = fl(q - p), is within 5u d64 and equals it when every fp32 intermediate is
-    exact.  Returns status [Q,N] int8: 1 decided hit, 0 decided miss, 2 undecided."""
+    exact.  Returns status [Q,N] int8: 1 decided hit, 0 decided miss, 2 undecided ([B,Q,N] for batched xyz [B,N,3],
+    qry [B,Q,3])."""
     p, q = _t64(xyz), _t64(qry)
     r = np.float32(radius)
     r2 = float(np.float32(r * r))
-    dd = q[:, None, :] - p[None, :, :]
+    dd = q[..., :, None, :] - p[..., None, :, :]
     sq = dd * dd
     s1 = sq[..., 0] + sq[..., 1]
     d = s1 + sq[..., 2]

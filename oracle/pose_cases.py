@@ -118,13 +118,13 @@ def report(name, out):
 
 
 # ------------------------------------------------------------------------------------------------ a10
-def _nn_side(M, best, second, got, Kother, what):
-    """One side of matching: outside the margin the first float64 minimum; inside it a candidate within the margin, and
-    never a later copy of a bitwise-equal row (the first minimum wins on exact ties)."""
+def _nn_side(M, best, second, got, Kother, what, C=32):
+    """One side of matching over C features: outside the margin KN (C + 3) u d the first float64 minimum; inside it a
+    candidate within the margin, and never a later copy of a bitwise-equal row (the first minimum wins on exact ties)."""
     K = M.shape[0]
     if K == 0:
         return 0.0, 0
-    eps = lambda d: KN * 35 * U * d + 1e-30
+    eps = lambda d: KN * (C + 3) * U * d + 1e-30
     dec = (second - best) > eps(best) + eps(second)
     ref = M.argmin(1)
     bad = dec & (got != ref)
