@@ -1,4 +1,5 @@
-"""BufferX on H100: the per-pair registration ``forward()`` and, in eval mode, the training stages' validation forward.
+"""BufferX on H100: the per-pair registration ``forward()``, in eval mode the training stages' validation forward, and in
+training mode the Pose stage's step (batch-statistics BatchNorm, ``pred_ind`` differentiable in ``Pose.conv``).
 
 Mirrors ``BufferX`` of /root/reference/models/BUFFERX.py (constructor :72-84, inference branch of
 ``forward`` :257-467, ``mutual_matching`` :469-496, ``post_refinement`` :522-556): same attribute names
@@ -134,6 +135,9 @@ class _PairSlot:
             self.graph = torch.cuda.CUDAGraph()
             with torch.cuda.device(dev), torch.cuda.graph(self.graph, stream=self.stream):
                 self.tail = self._enqueue()
+            # the graph replays the device pointers of the folded weights it captured: keep those tensors alive even when
+            # a later in-place weight change makes the caches rebuild (load_state_dict / .to() drop the slots themselves)
+            self.captured_weights = (model.Desc.prepared(dev), model.Desc.conv_net.folded(), model.Pose.conv.folded())
         # pinned landing buffer for the result block
         n_tail = 18 + (S + 1) + 1 + 1 + 16 + 1   # RANSAC block, scale offsets, consensus count, scales used, refined pose, fp16-range flag
         self.h_tail = torch.empty(n_tail, dtype=torch.float64).pin_memory()
@@ -683,7 +687,10 @@ class BufferX(nn.Module):
         return center
 
     def _train_forward(self, data_source, perms=None, aug_angles=None, match_choice=None):
-        """Validation forward of cfg.stage "Desc" / "Pose" in eval mode (reference BUFFERX.py:148-255): ground-truth
+        """Validation forward of cfg.stage "Desc" / "Pose" in eval mode (reference BUFFERX.py:148-255), or with the model in
+        training mode the forward of the Pose stage's training step (every BatchNorm on batch statistics, its running
+        statistics updated: the descriptor network's twice, source then target; ``pred_ind`` carries a grad_fn into
+        ``Pose.conv``'s weights and biases; the batch statistics land in ``self.last_train_stats``): ground-truth
         correspondences on the second-level clouds, descriptors of the (sub-sampled) matched key-points, then EquiMatch
         score + integer SO(2) label ("Desc") or CostNet soft arg-max + float SO(2) label of the augmented target ("Pose").
         NumPy's global RNG is consumed like the reference: match sub-sampling (only beyond cfg.train.pos_num), des_r,
@@ -698,7 +705,12 @@ class BufferX(nn.Module):
         def _pts(x, shape=(-1, 3)):
             return torch.as_tensor(x).to(dev, dtype=torch.float32, non_blocking=True).reshape(*shape).contiguous()
 
+        train = self.training
         rng_state = np.random.get_state()     # replayed if the pair has to be recomputed on the TF32 kernels
+        if train:
+            # the step moves every running statistic and optimizer.step() the weights: captured graphs hold the old folded ones
+            self._drop_captured_state()
+            stats = dict(src=[], tgt=[], pose=[])
         with torch.cuda.device(dev):
             src, tgt = _pts(data_source["src_fds_pcd"]), _pts(data_source["tgt_fds_pcd"])
             src_sds, tgt_sds = _pts(data_source["src_sds_pcd"]), _pts(data_source["tgt_sds_pcd"])
@@ -721,8 +733,13 @@ class BufferX(nn.Module):
             des_r = self._draw_des_r()
             aligned = bool(data_source["is_aligned_to_global_z"])
             ps, pt = (None, None) if perms is None else perms
-            src_d = self.Desc(src[None], src_kpt[None], des_r, aligned, perm=ps)
-            tgt_d = self.Desc(tgt[None], tgt_kpt[None], des_r, aligned, None, stage == "Pose", perm=pt, aug_angles=aug_angles)
+            if train:
+                src_d = self.Desc.forward_train(src[None], src_kpt[None], des_r, aligned, perm=ps, stats=stats["src"])
+                tgt_d = self.Desc.forward_train(tgt[None], tgt_kpt[None], des_r, aligned, True, perm=pt, aug_angles=aug_angles,
+                                                stats=stats["tgt"])
+            else:
+                src_d = self.Desc(src[None], src_kpt[None], des_r, aligned, perm=ps)
+                tgt_d = self.Desc(tgt[None], tgt_kpt[None], des_r, aligned, None, stage == "Pose", perm=pt, aug_angles=aug_angles)
             K = src_kpt.shape[0]
             if K < 2:
                 print(f"{data_source.get('src_id')} {data_source.get('tgt_id')} don't have enough patches")
@@ -731,6 +748,10 @@ class BufferX(nn.Module):
                 out = {"src_kpt": src_kpt, "tgt_kpt": tgt_kpt, "src_des": src_d["desc"], "tgt_des": tgt_d["desc"],
                        "equi_score": ops.equi_match(src_d["equi"], tgt_d["equi"]),
                        "gt_label": ops.so2_gt(src_d["rand_axis"], src_d["R"], tgt_d["R"], T, azi_n, True)}
+            elif train:
+                out = {"pred_ind": self.Pose.conv.forward_train(src_d["equi"], tgt_d["equi"], stats["pose"]),
+                       "gt_ind": ops.so2_gt(src_d["rand_axis"], src_d["R"], tgt_d["R"], T, azi_n, False, aug_R=tgt_d["aug_rotation"])}
+                self.last_train_stats = stats
             else:
                 # patch i of the source against patch i of the target: identity match lists through CostNet, the soft
                 # arg-max from the hypothesis kernel (its pose outputs land in scratch buffers)
@@ -745,7 +766,8 @@ class BufferX(nn.Module):
                                *scratch)
                 out = {"pred_ind": pred,
                        "gt_ind": ops.so2_gt(src_d["rand_axis"], src_d["R"], tgt_d["R"], T, azi_n, False, aug_R=tgt_d["aug_rotation"])}
-            overflow = self.Desc.conv_net.overflow_flag(dev).item() != 0
+            # the training step runs every convolution on the TF32 kernel, which has no fp16-range limit: nothing to recompute
+            overflow = not train and self.Desc.conv_net.overflow_flag(dev).item() != 0
         if overflow:      # an activation left fp16 range: recompute the pair with the TF32 kernels and the same draws
             np.random.set_state(rng_state)
             net = self.Desc.conv_net
@@ -759,10 +781,15 @@ class BufferX(nn.Module):
     def forward(self, data_source, perms=None, ransac_seed=None, debug=False, aug_angles=None, match_choice=None):
         cfg = self.config
         if cfg.stage != "test":
-            if cfg.stage not in ("Desc", "Pose") or self.training:
+            if cfg.stage not in ("Desc", "Pose") or (self.training and cfg.stage != "Pose"):
                 raise NotImplementedError(
-                    "bufferx_b200 runs cfg.stage 'test' and, in eval mode, the validation forward of the training stages "
-                    "'Desc' / 'Pose'; training-mode BatchNorm and the backward pass are not built (call model.eval())")
+                    "bufferx_b200 runs cfg.stage 'test', in eval mode the validation forward of the training stages "
+                    "'Desc' / 'Pose', and the training step of stage 'Pose'; training-mode BatchNorm and the backward pass of "
+                    "stage 'Desc' are not built (call model.eval())")
+            if self.training and any(p.requires_grad for p in self.Desc.parameters()):
+                raise NotImplementedError(
+                    "the Pose training step needs the descriptor network frozen (requires_grad=False on every Desc parameter, "
+                    "as train.py does for this stage): the backward pass through Desc is not built")
             if next(self.parameters()).device.type != "cuda":
                 raise ops.BufferXError("BufferX.forward needs the model on a CUDA device: there is no CPU path")
             return self._train_forward(data_source, perms, aug_angles, match_choice)

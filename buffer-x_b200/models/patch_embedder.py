@@ -2,8 +2,10 @@
 
 Mirrors ``MiniSpinNet`` of /root/reference/models/patch_embedder.py (constructor :16-42, forward :44-90,
 same sub-module names -> same state_dict keys ``pnt_layer.{0,1}``, ``pool_layer.{0,1,3,4}``,
-``conv_net.ops.*``).  Eval mode only: select_patches -> axis_align -> normalize -> SPT -> pnt_layer+max ->
-Cylindrical_Net -> attention pooling, every stage a hand-written CUDA kernel behind the C-ABI.
+``conv_net.ops.*``).  select_patches -> axis_align -> normalize -> SPT -> pnt_layer+max -> Cylindrical_Net -> attention
+pooling, every stage a hand-written CUDA kernel behind the C-ABI.  ``forward`` is the eval-mode forward; ``forward_train``
+normalises every BatchNorm with its batch statistics and updates the running statistics, as the module does under
+model.train() (the Pose training stage runs it with the descriptor network frozen: no gradients flow here).
 """
 import numpy as np
 import torch
@@ -47,6 +49,7 @@ class MiniSpinNet(nn.Module):
                                         nn.Conv2d(16, 1, kernel_size=(1, 1)), nn.BatchNorm2d(1), nn.ReLU(True))
         self.conv_net = pn.Cylindrical_Net(inchan=16, dim=32)
         self._prep = None
+        self._prep_key = None
 
     # ---- folded small layers + geometry tables, cached per device -------------------------------------
     def _apply(self, fn, *a, **k):
@@ -58,7 +61,9 @@ class MiniSpinNet(nn.Module):
         return super()._load_from_state_dict(*a, **k)
 
     def prepared(self, device):
-        if self._prep is None or self._prep["device"] != device:
+        key = pn.state_version(self.pnt_layer) + pn.state_version(self.pool_layer)
+        if self._prep is None or self._prep["device"] != device or self._prep_key != key:
+            self._prep_key = key
             bn = self.pnt_layer[1]
             Wt, b = pn.fold_conv_bn(self.pnt_layer[0].weight, self.pnt_layer[0].bias, bn.running_mean, bn.running_var,
                                     bn.weight, bn.bias, bn.eps)          # [1,3,16]
@@ -117,6 +122,71 @@ class MiniSpinNet(nn.Module):
             out.update(idx=idx, raw_patches=patches, vidx=res[1], inv=res[2], feat=ops.from_blocked(feat),
                        x=ops.from_blocked(x).view(K, -1, self.ele_n, self.azi_n))
         return out
+
+    def forward_train(self, pts, kpts, des_r, is_aligned_to_global_z, is_aug=False, perm=None, aug_angles=None, stats=None):
+        """MiniSpinNet.forward under model.train() (patch_embedder.py:44-90): the same patches, frames, augmentation and SPT
+        as ``forward``, but each of the ten BatchNorm layers normalises with its batch statistics and updates its running
+        statistics once.  The point layer's statistics over the K x 420 x 10 samples (zero slots included) follow from the
+        float64 moments of its de-rotated 3-vectors (it is linear: mean = W E[x] + b, var = diag(W Cov(x) W^T)); the pool
+        layer's from its 1x1 convolutions over K x 140 positions.  ``stats``: optional list receiving (batch mean, batch
+        variance) of every BatchNorm in module order (pnt_layer, conv_net, pool_layer), float64.  Returns ``forward``'s dict."""
+        pts = pts[0].contiguous()
+        kpts = kpts[0].contiguous()
+        dev = pts.device
+        N = pts.shape[0]
+        if perm is None:
+            perm = np.random.choice(N, N, replace=False)
+        if not isinstance(perm, torch.Tensor):
+            perm = torch.from_numpy(np.ascontiguousarray(perm, dtype=np.int32)).to(dev, non_blocking=True)
+        prep = self.prepared(dev)
+        pts4 = ops.permute_cloud(pts, perm)
+        patches, _ = ops.select_patches(pts4, kpts, des_r, self.patch_sample)
+        delta, R, rand_axis = ops.lrf(patches, des_r, bool(is_aligned_to_global_z))
+        aug_R = None
+        if is_aug:
+            if aug_angles is None:
+                aug_angles = (np.random.random([kpts.shape[0], 1]) * 2 * np.pi)[:, 0].astype(np.float32)
+            ang = torch.as_tensor(np.ascontiguousarray(aug_angles, dtype=np.float32)).to(dev, non_blocking=True)
+            aug_R = ops.so2_augment(delta, rand_axis, ang)
+        args = (delta, prep["voxels"], prep["rot"], self.delta / self.rad_n, self.voxel_sample)
+        _, _, inv = ops.spt_pnt(*args, prep["w_pnt"], prep["b_pnt"], self.azi_n, debug=True)   # the samples the point layer sees
+        # point layer: batch statistics of the linear 3 -> 16 map from the moments of its inputs
+        conv, bn = self.pnt_layer[0], self.pnt_layer[1]
+        R_n = inv.numel() // 3
+        mo = ops.moments3(inv) / R_n
+        Ex = mo[:3]
+        Exx = torch.stack([mo[[3, 4, 5]], mo[[4, 6, 7]], mo[[5, 7, 8]]])
+        cov = Exx - Ex[:, None] * Ex[None, :]
+        Wp = conv.weight.detach().double().view(16, 3)
+        mean = Wp @ Ex + conv.bias.detach().double()
+        var = torch.clamp(((Wp @ cov) * Wp).sum(dim=1), min=0.0)
+        pn.bn_batch_stats(torch.stack([mean * R_n, (var + mean * mean) * R_n]), R_n, bn)
+        if stats is not None:
+            stats.append((mean, var))
+        Wt, b = pn.fold_conv_bn(conv.weight, conv.bias, mean, var, bn.weight, bn.bias, bn.eps)
+        feat = ops.spt_pnt(*args, Wt[0].t().contiguous().to(dev), b.to(dev), self.azi_n)
+        x = self.conv_net.forward_train(feat, stats)                      # [K,8,140,4]
+        # pool layer: two 1x1 convolutions, each followed by a batch-statistics BatchNorm and ReLU
+        c1, b1n, c2, b2n = self.pool_layer[0], self.pool_layer[1], self.pool_layer[3], self.pool_layer[4]
+        K = x.shape[0]
+        W1, bb1 = pn.fold_conv_bn(c1.weight, c1.bias)                    # [1,32,16]
+        z1 = ops.conv1x1(x, W1[0].contiguous(), bb1)
+        m1, v1 = pn.bn_batch_stats(ops.channel_sums(z1), K * 140, b1n)
+        sc, sh = pn.bn_scale_shift(m1, v1, b1n)
+        h = ops.bn_apply(z1, sc, sh, True)
+        W2, bb2 = pn.fold_conv_bn(c2.weight, c2.bias)                    # [1,16,1]
+        w2p = torch.zeros((16, 4), dtype=torch.float32, device=dev)
+        w2p[:, :1] = W2[0]
+        b2p = torch.zeros(4, dtype=torch.float32, device=dev)
+        b2p[:1] = bb2
+        z2 = ops.conv1x1(h, w2p, b2p)                                     # channel 0 is the attention logit
+        m2, v2 = pn.bn_batch_stats(ops.channel_sums(z2)[:, :1], K * 140, b2n)
+        if stats is not None:
+            stats += [(m1, v1), (m2, v2)]
+        Wf1, bf1 = pn.fold_conv_bn(c1.weight, c1.bias, m1, v1, b1n.weight, b1n.bias, b1n.eps)
+        Wf2, bf2 = pn.fold_conv_bn(c2.weight, c2.bias, m2, v2, b2n.weight, b2n.bias, b2n.eps)
+        desc, equi = ops.pool_desc(x, Wf1[0].contiguous(), bf1, Wf2[0, :, 0].contiguous(), bf2, channels_last=True)
+        return {"desc": desc, "equi": equi, "rand_axis": rand_axis, "R": R, "patches": delta, "aug_rotation": aug_R}
 
     def forward_multi(self, jobs, is_aligned_to_global_z, radii=None, counts=None, npts=None):
         """Descriptors of several (cloud, key-points, radius, permutation) jobs in ONE pass through SPT, the

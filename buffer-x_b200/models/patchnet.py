@@ -5,12 +5,21 @@ Mirrors the state_dict layout of /root/reference/models/patchnet.py: ``Cylindric
 stacks have ``affine=False`` (:28,31).  The modules hold parameters only -- the arithmetic runs in
 the library's convolution kernels (``bx_conv_layer_sd``, ``bx_conv_layer_tc``, ``bx_costvol_ab``).  ``folded()``
 returns, per conv layer, the weight re-laid as [tap][Cin][Cout] with the eval-mode BatchNorm folded in (computed in
-fp64, stored fp32), and the kernels' operand images of it.
+fp64, stored fp32), and the kernels' operand images of it; the cache is keyed on the versions of the parameters and
+buffers, so an optimizer step or a training-mode forward (which moves the running statistics) invalidates it.
+
+Training mode (cfg.stage "Pose", model.train()): ``Cylindrical_Net.forward_train`` runs the convolutions on
+``bx_conv_layer_tc`` with the unfolded weights, ``CostNet.forward_train`` on float64 CUDA-core kernels, and both normalise
+every BatchNorm'd layer with its batch statistics (bx_train_step.cu), updating the running statistics as torch's BatchNorm
+does in training mode.  CostNet's forward sits behind one autograd Function whose backward (bx_ts_conv_backward and the
+BatchNorm backward, float64) gives the gradients of every ``ops.*`` weight and bias.
 """
+import itertools
+import os
+
 import torch
 import torch.nn as nn
-
-import os
+from torch.autograd.function import once_differentiable
 
 from bufferx_b200 import ops
 
@@ -42,6 +51,40 @@ def fold_conv_bn(conv_w, conv_b, bn_mean=None, bn_var=None, bn_w=None, bn_b=None
     return Wt, b.float().contiguous()
 
 
+def state_version(module):
+    """Identity of the current values of a module's parameters and buffers: changes with every in-place update
+    (optimizer.step(), the running statistics of a training-mode forward) and every replacement."""
+    return tuple((t.data_ptr(), t._version) for t in itertools.chain(module.parameters(), module.buffers()))
+
+
+def bn_batch_stats(sums, N, bn, update=True):
+    """Per-channel sums [2, C] (sum x, sum x^2, float64) over N samples -> the batch mean and biased variance (float64) that
+    a training-mode BatchNorm normalises with; with ``update`` also torch's running update: running_mean <- (1 - m)
+    running_mean + m mean, running_var <- (1 - m) running_var + m var N / (N - 1), num_batches_tracked += 1 (m =
+    bn.momentum, or the cumulative 1 / num_batches_tracked when it is None)."""
+    mean = sums[0] / N
+    var = torch.clamp(sums[1] / N - mean * mean, min=0.0)
+    if update:
+        with torch.no_grad():
+            bn.num_batches_tracked += 1
+            m = bn.momentum if bn.momentum is not None else 1.0 / float(bn.num_batches_tracked.item())
+            bn.running_mean.copy_((1.0 - m) * bn.running_mean.double() + m * mean)
+            bn.running_var.copy_((1.0 - m) * bn.running_var.double() + m * var * (N / max(N - 1, 1)))
+    return mean, var
+
+
+def bn_scale_shift(mean, var, bn, dtype=torch.float32):
+    """Normalisation by batch statistics as one per-channel affine map (computed in float64, stored as ``dtype``):
+    x^ = x scale + shift."""
+    scale = 1.0 / torch.sqrt(var + bn.eps)
+    if bn.affine:
+        scale = scale * bn.weight.detach().double()
+    shift = -mean * scale
+    if bn.affine:
+        shift = shift + bn.bias.detach().double()
+    return scale.to(dtype).contiguous(), shift.to(dtype).contiguous()
+
+
 class _ConvStack(nn.Module):
     """ModuleList ``ops`` with the reference's index layout: conv, [bn], [relu], conv, ..."""
 
@@ -63,6 +106,7 @@ class _ConvStack(nn.Module):
                 self.ops.append(nn.ReLU(inplace=True))
             self.layers.append((ci, bi, relu))
         self._folded = None
+        self._folded_key = None
         self.sd_kernel_sizes = ()    # kernel sizes whose layers also get the fp16-split weight image of bx_conv_layer_sd
 
     def invalidate(self):
@@ -77,7 +121,9 @@ class _ConvStack(nn.Module):
         return super()._load_from_state_dict(*a, **k)
 
     def folded(self):
-        if self._folded is None:
+        key = state_version(self)
+        if self._folded is None or self._folded_key != key:
+            self._folded_key = key
             out = []
             for (ci, bi, relu) in self.layers:
                 conv = self.ops[ci]
@@ -94,6 +140,36 @@ class _ConvStack(nn.Module):
                                 b=b, cin=conv.in_channels, cout=conv.out_channels, k=kk, relu=relu))
             self._folded = out
         return self._folded
+
+    def _layer_train(self, i, x, n, geom, D, H, W):
+        """Layer i in training mode on the blocked input x, then (BatchNorm'd layers) the batch statistics and normalise +
+        ReLU -> (output, record of what the backward needs).  The descriptor stack (cylindrical geometries) runs the unfolded
+        convolution on bx_conv_layer_tc in fp32; CostNet (GEOM_VALID3D) runs in float64 on bx_ts_conv_forward, the
+        precision its backward needs."""
+        ci, bi, relu = self.layers[i]
+        conv = self.ops[ci]
+        ks = tuple(conv.kernel_size)
+        kd, kh, kw = ks if len(ks) == 3 else (1,) + ks
+        f64 = geom == ops.GEOM_VALID3D
+        if f64:
+            OD, OH, OW = D - kd + 1, H - kh + 1, W - kw + 1
+            Wt = conv.weight.detach().double().reshape(conv.out_channels, conv.in_channels, -1).permute(2, 1, 0).contiguous()
+            z = ops.conv_forward(x, Wt, conv.bias.detach().double().contiguous(), D, H, W, kd, kh, kw)
+        else:
+            OD, OH, OW = 1, 7, 20
+            Wt, b = fold_conv_bn(conv.weight, conv.bias)
+            z = torch.empty((n, conv.out_channels // 4, OD * OH * OW, 4), dtype=torch.float32, device=x.device)
+            ops.conv_layer_tc(geom, x, ops.conv_tc_weights(Wt), b, z, n, conv.in_channels, conv.out_channels, D, H, W, kd, kh, kw,
+                              relu and bi is None)
+        rec = dict(x=x, z=z, Wt=Wt, geom=(D, H, W, kd, kh, kw), out=(OD, OH, OW))
+        if bi is None:
+            return z, rec
+        bn = self.ops[bi]
+        N = n * OD * OH * OW
+        mean, var = bn_batch_stats(ops.channel_sums(z), N, bn)
+        scale, shift = bn_scale_shift(mean, var, bn, z.dtype)
+        rec.update(scale=scale, shift=shift, N=N, batch_mean=mean, batch_var=var)
+        return ops.bn_apply(z, scale, shift, relu), rec
 
 
 class Cylindrical_Net(_ConvStack):
@@ -142,6 +218,34 @@ class Cylindrical_Net(_ConvStack):
                 ops.conv_layer_tc(ops.GEOM_CYL2D, cur, l["w_tc"], l["b"], out, K, l["cin"], l["cout"], 1, 7, 20, 1, 3, 3, l["relu"], d_n=d_n)
             cur = out
         return cur, None
+
+    def forward_train(self, x, stats=None):
+        """Training mode: x [K,4,420,4] channel-blocked features -> [K,8,140,4].  Every BatchNorm normalises with the batch
+        statistics over K x 140 positions and updates its running statistics once.  ``stats``: optional list that receives
+        (batch mean, batch variance) of each BatchNorm, float64."""
+        K = x.shape[0]
+        cur = x.contiguous()
+        for i in range(len(self.layers)):
+            cur, rec = self._layer_train(i, cur, K, ops.GEOM_CYL3D if i == 0 else ops.GEOM_CYL2D, 3 if i == 0 else 1, 7, 20)
+            if stats is not None and "batch_mean" in rec:
+                stats.append((rec["batch_mean"], rec["batch_var"]))
+        return cur
+
+
+class _CostNetTrain(torch.autograd.Function):
+    """pred_ind = soft arg-max of CostNet(cost volume) in training mode, differentiable in CostNet's weights and biases."""
+
+    @staticmethod
+    def forward(ctx, net, equi_s, equi_t, stats, *params):
+        ind, saved = net._forward_train(equi_s, equi_t, stats)
+        ctx.net, ctx.saved = net, saved
+        return ind
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, g):
+        grads = ctx.net._backward_train(ctx.saved, g.double().contiguous())
+        return (None, None, None, None) + tuple(grads)
 
 
 class CostNet(_ConvStack):
@@ -208,3 +312,46 @@ class CostNet(_ConvStack):
                                   d_n=d_M)
             cur, D, H, W = out, OD, OH, OW
         return cur.view(maxM, L[-1]["cout"])      # one output position: blocked [maxM, C/4, 1, 4] == [maxM, C]
+
+    def train_params(self):
+        """(weight, bias) of every convolution, in layer order: the inputs the training Function differentiates."""
+        return [t for (ci, _, _) in self.layers for t in (self.ops[ci].weight, self.ops[ci].bias)]
+
+    def forward_train(self, equi_s, equi_t, stats=None):
+        """Training mode, patch i of equi_s against patch i of equi_t ([M,32,7,20] full maps; rows 1..ele_n-2 enter the
+        cost volume) -> pred_ind [M] (reference CostVolume.forward, models/BUFFERX.py:52-69), carrying a grad_fn when
+        gradients are enabled and a convolution parameter requires them.  Each BatchNorm normalises with the batch
+        statistics over M x its output positions and updates its running statistics once."""
+        return _CostNetTrain.apply(self, equi_s.contiguous(), equi_t.contiguous(), stats, *self.train_params())
+
+    def _forward_train(self, equi_s, equi_t, stats):
+        M = equi_s.shape[0]
+        cur = ops.costvol(equi_s, equi_t)                 # float64 [M, 8, 20*5*20, 4]
+        D, H, W = 20, 5, 20
+        saved = []
+        for i in range(len(self.layers)):
+            cur, rec = self._layer_train(i, cur, M, ops.GEOM_VALID3D, D, H, W)
+            D, H, W = rec["out"]
+            saved.append(rec)
+            if stats is not None and "batch_mean" in rec:
+                stats.append((rec["batch_mean"], rec["batch_var"]))
+        logits = cur.view(M, -1)
+        return ops.softargmax(logits).float(), dict(layers=saved, logits=logits)
+
+    def _backward_train(self, saved, g):
+        dy = ops.softargmax(saved["logits"], g)           # dL/dlogits [M, 20] == blocked [M, 5, 1, 4]
+        grads = []
+        for i in reversed(range(len(self.layers))):
+            rec = saved["layers"][i]
+            conv = self.ops[self.layers[i][0]]
+            dy = dy.view(rec["z"].shape)
+            if "scale" in rec:                            # ReLU mask + batch-statistics BatchNorm backward
+                s = ops.channel_sums(dy, rec["z"], rec["scale"], rec["shift"]) / rec["N"]
+                dz = ops.bn_backward(dy, rec["z"], rec["scale"], rec["shift"], s[0].contiguous(), s[1].contiguous())
+            else:
+                dz = dy
+            db = ops.channel_sums(dz)[0]
+            dx, dW = ops.conv_backward(rec["x"], dz, rec["Wt"], *rec["geom"], want_dx=i > 0)
+            grads = [dW.permute(2, 1, 0).reshape(conv.weight.shape).to(conv.weight.dtype), db.to(conv.bias.dtype)] + grads
+            dy = dx
+        return grads

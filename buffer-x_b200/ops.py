@@ -32,6 +32,8 @@ SYMBOLS = [
     "bx_select_patches_grid_batched_counts",
     "bx_ball_query_batched", "bx_gather_channels", "bx_knn1", "bx_svd3", "bx_icp_workspace_bytes", "bx_icp",
     "bx_fps_large", "bx_fps_large_workspace_bytes", "bx_fps_large_n", "bx_fps_large_size_class", "bx_radius_estimate_n_sub",
+    "bx_ts_splits", "bx_ts_channel_sums", "bx_ts_channel_sums_f64", "bx_ts_moments3", "bx_ts_bn_apply", "bx_ts_bn_apply_f64",
+    "bx_ts_bn_backward", "bx_ts_conv1x1", "bx_ts_costvol", "bx_ts_softargmax", "bx_ts_conv_forward", "bx_ts_conv_backward",
 ]
 
 GEOM_CYL3D, GEOM_CYL2D, GEOM_VALID3D, GEOM_COSTAB = 0, 1, 2, 4
@@ -127,6 +129,17 @@ def load_library():
     lib.bx_icp_workspace_bytes.argtypes = [c_int, c_int]
     lib.bx_icp_workspace_bytes.restype = c_int64
     lib.bx_icp.argtypes = [P, c_int, P, c_int, c_double, P, c_double, c_double, c_int, P, P, P, P]
+    lib.bx_ts_channel_sums.argtypes = [P, c_int, c_int, c_int, P, P, P]
+    lib.bx_ts_channel_sums_f64.argtypes = [P, P, P, P, c_int, c_int, c_int, P, P, P]
+    lib.bx_ts_bn_apply_f64.argtypes = [P, P, P, c_int, c_int, c_int, c_int, P, P]
+    lib.bx_ts_conv_forward.argtypes = [P, P, P] + [c_int] * 9 + [P, P]
+    lib.bx_ts_moments3.argtypes = [P, c_int64, P, P, P]
+    lib.bx_ts_bn_apply.argtypes = [P, P, P, c_int, c_int, c_int, c_int, P, P]
+    lib.bx_ts_bn_backward.argtypes = [P, P, P, P, P, P, c_int, c_int, c_int, P, P]
+    lib.bx_ts_conv1x1.argtypes = [P, P, P, c_int, c_int, c_int, c_int, P, P]
+    lib.bx_ts_costvol.argtypes = [P, P, c_int, P, P]
+    lib.bx_ts_softargmax.argtypes = [P, c_int, c_int, P, P, P, P]
+    lib.bx_ts_conv_backward.argtypes = [P, P, P] + [c_int] * 9 + [P, P, P, P]
     _lib = lib
     return lib
 
@@ -1032,3 +1045,108 @@ def decode_icp_result(result_cpu: torch.Tensor):
     T = result_cpu[:16].reshape(4, 4).numpy().copy()
     ints = result_cpu[18:20].numpy().view(np.int32)
     return T, float(result_cpu[16]), float(result_cpu[17]), int(ints[0]), int(ints[1]), bool(ints[2])
+
+
+# --------------------------------------------------------------------------- #
+# the Pose-stage training step (bx_train_step.cu): activations channel-blocked fp32 [n, C/4, S, 4]
+# --------------------------------------------------------------------------- #
+F64 = torch.float64
+
+
+def _splits():
+    return int(load_library().bx_ts_splits())
+
+
+def channel_sums(x, z=None, scale=None, shift=None):
+    """-> float64 [2, C] per channel of the blocked x [n, C/4, S, 4] (fp32 or float64): (sum x, sum x^2); with z, scale,
+    shift (float64 only) the BatchNorm backward sums (sum dz, sum dz x^), x^ = z scale + shift, dz = x where x^ > 0."""
+    n, G, S, _ = x.shape
+    C = 4 * G
+    partial = torch.empty(_splits() * 2 * C, dtype=F64, device=x.device)
+    out = torch.empty(2 * C, dtype=F64, device=x.device)
+    lib = load_library()
+    if x.dtype == F64:
+        _check(lib.bx_ts_channel_sums_f64(_dp(x, F64, "x"), _dp(z, F64, "z"), _dp(scale, F64, "scale"), _dp(shift, F64, "shift"), n, C, S,
+                                          _dp(partial), _dp(out), _stream()), "bx_ts_channel_sums_f64")
+    else:
+        assert z is None
+        _check(lib.bx_ts_channel_sums(_dp(x, F32, "x"), n, C, S, _dp(partial), _dp(out), _stream()), "bx_ts_channel_sums")
+    return out.view(2, C)
+
+
+def moments3(v):
+    """[..., 3] fp32 -> float64 [9]: sums of x, y, z, xx, xy, xz, yy, yz, zz."""
+    R = v.numel() // 3
+    partial = torch.empty(_splits() * 9, dtype=F64, device=v.device)
+    out = torch.empty(9, dtype=F64, device=v.device)
+    _check(load_library().bx_ts_moments3(_dp(v, F32, "v"), R, _dp(partial), _dp(out), _stream()), "bx_ts_moments3")
+    return out
+
+
+def bn_apply(z, scale, shift, relu, out=None):
+    """y = z scale + shift per channel (ReLU if relu) on a blocked image, fp32 or float64 (scale / shift of the same dtype)."""
+    n, G, S, _ = z.shape
+    y = torch.empty_like(z) if out is None else out
+    dt = z.dtype
+    fn = load_library().bx_ts_bn_apply_f64 if dt == F64 else load_library().bx_ts_bn_apply
+    _check(fn(_dp(z, dt, "z"), _dp(scale, dt, "scale"), _dp(shift, dt, "shift"), n, 4 * G, S, int(bool(relu)), _dp(y, dt, "y"), _stream()),
+           "bx_ts_bn_apply")
+    return y
+
+
+def bn_backward(dy, z, scale, shift, m1, m2, out=None):
+    """float64 batch-statistics BatchNorm backward through the ReLU (see bx_ts_bn_backward)."""
+    n, G, S, _ = z.shape
+    dx = torch.empty_like(z) if out is None else out
+    _check(load_library().bx_ts_bn_backward(_dp(dy, F64, "dy"), _dp(z, F64, "z"), _dp(scale, F64, "scale"), _dp(shift, F64, "shift"),
+                                            _dp(m1, F64, "m1"), _dp(m2, F64, "m2"), n, 4 * G, S, _dp(dx, F64, "dx"), _stream()), "bx_ts_bn_backward")
+    return dx
+
+
+def conv1x1(x, w, b):
+    """blocked x [n, Cin/4, S, 4], w [Cin, Cout4], b [Cout4] (Cout4 a multiple of 4, <= 16) -> blocked [n, Cout4/4, S, 4]."""
+    n, G, S, _ = x.shape
+    Cout4 = w.shape[1]
+    out = torch.empty((n, Cout4 // 4, S, 4), dtype=F32, device=x.device)
+    _check(load_library().bx_ts_conv1x1(_dp(x, F32, "x"), _dp(w, F32, "w"), _dp(b, F32, "b"), n, 4 * G, Cout4, S, _dp(out), _stream()),
+           "bx_ts_conv1x1")
+    return out
+
+
+def costvol(equi_s, equi_t):
+    """Full fp32 maps [M,32,7,20] (patch i against patch i) -> the blocked float64 cost volume [M, 8, 2000, 4] of rows 1..5."""
+    M = equi_s.shape[0]
+    cv = torch.empty((M, 8, 2000, 4), dtype=F64, device=equi_s.device)
+    _check(load_library().bx_ts_costvol(_dp(equi_s, F32, "equi_s"), _dp(equi_t, F32, "equi_t"), M, _dp(cv), _stream()), "bx_ts_costvol")
+    return cv
+
+
+def softargmax(logits, g=None):
+    """float64 logits [M, L] -> ind [M]; with g [M] (dL/d ind, float64) -> dL/dlogits [M, L]."""
+    M, L = logits.shape
+    ind = None if g is not None else torch.empty(M, dtype=F64, device=logits.device)
+    dl = torch.empty_like(logits) if g is not None else None
+    _check(load_library().bx_ts_softargmax(_dp(logits, F64, "logits"), M, L, _dp(g, F64, "g"), _dp(ind), _dp(dl), _stream()), "bx_ts_softargmax")
+    return dl if g is not None else ind
+
+
+def conv_forward(x, Wt, b, D, H, W, kd, kh, kw):
+    """float64 valid 3-D convolution: x [n, Cin/4, D*H*W, 4], Wt [T, Cin, Cout], b [Cout] -> [n, Cout/4, OD*OH*OW, 4]."""
+    n, Cin, Cout = x.shape[0], Wt.shape[1], Wt.shape[2]
+    out = torch.empty((n, Cout // 4, (D - kd + 1) * (H - kh + 1) * (W - kw + 1), 4), dtype=F64, device=x.device)
+    _check(load_library().bx_ts_conv_forward(_dp(x, F64, "x"), _dp(Wt, F64, "Wt"), _dp(b, F64, "b"), n, Cin, Cout, D, H, W, kd, kh, kw,
+                                             _dp(out), _stream()), "bx_ts_conv_forward")
+    return out
+
+
+def conv_backward(x, dy, Wt, D, H, W, kd, kh, kw, want_dx=True):
+    """float64 valid 3-D convolution backward: x [n, Cin/4, D*H*W, 4], dy [n, Cout/4, OD*OH*OW, 4], Wt [T, Cin, Cout] ->
+    (dx like x or None, dW [T, Cin, Cout])."""
+    n, Cin, Cout = x.shape[0], Wt.shape[1], Wt.shape[2]
+    T = kd * kh * kw
+    wpart = torch.empty(_splits() * T * Cin * Cout, dtype=F64, device=x.device)
+    dW = torch.empty((T, Cin, Cout), dtype=F64, device=x.device)
+    dx = torch.empty_like(x) if want_dx else None
+    _check(load_library().bx_ts_conv_backward(_dp(x, F64, "x"), _dp(dy, F64, "dy"), _dp(Wt, F64, "Wt"), n, Cin, Cout, D, H, W, kd, kh, kw,
+                                              _dp(dx), _dp(wpart), _dp(dW), _stream()), "bx_ts_conv_backward")
+    return dx, dW

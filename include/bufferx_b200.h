@@ -451,6 +451,47 @@ int bx_equi_match(const float *D1, const float *D2, int B, int C, int K, int L, 
 int bx_so2_gt(const float *s_rand_axis, const float *s_R, const float *t_R, const float *T, const float *aug_R, int P,
               int azi_n, long long *label_int, float *label_float, void *stream);
 
+/* ---- SURVEY 8(f) row 3: the Pose-stage training step (trainer.py:93-167 with cfg.stage "Pose", model.train()) -------
+ * Activations are channel-blocked [n][C/4][S][4]: fp32 for the frozen descriptor network, float64 for CostNet (forward and
+ * backward).  Every reduction over samples x positions writes BX_TS_SPLITS per-block partials (workspace `partial`) that
+ * one thread per output then adds in split order in float64: no atomics, bit-identical across runs.
+ * bx_ts_channel_sums(_f64): out [2C] float64.  Without z: sum x and sum x^2 per channel (the batch statistics of the
+ *   BatchNorm layers in training mode, models/patchnet.py:28,31 and patch_embedder.py:26-39).  With z, scale, shift [C]
+ *   (_f64 only): the sums of the BatchNorm backward, sum dz and sum dz x^, where x^ = z scale + shift and dz = x [x^ > 0]
+ *   (x = dL/dy of the ReLU).  partial [BX_TS_SPLITS * 2C] float64.
+ * bx_ts_moments3: the 3 first and 6 second moments (xx, xy, xz, yy, yz, zz) of R fp32 3-vectors, out9 float64, partial
+ *   [BX_TS_SPLITS * 9]: the batch statistics of the linear 3 -> 16 point layer follow from them (patch_embedder.py:26-30).
+ * bx_ts_bn_apply(_f64): y = z scale + shift per channel (ReLU if relu); y may alias z.
+ * bx_ts_bn_backward: float64 dx = (dz - m1 - x^ m2) scale with x^, dz as above and m1 = mean dz, m2 = mean dz x^
+ *   (affine = False: scale = 1/sqrt(var + eps)); dx may alias dy.
+ * bx_ts_conv1x1: out [n][Cout4/4][S][4] = b + w^T x for w [Cin][Cout4] (the pool layer's 1x1 convolutions,
+ *   patch_embedder.py:32-39); Cin <= 32, Cout4 <= 16.
+ * bx_ts_costvol: the cost volume of CostVolume.forward (models/BUFFERX.py:52-64) on elevation rows 1..5 of the fp32 maps
+ *   equi_s, equi_t [M,32,7,20]: cv float64 [M][8][20*5*20][4], cv[c][n][k][l] = s[c][k+1][(l-n) mod 20] - t[c][k+1][l].
+ * bx_ts_softargmax: float64 ind [M] = sum_k softmax(logits)_k k (BUFFERX.py:66-68); with g = dL/dind [M] instead
+ *   dlogits [M][L] = g p_k (k - ind).
+ * bx_ts_conv_forward / bx_ts_conv_backward: a valid 3-D convolution of CostNet (models/patchnet.py:192-210) and its
+ *   backward, float64 on CUDA cores, with input x [n][Cin/4][D*H*W][4], output [n][Cout/4][OD*OH*OW][4], weight w
+ *   [kd*kh*kw][Cin][Cout] and bias b [Cout]; the backward gives dw [T][Cin][Cout] (wpartial [BX_TS_SPLITS * T*Cin*Cout]
+ *   workspace) and, when dx is not NULL, dx shaped like x.  Cin % 32 == 0, Cout % 4 == 0. */
+#define BX_TS_SPLITS 64
+int bx_ts_splits(void);
+int bx_ts_channel_sums(const float *x, int n, int C, int S, double *partial, double *out, void *stream);
+int bx_ts_channel_sums_f64(const double *x, const double *z, const double *scale, const double *shift, int n, int C, int S,
+                           double *partial, double *out, void *stream);
+int bx_ts_moments3(const float *v3, long long R, double *partial, double *out9, void *stream);
+int bx_ts_bn_apply(const float *z, const float *scale, const float *shift, int n, int C, int S, int relu, float *y, void *stream);
+int bx_ts_bn_apply_f64(const double *z, const double *scale, const double *shift, int n, int C, int S, int relu, double *y, void *stream);
+int bx_ts_bn_backward(const double *dy, const double *z, const double *scale, const double *shift, const double *m1, const double *m2,
+                      int n, int C, int S, double *dx, void *stream);
+int bx_ts_conv1x1(const float *x, const float *w, const float *b, int n, int Cin, int Cout4, int S, float *out, void *stream);
+int bx_ts_costvol(const float *equi_s, const float *equi_t, int M, double *cv, void *stream);
+int bx_ts_softargmax(const double *logits, int M, int L, const double *g, double *ind, double *dlogits, void *stream);
+int bx_ts_conv_forward(const double *x, const double *w, const double *b, int n, int Cin, int Cout, int D, int H, int W, int kd, int kh,
+                       int kw, double *out, void *stream);
+int bx_ts_conv_backward(const double *x, const double *dy, const double *w, int n, int Cin, int Cout, int D, int H, int W, int kd, int kh,
+                        int kw, double *dx, double *wpartial, double *dw, void *stream);
+
 /* ---- loader-side ground truth: point-to-point ICP ---------------------------------------------------
  * Replaces open3d.pipelines.registration.registration_icp(source, target, r, init, TransformationEstimationPointToPoint(),
  * ICPConvergenceCriteria(...)) (Open3D 0.18), which the KITTI loader runs on the CPU to refine every pair's ground-truth
