@@ -34,6 +34,18 @@ def derotation_table(azi_n):
     return np.stack([np.cos(ang), np.sin(ang)], axis=1).astype(np.float32)
 
 
+def pnt_stats_from_moments(mo, Wp, bp):
+    """Batch mean and biased variance of the linear point layer y = Wp x + bp over R samples, from the float64 moments
+    mo [9] / R of its inputs (E[x], E[y], E[z], E[xx], E[xy], E[xz], E[yy], E[yz], E[zz], as ops.moments3 orders them):
+    mean = Wp E[x] + bp, var = diag(Wp Cov(x) Wp^T), Cov(x) = E[x x^T] - E[x] E[x]^T (clamped at 0)."""
+    Ex = mo[:3]
+    Exx = torch.stack([mo[[3, 4, 5]], mo[[4, 6, 7]], mo[[5, 7, 8]]])
+    cov = Exx - Ex[:, None] * Ex[None, :]
+    mean = Wp @ Ex + bp
+    var = torch.clamp(((Wp @ cov) * Wp).sum(dim=1), min=0.0)
+    return mean, var
+
+
 class MiniSpinNet(nn.Module):
     def __init__(self, config):
         super().__init__()
@@ -153,13 +165,8 @@ class MiniSpinNet(nn.Module):
         # point layer: batch statistics of the linear 3 -> 16 map from the moments of its inputs
         conv, bn = self.pnt_layer[0], self.pnt_layer[1]
         R_n = inv.numel() // 3
-        mo = ops.moments3(inv) / R_n
-        Ex = mo[:3]
-        Exx = torch.stack([mo[[3, 4, 5]], mo[[4, 6, 7]], mo[[5, 7, 8]]])
-        cov = Exx - Ex[:, None] * Ex[None, :]
-        Wp = conv.weight.detach().double().view(16, 3)
-        mean = Wp @ Ex + conv.bias.detach().double()
-        var = torch.clamp(((Wp @ cov) * Wp).sum(dim=1), min=0.0)
+        mean, var = pnt_stats_from_moments(ops.moments3(inv) / R_n, conv.weight.detach().double().view(16, 3),
+                                           conv.bias.detach().double())
         pn.bn_batch_stats(torch.stack([mean * R_n, (var + mean * mean) * R_n]), R_n, bn)
         if stats is not None:
             stats.append((mean, var))

@@ -1057,11 +1057,29 @@ def _splits():
     return int(load_library().bx_ts_splits())
 
 
+def _ts_shape(what, t, shape, name):
+    """Refuse a mis-shaped input of a bx_ts_* kernel before launch (they index by the sizes passed, not the tensor's)."""
+    if not isinstance(t, torch.Tensor) or tuple(t.shape) != tuple(shape):
+        got = tuple(t.shape) if isinstance(t, torch.Tensor) else type(t).__name__
+        raise BufferXError(f"{what}: {name} must be {list(shape)}, got {got}")
+
+
+def _ts_blocked(what, x, name="x"):
+    if not isinstance(x, torch.Tensor) or x.dim() != 4 or x.shape[3] != 4:
+        raise BufferXError(f"{what}: {name} must be a blocked image [n, C/4, S, 4], got "
+                           f"{tuple(x.shape) if isinstance(x, torch.Tensor) else type(x).__name__}")
+    return x.shape[0], x.shape[1], x.shape[2]
+
+
 def channel_sums(x, z=None, scale=None, shift=None):
     """-> float64 [2, C] per channel of the blocked x [n, C/4, S, 4] (fp32 or float64): (sum x, sum x^2); with z, scale,
     shift (float64 only) the BatchNorm backward sums (sum dz, sum dz x^), x^ = z scale + shift, dz = x where x^ > 0."""
-    n, G, S, _ = x.shape
+    n, G, S = _ts_blocked("channel_sums", x)
     C = 4 * G
+    if z is not None or scale is not None or shift is not None:
+        _ts_shape("channel_sums", z, x.shape, "z")
+        _ts_shape("channel_sums", scale, (C,), "scale")
+        _ts_shape("channel_sums", shift, (C,), "shift")
     partial = torch.empty(_splits() * 2 * C, dtype=F64, device=x.device)
     out = torch.empty(2 * C, dtype=F64, device=x.device)
     lib = load_library()
@@ -1069,13 +1087,17 @@ def channel_sums(x, z=None, scale=None, shift=None):
         _check(lib.bx_ts_channel_sums_f64(_dp(x, F64, "x"), _dp(z, F64, "z"), _dp(scale, F64, "scale"), _dp(shift, F64, "shift"), n, C, S,
                                           _dp(partial), _dp(out), _stream()), "bx_ts_channel_sums_f64")
     else:
-        assert z is None
+        if z is not None:
+            raise BufferXError("channel_sums: the BatchNorm backward sums (z, scale, shift given) take float64 x only")
         _check(lib.bx_ts_channel_sums(_dp(x, F32, "x"), n, C, S, _dp(partial), _dp(out), _stream()), "bx_ts_channel_sums")
     return out.view(2, C)
 
 
 def moments3(v):
     """[..., 3] fp32 -> float64 [9]: sums of x, y, z, xx, xy, xz, yy, yz, zz."""
+    if not isinstance(v, torch.Tensor) or v.dim() < 1 or v.shape[-1] != 3 or v.numel() == 0:
+        raise BufferXError(f"moments3: v must be [..., 3] with at least one vector, got "
+                           f"{tuple(v.shape) if isinstance(v, torch.Tensor) else type(v).__name__}")
     R = v.numel() // 3
     partial = torch.empty(_splits() * 9, dtype=F64, device=v.device)
     out = torch.empty(9, dtype=F64, device=v.device)
@@ -1085,7 +1107,11 @@ def moments3(v):
 
 def bn_apply(z, scale, shift, relu, out=None):
     """y = z scale + shift per channel (ReLU if relu) on a blocked image, fp32 or float64 (scale / shift of the same dtype)."""
-    n, G, S, _ = z.shape
+    n, G, S = _ts_blocked("bn_apply", z, "z")
+    _ts_shape("bn_apply", scale, (4 * G,), "scale")
+    _ts_shape("bn_apply", shift, (4 * G,), "shift")
+    if out is not None:
+        _ts_shape("bn_apply", out, z.shape, "out")
     y = torch.empty_like(z) if out is None else out
     dt = z.dtype
     fn = load_library().bx_ts_bn_apply_f64 if dt == F64 else load_library().bx_ts_bn_apply
@@ -1096,7 +1122,12 @@ def bn_apply(z, scale, shift, relu, out=None):
 
 def bn_backward(dy, z, scale, shift, m1, m2, out=None):
     """float64 batch-statistics BatchNorm backward through the ReLU (see bx_ts_bn_backward)."""
-    n, G, S, _ = z.shape
+    n, G, S = _ts_blocked("bn_backward", z, "z")
+    _ts_shape("bn_backward", dy, z.shape, "dy")
+    for name, t in (("scale", scale), ("shift", shift), ("m1", m1), ("m2", m2)):
+        _ts_shape("bn_backward", t, (4 * G,), name)
+    if out is not None:
+        _ts_shape("bn_backward", out, z.shape, "out")
     dx = torch.empty_like(z) if out is None else out
     _check(load_library().bx_ts_bn_backward(_dp(dy, F64, "dy"), _dp(z, F64, "z"), _dp(scale, F64, "scale"), _dp(shift, F64, "shift"),
                                             _dp(m1, F64, "m1"), _dp(m2, F64, "m2"), n, 4 * G, S, _dp(dx, F64, "dx"), _stream()), "bx_ts_bn_backward")
@@ -1105,8 +1136,11 @@ def bn_backward(dy, z, scale, shift, m1, m2, out=None):
 
 def conv1x1(x, w, b):
     """blocked x [n, Cin/4, S, 4], w [Cin, Cout4], b [Cout4] (Cout4 a multiple of 4, <= 16) -> blocked [n, Cout4/4, S, 4]."""
-    n, G, S, _ = x.shape
+    n, G, S = _ts_blocked("conv1x1", x)
+    if not isinstance(w, torch.Tensor) or w.dim() != 2 or w.shape[0] != 4 * G:
+        raise BufferXError(f"conv1x1: w must be [{4 * G}, Cout4], got {tuple(w.shape) if isinstance(w, torch.Tensor) else w}")
     Cout4 = w.shape[1]
+    _ts_shape("conv1x1", b, (Cout4,), "b")
     out = torch.empty((n, Cout4 // 4, S, 4), dtype=F32, device=x.device)
     _check(load_library().bx_ts_conv1x1(_dp(x, F32, "x"), _dp(w, F32, "w"), _dp(b, F32, "b"), n, 4 * G, Cout4, S, _dp(out), _stream()),
            "bx_ts_conv1x1")
@@ -1115,7 +1149,9 @@ def conv1x1(x, w, b):
 
 def costvol(equi_s, equi_t):
     """Full fp32 maps [M,32,7,20] (patch i against patch i) -> the blocked float64 cost volume [M, 8, 2000, 4] of rows 1..5."""
-    M = equi_s.shape[0]
+    M = equi_s.shape[0] if isinstance(equi_s, torch.Tensor) and equi_s.dim() == 4 else -1
+    _ts_shape("costvol", equi_s, (M, 32, 7, 20), "equi_s")
+    _ts_shape("costvol", equi_t, (M, 32, 7, 20), "equi_t")
     cv = torch.empty((M, 8, 2000, 4), dtype=F64, device=equi_s.device)
     _check(load_library().bx_ts_costvol(_dp(equi_s, F32, "equi_s"), _dp(equi_t, F32, "equi_t"), M, _dp(cv), _stream()), "bx_ts_costvol")
     return cv
@@ -1123,16 +1159,37 @@ def costvol(equi_s, equi_t):
 
 def softargmax(logits, g=None):
     """float64 logits [M, L] -> ind [M]; with g [M] (dL/d ind, float64) -> dL/dlogits [M, L]."""
+    if not isinstance(logits, torch.Tensor) or logits.dim() != 2:
+        raise BufferXError(f"softargmax: logits must be [M, L], got {tuple(logits.shape) if isinstance(logits, torch.Tensor) else logits}")
     M, L = logits.shape
+    if g is not None:
+        _ts_shape("softargmax", g, (M,), "g")
     ind = None if g is not None else torch.empty(M, dtype=F64, device=logits.device)
     dl = torch.empty_like(logits) if g is not None else None
     _check(load_library().bx_ts_softargmax(_dp(logits, F64, "logits"), M, L, _dp(g, F64, "g"), _dp(ind), _dp(dl), _stream()), "bx_ts_softargmax")
     return dl if g is not None else ind
 
 
+def _conv_shapes(what, x, Wt, D, H, W, kd, kh, kw):
+    """x [n, Cin/4, D*H*W, 4] and Wt [kd*kh*kw, Cin, Cout] of one valid 3-D convolution -> (n, Cin, Cout); the kernel
+    itself refuses Cin % 32, Cout % 4, a kernel larger than the extent and n = 0."""
+    n, G, S = _ts_blocked(what, x)
+    if not isinstance(Wt, torch.Tensor) or Wt.dim() != 3:
+        raise BufferXError(f"{what}: Wt must be [kd*kh*kw, Cin, Cout], got {tuple(Wt.shape) if isinstance(Wt, torch.Tensor) else Wt}")
+    _ts_shape(what, Wt, (kd * kh * kw, 4 * G, Wt.shape[2]), "Wt")
+    if S != D * H * W:
+        raise BufferXError(f"{what}: x holds {S} positions per channel, the geometry {D}x{H}x{W} has {D * H * W}")
+    if Wt.shape[2] % 4:
+        raise BufferXError(f"{what}: Cout = {Wt.shape[2]} is not a multiple of 4")
+    if not (1 <= kd <= D and 1 <= kh <= H and 1 <= kw <= W):
+        raise BufferXError(f"{what}: kernel {kd}x{kh}x{kw} does not fit the extent {D}x{H}x{W}")
+    return n, 4 * G, Wt.shape[2]
+
+
 def conv_forward(x, Wt, b, D, H, W, kd, kh, kw):
     """float64 valid 3-D convolution: x [n, Cin/4, D*H*W, 4], Wt [T, Cin, Cout], b [Cout] -> [n, Cout/4, OD*OH*OW, 4]."""
-    n, Cin, Cout = x.shape[0], Wt.shape[1], Wt.shape[2]
+    n, Cin, Cout = _conv_shapes("conv_forward", x, Wt, D, H, W, kd, kh, kw)
+    _ts_shape("conv_forward", b, (Cout,), "b")
     out = torch.empty((n, Cout // 4, (D - kd + 1) * (H - kh + 1) * (W - kw + 1), 4), dtype=F64, device=x.device)
     _check(load_library().bx_ts_conv_forward(_dp(x, F64, "x"), _dp(Wt, F64, "Wt"), _dp(b, F64, "b"), n, Cin, Cout, D, H, W, kd, kh, kw,
                                              _dp(out), _stream()), "bx_ts_conv_forward")
@@ -1142,7 +1199,8 @@ def conv_forward(x, Wt, b, D, H, W, kd, kh, kw):
 def conv_backward(x, dy, Wt, D, H, W, kd, kh, kw, want_dx=True):
     """float64 valid 3-D convolution backward: x [n, Cin/4, D*H*W, 4], dy [n, Cout/4, OD*OH*OW, 4], Wt [T, Cin, Cout] ->
     (dx like x or None, dW [T, Cin, Cout])."""
-    n, Cin, Cout = x.shape[0], Wt.shape[1], Wt.shape[2]
+    n, Cin, Cout = _conv_shapes("conv_backward", x, Wt, D, H, W, kd, kh, kw)
+    _ts_shape("conv_backward", dy, (n, Cout // 4, (D - kd + 1) * (H - kh + 1) * (W - kw + 1), 4), "dy")
     T = kd * kh * kw
     wpart = torch.empty(_splits() * T * Cin * Cout, dtype=F64, device=x.device)
     dW = torch.empty((T, Cin, Cout), dtype=F64, device=x.device)

@@ -8,12 +8,9 @@ import numpy as np
 import pytest
 import torch
 
-pytestmark = pytest.mark.gpu
+from oracle.train_step_cases import G_ELEM, G_NORM, POSE_BN
 
-ETA = 1e-4          # the forward's fp32-grade bound (a8 / a11): relative to a channel's magnitude sqrt(E[x^2])
-G_ELEM = 2e-5       # gradient error against the contraction on absolute values |dz|^T |x| (weights), sum |dz| (biases)
-G_NORM = 1e-4       # gradient error per tensor, relative to the float64 gradient's norm
-BN_CONVS = [0, 3, 6, 9, 12, 15, 18, 21, 24]
+pytestmark = pytest.mark.gpu
 
 
 @pytest.fixture(scope="module")
@@ -70,17 +67,6 @@ def _oracle(TP, sd, hp, cfg, data, seed):
     return r, keep, st
 
 
-def _stat_bound(mean, var):
-    """|batch mean error| and |batch variance error| allowed for a channel: the layer's values carry an error of at most
-    ETA sqrt(E[x^2]), so the mean moves by at most that and the variance by at most 2 ETA E[x^2] (+ ETA^2 E[x^2])."""
-    ex2 = var + mean * mean
-    return ETA * torch.sqrt(ex2) + 1e-12, (2 * ETA + ETA * ETA) * ex2 + 1e-12
-
-
-DESC_BN = ["Desc.pnt_layer.1"] + [f"Desc.conv_net.ops.{i}" for i in (1, 4, 7, 10, 13, 16, 19)] + ["Desc.pool_layer.1", "Desc.pool_layer.4"]
-POSE_BN = [f"Pose.conv.ops.{i + 1}" for i in BN_CONVS]
-
-
 def _spy_costnet(model):
     """Record the equivariant maps the training step feeds CostNet (cap["es"], cap["et"], full height, on the CPU)."""
     cap = {}
@@ -104,58 +90,30 @@ def _costnet_oracle(TP, sd, hp, cap, gt_ind):
 
 def _check_stats_and_running(model, sd0, r, sides):
     """Batch statistics and running buffers of the BatchNorms of ``sides`` ("src"/"tgt": Desc, "pose": Pose.conv) against
-    the float64 oracle result ``r``; num_batches_tracked moved by exactly one per call."""
+    the float64 oracle result ``r``; num_batches_tracked moved by exactly one per call.  Momentum comes from the model's
+    modules and N / (N - 1) from the batch's sample count (oracle/train_step_cases.py)."""
+    from oracle import train_step_cases as SC
+    from oracle.train_step import bn_hparams
     got = model.last_train_stats
+    hp = bn_hparams(model)
+    K = int(r["pred_ind"].shape[0])
     bounds = {}
     for side in sides:
-        keys = POSE_BN if side == "pose" else DESC_BN
-        assert len(got[side]) == len(r["stats"][side]) == len(keys)
-        for key, (gm, gv), (om, ov) in zip(keys, got[side], r["stats"][side]):
-            bm, bv = _stat_bound(om, ov)
-            em, ev = (gm.cpu() - om).abs(), (gv.cpu() - ov).abs()
-            assert (em <= bm).all(), f"{side} {key}: batch mean err {(em / bm).max()} x bound"
-            assert (ev <= bv).all(), f"{side} {key}: batch var err {(ev / bv).max()} x bound"
-            bounds.setdefault(key, []).append((bm, bv))
+        keys = SC.POSE_BN if side == "pose" else SC.DESC_BN
+        for key, b in zip(keys, SC.check_batch_stats(got[side], r["stats"][side], keys, side)):
+            bounds.setdefault(key, []).append(b)
     msd = model.state_dict()
     for key in bounds:
         calls = 2 if key.startswith("Desc") else 1
-        assert int(msd[key + ".num_batches_tracked"]) == int(sd0[key + ".num_batches_tracked"]) + calls, key
+        nbt0 = int(sd0[key + ".num_batches_tracked"])
+        assert int(msd[key + ".num_batches_tracked"]) == nbt0 + calls, key
         assert int(r["state"][key + ".num_batches_tracked"]) == int(msd[key + ".num_batches_tracked"]), key
-        m = 0.1
-        n_rel = 1.0 + 1e-3                       # n / (n - 1) for n >= 1000 samples
-        bm = sum(b[0] for b in bounds[key]) * m
-        bv = sum(b[1] for b in bounds[key]) * m * n_rel
-        for buf, b in (("running_mean", bm), ("running_var", bv)):
-            g, o = msd[key + "." + buf].cpu().double(), r["state"][key + "." + buf]
-            err = (g - o).abs()
-            lim = b + 2.0 ** -22 * o.abs()       # + the fp32 storage of the running buffers
-            assert (err <= lim).all(), f"{key}.{buf}: err {(err / lim).max()} x bound"
+        SC.check_running_buffers(msd, r["state"], key, bounds[key], hp[key][0], nbt0, SC.bn_count(key, K))
 
 
 def _check_grads(model, r, keep, TP, what):
-    absb = TP.grad_abs_bounds(keep, r["params"])
-    bad, ratios = [], {}
-    for i in [0, 3, 6, 9, 12, 15, 18, 21, 24, 27]:
-        for kind in ("weight", "bias"):
-            k = f"ops.{i}.{kind}"
-            p = getattr(model.Pose.conv.ops[i], kind)
-            assert p.grad is not None, k
-            g, g64 = p.grad.detach().cpu().double(), r["params"][k].grad
-            lim = G_ELEM * absb[k] + 1e-30
-            e = float(((g - g64).abs() / lim).max())
-            ratios[k] = e
-            if e > 1.0:
-                bad.append(f"{k}: elementwise err {e:.3g} x bound")
-            if kind == "bias" and i in BN_CONVS:
-                if not (g.abs() <= lim).all():
-                    bad.append(f"{k}: the analytically zero gradient is {float(g.abs().max()):.3g}")
-            else:
-                n = float((g - g64).norm()) / float(g64.norm())
-                ratios[k + "/norm"] = n / G_NORM
-                if n > G_NORM:
-                    bad.append(f"{k}: norm err {n:.3g}")
-    print(what, "gradient error / bound:", {k: round(v, 3) for k, v in ratios.items()})
-    assert not bad, f"{what}: " + "; ".join(bad)
+    from oracle import train_step_cases as SC
+    SC.check_grads(model.Pose.conv, r["params"], TP.grad_abs_bounds(keep, r["params"]), what)
 
 
 @pytest.mark.parametrize("name,aligned", [("C1", False), ("C1", True), ("C2", False), ("C2", True)])
