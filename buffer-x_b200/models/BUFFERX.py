@@ -8,7 +8,8 @@ Mirrors ``BufferX`` of /root/reference/models/BUFFERX.py (constructor :72-84, in
 scales_used)``.  Differences that do not change results:
   * FPS runs once per cloud for max(num_points_radius_estimate, num_fps) points -- the reference's
     per-scale calls return the same indices and FPS(k) is a prefix of FPS(k') (SURVEY 8.1 item 8);
-  * the radius histogram is built once and serves every scale's bisection, on the device;
+  * the radius histogram is built once and serves every scale's bisection, on the device (a larger cloud of more than
+    200000 points keeps the reference's per-scale sub-sample: one draw and one histogram per scale);
   * data-dependent sizes stay in device counters, so the whole pair is enqueued without a host round
     trip; the host reads one small result block at the end (early-exit mode in ``forward`` adds one read after scale 0;
     ``forward_async`` decides early exit on the device).
@@ -95,7 +96,8 @@ class _PairSlot:
     whose clouds fit the capacities: the true counts are copied to the device before each replay and the N-dependent
     kernels (FPS, radius histogram, permutation, patch gathering) stop at them, so the padding rows are never read.
     A large-class slot (``subsample`` True: a size-class slot whose larger capacity exceeds MAX_CLASS_POINTS) also holds the
-    reference's 200000-index radius sub-sample, drawn at launch from torch's CPU generator as eager ``forward`` draws it."""
+    reference's [S, 200000] radius sub-samples, one per scale, drawn at launch from torch's CPU generator in scale order as
+    eager ``forward`` draws them."""
 
     def __init__(self, model, Cs, Ct, aligned, use_graph, counted=False, subsample=False):
         cfg = model.config
@@ -116,8 +118,8 @@ class _PairSlot:
         self.counts = torch.tensor([Cs, Ct], dtype=torch.int32, device=dev) if counted else None
         self.h_counts = torch.empty(2, dtype=torch.int32).pin_memory() if counted else None
         # index 0 is valid in any cloud: the warm-up and the capture read it before the first launch draws
-        self.sub = torch.zeros(ops.RADIUS_SUBSAMPLE, dtype=torch.int32, device=dev) if subsample else None
-        self.h_sub = torch.empty(ops.RADIUS_SUBSAMPLE, dtype=torch.int32).pin_memory() if subsample else None
+        self.sub = torch.zeros((S, ops.RADIUS_SUBSAMPLE), dtype=torch.int32, device=dev) if subsample else None
+        self.h_sub = torch.empty((S, ops.RADIUS_SUBSAMPLE), dtype=torch.int32).pin_memory() if subsample else None
         self.h_tail = None
         self.done = torch.cuda.Event()
         self.graph = None
@@ -195,8 +197,10 @@ class _PairSlot:
                 self.h_counts[0], self.h_counts[1] = n_s, n_t
                 self.counts.copy_(self.h_counts, non_blocking=True)
             if self.sub is not None and max(n_s, n_t) > ops.RADIUS_SUBSAMPLE:
-                # eager forward's draw (reference BUFFERX.py:664-665) on the cloud it picks: the source iff n_s > n_t
-                self.h_sub.copy_(torch.randint(0, n_s if n_s > n_t else n_t, (ops.RADIUS_SUBSAMPLE,)))
+                # eager forward's draws (reference BUFFERX.py:664-665, one per scale) on the cloud it picks: the source iff
+                # n_s > n_t.  All S are drawn, also when the device then exits after scale 0 (the reference draws one)
+                for i in range(S):
+                    self.h_sub[i].copy_(torch.randint(0, n_s if n_s > n_t else n_t, (ops.RADIUS_SUBSAMPLE,)))
                 self.sub.copy_(self.h_sub, non_blocking=True)
             if self.graph is not None:
                 self.graph.replay()
@@ -301,8 +305,11 @@ class BufferX(nn.Module):
         than 200000 points keeps an exact-shape slot (the reference sub-samples such a cloud with a draw sized by N), unless
         ``large_classes=True``: such pairs then get size-class slots too (``ops.fps_large_size_class``: above 524288 points,
         capacities at most 1.25x the cloud, up to 1638400 points), and each launch draws the 200000-index sub-sample on the
-        host from torch's CPU generator and uploads it with the counts -- results byte-identical to eager ``forward`` with
-        the same ``perms`` and the same generator state, graphs on or off.
+        host from torch's CPU generator (one draw per scale, in scale order, as the reference draws them) and uploads them
+        with the counts -- results byte-identical to eager ``forward`` with the same ``perms`` and the same generator state,
+        graphs on or off.  With early exit the device decides after the launch, so a launch always makes all S draws: after
+        a pair that exits at scale 0 the generator is S - 1 draws ahead of the reference's (as the NumPy permutations are,
+        see ``_graphable``); the scales that run use the reference's draws.
         ``slots_per_shape`` slots (pairs in flight) are kept per key.  These options also apply to ``forward_async``
         without graphs."""
         if large_classes and not size_classes:
@@ -324,7 +331,9 @@ class BufferX(nn.Module):
     def _graphable(self):
         """Whether ``forward`` may route through the slots.  Early exit stays on the host decision in ``forward``: only that
         reproduces the reference's NumPy draw order (scales 1..S-1 draw their permutations only when the pair does not exit),
-        the drop-in contract of ``forward``.  ``forward_async`` draws all 2*S permutations at launch and decides on the device."""
+        the drop-in contract of ``forward``; likewise torch's CPU generator, which ``forward`` rewinds to after scale 0's radius
+        sub-sample when a pair above 200000 points exits.  ``forward_async`` draws all 2*S permutations (and S sub-samples) at
+        launch and decides on the device."""
         cfg = self.config
         return not cfg.match.get("enable_early_exit", True) and not cfg.test.get("enable_timing", False)
 
@@ -414,9 +423,9 @@ class BufferX(nn.Module):
         """Everything of one pair on the current stream, no host synchronisation unless early exit is on and the decision is
         the host's (``device_exit`` False: ``forward``).  Returns (tail block on the device, debug dict).
         ``counts`` (size-class slots): [2] int32 CUDA point counts; src / tgt are then capacity buffers whose first counts
-        rows are the clouds, and ``perms`` rows likewise.  ``sub`` (large-class slots, with ``counts``): [200000] int32 CUDA
-        radius sub-sample, read when the larger cloud has more than 200000 points; without it the counted clouds have at most
-        MAX_CLASS_POINTS points.  ``xyz``: src and tgt back to back, when the caller holds them so (saves the concatenation
+        rows are the clouds, and ``perms`` rows likewise.  ``sub`` (large-class slots, with ``counts``): [S, 200000] int32 CUDA
+        radius sub-samples, row i read by scale i when the larger cloud has more than 200000 points; without it the counted
+        clouds have at most MAX_CLASS_POINTS points.  ``xyz``: src and tgt back to back, when the caller holds them so (saves the concatenation
         before FPS)."""
         cfg = self.config
         dev = src.device
@@ -447,21 +456,28 @@ class BufferX(nn.Module):
             fk = torch.stack([k.reshape(nfps, 3) for _, k in per])
         kpts1, kpts2 = fk[0, :Kr].contiguous(), fk[1, :Kr].contiguous()
         src_kpts, tgt_kpts = fk[0, :K].contiguous(), fk[1, :K].contiguous()
-        # ---- density-aware radii of every scale from one histogram ------------------------------------
+        # ---- density-aware radii of every scale: one histogram, or one per scale for a cloud above 200000 points ------
+        rng_after_first = None      # torch's CPU generator after scale 0's draw: where the reference leaves it on an exit
         if counts is not None:      # the device picks the larger cloud from the counts (and sub-samples it through ``sub``)
             r_dev, m_dev, _ = ops.radius_estimate_pair(kpts1, src, kpts2, tgt, thresholds, counts, d_sub=sub)
         else:
             pts_r, kpts_r = (src, kpts1) if Ns > Nt else (tgt, kpts2)
-            denom = pts_r.shape[0] * Kr
-            if pts_r.shape[0] > 200000:  # reference BUFFERX.py:664-665 (denominator keeps the original size)
-                # eager: the reference's draw from the CPU generator (same indices under torch.manual_seed); under CUDA-graph
-                # capture a host draw would be frozen into the graph, so the capture draws on the device (DESIGN.md section 2)
-                if torch.cuda.is_current_stream_capturing():
-                    sub = torch.randint(0, pts_r.shape[0], (200000,), device=dev)
-                else:
-                    sub = torch.randint(0, pts_r.shape[0], (200000,)).to(dev, non_blocking=True)
-                pts_r = pts_r[sub].contiguous()
-            r_dev, m_dev, _ = ops.radius_estimate(kpts_r, pts_r, thresholds, denom=denom)
+            N = pts_r.shape[0]
+            if N > ops.RADIUS_SUBSAMPLE:
+                # reference BUFFERX.py:320-329 + 664-665: each scale estimates its radius on its own 200000-index draw,
+                # the denominator keeping N.  Eager: the reference's draws from the CPU generator in scale order (the same
+                # indices under torch.manual_seed); under CUDA-graph capture a host draw would be frozen into the graph, so
+                # the capture draws on the device (DESIGN.md section 2)
+                on_dev = {"device": dev} if torch.cuda.is_current_stream_capturing() else {}
+                subs = []
+                for i in range(S):
+                    subs.append(torch.randint(0, N, (ops.RADIUS_SUBSAMPLE,), **on_dev).to(dev, non_blocking=True))
+                    if i == 0 and not on_dev:
+                        rng_after_first = torch.get_rng_state()
+                est = [ops.radius_estimate(kpts_r, pts_r[subs[i]].contiguous(), thresholds[i:i + 1], denom=N * Kr) for i in range(S)]
+                r_dev, m_dev = torch.cat([e[0] for e in est]), torch.cat([e[1] for e in est])
+            else:
+                r_dev, m_dev, _ = ops.radius_estimate(kpts_r, pts_r, thresholds, denom=N * Kr)
         desc_t.toc()
 
         maxMc = S * K
@@ -555,6 +571,8 @@ class BufferX(nn.Module):
                 opt_t.toc()
                 should_exit = self.pose_estimator.compute_confidence_score(num_inliers)
                 if should_exit:
+                    if rng_after_first is not None:     # the reference made only scale 0's sub-sample draw
+                        torch.set_rng_state(rng_after_first)
                     break
 
         opt_t.tic()
@@ -796,7 +814,7 @@ class BufferX(nn.Module):
         dev = next(self.parameters()).device
         if dev.type != "cuda":
             raise ops.BufferXError("BufferX.forward needs the model on a CUDA device: there is no CPU path")
-        self._cloud_sizes(data_source)
+        sizes = self._cloud_sizes(data_source)
         if self._use_graphs and not debug and ransac_seed is None and self._graphable():
             return self.forward_async(data_source, perms).result()
 
@@ -807,6 +825,8 @@ class BufferX(nn.Module):
         aligned = bool(data_source["is_aligned_to_global_z"])
         enable_timing = cfg.test.get("enable_timing", False)
         rng_state = np.random.get_state() if perms is None else None     # replayed if the pair has to be recomputed
+        # ... and torch's CPU generator, when the pair draws its radius sub-samples from it
+        torch_rng = torch.get_rng_state() if max(sizes) > ops.RADIUS_SUBSAMPLE else None
         with torch.cuda.device(dev):        # kernels launch on the model's device, whatever the caller's current device
             src, tgt = _cloud(data_source["src_fds_pcd"]), _cloud(data_source["tgt_fds_pcd"])
             timers = (_Timer(enable_timing), _Timer(enable_timing), _Timer(enable_timing))
@@ -817,6 +837,8 @@ class BufferX(nn.Module):
         if self._overflow:
             if rng_state is not None:
                 np.random.set_state(rng_state)
+            if torch_rng is not None:
+                torch.set_rng_state(torch_rng)
             return self._rerun_tf32(data_source, perms, ransac_seed, debug)
         if debug:
             dbg.update(self._last_ransac)

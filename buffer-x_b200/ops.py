@@ -315,17 +315,24 @@ RADIUS_SUBSAMPLE = 200000       # the reference's sub-sample of a larger cloud (
 def radius_estimate_pair(kpts_s, pts_s, kpts_t, pts_t, thresholds, d_counts, tolerance=0.01, hist=None, d_sub=None):
     """Both clouds (capacity buffers) and their [Kr,3] key-points, d_counts [2] int32 CUDA = (ns, nt): the device picks the
     larger cloud (source iff ns > nt) and denom = N * Kr.  Returns (r, m, hist) like radius_estimate.
-    d_sub: optional [RADIUS_SUBSAMPLE] int32 CUDA indices (bx_radius_estimate_n_sub): when the chosen cloud has more than
-    RADIUS_SUBSAMPLE points, the histogram runs over its points d_sub, as radius_estimate(kpts, pts[d_sub], denom=N * Kr)."""
+    d_sub: optional int32 CUDA indices into the chosen cloud, read when it has more than RADIUS_SUBSAMPLE points
+    (bx_radius_estimate_n_sub):
+      [RADIUS_SUBSAMPLE]: one histogram over pts[d_sub] serves every threshold, as
+        radius_estimate(kpts, pts[d_sub], thresholds, denom=N * Kr);
+      [len(thresholds), RADIUS_SUBSAMPLE]: one row per threshold (the reference draws one sub-sample per scale): threshold i
+        has its own histogram (hist [len(thresholds), RADIUS_BINS + 2]) over pts[d_sub[i]], as
+        radius_estimate(kpts, pts[d_sub[i]], thresholds[i:i + 1], denom=N * Kr), one launch per threshold."""
     lib = load_library()
     th = np.ascontiguousarray(thresholds, dtype=np.float64)
     Kr = kpts_s.shape[0]
     assert kpts_t.shape[0] == Kr
-    if d_sub is not None and tuple(d_sub.shape) != (RADIUS_SUBSAMPLE,):
-        raise BufferXError(f"radius_estimate_pair: d_sub must be [{RADIUS_SUBSAMPLE}], got {tuple(d_sub.shape)}")
+    per_threshold = d_sub is not None and d_sub.dim() == 2
+    if d_sub is not None and tuple(d_sub.shape) not in ((RADIUS_SUBSAMPLE,), (len(th), RADIUS_SUBSAMPLE)):
+        raise BufferXError(f"radius_estimate_pair: d_sub must be [{RADIUS_SUBSAMPLE}] or [{len(th)}, {RADIUS_SUBSAMPLE}], "
+                           f"got {tuple(d_sub.shape)}")
     dev = pts_s.device
     if hist is None:
-        hist = torch.empty(RADIUS_BINS + 2, dtype=I32, device=dev)
+        hist = torch.empty((len(th), RADIUS_BINS + 2) if per_threshold else (RADIUS_BINS + 2,), dtype=I32, device=dev)
     out_r = torch.empty(len(th), dtype=F32, device=dev)
     out_m = torch.empty(len(th), dtype=I32, device=dev)
     if d_sub is None:
@@ -333,11 +340,18 @@ def radius_estimate_pair(kpts_s, pts_s, kpts_t, pts_t, thresholds, d_counts, tol
                                         _dp(pts_t, F32, "pts_t"), pts_t.shape[0], Kr, _dp(d_counts, I32, "d_counts"), th.ctypes.data_as(c_void_p),
                                         len(th), float(tolerance), _dp(radius_round_table(dev)), _dp(hist), _dp(out_r), _dp(out_m), _stream()),
                "bx_radius_estimate_n")
-    else:
+        return out_r, out_m, hist
+    if not per_threshold:
         _check(lib.bx_radius_estimate_n_sub(_dp(kpts_s, F32, "kpts_s"), _dp(pts_s, F32, "pts_s"), pts_s.shape[0], _dp(kpts_t, F32, "kpts_t"),
                                             _dp(pts_t, F32, "pts_t"), pts_t.shape[0], Kr, _dp(d_counts, I32, "d_counts"), _dp(d_sub, I32, "d_sub"),
                                             th.ctypes.data_as(c_void_p), len(th), float(tolerance), _dp(radius_round_table(dev)), _dp(hist),
                                             _dp(out_r), _dp(out_m), _stream()), "bx_radius_estimate_n_sub")
+        return out_r, out_m, hist
+    for i in range(len(th)):
+        _check(lib.bx_radius_estimate_n_sub(_dp(kpts_s, F32, "kpts_s"), _dp(pts_s, F32, "pts_s"), pts_s.shape[0], _dp(kpts_t, F32, "kpts_t"),
+                                            _dp(pts_t, F32, "pts_t"), pts_t.shape[0], Kr, _dp(d_counts, I32, "d_counts"), _dp(d_sub[i], I32, "d_sub"),
+                                            th[i:i + 1].ctypes.data_as(c_void_p), 1, float(tolerance), _dp(radius_round_table(dev)), _dp(hist[i]),
+                                            _dp(out_r[i:i + 1]), _dp(out_m[i:i + 1]), _stream()), "bx_radius_estimate_n_sub")
     return out_r, out_m, hist
 
 

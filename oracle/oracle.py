@@ -250,7 +250,9 @@ def radius_hist(kpts, pts) -> np.ndarray:
 def radius_estimation(src_pts, src_kpts, tgt_pts, tgt_kpts, thresholds, tolerance=0.01, cum=None, sub_idx=None):
     """``density_aware_radius_estimation`` (models/BUFFERX.py:627-696): the larger cloud wins
     (strict >, else target); returns the list of 2-decimal radii.  Above 200000 points the reference histograms
-    ``pts[sub_idx]`` (its ``torch.randint`` draw, passed in here) and keeps the original size in the denominator."""
+    ``pts[sub_idx]`` and keeps the original size in the denominator; without ``sub_idx`` this call makes the reference's
+    draw itself, ``torch.randint(0, N, (200000,))`` from torch's CPU generator (the reference calls this function once per
+    scale, so each scale draws its own sub-sample)."""
     if src_pts.shape[0] > tgt_pts.shape[0]:
         pts, kpts = src_pts, src_kpts
     else:
@@ -258,7 +260,7 @@ def radius_estimation(src_pts, src_kpts, tgt_pts, tgt_kpts, thresholds, toleranc
     denom = int(pts.shape[0]) * int(kpts.shape[0])
     if pts.shape[0] > 200000:
         if sub_idx is None:
-            raise NotImplementedError("random 200k sub-sampling (BUFFERX.py:664-665) needs explicit indices")
+            sub_idx = torch.randint(0, pts.shape[0], (200000,)).numpy()
         pts = np.asarray(pts)[np.asarray(sub_idx)]
     if cum is None:
         cum = radius_hist(kpts, pts)
@@ -1014,10 +1016,18 @@ def draw_perms(cfg, n_src, n_tgt, seed):
     return perms
 
 
-def register_pair(sd, cfg, data, perms, ransac_seed=0, keep=False, timings=None, z_axes=None):
+def should_exit(cfg, num_inliers):
+    """``PoseEstimator.compute_confidence_score`` (pose_estimator.py:119-126)."""
+    return num_inliers >= cfg.match.get("early_exit_min_inliers", 15)
+
+
+def register_pair(sd, cfg, data, perms, ransac_seed=0, keep=False, timings=None, z_axes=None, sub_idx=None):
     """``BufferX.forward`` inference branch (models/BUFFERX.py:257-467), early exit disabled or enabled
     as configured.  Returns (pose, num_inliers, num_mutual, num_inlier_ind, scales_used, aux).
-    ``z_axes`` (ref_check.py only): per scale a (src [K,3], tgt [K,3]) pair of LRF z axes to impose."""
+    ``z_axes`` (ref_check.py only): per scale a (src [K,3], tgt [K,3]) pair of LRF z axes to impose.
+    A larger cloud of more than 200000 points is sub-sampled once per scale that runs, as the reference does
+    (BUFFERX.py:320-329 calls the radius estimation inside the scale loop): scale i histograms ``sub_idx[i]``, or without
+    ``sub_idx`` its own draw from torch's CPU generator, made in scale order (one draw after an early exit at scale 0)."""
     src = _f32(data["src_fds_pcd"])
     tgt = _f32(data["tgt_fds_pcd"])
     aligned = bool(data["is_aligned_to_global_z"])
@@ -1040,19 +1050,24 @@ def register_pair(sd, cfg, data, perms, ransac_seed=0, keep=False, timings=None,
     src_kpts, tgt_kpts = src[s_idx], tgt[t_idx]
 
     t0 = time.perf_counter()
-    if src.shape[0] > tgt.shape[0]:
-        cum = radius_hist(kpts1, src)
-    else:
-        cum = radius_hist(kpts2, tgt)
+    cum = None                      # up to 200000 points one histogram serves every scale
+    if max(src.shape[0], tgt.shape[0]) <= 200000:
+        cum = radius_hist(kpts1, src) if src.shape[0] > tgt.shape[0] else radius_hist(kpts2, tgt)
     _t("radius_estimation", t0)
 
     enable_early_exit = cfg.match.get("enable_early_exit", True)
-    aux = dict(des_r=[], scales=[], s_fps=s_idx_r, t_fps=t_idx_r)
+    aux = dict(des_r=[], scales=[], s_fps=s_idx_r, t_fps=t_idx_r, ransac_calls=[])
     R_acc, t_acc, ss_acc, tt_acc = [], [], [], []
-    init_pose, num_inliers, scales_used, should_exit = None, 0, 0, False
+    init_pose, num_inliers, scales_used, exit_now = None, 0, 0, False
     inlier_ind = np.zeros(0, dtype=np.int32)
     for i in range(cfg.patch.num_scales):
-        des_r = radius_estimation(src, kpts1, tgt, kpts2, [cfg.patch.search_radius_thresholds[i]], cum=cum)[0]
+        t0 = time.perf_counter()
+        th = [cfg.patch.search_radius_thresholds[i]]
+        if sub_idx is None:
+            des_r = radius_estimation(src, kpts1, tgt, kpts2, th, cum=cum)[0]
+        else:
+            des_r = radius_estimation(src, kpts1, tgt, kpts2, th, cum=cum, sub_idx=sub_idx[i])[0]
+        _t("radius_estimation", t0)
         aux["des_r"].append(des_r)
         zs, zt = (None, None) if z_axes is None else z_axes[i]
         s = describe(sd, cfg, src, src_kpts, des_r, aligned, perms[i][0], keep=keep, timings=tm, z_axis=zs)
@@ -1083,16 +1098,18 @@ def register_pair(sd, cfg, data, perms, ransac_seed=0, keep=False, timings=None,
             r = ransac(ss_cat.numpy(), tt_cat.numpy(), inlier_ind, cfg.match.dist_th, cfg.match.similar_th,
                        cfg.match.confidence, cfg.match.iter_n, ransac_seed)
             _t("ransac", t0)
+            aux["ransac_calls"].append(dict(inlier_ind=inlier_ind.copy(), **r))
             init_pose, num_inliers = r["T"], r["num_inliers"]
-            should_exit = num_inliers >= cfg.match.get("early_exit_min_inliers", 15)
-            if should_exit:
+            exit_now = should_exit(cfg, num_inliers)
+            if exit_now:
                 break
     num_mutual = int(ss_cat.shape[0])
-    if (not enable_early_exit) or (enable_early_exit and not should_exit):
+    if (not enable_early_exit) or (enable_early_exit and not exit_now):
         t0 = time.perf_counter()
         r = ransac(ss_cat.numpy(), tt_cat.numpy(), inlier_ind, cfg.match.dist_th, cfg.match.similar_th,
                    cfg.match.confidence, cfg.match.iter_n, ransac_seed)
         _t("ransac", t0)
+        aux["ransac_calls"].append(dict(inlier_ind=inlier_ind.copy(), **r))
         init_pose, num_inliers = r["T"], r["num_inliers"]
         aux["ransac"] = r
     aux["init_pose"] = init_pose

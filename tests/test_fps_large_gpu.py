@@ -5,10 +5,10 @@ ops.fps_large must equal the C oracle bit for bit (indices, and key points = xyz
 must also equal ops.fps.  Whole pairs with one or both clouds above 524288 points go through BufferX.forward against the
 oracle pair, and through captured slots, exact-shape and size-class, against eager forward.
 
-Both clouds of such a pair exceed 200000 points, so the radius estimation histograms 200000 indices the reference draws
-with torch.randint (BUFFERX.py:664-665).  The tests pin that draw to one fixed set per cloud size -- in eager forward, in
-the captures (which otherwise draw on the device, DESIGN.md section 2) and in the oracle -- so that every route sees the
-same sub-sample and results can be compared byte for byte."""
+Both clouds of such a pair exceed 200000 points, so each scale's radius estimation histograms 200000 indices the reference
+draws with torch.randint (BUFFERX.py:664-665), one draw per scale.  The tests pin those draws to fixed sets per cloud size,
+a distinct one per scale -- in eager forward, in the captures (which otherwise draw on the device, DESIGN.md section 2) and
+in the oracle -- so that every route sees the same sub-samples and results can be compared byte for byte."""
 import functools
 import os
 import sys
@@ -98,35 +98,35 @@ def _cfg():
 
 
 _SUBS = {}
+SCALES = 3      # the C3 configuration's scales: a pair draws one sub-sample per scale
 
 
-def _sub(n, device="cpu"):
-    """The fixed 200000-index sub-sample of an n-point cloud (device copies are made outside any capture and kept)."""
-    key = (n, str(torch.device(device)))
+def _sub(n, k=0, device="cpu"):
+    """The k-th fixed 200000-index sub-sample of an n-point cloud, k < SCALES, all distinct (so that scales sharing one
+    draw would be seen); device copies are made outside any capture and kept."""
+    key = (n, k, str(torch.device(device)))
     if key not in _SUBS:
         assert torch.device(device).type == "cpu" or not torch.cuda.is_current_stream_capturing()
-        _SUBS[key] = torch.from_numpy(np.random.default_rng(n).integers(0, n, 200000)).to(device)
+        _SUBS[key] = torch.from_numpy(np.random.default_rng([n, k]).integers(0, n, 200000)).to(device)
     return _SUBS[key]
 
 
 @pytest.fixture
-def pinned_draw(monkeypatch, oracle):
+def pinned_draw(monkeypatch):
+    """torch.randint(0, n, (200000,)) returns the pinned draws of an n-point cloud in turn (0, 1, .., SCALES - 1, 0, ..),
+    so every pair -- eager forward, a capture, a slot launch, the oracle's per-scale draws -- takes draw i at scale i."""
     randint = torch.randint
+    turn = {}
 
     def fixed(*a, **kw):
         if len(a) >= 3 and a[0] == 0 and tuple(a[2]) == (200000,):
-            return _sub(int(a[1]), kw.get("device", "cpu"))
+            n, device = int(a[1]), kw.get("device", "cpu")
+            k = turn.get(n, 0)
+            turn[n] = (k + 1) % SCALES
+            return _sub(n, k, device)
         return randint(*a, **kw)
 
     monkeypatch.setattr(torch, "randint", fixed)
-    hist, est = oracle.radius_hist, oracle.radius_estimation
-    monkeypatch.setattr(oracle, "radius_hist", lambda kp, pts: hist(kp, pts[_sub(len(pts)).numpy()] if len(pts) > 200000 else pts))
-
-    def est_sub(src, skp, tgt, tkp, *a, **kw):
-        n = len(src) if len(src) > len(tgt) else len(tgt)      # the reference's cloud choice (BUFFERX.py:654)
-        return est(src, skp, tgt, tkp, *a, sub_idx=_sub(n).numpy(), **kw)
-
-    monkeypatch.setattr(oracle, "radius_estimation", est_sub)
 
 
 PAIRS = [(700000, 600000), (560000, 300000)]
@@ -183,7 +183,8 @@ def test_large_pairs_on_captured_slots(dev, oracle, pinned_draw, size_classes):
     model = model.to(dev).eval()
     items = [(_pair(ns, nt), oracle.draw_perms(model.config, ns, nt, 1)) for ns, nt in PAIRS]
     for ns, nt in PAIRS:
-        _sub(max(ns, nt), dev)          # the device copy the captures index with, made before any capture
+        for k in range(SCALES):
+            _sub(max(ns, nt), k, dev)   # the device copies the captures index with, made before any capture
     with torch.no_grad():
         eager = [model(d, perms=p) for d, p in items]
         model.enable_cuda_graphs(True, slots_per_shape=1, size_classes=size_classes)

@@ -154,14 +154,28 @@ def test_radius_estimate_pair_counts(dev, ns, nt):
     report(f"radius pair ns={ns} nt={nt}", out)
 
 
-def test_radius_subsampled_route_of_the_model(dev, monkeypatch):
-    """BufferX.forward on a pair whose larger cloud has 250000 points: the 200000 indices are drawn from the CPU
-    generator as the reference's torch.randint(0, N, (200000,)) (same indices under torch.manual_seed), the histogram is
-    built on pts[indices] and the denominator keeps N."""
+def test_radius_subsampled_route_draws_once_per_scale(dev, monkeypatch):
+    """BufferX.forward on a pair whose larger cloud has 250000 points: as the reference (BUFFERX.py:320-329, 664-665), each
+    scale draws its own 200000 indices from the CPU generator, torch.randint(0, N, (200000,)) in scale order (the same
+    indices under torch.manual_seed), builds its histogram on pts[indices] with the denominator keeping N, and takes its
+    radius with its own threshold."""
+    _subsampled_route(dev, monkeypatch, early_exit=False)
+
+
+def test_radius_subsampled_route_after_an_early_exit(dev, monkeypatch):
+    """The same with early exit on and every pair exiting after scale 0: forward draws the S sub-samples, and leaves
+    torch's generator after one draw, where the reference leaves it."""
+    _subsampled_route(dev, monkeypatch, early_exit=True)
+
+
+def _subsampled_route(dev, monkeypatch, early_exit):
     import bufferx_b200 as bx
     from bufferx_b200 import ops
     from bufferx_b200.synth import init_synthetic_weights, make_pair, workload_cfg
     cfg = workload_cfg("C3")
+    cfg.match.enable_early_exit = early_exit
+    cfg.match.early_exit_min_inliers = 0          # with early exit on, every pair exits after scale 0
+    S, ths_all = cfg.patch.num_scales, list(cfg.patch.search_radius_thresholds)
     model = init_synthetic_weights(bx.BufferX(cfg)).to(dev).eval()
     data = make_pair("C3", 0, n_src=250000, n_tgt=30000)
     draws, calls = [], []
@@ -181,19 +195,26 @@ def test_radius_subsampled_route_of_the_model(dev, monkeypatch):
     monkeypatch.setattr(ops, "radius_estimate", rec_est)
     torch.manual_seed(1234)
     with torch.no_grad():
-        model(data)
+        _, _, _, _, _, su = model(data)
+    after = torch.get_rng_state()
     monkeypatch.undo()
+    assert su == (1 if early_exit else S)
     torch.manual_seed(1234)
-    want = torch.randint(0, 250000, (200000,))
+    want = [torch.randint(0, 250000, (200000,)) for _ in range(S)]
     sub = [t for a, kw, t in draws if len(a) >= 3 and a[0] == 0 and tuple(a[2]) == (200000,)]
-    assert len(sub) == 1 and sub[0].device.type == "cpu" and torch.equal(sub[0], want), "not the reference's CPU draw"
-    assert len(calls) == 1
-    kp, pts, ths, denom, (r, m, hist) = calls[0]
+    assert len(sub) == S and all(t.device.type == "cpu" and torch.equal(t, w) for t, w in zip(sub, want)), "not the reference's CPU draws"
+    torch.manual_seed(1234)
+    for _ in range(su):
+        torch.randint(0, 250000, (200000,))
+    assert torch.equal(after, torch.get_rng_state()), "the generator is not where the reference leaves it"
+    assert len(calls) == S
     src = cu(np.ascontiguousarray(data["src_fds_pcd"], np.float32), dev)
-    assert denom == 250000 * kp.shape[0] and torch.equal(pts, src[want.to(dev)])
-    lo, hi = F.O.radius_count_bounds(kp, pts)
-    report("radius model route, 250000 points", F.check_radius(hist[:8193].cpu().numpy(), denom, ths, 0.01, m.cpu().numpy(),
-                                                               r.cpu().numpy(), lo, hi))
+    for i, (kp, pts, ths, denom, (r, m, hist)) in enumerate(calls):
+        assert ths == [ths_all[i]], f"scale {i} bisects with {ths}"
+        assert denom == 250000 * kp.shape[0] and torch.equal(pts, src[want[i].to(dev)]), f"scale {i} is not on draw {i}"
+        lo, hi = F.O.radius_count_bounds(kp, pts)
+        report(f"radius model route, 250000 points, scale {i}", F.check_radius(hist[:8193].cpu().numpy(), denom, ths, 0.01,
+                                                                             m.cpu().numpy(), r.cpu().numpy(), lo, hi))
 
 
 def test_radius_subsampled_route_under_capture(dev, monkeypatch):

@@ -4,10 +4,11 @@ large_classes=True)) and the two device forms they run on.
   * ops.fps_large with a device count (bx_fps_large_n) on a capacity buffer whose padding rows would win if they were read:
     the indices and key-points of ops.fps_large on the exact cloud, also when one captured launch is replayed with two counts.
   * ops.radius_estimate_pair with the 200000-index sub-sample (bx_radius_estimate_n_sub): the histogram, radii and m of
-    ops.radius_estimate on the gathered larger cloud with denom = N * Kr.
+    ops.radius_estimate on the gathered larger cloud with denom = N * Kr; with one sub-sample per scale ([S, 200000], one
+    launch per scale) each scale's histogram, radius and m on its own gathered cloud.
   * Whole pairs through large-class slots: with the same perms and the same torch.manual_seed, the bytes of eager forward.
-    The sub-sample is the reference's own torch.randint draw on the CPU generator, made by eager forward and by each slot
-    launch alike; nothing is pinned here."""
+    The sub-samples are the reference's own torch.randint draws on the CPU generator, one per scale, made by eager
+    forward and by each slot launch alike; nothing is pinned here."""
 import functools
 
 import numpy as np
@@ -122,6 +123,44 @@ def test_radius_sub_sampled_pair_form(dev, counts, caps):
     assert torch.equal(hist, hist_e)
     assert torch.equal(m, m_e) and torch.equal(r.view(torch.int32), r_e.view(torch.int32))
     assert int(hist_e[-2]) > 0
+
+
+@pytest.mark.parametrize("counts,caps", RADIUS_CASES)
+def test_radius_sub_sampled_pair_form_per_scale(dev, counts, caps):
+    """d_sub [S, 200000], one sub-sample per scale: scale i's histogram, radius and m are those of ops.radius_estimate on
+    its own gathered cloud with its own threshold (the padding rows of both buffers would count if read)."""
+    from bufferx_b200 import ops
+    from bufferx_b200.synth import workload_cfg
+    thresholds = workload_cfg("C3").patch.search_radius_thresholds
+    S = len(thresholds)
+    Kr = 2000
+    (ns, nt), (cs, ct) = counts, caps
+    g = torch.Generator().manual_seed(ns + nt)
+    clouds, kpts = [], []
+    for n, cap, seed in ((ns, cs, 3), (nt, ct, 4)):
+        x = _cloud(n, seed)[:n]
+        k = torch.from_numpy(x[torch.randint(0, n, (Kr,), generator=g).numpy()]).to(dev).contiguous()
+        clouds.append(_poisoned(x, cap, dev, k.cpu()))     # padding rows on the key-points: each would count if read
+        kpts.append(k)
+    N = ns if ns > nt else nt
+    pts_r, kpts_r = (clouds[0], kpts[0]) if ns > nt else (clouds[1], kpts[1])
+    sub = torch.randint(0, N, (S, SUB), generator=g)
+    d_sub = sub.to(dev, torch.int32)
+    if ns == 200000:
+        d_sub.fill_(-1)       # not read: any value would do
+    d_counts = torch.tensor([ns, nt], dtype=torch.int32, device=dev)
+    r, m, hist = ops.radius_estimate_pair(kpts[0], clouds[0], kpts[1], clouds[1], thresholds, d_counts, d_sub=d_sub)
+    assert tuple(hist.shape) == (S, ops.RADIUS_BINS + 2)
+    for i in range(S):
+        pts_e = pts_r[:N][sub[i].to(dev)].contiguous() if N > SUB else pts_r[:N].contiguous()
+        r_e, m_e, hist_e = ops.radius_estimate(kpts_r, pts_e, thresholds[i:i + 1], denom=N * Kr)
+        assert torch.equal(hist[i], hist_e), f"scale {i}: histogram"
+        assert torch.equal(m[i:i + 1], m_e) and torch.equal(r[i:i + 1].view(torch.int32), r_e.view(torch.int32)), f"scale {i}: radius"
+        assert int(hist_e[-2]) > 0
+    if N > SUB:     # three draws, three histograms
+        assert not torch.equal(hist[0], hist[1]) and not torch.equal(hist[1], hist[2])
+    with pytest.raises(ops.BufferXError, match="d_sub must be"):
+        ops.radius_estimate_pair(kpts[0], clouds[0], kpts[1], clouds[1], thresholds, d_counts, d_sub=d_sub[:2])
 
 
 # ------------------------------------------------------------------------------------------------ whole pairs
