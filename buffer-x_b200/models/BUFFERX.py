@@ -1,5 +1,6 @@
 """BufferX on H100: the per-pair registration ``forward()``, in eval mode the training stages' validation forward, and in
-training mode the Pose stage's step (batch-statistics BatchNorm, ``pred_ind`` differentiable in ``Pose.conv``).
+training mode the Pose stage's step (batch-statistics BatchNorm, ``pred_ind`` differentiable in ``Pose.conv``) and the Desc
+stage's step (``src_des``, ``tgt_des`` and ``equi_score`` differentiable in the descriptor network's parameters).
 
 Mirrors ``BufferX`` of /root/reference/models/BUFFERX.py (constructor :72-84, inference branch of
 ``forward`` :257-467, ``mutual_matching`` :469-496, ``post_refinement`` :522-556): same attribute names
@@ -30,6 +31,7 @@ import os
 import numpy as np
 import torch
 import torch.nn as nn
+from torch.autograd.function import once_differentiable
 
 from bufferx_b200 import ops
 from . import patchnet as pn
@@ -55,6 +57,21 @@ class EquiMatch(nn.Module):
         idx = torch.from_numpy(self.index_list).to(Des1.device).reshape(-1)
         d1 = Des1[:, :, :, idx].reshape(B, C, K, self.azi_n, self.azi_n).permute(0, 1, 3, 2, 4).reshape(B, C, -1, K * L)
         return torch.einsum("bfag,bfg->ba", d1, Des2.reshape(B, C, K * L))
+
+
+class _EquiMatchFn(torch.autograd.Function):
+    """EquiMatch score of two equivariant maps on bx_equi_match, differentiable in both (bx_td_equi_match_backward)."""
+
+    @staticmethod
+    def forward(ctx, d1, d2):
+        ctx.save_for_backward(d1, d2)
+        return ops.equi_match(d1, d2)
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, g):
+        d1, d2 = ctx.saved_tensors
+        return ops.equi_match_backward(d1, d2, g.float().contiguous())
 
 
 class CostVolume(nn.Module):
@@ -706,9 +723,10 @@ class BufferX(nn.Module):
 
     def _train_forward(self, data_source, perms=None, aug_angles=None, match_choice=None):
         """Validation forward of cfg.stage "Desc" / "Pose" in eval mode (reference BUFFERX.py:148-255), or with the model in
-        training mode the forward of the Pose stage's training step (every BatchNorm on batch statistics, its running
-        statistics updated: the descriptor network's twice, source then target; ``pred_ind`` carries a grad_fn into
-        ``Pose.conv``'s weights and biases; the batch statistics land in ``self.last_train_stats``): ground-truth
+        training mode the forward of the stage's training step (every BatchNorm on batch statistics, its running
+        statistics updated: the descriptor network's twice, source then target; "Pose": ``pred_ind`` carries a grad_fn into
+        ``Pose.conv``'s weights and biases, "Desc": ``src_des``, ``tgt_des`` and ``equi_score`` into the descriptor
+        network's parameters; the batch statistics land in ``self.last_train_stats``): ground-truth
         correspondences on the second-level clouds, descriptors of the (sub-sampled) matched key-points, then EquiMatch
         score + integer SO(2) label ("Desc") or CostNet soft arg-max + float SO(2) label of the augmented target ("Pose").
         NumPy's global RNG is consumed like the reference: match sub-sampling (only beyond cfg.train.pos_num), des_r,
@@ -728,7 +746,7 @@ class BufferX(nn.Module):
         if train:
             # the step moves every running statistic and optimizer.step() the weights: captured graphs hold the old folded ones
             self._drop_captured_state()
-            stats = dict(src=[], tgt=[], pose=[])
+            stats = dict(src=[], tgt=[], pose=[]) if stage == "Pose" else dict(src=[], tgt=[])
         with torch.cuda.device(dev):
             src, tgt = _pts(data_source["src_fds_pcd"]), _pts(data_source["tgt_fds_pcd"])
             src_sds, tgt_sds = _pts(data_source["src_sds_pcd"]), _pts(data_source["tgt_sds_pcd"])
@@ -751,7 +769,10 @@ class BufferX(nn.Module):
             des_r = self._draw_des_r()
             aligned = bool(data_source["is_aligned_to_global_z"])
             ps, pt = (None, None) if perms is None else perms
-            if train:
+            if train and stage == "Desc":
+                src_d = self.Desc.forward_desc_train(src[None], src_kpt[None], des_r, aligned, perm=ps, stats=stats["src"])
+                tgt_d = self.Desc.forward_desc_train(tgt[None], tgt_kpt[None], des_r, aligned, perm=pt, stats=stats["tgt"])
+            elif train:
                 src_d = self.Desc.forward_train(src[None], src_kpt[None], des_r, aligned, perm=ps, stats=stats["src"])
                 tgt_d = self.Desc.forward_train(tgt[None], tgt_kpt[None], des_r, aligned, True, perm=pt, aug_angles=aug_angles,
                                                 stats=stats["tgt"])
@@ -764,8 +785,11 @@ class BufferX(nn.Module):
                 return None
             if stage == "Desc":
                 out = {"src_kpt": src_kpt, "tgt_kpt": tgt_kpt, "src_des": src_d["desc"], "tgt_des": tgt_d["desc"],
-                       "equi_score": ops.equi_match(src_d["equi"], tgt_d["equi"]),
+                       "equi_score": _EquiMatchFn.apply(src_d["equi"], tgt_d["equi"]) if train
+                       else ops.equi_match(src_d["equi"], tgt_d["equi"]),
                        "gt_label": ops.so2_gt(src_d["rand_axis"], src_d["R"], tgt_d["R"], T, azi_n, True)}
+                if train:
+                    self.last_train_stats = stats
             elif train:
                 out = {"pred_ind": self.Pose.conv.forward_train(src_d["equi"], tgt_d["equi"], stats["pose"]),
                        "gt_ind": ops.so2_gt(src_d["rand_axis"], src_d["R"], tgt_d["R"], T, azi_n, False, aug_R=tgt_d["aug_rotation"])}
@@ -799,12 +823,15 @@ class BufferX(nn.Module):
     def forward(self, data_source, perms=None, ransac_seed=None, debug=False, aug_angles=None, match_choice=None):
         cfg = self.config
         if cfg.stage != "test":
-            if cfg.stage not in ("Desc", "Pose") or (self.training and cfg.stage != "Pose"):
+            if cfg.stage not in ("Desc", "Pose"):
                 raise NotImplementedError(
-                    "bufferx_b200 runs cfg.stage 'test', in eval mode the validation forward of the training stages "
-                    "'Desc' / 'Pose', and the training step of stage 'Pose'; training-mode BatchNorm and the backward pass of "
-                    "stage 'Desc' are not built (call model.eval())")
-            if self.training and any(p.requires_grad for p in self.Desc.parameters()):
+                    "bufferx_b200 runs cfg.stage 'test', and for the training stages 'Desc' / 'Pose' their validation forward "
+                    "(eval mode) and their training step (train mode)")
+            if self.training and cfg.stage == "Desc" and any(p.requires_grad for p in self.Pose.parameters()):
+                raise NotImplementedError(
+                    "the Desc training step (training-mode BatchNorm and the backward pass through Desc) needs CostNet frozen "
+                    "(requires_grad=False on every Pose parameter, as train.py does for this stage)")
+            if self.training and cfg.stage == "Pose" and any(p.requires_grad for p in self.Desc.parameters()):
                 raise NotImplementedError(
                     "the Pose training step needs the descriptor network frozen (requires_grad=False on every Desc parameter, "
                     "as train.py does for this stage): the backward pass through Desc is not built")

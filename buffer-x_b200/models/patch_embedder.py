@@ -6,10 +6,13 @@ same sub-module names -> same state_dict keys ``pnt_layer.{0,1}``, ``pool_layer.
 pooling, every stage a hand-written CUDA kernel behind the C-ABI.  ``forward`` is the eval-mode forward; ``forward_train``
 normalises every BatchNorm with its batch statistics and updates the running statistics, as the module does under
 model.train() (the Pose training stage runs it with the descriptor network frozen: no gradients flow here).
+``forward_desc_train`` is the Desc training stage's forward: float64 from the point layer on (bx_train_desc.cu), behind
+one autograd Function whose backward gives the gradients of every MiniSpinNet parameter.
 """
 import numpy as np
 import torch
 import torch.nn as nn
+from torch.autograd.function import once_differentiable
 
 from bufferx_b200 import ops
 from . import patchnet as pn
@@ -44,6 +47,22 @@ def pnt_stats_from_moments(mo, Wp, bp):
     mean = Wp @ Ex + bp
     var = torch.clamp(((Wp @ cov) * Wp).sum(dim=1), min=0.0)
     return mean, var
+
+
+class _DescTrain(torch.autograd.Function):
+    """(desc, equi) of MiniSpinNet in training mode from the de-rotated point-layer inputs, differentiable in its parameters."""
+
+    @staticmethod
+    def forward(ctx, net, inv, stats, *params):
+        desc, equi, saved = net._desc_forward_train(inv, stats)
+        ctx.net, ctx.saved = net, saved
+        return desc, equi
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, ddesc, dequi):
+        grads = ctx.net._desc_backward_train(ctx.saved, ddesc, dequi)
+        return (None, None, None) + tuple(g if need else None for g, need in zip(grads, ctx.needs_input_grad[3:]))
 
 
 class MiniSpinNet(nn.Module):
@@ -194,6 +213,136 @@ class MiniSpinNet(nn.Module):
         Wf2, bf2 = pn.fold_conv_bn(c2.weight, c2.bias, m2, v2, b2n.weight, b2n.bias, b2n.eps)
         desc, equi = ops.pool_desc(x, Wf1[0].contiguous(), bf1, Wf2[0, :, 0].contiguous(), bf2, channels_last=True)
         return {"desc": desc, "equi": equi, "rand_axis": rand_axis, "R": R, "patches": delta, "aug_rotation": aug_R}
+
+    def forward_desc_train(self, pts, kpts, des_r, is_aligned_to_global_z, perm=None, stats=None):
+        """MiniSpinNet.forward of the Desc training stage (patch_embedder.py:44-90 under model.train(), no augmentation): the
+        patches, frames and SPT of ``forward``, then ``train_desc``.  ``desc`` and ``equi`` carry a grad_fn into the
+        parameters that require grad.  Returns ``forward``'s dict."""
+        pts = pts[0].contiguous()
+        kpts = kpts[0].contiguous()
+        dev = pts.device
+        N = pts.shape[0]
+        if perm is None:
+            perm = np.random.choice(N, N, replace=False)
+        if not isinstance(perm, torch.Tensor):
+            perm = torch.from_numpy(np.ascontiguousarray(perm, dtype=np.int32)).to(dev, non_blocking=True)
+        prep = self.prepared(dev)
+        pts4 = ops.permute_cloud(pts, perm)
+        patches, _ = ops.select_patches(pts4, kpts, des_r, self.patch_sample)
+        delta, R, rand_axis = ops.lrf(patches, des_r, bool(is_aligned_to_global_z))
+        _, _, inv = ops.spt_pnt(delta, prep["voxels"], prep["rot"], self.delta / self.rad_n, self.voxel_sample, prep["w_pnt"],
+                                prep["b_pnt"], self.azi_n, debug=True)
+        desc, equi = self.train_desc(inv, stats)
+        return {"desc": desc, "equi": equi, "rand_axis": rand_axis, "R": R, "patches": delta, "aug_rotation": None}
+
+    def train_desc(self, inv, stats=None):
+        """Training mode from the de-rotated samples inv [K, V, nv, 3] (fp32, zero slots included) -> (desc [K, 32], equi
+        [K, 32, ele_n, azi_n]) fp32, evaluated in float64.  Every BatchNorm normalises with its batch statistics and updates
+        its running statistics once (also under torch.no_grad()).  ``stats``: optional list receiving (batch mean, batch
+        variance) of every BatchNorm in module order (pnt_layer, conv_net, pool_layer), float64."""
+        if self.rad_n * self.ele_n * self.azi_n != 420 or self.azi_n != 20 or self.rad_n != 3:
+            raise ops.BufferXError("train_desc: the Desc training kernels are built for 3 x 7 x 20 cylindrical voxels")
+        return _DescTrain.apply(self, inv.contiguous(), [] if stats is None else stats, *self.parameters())
+
+    def _desc_forward_train(self, inv, stats):
+        F64 = torch.float64
+        dev = inv.device
+        K, V, nv = inv.shape[0], inv.shape[1], inv.shape[2]
+        # point layer: batch statistics of the linear 3 -> 16 map from the float64 moments of its inputs
+        conv, bn = self.pnt_layer[0], self.pnt_layer[1]
+        R_n = K * V * nv
+        mo = ops.moments3(inv)
+        Wp = conv.weight.detach().double().view(16, 3).contiguous()
+        bp = conv.bias.detach().double().contiguous()
+        mean, var = pnt_stats_from_moments(mo / R_n, Wp, bp)
+        pn.bn_batch_stats(torch.stack([mean * R_n, (var + mean * mean) * R_n]), R_n, bn)
+        stats.append((mean, var))
+        scale, shift = pn.bn_scale_shift(mean, var, bn, F64)
+        feat, arg = ops.pnt_forward(inv, Wp, bp, scale, shift)
+        pnt = dict(inv=inv, arg=arg, W=Wp, b=bp, mean=mean.contiguous(), rstd=(1.0 / torch.sqrt(var + bn.eps)).contiguous(),
+                   gamma=bn.weight.detach().double().contiguous(), scale=scale, shift=shift, mo=mo)
+        # Cylindrical_Net on the fp64 tensor cores, each BatchNorm'd layer normalised with its batch statistics
+        net = self.conv_net
+        N = K * 140
+        cur, layers = feat, []
+        for i, (ci, bi, _) in enumerate(net.layers):
+            c = net.ops[ci]
+            Din = 3 if i == 0 else 1
+            Wt = c.weight.detach().double().reshape(c.out_channels, c.in_channels, -1).permute(2, 1, 0).contiguous()
+            z = ops.cyl_forward(cur, Wt, c.bias.detach().double().contiguous(), Din)
+            rec = dict(x=cur, z=z, Wt=Wt, Din=Din)
+            if bi is not None:
+                m, v = pn.bn_batch_stats(ops.channel_sums(z), N, net.ops[bi])
+                sc, sh = pn.bn_scale_shift(m, v, net.ops[bi], F64)
+                rec.update(scale=sc, shift=sh)
+                stats.append((m, v))
+                cur = ops.bn_apply(z, sc, sh, True)
+            else:
+                cur = z
+            layers.append(rec)
+        x = cur
+        # pool layer: two 1x1 convolutions with affine batch-statistics BatchNorm and ReLU -> attention w; pooling
+        c1, b1n, c2, b2n = self.pool_layer[0], self.pool_layer[1], self.pool_layer[3], self.pool_layer[4]
+        W1 = c1.weight.detach().double().view(16, 32).t().contiguous()                    # [32, 16]
+        z1 = ops.conv1x1_f64(x, W1, c1.bias.detach().double().contiguous())
+        m1, v1 = pn.bn_batch_stats(ops.channel_sums(z1), N, b1n)
+        sc1, sh1 = pn.bn_scale_shift(m1, v1, b1n, F64)
+        h = ops.bn_apply(z1, sc1, sh1, True)
+        W2 = torch.zeros((16, 4), dtype=F64, device=dev)                                   # one output channel, padded to 4
+        W2[:, 0] = c2.weight.detach().double().view(16)
+        b2 = torch.zeros(4, dtype=F64, device=dev)
+        b2[0] = c2.bias.detach().double()[0]
+        z2 = ops.conv1x1_f64(h, W2, b2)
+        m2, v2 = pn.bn_batch_stats(ops.channel_sums(z2)[:, :1], N, b2n)
+        sc2, sh2 = pn.bn_scale_shift(m2, v2, b2n, F64)
+
+        def pad(t):                      # the one attention channel, padded to the 4 of a blocked image
+            return torch.cat([t.reshape(1).double(), torch.zeros(3, dtype=F64, device=dev)])
+        w = ops.bn_apply(z2, pad(sc2), pad(sh2), True)
+        stats += [(m1, v1), (m2, v2)]
+        f, desc, equi = ops.pool_forward(x, w)
+        pool = dict(x=x, z1=z1, h=h, z2=z2, w=w, f=f, W1=W1, W2=W2,
+                    bn1=(m1.contiguous(), (1.0 / torch.sqrt(v1 + b1n.eps)).contiguous(), b1n.weight.detach().double().contiguous(),
+                         b1n.bias.detach().double().contiguous()),
+                    bn2=tuple(pad(t) for t in (m2, 1.0 / torch.sqrt(v2 + b2n.eps), b2n.weight.detach(), b2n.bias.detach())))
+        return desc, equi.view(K, 32, self.ele_n, self.azi_n), dict(pnt=pnt, layers=layers, pool=pool, K=K)
+
+    def _desc_backward_train(self, saved, ddesc, dequi):
+        """The gradients of every parameter (in self.parameters() order) from dL/ddesc, dL/dequi (either may be None)."""
+        K = saved["K"]
+        dev = saved["pool"]["x"].device
+        ddesc = torch.zeros((K, 32), dtype=torch.float32, device=dev) if ddesc is None else ddesc.float().contiguous()
+        dequi = torch.zeros((K, 32, self.ele_n, self.azi_n), dtype=torch.float32, device=dev) if dequi is None else dequi.float().contiguous()
+        g = {}
+        P = saved["pool"]
+        dx, dw = ops.pool_backward(P["x"], P["w"], P["f"], ddesc, dequi)
+        dz2, s2 = ops.bn_affine_backward(dw, P["z2"], *P["bn2"])
+        g["pool_layer.4.weight"], g["pool_layer.4.bias"] = s2[1, :1], s2[0, :1]
+        g["pool_layer.3.weight"] = ops.cross_sums(P["h"], dz2)[:, :1].t()
+        g["pool_layer.3.bias"] = ops.channel_sums(dz2)[0, :1]
+        dh = ops.conv1x1_f64(dz2, P["W2"].t().contiguous())
+        dz1, s1 = ops.bn_affine_backward(dh, P["z1"], *P["bn1"])
+        g["pool_layer.1.weight"], g["pool_layer.1.bias"] = s1[1], s1[0]
+        g["pool_layer.0.weight"] = ops.cross_sums(P["x"], dz1).t()
+        g["pool_layer.0.bias"] = ops.channel_sums(dz1)[0]
+        dy = ops.conv1x1_f64(dz1, P["W1"].t().contiguous(), out=dx)
+        net = self.conv_net
+        for i in reversed(range(len(net.layers))):
+            rec = saved["layers"][i]
+            if "scale" in rec:                        # ReLU mask + batch-statistics BatchNorm backward
+                s = ops.channel_sums(dy, rec["z"], rec["scale"], rec["shift"]) / (K * 140)
+                dz = ops.bn_backward(dy, rec["z"], rec["scale"], rec["shift"], s[0].contiguous(), s[1].contiguous())
+            else:
+                dz = dy
+            ci = net.layers[i][0]
+            g[f"conv_net.ops.{ci}.bias"] = ops.channel_sums(dz)[0]
+            dy, dW = ops.cyl_backward(rec["x"], dz, rec["Wt"], rec["Din"])
+            g[f"conv_net.ops.{ci}.weight"] = dW.permute(2, 1, 0)
+        Q = saved["pnt"]
+        o = ops.pnt_backward(Q["inv"], Q["arg"], dy, Q["W"], Q["b"], Q["mean"], Q["rstd"], Q["gamma"], Q["scale"], Q["shift"], Q["mo"])
+        g["pnt_layer.0.weight"], g["pnt_layer.0.bias"] = o[:, :3], o[:, 3]
+        g["pnt_layer.1.weight"], g["pnt_layer.1.bias"] = o[:, 4], o[:, 5]
+        return [g[name].reshape(p.shape).to(p.dtype).contiguous() for name, p in self.named_parameters()]
 
     def forward_multi(self, jobs, is_aligned_to_global_z, radii=None, counts=None, npts=None):
         """Descriptors of several (cloud, key-points, radius, permutation) jobs in ONE pass through SPT, the

@@ -34,6 +34,8 @@ SYMBOLS = [
     "bx_fps_large", "bx_fps_large_workspace_bytes", "bx_fps_large_n", "bx_fps_large_size_class", "bx_radius_estimate_n_sub",
     "bx_ts_splits", "bx_ts_channel_sums", "bx_ts_channel_sums_f64", "bx_ts_moments3", "bx_ts_bn_apply", "bx_ts_bn_apply_f64",
     "bx_ts_bn_backward", "bx_ts_conv1x1", "bx_ts_costvol", "bx_ts_softargmax", "bx_ts_conv_forward", "bx_ts_conv_backward",
+    "bx_td_cyl_forward", "bx_td_cyl_dgrad", "bx_td_cyl_wgrad", "bx_td_pnt_forward", "bx_td_pnt_backward", "bx_td_conv1x1",
+    "bx_td_cross_sums", "bx_td_bn_affine_backward", "bx_td_pool_forward", "bx_td_pool_backward", "bx_td_equi_match_backward",
 ]
 
 GEOM_CYL3D, GEOM_CYL2D, GEOM_VALID3D, GEOM_COSTAB = 0, 1, 2, 4
@@ -140,6 +142,17 @@ def load_library():
     lib.bx_ts_costvol.argtypes = [P, P, c_int, P, P]
     lib.bx_ts_softargmax.argtypes = [P, c_int, c_int, P, P, P, P]
     lib.bx_ts_conv_backward.argtypes = [P, P, P] + [c_int] * 9 + [P, P, P, P]
+    lib.bx_td_cyl_forward.argtypes = [P, P, P, c_int, c_int, c_int, c_int, P, P]
+    lib.bx_td_cyl_dgrad.argtypes = [P, P, c_int, c_int, c_int, c_int, P, P]
+    lib.bx_td_cyl_wgrad.argtypes = [P, P, c_int, c_int, c_int, c_int, P, P, P]
+    lib.bx_td_pnt_forward.argtypes = [P, P, P, P, P, c_int, c_int, c_int, P, P, P]
+    lib.bx_td_pnt_backward.argtypes = [P] * 11 + [c_int, c_int, c_int, P, P, P]
+    lib.bx_td_conv1x1.argtypes = [P, P, P, c_int, c_int, c_int, c_int, c_int, P, P]
+    lib.bx_td_cross_sums.argtypes = [P, P, c_int, c_int, c_int, c_int, P, P, P]
+    lib.bx_td_bn_affine_backward.argtypes = [P] * 6 + [c_int, c_int, c_int, P, P, P, P]
+    lib.bx_td_pool_forward.argtypes = [P, P, c_int, P, P, P, P]
+    lib.bx_td_pool_backward.argtypes = [P, P, P, P, P, c_int, P, P, P]
+    lib.bx_td_equi_match_backward.argtypes = [P, P, P, c_int, c_int, c_int, c_int, P, P, P]
     _lib = lib
     return lib
 
@@ -1222,3 +1235,196 @@ def conv_backward(x, dy, Wt, D, H, W, kd, kh, kw, want_dx=True):
     _check(load_library().bx_ts_conv_backward(_dp(x, F64, "x"), _dp(dy, F64, "dy"), _dp(Wt, F64, "Wt"), n, Cin, Cout, D, H, W, kd, kh, kw,
                                               _dp(dx), _dp(wpart), _dp(dW), _stream()), "bx_ts_conv_backward")
     return dx, dW
+
+
+# --------------------------------------------------------------------------- #
+# the Desc-stage training step (bx_train_desc.cu): float64 activations channel-blocked [n, C/4, S, 4]; a cylindrical
+# raster has 140 = 7 x 20 positions per depth slice
+# --------------------------------------------------------------------------- #
+CYL_S = 140
+U8 = torch.uint8
+
+
+def _cyl_shapes(what, x, Din, C=None):
+    n, G, S = _ts_blocked(what, x)
+    if x.dtype != F64:
+        raise BufferXError(f"{what}: x must be float64, got {x.dtype}")
+    if S != Din * CYL_S:
+        raise BufferXError(f"{what}: x holds {S} positions per channel, a cylindrical raster of depth {Din} has {Din * CYL_S}")
+    if C is not None and 4 * G != C:
+        raise BufferXError(f"{what}: x has {4 * G} channels, expected {C}")
+    return n, 4 * G
+
+
+def cyl_forward(x, Wt, b, Din):
+    """One Cylindrical_Net convolution on the fp64 tensor cores: x [n, Cin/4, Din*140, 4], Wt [Din*9, Cin, Cout], b [Cout]
+    (float64) -> [n, Cout/4, 140, 4].  Circular azimuth / zero elevation padding is applied by the kernel."""
+    n, Cin = _cyl_shapes("cyl_forward", x, Din)
+    if not isinstance(Wt, torch.Tensor) or Wt.dim() != 3:
+        raise BufferXError(f"cyl_forward: Wt must be [Din*9, Cin, Cout], got {tuple(Wt.shape) if isinstance(Wt, torch.Tensor) else Wt}")
+    Cout = Wt.shape[2]
+    _ts_shape("cyl_forward", Wt, (Din * 9, Cin, Cout), "Wt")
+    _ts_shape("cyl_forward", b, (Cout,), "b")
+    if Cin % 16 or Cout % 8:
+        raise BufferXError(f"cyl_forward: Cin = {Cin} must be a multiple of 16 and Cout = {Cout} of 8")
+    out = torch.empty((n, Cout // 4, CYL_S, 4), dtype=F64, device=x.device)
+    _check(load_library().bx_td_cyl_forward(_dp(x, F64, "x"), _dp(Wt, F64, "Wt"), _dp(b, F64, "b"), n, Cin, Cout, Din, _dp(out), _stream()),
+           "bx_td_cyl_forward")
+    return out
+
+
+def cyl_backward(x, dy, Wt, Din, want_dx=True):
+    """Backward of cyl_forward: x [n, Cin/4, Din*140, 4], dy [n, Cout/4, 140, 4], Wt [Din*9, Cin, Cout] -> (dx like x or
+    None, dW [Din*9, Cin, Cout]); the bias gradient is channel_sums(dy)[0]."""
+    n, Cin = _cyl_shapes("cyl_backward", x, Din)
+    if not isinstance(Wt, torch.Tensor) or Wt.dim() != 3:
+        raise BufferXError(f"cyl_backward: Wt must be [Din*9, Cin, Cout], got {tuple(Wt.shape) if isinstance(Wt, torch.Tensor) else Wt}")
+    Cout = Wt.shape[2]
+    _ts_shape("cyl_backward", Wt, (Din * 9, Cin, Cout), "Wt")
+    _ts_shape("cyl_backward", dy, (n, Cout // 4, CYL_S, 4), "dy")
+    if Cout % 16 or Cin % 8:
+        raise BufferXError(f"cyl_backward: Cin = {Cin} must be a multiple of 8 and Cout = {Cout} of 16")
+    lib = load_library()
+    wpart = torch.empty(_splits() * Din * 9 * Cin * Cout, dtype=F64, device=x.device)
+    dW = torch.empty((Din * 9, Cin, Cout), dtype=F64, device=x.device)
+    _check(lib.bx_td_cyl_wgrad(_dp(x, F64, "x"), _dp(dy, F64, "dy"), n, Cin, Cout, Din, _dp(wpart), _dp(dW), _stream()), "bx_td_cyl_wgrad")
+    dx = None
+    if want_dx:
+        dx = torch.empty_like(x)
+        _check(lib.bx_td_cyl_dgrad(_dp(dy, F64, "dy"), _dp(Wt, F64, "Wt"), n, Cin, Cout, Din, _dp(dx), _stream()), "bx_td_cyl_dgrad")
+    return dx, dW
+
+
+def _pnt_inv(what, inv):
+    if not isinstance(inv, torch.Tensor) or inv.dim() != 4 or inv.shape[3] != 3 or inv.numel() == 0 or inv.shape[2] > 255:
+        raise BufferXError(f"{what}: inv must be [K, V, nv, 3] with 1 <= nv <= 255, got "
+                           f"{tuple(inv.shape) if isinstance(inv, torch.Tensor) else type(inv).__name__}")
+    return inv.shape[0], inv.shape[1], inv.shape[2]
+
+
+def pnt_forward(inv, W, b, scale, shift):
+    """The point layer in training mode on the de-rotated samples inv [K, V, nv, 3] fp32: W [16, 3], b, scale, shift [16]
+    (float64; x^ = (W inv + b) scale + shift) -> (feat [K, 4, V, 4] float64 = max over the samples of relu(x^), arg [K, 16, V]
+    uint8 = the first maximal sample)."""
+    K, V, nv = _pnt_inv("pnt_forward", inv)
+    _ts_shape("pnt_forward", W, (16, 3), "W")
+    for name, t in (("b", b), ("scale", scale), ("shift", shift)):
+        _ts_shape("pnt_forward", t, (16,), name)
+    feat = torch.empty((K, 4, V, 4), dtype=F64, device=inv.device)
+    arg = torch.empty((K, 16, V), dtype=U8, device=inv.device)
+    _check(load_library().bx_td_pnt_forward(_dp(inv, F32, "inv"), _dp(W, F64, "W"), _dp(b, F64, "b"), _dp(scale, F64, "scale"),
+                                            _dp(shift, F64, "shift"), K, V, nv, _dp(feat), _dp(arg), _stream()), "bx_td_pnt_forward")
+    return feat, arg
+
+
+def pnt_backward(inv, arg, dfeat, W, b, mean, rstd, gamma, scale, shift, mo9):
+    """Backward of pnt_forward from dfeat (like feat): -> float64 [16, 6] = dW (3 columns), db, dgamma, dbeta.  mean, rstd:
+    the batch statistics; gamma: the BatchNorm weight; mo9: moments3(inv)."""
+    K, V, nv = _pnt_inv("pnt_backward", inv)
+    _ts_shape("pnt_backward", arg, (K, 16, V), "arg")
+    _ts_shape("pnt_backward", dfeat, (K, 4, V, 4), "dfeat")
+    _ts_shape("pnt_backward", W, (16, 3), "W")
+    for name, t in (("b", b), ("mean", mean), ("rstd", rstd), ("gamma", gamma), ("scale", scale), ("shift", shift)):
+        _ts_shape("pnt_backward", t, (16,), name)
+    _ts_shape("pnt_backward", mo9, (9,), "mo9")
+    partial = torch.empty(_splits() * 80, dtype=F64, device=inv.device)
+    out = torch.empty((16, 6), dtype=F64, device=inv.device)
+    _check(load_library().bx_td_pnt_backward(_dp(inv, F32, "inv"), _dp(arg, U8, "arg"), _dp(dfeat, F64, "dfeat"), _dp(W, F64, "W"),
+                                             _dp(b, F64, "b"), _dp(mean, F64, "mean"), _dp(rstd, F64, "rstd"), _dp(gamma, F64, "gamma"),
+                                             _dp(scale, F64, "scale"), _dp(shift, F64, "shift"), _dp(mo9, F64, "mo9"), K, V, nv, _dp(partial),
+                                             _dp(out), _stream()), "bx_td_pnt_backward")
+    return out
+
+
+def conv1x1_f64(x, w, b=None, out=None):
+    """float64 1x1 convolution of a blocked image: x [n, Cin/4, S, 4], w [Cin, Cout], b [Cout] or None -> [n, Cout/4, S, 4];
+    with ``out`` the result is added to it.  Cin, Cout <= 32, multiples of 4."""
+    n, G, S = _ts_blocked("conv1x1_f64", x)
+    if not isinstance(w, torch.Tensor) or w.dim() != 2 or w.shape[0] != 4 * G:
+        raise BufferXError(f"conv1x1_f64: w must be [{4 * G}, Cout], got {tuple(w.shape) if isinstance(w, torch.Tensor) else w}")
+    Cout = w.shape[1]
+    if Cout % 4 or not 4 <= Cout <= 32 or 4 * G > 32:
+        raise BufferXError(f"conv1x1_f64: {4 * G} -> {Cout} channels: both must be multiples of 4, at most 32")
+    if b is not None:
+        _ts_shape("conv1x1_f64", b, (Cout,), "b")
+    acc = out is not None
+    if acc:
+        _ts_shape("conv1x1_f64", out, (n, Cout // 4, S, 4), "out")
+    else:
+        out = torch.empty((n, Cout // 4, S, 4), dtype=F64, device=x.device)
+    _check(load_library().bx_td_conv1x1(_dp(x, F64, "x"), _dp(w, F64, "w"), _dp(b, F64, "b"), n, 4 * G, Cout, S, int(acc), _dp(out, F64, "out"),
+                                        _stream()), "bx_td_conv1x1")
+    return out
+
+
+def cross_sums(X, D):
+    """X [n, Ca/4, S, 4], D [n, Cb/4, S, 4] float64 -> [Ca, Cb] = sum over samples and positions of X[a] D[b]."""
+    n, Ga, S = _ts_blocked("cross_sums", X, "X")
+    _ts_blocked("cross_sums", D, "D")
+    _ts_shape("cross_sums", D, (n, D.shape[1], S, 4), "D")
+    Ca, Cb = 4 * Ga, 4 * D.shape[1]
+    partial = torch.empty(_splits() * Ca * Cb, dtype=F64, device=X.device)
+    out = torch.empty((Ca, Cb), dtype=F64, device=X.device)
+    _check(load_library().bx_td_cross_sums(_dp(X, F64, "X"), _dp(D, F64, "D"), n, Ca, Cb, S, _dp(partial), _dp(out), _stream()),
+           "bx_td_cross_sums")
+    return out
+
+
+def bn_affine_backward(dy, z, mean, rstd, gamma, beta):
+    """Affine batch-statistics BatchNorm + ReLU backward, float64 blocked: -> (dz like z, sums [2, C] = (sum dz', sum dz' x^)
+    = (dbeta, dgamma)), dz' = dy [gamma x^ + beta > 0], x^ = (z - mean) rstd."""
+    n, G, S = _ts_blocked("bn_affine_backward", z, "z")
+    _ts_shape("bn_affine_backward", dy, z.shape, "dy")
+    for name, t in (("mean", mean), ("rstd", rstd), ("gamma", gamma), ("beta", beta)):
+        _ts_shape("bn_affine_backward", t, (4 * G,), name)
+    C = 4 * G
+    partial = torch.empty(_splits() * 2 * C, dtype=F64, device=z.device)
+    sums = torch.empty(2 * C, dtype=F64, device=z.device)
+    dx = torch.empty_like(z)
+    _check(load_library().bx_td_bn_affine_backward(_dp(dy, F64, "dy"), _dp(z, F64, "z"), _dp(mean, F64, "mean"), _dp(rstd, F64, "rstd"),
+                                                   _dp(gamma, F64, "gamma"), _dp(beta, F64, "beta"), n, C, S, _dp(partial), _dp(sums),
+                                                   _dp(dx), _stream()), "bx_td_bn_affine_backward")
+    return dx, sums.view(2, C)
+
+
+def pool_forward(x, w):
+    """x [K, 8, 140, 4], w [K, 1, 140, 4] (the attention in channel 0), float64 -> (f [K, 32] float64, desc [K, 32],
+    equi [K, 32, 7, 20] fp32)."""
+    _ts_shape("pool_forward", x, (x.shape[0] if isinstance(x, torch.Tensor) else -1, 8, CYL_S, 4), "x")
+    K = x.shape[0]
+    _ts_shape("pool_forward", w, (K, 1, CYL_S, 4), "w")
+    f = torch.empty((K, 32), dtype=F64, device=x.device)
+    desc = torch.empty((K, 32), dtype=F32, device=x.device)
+    equi = torch.empty((K, 32, 7, 20), dtype=F32, device=x.device)
+    _check(load_library().bx_td_pool_forward(_dp(x, F64, "x"), _dp(w, F64, "w"), K, _dp(f), _dp(desc), _dp(equi), _stream()), "bx_td_pool_forward")
+    return f, desc, equi
+
+
+def pool_backward(x, w, f, ddesc, dequi):
+    """Backward of pool_forward from ddesc [K, 32], dequi [K, 32, 7, 20] (fp32) -> (dx like x, dw like w)."""
+    _ts_shape("pool_backward", x, (x.shape[0] if isinstance(x, torch.Tensor) else -1, 8, CYL_S, 4), "x")
+    K = x.shape[0]
+    _ts_shape("pool_backward", w, (K, 1, CYL_S, 4), "w")
+    _ts_shape("pool_backward", f, (K, 32), "f")
+    _ts_shape("pool_backward", ddesc, (K, 32), "ddesc")
+    _ts_shape("pool_backward", dequi, (K, 32, 7, 20), "dequi")
+    dx = torch.empty_like(x)
+    dw = torch.empty_like(w)
+    _check(load_library().bx_td_pool_backward(_dp(x, F64, "x"), _dp(w, F64, "w"), _dp(f, F64, "f"), _dp(ddesc, F32, "ddesc"),
+                                              _dp(dequi, F32, "dequi"), K, _dp(dx), _dp(dw), _stream()), "bx_td_pool_backward")
+    return dx, dw
+
+
+def equi_match_backward(d1, d2, dcor):
+    """Gradients of equi_match(d1, d2) [B, L] with respect to d1 and d2 ([B, C, K, L] fp32) from dcor [B, L]."""
+    if not isinstance(d1, torch.Tensor) or d1.dim() != 4:
+        raise BufferXError(f"equi_match_backward: d1 must be [B, C, K, L], got {tuple(d1.shape) if isinstance(d1, torch.Tensor) else d1}")
+    B, C, K, L = d1.shape
+    _ts_shape("equi_match_backward", d2, (B, C, K, L), "d2")
+    _ts_shape("equi_match_backward", dcor, (B, L), "dcor")
+    g1, g2 = torch.empty_like(d1), torch.empty_like(d2)
+    if B == 0:
+        return g1, g2
+    _check(load_library().bx_td_equi_match_backward(_dp(d1, F32, "d1"), _dp(d2, F32, "d2"), _dp(dcor, F32, "dcor"), B, C, K, L, _dp(g1),
+                                                    _dp(g2), _stream()), "bx_td_equi_match_backward")
+    return g1, g2

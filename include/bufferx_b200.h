@@ -492,6 +492,58 @@ int bx_ts_conv_forward(const double *x, const double *w, const double *b, int n,
 int bx_ts_conv_backward(const double *x, const double *dy, const double *w, int n, int Cin, int Cout, int D, int H, int W, int kd, int kh,
                         int kw, double *dx, double *wpartial, double *dw, void *stream);
 
+/* ---- SURVEY 8(f) row 3: the Desc-stage training step (trainer.py:93-167 with cfg.stage "Desc", model.train()) -------
+ * MiniSpinNet's forward with batch-statistics BatchNorm and its backward, float64 throughout (bx_train_desc.cu).  Images are
+ * channel-blocked float64 [n][C/4][S][4]; a cylindrical raster has S = 140 (7 elevation x 20 azimuth) positions per depth
+ * slice.  Reductions over samples x positions go through BX_TS_SPLITS partials (workspace `partial` / `wpartial`) added in
+ * split order: bit-identical across runs.
+ * bx_td_cyl_forward: one layer of Cylindrical_Net (models/patchnet.py:68-84) without its BatchNorm: the input padded
+ *   circularly in azimuth and with zeros in elevation (utils/common.py:265-310), then a valid 3x3 (Din = 1) or 3x3x3
+ *   (Din = 3, the depth collapsed) convolution.  x [n][Cin/4][Din*140][4], w [Din*9][Cin][Cout] (tap = (d, e, a) row-major),
+ *   b [Cout] -> out [n][Cout/4][140][4].  Runs on the fp64 tensor-core MMA.  Cin % 16 == 0, Cout % 8 == 0.
+ * bx_td_cyl_dgrad: its data gradient dx [n][Cin/4][Din*140][4] from dy [n][Cout/4][140][4] (replaces autograd through
+ *   F.conv3d / F.conv2d of patchnet.py:68-84 and the padding of utils/common.py:265-310).  Cin % 8 == 0, Cout % 16 == 0.
+ * bx_td_cyl_wgrad: its weight gradient dw [Din*9][Cin][Cout]; wpartial [BX_TS_SPLITS * Din*9*Cin*Cout].  The bias
+ *   gradient is bx_ts_channel_sums_f64 of dy.
+ * bx_td_pnt_forward: the point layer in training mode (patch_embedder.py:78-90: pnt_layer = 1x1 conv 3 -> 16, affine
+ *   BatchNorm, ReLU, then max_pool2d over the nv samples): inv [K][V][nv][3] fp32 (the de-rotated samples, zero slots
+ *   included), W [16][3], b [16], the BatchNorm as x^ = y scale + shift [16] -> feat [K][4][V][4] and arg [K][16][V] (the
+ *   first maximal sample).
+ * bx_td_pnt_backward: its backward from dfeat (shaped like feat): one pass over the K*16*V selected samples gives sum dz,
+ *   sum dz x^ and sum dz inv; the dense sums over every sample follow from mo9 (bx_ts_moments3 of inv).  mean, rstd, gamma
+ *   [16] are the batch statistics and BatchNorm weight, scale / shift as in the forward.  out [16][6] = dW[c][0..2], db[c],
+ *   dgamma[c], dbeta[c]; partial [BX_TS_SPLITS * 80].
+ * bx_td_conv1x1: out (+= if accumulate) b + w^T x for w [Cin][Cout], b [Cout] or NULL (the pool layer's 1x1 convolutions,
+ *   patch_embedder.py:32-39, and their data gradients); Cin, Cout <= 32, multiples of 4.
+ * bx_td_cross_sums: out [Ca][Cb] = sum over (s, p) of X[s][a][p] D[s][b][p] (a 1x1 convolution's weight gradient);
+ *   partial [BX_TS_SPLITS * Ca*Cb].
+ * bx_td_bn_affine_backward: affine batch-statistics BatchNorm + ReLU backward (pool_layer.{1,4}): x^ = (z - mean) rstd,
+ *   dz = dy [gamma x^ + beta > 0]; sums [2C] = (sum dz, sum dz x^) (= dbeta, dgamma), dx = gamma rstd (dz - m1 - x^ m2) with
+ *   m1, m2 the sums over n*S.  partial [BX_TS_SPLITS * 2C].
+ * bx_td_pool_forward / bx_td_pool_backward: attention pooling and the L2 normalisations (patch_embedder.py:86-90):
+ *   x [K][8][140][4], w the attention [K][1][140][4] (channel 0) -> f [K][32] float64, desc [K][32] and equi [K][32][140]
+ *   fp32 (v / max(|v|, 1e-12)); the backward from ddesc, dequi (fp32) gives dx like x and dw like w.
+ * bx_td_equi_match_backward: the gradients ds, dt [B][C][E][L] (fp32, float64 accumulation) of bx_equi_match's
+ *   cor[b][a] = sum s[b][c][e][(l - a) mod L] t[b][c][e][l] (EquiMatch, models/BUFFERX.py:72-86) from dcor [B][L]. */
+int bx_td_cyl_forward(const double *x, const double *w, const double *b, int n, int Cin, int Cout, int Din, double *out, void *stream);
+int bx_td_cyl_dgrad(const double *dy, const double *w, int n, int Cin, int Cout, int Din, double *dx, void *stream);
+int bx_td_cyl_wgrad(const double *x, const double *dy, int n, int Cin, int Cout, int Din, double *wpartial, double *dw, void *stream);
+int bx_td_pnt_forward(const float *inv, const double *W, const double *b, const double *scale, const double *shift, int K, int V, int nv,
+                      double *feat, unsigned char *arg, void *stream);
+int bx_td_pnt_backward(const float *inv, const unsigned char *arg, const double *dfeat, const double *W, const double *b, const double *mean,
+                       const double *rstd, const double *gamma, const double *scale, const double *shift, const double *mo9, int K, int V,
+                       int nv, double *partial, double *out, void *stream);
+int bx_td_conv1x1(const double *x, const double *w, const double *b, int n, int Cin, int Cout, int S, int accumulate, double *out,
+                  void *stream);
+int bx_td_cross_sums(const double *X, const double *D, int n, int Ca, int Cb, int S, double *partial, double *out, void *stream);
+int bx_td_bn_affine_backward(const double *dy, const double *z, const double *mean, const double *rstd, const double *gamma,
+                             const double *beta, int n, int C, int S, double *partial, double *sums, double *dx, void *stream);
+int bx_td_pool_forward(const double *x, const double *w, int K, double *f, float *desc, float *equi, void *stream);
+int bx_td_pool_backward(const double *x, const double *w, const double *f, const float *ddesc, const float *dequi, int K, double *dx,
+                        double *dw, void *stream);
+int bx_td_equi_match_backward(const float *s, const float *t, const float *dcor, int B, int C, int E, int L, float *ds, float *dt,
+                              void *stream);
+
 /* ---- loader-side ground truth: point-to-point ICP ---------------------------------------------------
  * Replaces open3d.pipelines.registration.registration_icp(source, target, r, init, TransformationEstimationPointToPoint(),
  * ICPConvergenceCriteria(...)) (Open3D 0.18), which the KITTI loader runs on the CPU to refine every pair's ground-truth
