@@ -417,28 +417,30 @@ __global__ void __launch_bounds__(TD_THREADS) cross_sums_kernel(const double *__
 }
 
 // Affine batch-statistics BatchNorm + ReLU backward (the pool layer's, patch_embedder.py:32-39), float64, blocked:
-//   x^ = (z - mean) rstd, y = gamma x^ + beta, dz = dy [y > 0].
+//   x^ = (z - mean) rstd, dz = dy [y > 0] with y the forward's ReLU output (bn_apply's z scale + shift: recomputing the
+//   sign as gamma x^ + beta rounds differently near the boundary, so the mask is read from y, as torch's threshold_backward).
 // First the per-channel sums sum dz, sum dz x^ (grid (C/4, BX_TS_SPLITS), partial [split][2C], then in split order),
 // then dx = gamma rstd (dz - m1 - x^ m2) with m1, m2 those sums over N (one thread per element).
 struct AffBN {
-    const double *mean, *rstd, *gamma, *beta;
+    const double *mean, *rstd, *gamma;
 };
 
-__global__ void __launch_bounds__(TD_THREADS) bn_aff_sums_kernel(const double *__restrict__ dy, const double *__restrict__ z, AffBN q, int n,
-                                                                 int G, int S, double *__restrict__ partial) {
+__global__ void __launch_bounds__(TD_THREADS) bn_aff_sums_kernel(const double *__restrict__ dy, const double *__restrict__ z,
+                                                                 const double *__restrict__ y, AffBN q, int n, int G, int S,
+                                                                 double *__restrict__ partial) {
     __shared__ double sh[8 * TD_THREADS];
     const int g = blockIdx.x, split = blockIdx.y, nsplit = gridDim.y;
     double v[8] = {0, 0, 0, 0, 0, 0, 0, 0};
-    double mu[4], rs[4], ga[4], be[4];
+    double mu[4], rs[4];
 #pragma unroll
-    for (int j = 0; j < 4; ++j) mu[j] = q.mean[4 * g + j], rs[j] = q.rstd[4 * g + j], ga[j] = q.gamma[4 * g + j], be[j] = q.beta[4 * g + j];
+    for (int j = 0; j < 4; ++j) mu[j] = q.mean[4 * g + j], rs[j] = q.rstd[4 * g + j];
     for (int s = split; s < n; s += nsplit) {
         const size_t base = ((size_t)s * G + g) * S * 4;
         for (int p = threadIdx.x; p < S; p += TD_THREADS) {
 #pragma unroll
             for (int j = 0; j < 4; ++j) {
                 const double xh = (z[base + 4 * p + j] - mu[j]) * rs[j];
-                const double dz = ga[j] * xh + be[j] > 0.0 ? dy[base + 4 * p + j] : 0.0;
+                const double dz = y[base + 4 * p + j] > 0.0 ? dy[base + 4 * p + j] : 0.0;
                 v[j] += dz;
                 v[4 + j] += dz * xh;
             }
@@ -456,13 +458,13 @@ __global__ void __launch_bounds__(TD_THREADS) bn_aff_sums_kernel(const double *_
     }
 }
 
-__global__ void bn_aff_bwd_kernel(const double *__restrict__ dy, const double *__restrict__ z, AffBN q, const double *__restrict__ sums,
-                                  double N, long long total, int G, int S, double *__restrict__ dx) {
+__global__ void bn_aff_bwd_kernel(const double *__restrict__ dy, const double *__restrict__ z, const double *__restrict__ y, AffBN q,
+                                  const double *__restrict__ sums, double N, long long total, int G, int S, double *__restrict__ dx) {
     const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= total) return;
     const int c = (int)((i / (4LL * S)) % G) * 4 + (int)(i & 3);
     const double xh = (z[i] - q.mean[c]) * q.rstd[c];
-    const double dz = q.gamma[c] * xh + q.beta[c] > 0.0 ? dy[i] : 0.0;
+    const double dz = y[i] > 0.0 ? dy[i] : 0.0;
     dx[i] = q.gamma[c] * q.rstd[c] * (dz - sums[c] / N - xh * (sums[4 * G + c] / N));
 }
 
@@ -502,7 +504,7 @@ __global__ void __launch_bounds__(CYL_S) pool_fwd_kernel(const double *__restric
 
 // backward of pool_fwd_kernel: ddesc [K][32], dequi [K][32][140] (fp32, upstream) -> dx blocked [K][8][140][4] (the equi
 // path and the direct x w path) and dw blocked [K][1][140][4] (channel 0; channels 1-3 zero).  Normalisation backward:
-// |v| > eps: (g - y (y . g)) / |v|, else g / eps (torch's clamp_min).
+// |v| >= eps: (g - y (y . g)) / |v|, else g / eps (torch's clamp_min, whose backward passes the gradient at equality).
 __global__ void __launch_bounds__(CYL_S) pool_bwd_kernel(const double *__restrict__ x, const double *__restrict__ w, const double *__restrict__ f,
                                                          const float *__restrict__ ddesc, const float *__restrict__ dequi,
                                                          double *__restrict__ dx, double *__restrict__ dw) {
@@ -514,7 +516,7 @@ __global__ void __launch_bounds__(CYL_S) pool_bwd_kernel(const double *__restric
         const double *fk = f + (size_t)k * 32;
         for (int c = 0; c < 32; ++c) n2 += fk[c] * fk[c];
         const double nf = sqrt(n2);
-        const bool big = nf > NORM_EPS;
+        const bool big = nf >= NORM_EPS;
         const double den = big ? nf : NORM_EPS;
         for (int c = 0; c < 32; ++c) yg += (fk[c] / den) * (double)ddesc[(size_t)k * 32 + c];
         for (int c = 0; c < 32; ++c) {
@@ -529,7 +531,7 @@ __global__ void __launch_bounds__(CYL_S) pool_bwd_kernel(const double *__restric
         n2 += v * v;
     }
     const double nx = sqrt(n2);
-    const bool big = nx > NORM_EPS;
+    const bool big = nx >= NORM_EPS;
     const double den = big ? nx : NORM_EPS;
     for (int c = 0; c < 32; ++c)
         yg += (xk[((c / 4) * CYL_S + p) * 4 + (c & 3)] / den) * (double)dequi[((size_t)k * 32 + c) * CYL_S + p];
@@ -660,18 +662,18 @@ BX_API int bx_td_cross_sums(const double *X, const double *D, int n, int Ca, int
     return BX_OK;
 }
 
-BX_API int bx_td_bn_affine_backward(const double *dy, const double *z, const double *mean, const double *rstd, const double *gamma,
-                                    const double *beta, int n, int C, int S, double *partial, double *sums, double *dx, void *stream) {
+BX_API int bx_td_bn_affine_backward(const double *dy, const double *z, const double *y, const double *mean, const double *rstd,
+                                    const double *gamma, int n, int C, int S, double *partial, double *sums, double *dx, void *stream) {
     BX_REQUIRE(n >= 1 && C >= 4 && C % 4 == 0 && S >= 1, "bx_td_bn_affine_backward: bad sizes");
-    BX_REQUIRE(dy && z && mean && rstd && gamma && beta && partial && sums && dx, "bx_td_bn_affine_backward: null pointer");
+    BX_REQUIRE(dy && z && y && mean && rstd && gamma && partial && sums && dx, "bx_td_bn_affine_backward: null pointer");
     cudaStream_t st = bx_stream(stream);
-    AffBN q{mean, rstd, gamma, beta};
-    bn_aff_sums_kernel<<<dim3(C / 4, BX_TS_SPLITS), TD_THREADS, 0, st>>>(dy, z, q, n, C / 4, S, partial);
+    AffBN q{mean, rstd, gamma};
+    bn_aff_sums_kernel<<<dim3(C / 4, BX_TS_SPLITS), TD_THREADS, 0, st>>>(dy, z, y, q, n, C / 4, S, partial);
     BX_LAUNCH_CHECK();
     sum_splits_kernel<<<blocks_for(2 * C, 128), 128, 0, st>>>(partial, BX_TS_SPLITS, 2 * C, sums);
     BX_LAUNCH_CHECK();
     const long long total = (long long)n * C * S;
-    bn_aff_bwd_kernel<<<blocks_for(total, 256), 256, 0, st>>>(dy, z, q, sums, (double)n * S, total, C / 4, S, dx);
+    bn_aff_bwd_kernel<<<blocks_for(total, 256), 256, 0, st>>>(dy, z, y, q, sums, (double)n * S, total, C / 4, S, dx);
     BX_LAUNCH_CHECK();
     return BX_OK;
 }

@@ -302,9 +302,8 @@ class MiniSpinNet(nn.Module):
         stats += [(m1, v1), (m2, v2)]
         f, desc, equi = ops.pool_forward(x, w)
         pool = dict(x=x, z1=z1, h=h, z2=z2, w=w, f=f, W1=W1, W2=W2,
-                    bn1=(m1.contiguous(), (1.0 / torch.sqrt(v1 + b1n.eps)).contiguous(), b1n.weight.detach().double().contiguous(),
-                         b1n.bias.detach().double().contiguous()),
-                    bn2=tuple(pad(t) for t in (m2, 1.0 / torch.sqrt(v2 + b2n.eps), b2n.weight.detach(), b2n.bias.detach())))
+                    bn1=(m1.contiguous(), (1.0 / torch.sqrt(v1 + b1n.eps)).contiguous(), b1n.weight.detach().double().contiguous()),
+                    bn2=tuple(pad(t) for t in (m2, 1.0 / torch.sqrt(v2 + b2n.eps), b2n.weight.detach())))
         return desc, equi.view(K, 32, self.ele_n, self.azi_n), dict(pnt=pnt, layers=layers, pool=pool, K=K)
 
     def _desc_backward_train(self, saved, ddesc, dequi):
@@ -316,12 +315,12 @@ class MiniSpinNet(nn.Module):
         g = {}
         P = saved["pool"]
         dx, dw = ops.pool_backward(P["x"], P["w"], P["f"], ddesc, dequi)
-        dz2, s2 = ops.bn_affine_backward(dw, P["z2"], *P["bn2"])
+        dz2, s2 = ops.bn_affine_backward(dw, P["z2"], P["w"], *P["bn2"])        # masked by the forward's ReLU output
         g["pool_layer.4.weight"], g["pool_layer.4.bias"] = s2[1, :1], s2[0, :1]
         g["pool_layer.3.weight"] = ops.cross_sums(P["h"], dz2)[:, :1].t()
         g["pool_layer.3.bias"] = ops.channel_sums(dz2)[0, :1]
         dh = ops.conv1x1_f64(dz2, P["W2"].t().contiguous())
-        dz1, s1 = ops.bn_affine_backward(dh, P["z1"], *P["bn1"])
+        dz1, s1 = ops.bn_affine_backward(dh, P["z1"], P["h"], *P["bn1"])
         g["pool_layer.1.weight"], g["pool_layer.1.bias"] = s1[1], s1[0]
         g["pool_layer.0.weight"] = ops.cross_sums(P["x"], dz1).t()
         g["pool_layer.0.bias"] = ops.channel_sums(dz1)[0]

@@ -1370,19 +1370,21 @@ def cross_sums(X, D):
     return out
 
 
-def bn_affine_backward(dy, z, mean, rstd, gamma, beta):
+def bn_affine_backward(dy, z, y, mean, rstd, gamma):
     """Affine batch-statistics BatchNorm + ReLU backward, float64 blocked: -> (dz like z, sums [2, C] = (sum dz', sum dz' x^)
-    = (dbeta, dgamma)), dz' = dy [gamma x^ + beta > 0], x^ = (z - mean) rstd."""
+    = (dbeta, dgamma)), dz' = dy [y > 0], x^ = (z - mean) rstd.  y is the forward's ReLU output (bn_apply's), so the
+    mask is the forward's bit for bit."""
     n, G, S = _ts_blocked("bn_affine_backward", z, "z")
     _ts_shape("bn_affine_backward", dy, z.shape, "dy")
-    for name, t in (("mean", mean), ("rstd", rstd), ("gamma", gamma), ("beta", beta)):
+    _ts_shape("bn_affine_backward", y, z.shape, "y")
+    for name, t in (("mean", mean), ("rstd", rstd), ("gamma", gamma)):
         _ts_shape("bn_affine_backward", t, (4 * G,), name)
     C = 4 * G
     partial = torch.empty(_splits() * 2 * C, dtype=F64, device=z.device)
     sums = torch.empty(2 * C, dtype=F64, device=z.device)
     dx = torch.empty_like(z)
-    _check(load_library().bx_td_bn_affine_backward(_dp(dy, F64, "dy"), _dp(z, F64, "z"), _dp(mean, F64, "mean"), _dp(rstd, F64, "rstd"),
-                                                   _dp(gamma, F64, "gamma"), _dp(beta, F64, "beta"), n, C, S, _dp(partial), _dp(sums),
+    _check(load_library().bx_td_bn_affine_backward(_dp(dy, F64, "dy"), _dp(z, F64, "z"), _dp(y, F64, "y"), _dp(mean, F64, "mean"),
+                                                   _dp(rstd, F64, "rstd"), _dp(gamma, F64, "gamma"), n, C, S, _dp(partial), _dp(sums),
                                                    _dp(dx), _stream()), "bx_td_bn_affine_backward")
     return dx, sums.view(2, C)
 

@@ -518,7 +518,7 @@ int bx_ts_conv_backward(const double *x, const double *dy, const double *w, int 
  * bx_td_cross_sums: out [Ca][Cb] = sum over (s, p) of X[s][a][p] D[s][b][p] (a 1x1 convolution's weight gradient);
  *   partial [BX_TS_SPLITS * Ca*Cb].
  * bx_td_bn_affine_backward: affine batch-statistics BatchNorm + ReLU backward (pool_layer.{1,4}): x^ = (z - mean) rstd,
- *   dz = dy [gamma x^ + beta > 0]; sums [2C] = (sum dz, sum dz x^) (= dbeta, dgamma), dx = gamma rstd (dz - m1 - x^ m2) with
+ *   dz = dy [y > 0] with y the forward's ReLU output (bn_apply's, so the mask is the forward's bit for bit); sums [2C] = (sum dz, sum dz x^) (= dbeta, dgamma), dx = gamma rstd (dz - m1 - x^ m2) with
  *   m1, m2 the sums over n*S.  partial [BX_TS_SPLITS * 2C].
  * bx_td_pool_forward / bx_td_pool_backward: attention pooling and the L2 normalisations (patch_embedder.py:86-90):
  *   x [K][8][140][4], w the attention [K][1][140][4] (channel 0) -> f [K][32] float64, desc [K][32] and equi [K][32][140]
@@ -536,8 +536,8 @@ int bx_td_pnt_backward(const float *inv, const unsigned char *arg, const double 
 int bx_td_conv1x1(const double *x, const double *w, const double *b, int n, int Cin, int Cout, int S, int accumulate, double *out,
                   void *stream);
 int bx_td_cross_sums(const double *X, const double *D, int n, int Ca, int Cb, int S, double *partial, double *out, void *stream);
-int bx_td_bn_affine_backward(const double *dy, const double *z, const double *mean, const double *rstd, const double *gamma,
-                             const double *beta, int n, int C, int S, double *partial, double *sums, double *dx, void *stream);
+int bx_td_bn_affine_backward(const double *dy, const double *z, const double *y, const double *mean, const double *rstd,
+                             const double *gamma, int n, int C, int S, double *partial, double *sums, double *dx, void *stream);
 int bx_td_pool_forward(const double *x, const double *w, int K, double *f, float *desc, float *equi, void *stream);
 int bx_td_pool_backward(const double *x, const double *w, const double *f, const float *ddesc, const float *dequi, int K, double *dx,
                         double *dw, void *stream);
