@@ -14,38 +14,17 @@
 // elevation range loads a zero, an azimuth index wraps.  The data gradient is the same cylindrical convolution with the taps
 // flipped and the weight transposed (the padding rule maps onto itself), one launch per input depth slice.
 //
+// The 1x1 convolution (fp32 and float64) and the BatchNorm + ReLU backward carry the bx_ts_ prefix: the Pose step runs
+// them too (its frozen descriptor's pool layer, CostNet's BatchNorms with gamma = 1).
+//
 // Determinism: every reduction over samples x positions goes through BX_TS_SPLITS per-block partials summed in index
 // order by one thread per output; no floating-point atomics.  Two runs on the same inputs are bit-identical.
-#include "bx_common.cuh"
+#include "bx_splits.cuh"
 
 namespace {
 
-constexpr int TD_THREADS = 256;
 constexpr int CYL_E = 7, CYL_A = 20, CYL_S = CYL_E * CYL_A;
 constexpr double NORM_EPS = 1e-12;        // F.normalize's eps
-
-template <int NV>
-__device__ __forceinline__ void block_sum(double (&v)[NV], double *sh) {
-    const int t = threadIdx.x;
-#pragma unroll
-    for (int i = 0; i < NV; ++i) sh[i * TD_THREADS + t] = v[i];
-    __syncthreads();
-    for (int s = TD_THREADS / 2; s > 0; s >>= 1) {
-        if (t < s) {
-#pragma unroll
-            for (int i = 0; i < NV; ++i) sh[i * TD_THREADS + t] += sh[i * TD_THREADS + t + s];
-        }
-        __syncthreads();
-    }
-}
-
-__global__ void sum_splits_kernel(const double *__restrict__ partial, int nsplit, long long L, double *__restrict__ out) {
-    const long long l = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-    if (l >= L) return;
-    double s = 0.0;
-    for (int i = 0; i < nsplit; ++i) s += partial[(size_t)i * L + l];
-    out[l] = s;
-}
 
 __device__ __forceinline__ void dmma16816(double (&d)[4], const double (&a)[8], const double (&b)[4]) {
     asm volatile(
@@ -291,20 +270,20 @@ __global__ void pnt_forward_kernel(const float *__restrict__ inv, const double *
 // Point layer backward, the sparse pass: the feature gradient goes to the selected sample of each (patch, channel, voxel),
 // masked by the ReLU (dz).  Per channel the sums sum dz, sum dz x^ (x^ = (y - mean) rstd) and sum dz inv (3).
 // grid (16, BX_TS_SPLITS); partial [split][16][5].
-__global__ void __launch_bounds__(TD_THREADS) pnt_bwd_sums_kernel(const float *__restrict__ inv, const unsigned char *__restrict__ arg,
+__global__ void __launch_bounds__(TS_THREADS) pnt_bwd_sums_kernel(const float *__restrict__ inv, const unsigned char *__restrict__ arg,
                                                                   const double *__restrict__ dfeat, const double *__restrict__ W,
                                                                   const double *__restrict__ b, const double *__restrict__ mean,
                                                                   const double *__restrict__ rstd, const double *__restrict__ scale,
                                                                   const double *__restrict__ shift, int K, int V, int nv,
                                                                   double *__restrict__ partial) {
-    __shared__ double sh[5 * TD_THREADS];
+    __shared__ double sh[5 * TS_THREADS];
     const int c = blockIdx.x, split = blockIdx.y, nsplit = gridDim.y;
     const long long R = (long long)K * V;
     const long long per = (R + nsplit - 1) / nsplit;
     const long long rb = min(R, per * split), re = min(R, rb + per);
     double acc[5] = {0, 0, 0, 0, 0};
     const double w0 = W[3 * c], w1 = W[3 * c + 1], w2 = W[3 * c + 2];
-    for (long long i = rb + threadIdx.x; i < re; i += TD_THREADS) {
+    for (long long i = rb + threadIdx.x; i < re; i += TS_THREADS) {
         const int k = (int)(i / V), v = (int)(i % V);
         const int a = arg[((size_t)k * 16 + c) * V + v];
         const float *q = inv + ((size_t)i * nv + a) * 3;
@@ -321,7 +300,7 @@ __global__ void __launch_bounds__(TD_THREADS) pnt_bwd_sums_kernel(const float *_
     }
     block_sum<5>(acc, sh);
     if (threadIdx.x == 0)
-        for (int j = 0; j < 5; ++j) partial[((size_t)split * 16 + c) * 5 + j] = sh[j * TD_THREADS];
+        for (int j = 0; j < 5; ++j) partial[((size_t)split * 16 + c) * 5 + j] = sh[j * TS_THREADS];
 }
 
 // Point layer backward, the closing step (one thread per channel): with S the split sums of pnt_bwd_sums_kernel and the
@@ -354,24 +333,27 @@ __global__ void pnt_bwd_final_kernel(const double *__restrict__ partial, int nsp
     out[6 * c + 5] = S[0];
 }
 
-// 1x1 convolution of a blocked float64 image: out[s][co][p] (+)= b[co] + sum_ci w[ci][co] x[s][ci][p]; Cin, Cout <= 32
-__global__ void conv1x1_f64_kernel(const double *__restrict__ x, const double *__restrict__ w, const double *__restrict__ b, int n, int Cin,
-                                   int Cout, int S, int accumulate, double *__restrict__ out) {
-    __shared__ double ws[32 * 32 + 32];
+// 1x1 convolution of a blocked image, fp32 or float64: out[s][co][p] (+)= b[co] + sum_ci w[ci][co] x[s][ci][p], the
+// accumulator starting at the bias (0 without one), then one fused multiply-add per input channel in channel order.
+// Cin, Cout <= 32, multiples of 4.
+template <typename T>
+__global__ void conv1x1_kernel(const T *__restrict__ x, const T *__restrict__ w, const T *__restrict__ b, int n, int Cin, int Cout,
+                               int S, int accumulate, T *__restrict__ out) {
+    __shared__ T ws[32 * 32 + 32];
     for (int i = threadIdx.x; i < Cin * Cout; i += blockDim.x) ws[i] = w[i];
-    for (int i = threadIdx.x; i < Cout; i += blockDim.x) ws[Cin * Cout + i] = b ? b[i] : 0.0;
+    for (int i = threadIdx.x; i < Cout; i += blockDim.x) ws[Cin * Cout + i] = b ? b[i] : T(0);
     __syncthreads();
     const long long t = (long long)blockIdx.x * blockDim.x + threadIdx.x;
     if (t >= (long long)n * S) return;
     const int s = (int)(t / S), p = (int)(t % S);
-    double acc[32];
+    T acc[32];
 #pragma unroll
-    for (int co = 0; co < 32; ++co) acc[co] = co < Cout ? ws[Cin * Cout + co] : 0.0;
+    for (int co = 0; co < 32; ++co) acc[co] = co < Cout ? ws[Cin * Cout + co] : T(0);
     const int Gi = Cin / 4, Go = Cout / 4;
     for (int g = 0; g < Gi; ++g) {
-        const double *xp = x + (((size_t)s * Gi + g) * S + p) * 4;
+        const T *xp = x + (((size_t)s * Gi + g) * S + p) * 4;
         for (int j = 0; j < 4; ++j) {
-            const double a = xp[j];
+            const T a = xp[j];
 #pragma unroll
             for (int co = 0; co < 32; ++co)
                 if (co < Cout) acc[co] = fma(ws[(4 * g + j) * Cout + co], a, acc[co]);
@@ -380,16 +362,16 @@ __global__ void conv1x1_f64_kernel(const double *__restrict__ x, const double *_
 #pragma unroll
     for (int co = 0; co < 32; ++co) {
         if (co >= Cout) break;
-        double *o = out + (((size_t)s * Go + co / 4) * S + p) * 4 + (co & 3);
+        T *o = out + (((size_t)s * Go + co / 4) * S + p) * 4 + (co & 3);
         *o = accumulate ? *o + acc[co] : acc[co];
     }
 }
 
 // sum over (s, p) of X[s][a][p] D[s][b][p] for every channel pair (the weight gradient of a 1x1 convolution); grid
 // (Ca/4 * Cb/4, BX_TS_SPLITS), each thread a 4 x 4 block of pairs; partial [split][Ca][Cb]
-__global__ void __launch_bounds__(TD_THREADS) cross_sums_kernel(const double *__restrict__ X, const double *__restrict__ D, int n, int Ca,
+__global__ void __launch_bounds__(TS_THREADS) cross_sums_kernel(const double *__restrict__ X, const double *__restrict__ D, int n, int Ca,
                                                                 int Cb, int S, double *__restrict__ partial) {
-    __shared__ double sh[16 * TD_THREADS];
+    __shared__ double sh[16 * TS_THREADS];
     const int Gb = Cb / 4, ga = blockIdx.x / Gb, gb = blockIdx.x % Gb, split = blockIdx.y, nsplit = gridDim.y;
     const long long R = (long long)n * S;
     const long long per = (R + nsplit - 1) / nsplit;
@@ -397,7 +379,7 @@ __global__ void __launch_bounds__(TD_THREADS) cross_sums_kernel(const double *__
     double acc[16];
 #pragma unroll
     for (int i = 0; i < 16; ++i) acc[i] = 0.0;
-    for (long long r = rb + threadIdx.x; r < re; r += TD_THREADS) {
+    for (long long r = rb + threadIdx.x; r < re; r += TS_THREADS) {
         const int s = (int)(r / S), p = (int)(r % S);
         const double *xp = X + (((size_t)s * (Ca / 4) + ga) * S + p) * 4;
         const double *dp = D + (((size_t)s * Gb + gb) * S + p) * 4;
@@ -413,22 +395,23 @@ __global__ void __launch_bounds__(TD_THREADS) cross_sums_kernel(const double *__
     if (threadIdx.x == 0)
         for (int i = 0; i < 4; ++i)
             for (int j = 0; j < 4; ++j)
-                partial[((size_t)split * Ca + 4 * ga + i) * Cb + 4 * gb + j] = sh[(4 * i + j) * TD_THREADS];
+                partial[((size_t)split * Ca + 4 * ga + i) * Cb + 4 * gb + j] = sh[(4 * i + j) * TS_THREADS];
 }
 
-// Affine batch-statistics BatchNorm + ReLU backward (the pool layer's, patch_embedder.py:32-39), float64, blocked:
-//   x^ = (z - mean) rstd, dz = dy [y > 0] with y the forward's ReLU output (bn_apply's z scale + shift: recomputing the
-//   sign as gamma x^ + beta rounds differently near the boundary, so the mask is read from y, as torch's threshold_backward).
+// Batch-statistics BatchNorm + ReLU backward, float64, blocked (patchnet.py:28,31 with affine = False: gamma = 1; the pool
+// layer's, patch_embedder.py:32-39):
+//   x^ = (z - mean) rstd, dz = dy [y > 0] with y the forward's ReLU output (bn_apply's fma(z, scale, shift): a mask
+//   recomputed from x^ can round to the other sign near the boundary, so it is read from y, as torch's threshold_backward).
 // First the per-channel sums sum dz, sum dz x^ (grid (C/4, BX_TS_SPLITS), partial [split][2C], then in split order),
 // then dx = gamma rstd (dz - m1 - x^ m2) with m1, m2 those sums over N (one thread per element).
-struct AffBN {
+struct BnBwd {
     const double *mean, *rstd, *gamma;
 };
 
-__global__ void __launch_bounds__(TD_THREADS) bn_aff_sums_kernel(const double *__restrict__ dy, const double *__restrict__ z,
-                                                                 const double *__restrict__ y, AffBN q, int n, int G, int S,
+__global__ void __launch_bounds__(TS_THREADS) bn_bwd_sums_kernel(const double *__restrict__ dy, const double *__restrict__ z,
+                                                                 const double *__restrict__ y, BnBwd q, int n, int G, int S,
                                                                  double *__restrict__ partial) {
-    __shared__ double sh[8 * TD_THREADS];
+    __shared__ double sh[8 * TS_THREADS];
     const int g = blockIdx.x, split = blockIdx.y, nsplit = gridDim.y;
     double v[8] = {0, 0, 0, 0, 0, 0, 0, 0};
     double mu[4], rs[4];
@@ -436,7 +419,7 @@ __global__ void __launch_bounds__(TD_THREADS) bn_aff_sums_kernel(const double *_
     for (int j = 0; j < 4; ++j) mu[j] = q.mean[4 * g + j], rs[j] = q.rstd[4 * g + j];
     for (int s = split; s < n; s += nsplit) {
         const size_t base = ((size_t)s * G + g) * S * 4;
-        for (int p = threadIdx.x; p < S; p += TD_THREADS) {
+        for (int p = threadIdx.x; p < S; p += TS_THREADS) {
 #pragma unroll
             for (int j = 0; j < 4; ++j) {
                 const double xh = (z[base + 4 * p + j] - mu[j]) * rs[j];
@@ -452,14 +435,14 @@ __global__ void __launch_bounds__(TD_THREADS) bn_aff_sums_kernel(const double *_
         double *o = partial + (size_t)split * 2 * C;
 #pragma unroll
         for (int j = 0; j < 4; ++j) {
-            o[4 * g + j] = sh[j * TD_THREADS];
-            o[C + 4 * g + j] = sh[(4 + j) * TD_THREADS];
+            o[4 * g + j] = sh[j * TS_THREADS];
+            o[C + 4 * g + j] = sh[(4 + j) * TS_THREADS];
         }
     }
 }
 
-__global__ void bn_aff_bwd_kernel(const double *__restrict__ dy, const double *__restrict__ z, const double *__restrict__ y, AffBN q,
-                                  const double *__restrict__ sums, double N, long long total, int G, int S, double *__restrict__ dx) {
+__global__ void bn_bwd_kernel(const double *__restrict__ dy, const double *__restrict__ z, const double *__restrict__ y, BnBwd q,
+                              const double *__restrict__ sums, double N, long long total, int G, int S, double *__restrict__ dx) {
     const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= total) return;
     const int c = (int)((i / (4LL * S)) % G) * 4 + (int)(i & 3);
@@ -575,8 +558,6 @@ __global__ void equi_match_bwd_kernel(const float *__restrict__ s, const float *
     dt[i] = (float)at;
 }
 
-inline int blocks_for(long long n, int t) { return (int)((n + t - 1) / t); }
-
 }  // namespace
 
 static bool cyl_sizes_ok(int n, int Kc, int Nc, int Din) {
@@ -635,45 +616,55 @@ BX_API int bx_td_pnt_backward(const float *inv, const unsigned char *arg, const 
     BX_REQUIRE(inv && arg && dfeat && W && b && mean && rstd && gamma && scale && shift && mo9 && partial && out,
                "bx_td_pnt_backward: null pointer");
     cudaStream_t st = bx_stream(stream);
-    pnt_bwd_sums_kernel<<<dim3(16, BX_TS_SPLITS), TD_THREADS, 0, st>>>(inv, arg, dfeat, W, b, mean, rstd, scale, shift, K, V, nv, partial);
+    pnt_bwd_sums_kernel<<<dim3(16, BX_TS_SPLITS), TS_THREADS, 0, st>>>(inv, arg, dfeat, W, b, mean, rstd, scale, shift, K, V, nv, partial);
     BX_LAUNCH_CHECK();
     pnt_bwd_final_kernel<<<1, 32, 0, st>>>(partial, BX_TS_SPLITS, mo9, (double)K * V * nv, W, b, mean, rstd, gamma, out);
     BX_LAUNCH_CHECK();
     return BX_OK;
 }
 
-BX_API int bx_td_conv1x1(const double *x, const double *w, const double *b, int n, int Cin, int Cout, int S, int accumulate, double *out,
-                         void *stream) {
-    BX_REQUIRE(n >= 1 && Cin >= 4 && Cin % 4 == 0 && Cin <= 32 && Cout >= 4 && Cout % 4 == 0 && Cout <= 32 && S >= 1, "bx_td_conv1x1: bad sizes");
-    BX_REQUIRE(x && w && out, "bx_td_conv1x1: null pointer");
-    conv1x1_f64_kernel<<<blocks_for((long long)n * S, 128), 128, 0, bx_stream(stream)>>>(x, w, b, n, Cin, Cout, S, accumulate, out);
+template <typename T>
+static int conv1x1(const T *x, const T *w, const T *b, int n, int Cin, int Cout, int S, int accumulate, T *out, void *stream) {
+    BX_REQUIRE(n >= 1 && Cin >= 4 && Cin % 4 == 0 && Cin <= 32 && Cout >= 4 && Cout % 4 == 0 && Cout <= 32 && S >= 1, "bx_ts_conv1x1: bad sizes");
+    BX_REQUIRE(x && w && out, "bx_ts_conv1x1: null pointer");
+    conv1x1_kernel<T><<<blocks_for((long long)n * S, 128), 128, 0, bx_stream(stream)>>>(x, w, b, n, Cin, Cout, S, accumulate, out);
     BX_LAUNCH_CHECK();
     return BX_OK;
+}
+
+BX_API int bx_ts_conv1x1(const float *x, const float *w, const float *b, int n, int Cin, int Cout, int S, int accumulate, float *out,
+                         void *stream) {
+    return conv1x1<float>(x, w, b, n, Cin, Cout, S, accumulate, out, stream);
+}
+
+BX_API int bx_ts_conv1x1_f64(const double *x, const double *w, const double *b, int n, int Cin, int Cout, int S, int accumulate, double *out,
+                             void *stream) {
+    return conv1x1<double>(x, w, b, n, Cin, Cout, S, accumulate, out, stream);
 }
 
 BX_API int bx_td_cross_sums(const double *X, const double *D, int n, int Ca, int Cb, int S, double *partial, double *out, void *stream) {
     BX_REQUIRE(n >= 1 && Ca >= 4 && Ca % 4 == 0 && Cb >= 4 && Cb % 4 == 0 && S >= 1, "bx_td_cross_sums: bad sizes");
     BX_REQUIRE(X && D && partial && out, "bx_td_cross_sums: null pointer");
     cudaStream_t st = bx_stream(stream);
-    cross_sums_kernel<<<dim3((Ca / 4) * (Cb / 4), BX_TS_SPLITS), TD_THREADS, 0, st>>>(X, D, n, Ca, Cb, S, partial);
+    cross_sums_kernel<<<dim3((Ca / 4) * (Cb / 4), BX_TS_SPLITS), TS_THREADS, 0, st>>>(X, D, n, Ca, Cb, S, partial);
     BX_LAUNCH_CHECK();
     sum_splits_kernel<<<blocks_for((long long)Ca * Cb, 256), 256, 0, st>>>(partial, BX_TS_SPLITS, (long long)Ca * Cb, out);
     BX_LAUNCH_CHECK();
     return BX_OK;
 }
 
-BX_API int bx_td_bn_affine_backward(const double *dy, const double *z, const double *y, const double *mean, const double *rstd,
-                                    const double *gamma, int n, int C, int S, double *partial, double *sums, double *dx, void *stream) {
-    BX_REQUIRE(n >= 1 && C >= 4 && C % 4 == 0 && S >= 1, "bx_td_bn_affine_backward: bad sizes");
-    BX_REQUIRE(dy && z && y && mean && rstd && gamma && partial && sums && dx, "bx_td_bn_affine_backward: null pointer");
+BX_API int bx_ts_bn_backward(const double *dy, const double *z, const double *y, const double *mean, const double *rstd,
+                             const double *gamma, int n, int C, int S, double *partial, double *sums, double *dx, void *stream) {
+    BX_REQUIRE(n >= 1 && C >= 4 && C % 4 == 0 && S >= 1, "bx_ts_bn_backward: bad sizes");
+    BX_REQUIRE(dy && z && y && mean && rstd && gamma && partial && sums && dx, "bx_ts_bn_backward: null pointer");
     cudaStream_t st = bx_stream(stream);
-    AffBN q{mean, rstd, gamma};
-    bn_aff_sums_kernel<<<dim3(C / 4, BX_TS_SPLITS), TD_THREADS, 0, st>>>(dy, z, y, q, n, C / 4, S, partial);
+    BnBwd q{mean, rstd, gamma};
+    bn_bwd_sums_kernel<<<dim3(C / 4, BX_TS_SPLITS), TS_THREADS, 0, st>>>(dy, z, y, q, n, C / 4, S, partial);
     BX_LAUNCH_CHECK();
     sum_splits_kernel<<<blocks_for(2 * C, 128), 128, 0, st>>>(partial, BX_TS_SPLITS, 2 * C, sums);
     BX_LAUNCH_CHECK();
     const long long total = (long long)n * C * S;
-    bn_aff_bwd_kernel<<<blocks_for(total, 256), 256, 0, st>>>(dy, z, y, q, sums, (double)n * S, total, C / 4, S, dx);
+    bn_bwd_kernel<<<blocks_for(total, 256), 256, 0, st>>>(dy, z, y, q, sums, (double)n * S, total, C / 4, S, dx);
     BX_LAUNCH_CHECK();
     return BX_OK;
 }

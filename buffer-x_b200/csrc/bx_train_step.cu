@@ -9,68 +9,30 @@
 //   most of its input (dx = (dz - mean dz - x^ mean dz x^) / sigma); an fp32 evaluation of the chain (3xTF32 forward or
 //   plain fp32 on CUDA cores alike) carries that cancellation into the weight gradients of the lower layers, a float64 one
 //   does not.
+// The channel sums and bn_apply serve the Desc step (bx_train_desc.cu) too; the BatchNorm backward and the 1x1
+// convolution that both steps run are in bx_train_desc.cu, beside the pool layer's other kernels.
 //
-// Determinism: every reduction over samples x positions goes through a fixed number of per-block partials (BX_TS_SPLITS)
-// that are summed in index order by one thread per output; no floating-point atomics.  Two runs on the same inputs give
-// bit-identical statistics and gradients.
-#include "bx_common.cuh"
+// Determinism: every reduction over samples x positions goes through the fixed-order split reductions of bx_splits.cuh;
+// two runs on the same inputs give bit-identical statistics and gradients.
+#include "bx_splits.cuh"
 
 namespace {
 
-constexpr int TS_THREADS = 256;
-
-// in-block fixed-order tree reduction of NV doubles per thread; thread 0 ends with the block totals in sh[0..NV)
-template <int NV>
-__device__ __forceinline__ void block_sum(double (&v)[NV], double *sh) {
-    const int t = threadIdx.x;
-#pragma unroll
-    for (int i = 0; i < NV; ++i) sh[i * TS_THREADS + t] = v[i];
-    __syncthreads();
-    for (int s = TS_THREADS / 2; s > 0; s >>= 1) {
-        if (t < s) {
-#pragma unroll
-            for (int i = 0; i < NV; ++i) sh[i * TS_THREADS + t] += sh[i * TS_THREADS + t + s];
-        }
-        __syncthreads();
-    }
-}
-
-// MODE 0: per-channel sum x and sum x^2 of a blocked image.
-// MODE 1: the BatchNorm backward sums: dz = dy where x^ = z * scale + shift > 0 (else 0); sum dz and sum dz * x^.
-// grid (C/4, BX_TS_SPLITS); partial [split][2C]: the first sums at [c], the second at [C + c].
-template <int MODE, typename T>
-__global__ void __launch_bounds__(TS_THREADS) chan_sums_kernel(const T *__restrict__ x, const T *__restrict__ z,
-                                                               const T *__restrict__ scale, const T *__restrict__ shift,
-                                                               int n, int G, int S, double *__restrict__ partial) {
+// per-channel sum x and sum x^2 of a blocked image; grid (C/4, BX_TS_SPLITS); partial [split][2C]: sum x at [c], sum x^2
+// at [C + c]
+template <typename T>
+__global__ void __launch_bounds__(TS_THREADS) chan_sums_kernel(const T *__restrict__ x, int n, int G, int S, double *__restrict__ partial) {
     __shared__ double sh[8 * TS_THREADS];
     const int g = blockIdx.x, split = blockIdx.y, nsplit = gridDim.y;
     double v[8] = {0, 0, 0, 0, 0, 0, 0, 0};
-    T scv[4] = {0, 0, 0, 0}, sfv[4] = {0, 0, 0, 0};
-    if (MODE == 1)
-        for (int j = 0; j < 4; ++j) scv[j] = scale[4 * g + j], sfv[j] = shift[4 * g + j];
     for (int s = split; s < n; s += nsplit) {
         const T *xs = x + ((size_t)s * G + g) * S * 4;
-        const T *zs = MODE == 1 ? z + ((size_t)s * G + g) * S * 4 : nullptr;
         for (int p = threadIdx.x; p < S; p += TS_THREADS) {
-            T av[4], zv[4];
 #pragma unroll
-            for (int j = 0; j < 4; ++j) av[j] = xs[4 * p + j];
-            if (MODE == 0) {
-#pragma unroll
-                for (int j = 0; j < 4; ++j) {
-                    v[j] += (double)av[j];
-                    v[4 + j] += (double)av[j] * (double)av[j];
-                }
-            } else {
-#pragma unroll
-                for (int j = 0; j < 4; ++j) zv[j] = zs[4 * p + j];
-#pragma unroll
-                for (int j = 0; j < 4; ++j) {
-                    const T xh = zv[j] * scv[j] + sfv[j];
-                    const T dz = xh > T(0) ? av[j] : T(0);
-                    v[j] += (double)dz;
-                    v[4 + j] += (double)dz * (double)xh;
-                }
+            for (int j = 0; j < 4; ++j) {
+                const double a = (double)xs[4 * p + j];
+                v[j] += a;
+                v[4 + j] += a * a;
             }
         }
     }
@@ -100,16 +62,6 @@ __global__ void __launch_bounds__(TS_THREADS) moments3_kernel(const float *__res
         for (int i = 0; i < 9; ++i) partial[(size_t)blockIdx.x * 9 + i] = sh[i * TS_THREADS];
 }
 
-// out[l] = sum over splits of partial[split][l], in split order, in float64
-template <typename T>
-__global__ void sum_splits_kernel(const T *__restrict__ partial, int nsplit, long long L, double *__restrict__ out) {
-    const long long l = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-    if (l >= L) return;
-    double s = 0.0;
-    for (int i = 0; i < nsplit; ++i) s += (double)partial[(size_t)i * L + l];
-    out[l] = s;
-}
-
 // y = z * scale[c] + shift[c] (ReLU if relu), blocked, one element per thread; y may alias z
 template <typename T>
 __global__ void bn_apply_kernel(const T *__restrict__ z, const T *__restrict__ scale, const T *__restrict__ shift, long long total,
@@ -120,43 +72,6 @@ __global__ void bn_apply_kernel(const T *__restrict__ z, const T *__restrict__ s
     T r = z[i] * scale[c] + shift[c];
     if (relu) r = r > T(0) ? r : T(0);
     y[i] = r;
-}
-
-// batch-statistics BatchNorm backward through the ReLU (affine = False, rstd = scale), float64:
-//   x^ = z * scale + shift, dz = dy [x^ > 0], dx = (dz - m1 - x^ m2) * scale with m1 = mean dz, m2 = mean dz x^.  dx may alias dy.
-__global__ void bn_bwd_kernel(const double *__restrict__ dy, const double *__restrict__ z, const double *__restrict__ scale,
-                              const double *__restrict__ shift, const double *__restrict__ m1, const double *__restrict__ m2,
-                              long long total, int G, int S, double *__restrict__ dx) {
-    const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= total) return;
-    const int c = (int)((i / (4LL * S)) % G) * 4 + (int)(i & 3);
-    const double xh = z[i] * scale[c] + shift[c];
-    const double dz = xh > 0.0 ? dy[i] : 0.0;
-    dx[i] = (dz - m1[c] - xh * m2[c]) * scale[c];
-}
-
-// 1x1 convolution of a blocked image: out[s][co][p] = b[co] + sum_ci w[ci][co] x[s][ci][p]; Cin <= 32, Cout4 <= 16
-// (Cout4 = Cout rounded up to 4; the padding channels get w = b = 0 from the caller)
-__global__ void conv1x1_kernel(const float *__restrict__ x, const float *__restrict__ w, const float *__restrict__ b, int n,
-                               int Cin, int Cout4, int S, float *__restrict__ out) {
-    __shared__ float ws[32 * 16 + 16];
-    for (int i = threadIdx.x; i < Cin * Cout4; i += blockDim.x) ws[i] = w[i];
-    for (int i = threadIdx.x; i < Cout4; i += blockDim.x) ws[Cin * Cout4 + i] = b[i];
-    __syncthreads();
-    const long long t = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-    if (t >= (long long)n * S) return;
-    const int s = (int)(t / S), p = (int)(t % S);
-    float acc[16];
-    for (int co = 0; co < Cout4; ++co) acc[co] = ws[Cin * Cout4 + co];
-    const int Gi = Cin / 4, Go = Cout4 / 4;
-    for (int g = 0; g < Gi; ++g) {
-        const float4 a = reinterpret_cast<const float4 *>(x)[((size_t)s * Gi + g) * S + p];
-        const float av[4] = {a.x, a.y, a.z, a.w};
-        for (int j = 0; j < 4; ++j)
-            for (int co = 0; co < Cout4; ++co) acc[co] = fmaf(ws[(4 * g + j) * Cout4 + co], av[j], acc[co]);
-    }
-    for (int g = 0; g < Go; ++g)
-        reinterpret_cast<float4 *>(out)[((size_t)s * Go + g) * S + p] = make_float4(acc[4 * g], acc[4 * g + 1], acc[4 * g + 2], acc[4 * g + 3]);
 }
 
 // cost volume of the reference's CostVolume.forward (models/BUFFERX.py:52-64) over elevation rows 1..5 of the full maps:
@@ -352,35 +267,28 @@ __global__ void __launch_bounds__(TS_THREADS) wgrad_kernel(const double *__restr
     }
 }
 
-inline int blocks_for(long long n, int t) { return (int)((n + t - 1) / t); }
-
 }  // namespace
 
 BX_API int bx_ts_splits(void) { return BX_TS_SPLITS; }
 
 template <typename T>
-static int channel_sums(const T *x, const T *z, const T *scale, const T *shift, int n, int C, int S, double *partial, double *out,
-                        void *stream) {
+static int channel_sums(const T *x, int n, int C, int S, double *partial, double *out, void *stream) {
     BX_REQUIRE(n >= 1 && C >= 4 && C % 4 == 0 && S >= 1, "bx_ts_channel_sums: bad sizes");
     BX_REQUIRE(x && partial && out, "bx_ts_channel_sums: null pointer");
-    BX_REQUIRE((z == nullptr) == (scale == nullptr) && (z == nullptr) == (shift == nullptr), "bx_ts_channel_sums: z, scale, shift go together");
     cudaStream_t st = bx_stream(stream);
-    dim3 grid(C / 4, BX_TS_SPLITS);
-    if (z) chan_sums_kernel<1, T><<<grid, TS_THREADS, 0, st>>>(x, z, scale, shift, n, C / 4, S, partial);
-    else chan_sums_kernel<0, T><<<grid, TS_THREADS, 0, st>>>(x, nullptr, nullptr, nullptr, n, C / 4, S, partial);
+    chan_sums_kernel<T><<<dim3(C / 4, BX_TS_SPLITS), TS_THREADS, 0, st>>>(x, n, C / 4, S, partial);
     BX_LAUNCH_CHECK();
-    sum_splits_kernel<double><<<blocks_for(2 * C, 128), 128, 0, st>>>(partial, BX_TS_SPLITS, 2 * C, out);
+    sum_splits_kernel<<<blocks_for(2 * C, 128), 128, 0, st>>>(partial, BX_TS_SPLITS, 2 * C, out);
     BX_LAUNCH_CHECK();
     return BX_OK;
 }
 
 BX_API int bx_ts_channel_sums(const float *x, int n, int C, int S, double *partial, double *out, void *stream) {
-    return channel_sums<float>(x, nullptr, nullptr, nullptr, n, C, S, partial, out, stream);
+    return channel_sums<float>(x, n, C, S, partial, out, stream);
 }
 
-BX_API int bx_ts_channel_sums_f64(const double *x, const double *z, const double *scale, const double *shift, int n, int C, int S,
-                                  double *partial, double *out, void *stream) {
-    return channel_sums<double>(x, z, scale, shift, n, C, S, partial, out, stream);
+BX_API int bx_ts_channel_sums_f64(const double *x, int n, int C, int S, double *partial, double *out, void *stream) {
+    return channel_sums<double>(x, n, C, S, partial, out, stream);
 }
 
 BX_API int bx_ts_moments3(const float *v3, long long R, double *partial, double *out9, void *stream) {
@@ -388,7 +296,7 @@ BX_API int bx_ts_moments3(const float *v3, long long R, double *partial, double 
     cudaStream_t st = bx_stream(stream);
     moments3_kernel<<<BX_TS_SPLITS, TS_THREADS, 0, st>>>(v3, R, partial);
     BX_LAUNCH_CHECK();
-    sum_splits_kernel<double><<<1, 32, 0, st>>>(partial, BX_TS_SPLITS, 9, out9);
+    sum_splits_kernel<<<1, 32, 0, st>>>(partial, BX_TS_SPLITS, 9, out9);
     BX_LAUNCH_CHECK();
     return BX_OK;
 }
@@ -409,23 +317,6 @@ BX_API int bx_ts_bn_apply(const float *z, const float *scale, const float *shift
 BX_API int bx_ts_bn_apply_f64(const double *z, const double *scale, const double *shift, int n, int C, int S, int relu, double *y,
                               void *stream) {
     return bn_apply<double>(z, scale, shift, n, C, S, relu, y, stream);
-}
-
-BX_API int bx_ts_bn_backward(const double *dy, const double *z, const double *scale, const double *shift, const double *m1,
-                             const double *m2, int n, int C, int S, double *dx, void *stream) {
-    BX_REQUIRE(n >= 1 && C % 4 == 0 && S >= 1 && dy && z && scale && shift && m1 && m2 && dx, "bx_ts_bn_backward: bad arguments");
-    const long long total = (long long)n * C * S;
-    bn_bwd_kernel<<<blocks_for(total, 256), 256, 0, bx_stream(stream)>>>(dy, z, scale, shift, m1, m2, total, C / 4, S, dx);
-    BX_LAUNCH_CHECK();
-    return BX_OK;
-}
-
-BX_API int bx_ts_conv1x1(const float *x, const float *w, const float *b, int n, int Cin, int Cout4, int S, float *out, void *stream) {
-    BX_REQUIRE(n >= 1 && Cin % 4 == 0 && Cin <= 32 && Cout4 % 4 == 0 && Cout4 >= 4 && Cout4 <= 16 && S >= 1, "bx_ts_conv1x1: bad sizes");
-    BX_REQUIRE(x && w && b && out, "bx_ts_conv1x1: null pointer");
-    conv1x1_kernel<<<blocks_for((long long)n * S, 128), 128, 0, bx_stream(stream)>>>(x, w, b, n, Cin, Cout4, S, out);
-    BX_LAUNCH_CHECK();
-    return BX_OK;
 }
 
 BX_API int bx_ts_costvol(const float *equi_s, const float *equi_t, int M, double *cv, void *stream) {
@@ -468,7 +359,7 @@ BX_API int bx_ts_conv_backward(const double *x, const double *dy, const double *
     wgrad_kernel<<<wg, TS_THREADS, 0, st>>>(x, dy, n, Cin, Cout, q, wpartial);
     BX_LAUNCH_CHECK();
     const long long L = (long long)T * Cin * Cout;
-    sum_splits_kernel<double><<<blocks_for(L, 256), 256, 0, st>>>(wpartial, BX_TS_SPLITS, L, dw);
+    sum_splits_kernel<<<blocks_for(L, 256), 256, 0, st>>>(wpartial, BX_TS_SPLITS, L, dw);
     BX_LAUNCH_CHECK();
     if (dx) {
         dim3 dg(blocks_for((long long)n * D * H * W, 64), Cin / 32);

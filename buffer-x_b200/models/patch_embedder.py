@@ -114,14 +114,9 @@ class MiniSpinNet(nn.Module):
             )
         return self._prep
 
-    def forward(self, pts, kpts, des_r, is_aligned_to_global_z, z_axis=None, is_aug=False, perm=None, debug=False, aug_angles=None):
-        """pts [1,N,3], kpts [1,K,3] CUDA f32; des_r python float or 1-element CUDA tensor.
-        ``perm`` (optional int32 [N]) replaces the host draw of the reference (patch_embedder.py:96).
-        ``is_aug``: SO(2) augmentation of the normalised patches and rand_axis (patch_embedder.py:54-67), one z-rotation per
-        patch; the angles are drawn from NumPy's global RNG after the permutation, like the reference, unless ``aug_angles``
-        ([K] fp32) are given.  ``aug_rotation`` is then the [K,3,3] rotations (None without augmentation)."""
-        if z_axis is not None:
-            raise NotImplementedError("an externally supplied z_axis is a training-time option outside the forward built here")
+    def _front(self, pts, kpts, des_r, is_aligned_to_global_z, is_aug, perm, aug_angles, want_idx=False):
+        """The front end every forward shares (patch_embedder.py:44-67): the permutation, patch selection, local reference
+        frames and, with ``is_aug``, the SO(2) augmentation -> (prep, patches, idx, delta, R, rand_axis, aug_R)."""
         pts = pts[0].contiguous()
         kpts = kpts[0].contiguous()
         dev = pts.device
@@ -133,19 +128,46 @@ class MiniSpinNet(nn.Module):
             perm = torch.from_numpy(np.ascontiguousarray(perm, dtype=np.int32)).to(dev, non_blocking=True)
         prep = self.prepared(dev)
         pts4 = ops.permute_cloud(pts, perm)
-        patches, idx = ops.select_patches(pts4, kpts, des_r, self.patch_sample, want_idx=debug)
+        patches, idx = ops.select_patches(pts4, kpts, des_r, self.patch_sample, want_idx=want_idx)
         delta, R, rand_axis = ops.lrf(patches, des_r, bool(is_aligned_to_global_z))
         aug_R = None
         if is_aug:
             if aug_angles is None:
-                # the reference draws angles = r * 2 * pi in fp64 and casts them to fp32
+                # the reference draws angles = r * 2 * pi in fp64 (after the permutation) and casts them to fp32
                 aug_angles = (np.random.random([kpts.shape[0], 1]) * 2 * np.pi)[:, 0].astype(np.float32)
             ang = torch.as_tensor(np.ascontiguousarray(aug_angles, dtype=np.float32)).to(dev, non_blocking=True)
             aug_R = ops.so2_augment(delta, rand_axis, ang)
+        return prep, patches, idx, delta, R, rand_axis, aug_R
+
+    def _pnt_batch_stats(self, inv, stats):
+        """The point layer's batch statistics over every sample of inv [..., 3] (zero slots included) from the float64
+        moments of its inputs (it is linear: mean = W E[x] + b, var = diag(W Cov(x) W^T)); updates its running statistics
+        once and appends (mean, var) to ``stats`` -> (mean, var, W [16, 3], b [16] float64, moments [9])."""
+        conv, bn = self.pnt_layer[0], self.pnt_layer[1]
+        R_n = inv.numel() // 3
+        mo = ops.moments3(inv)
+        Wp = conv.weight.detach().double().view(16, 3).contiguous()
+        bp = conv.bias.detach().double().contiguous()
+        mean, var = pnt_stats_from_moments(mo / R_n, Wp, bp)
+        pn.bn_batch_stats(torch.stack([mean * R_n, (var + mean * mean) * R_n]), R_n, bn)
+        if stats is not None:
+            stats.append((mean, var))
+        return mean, var, Wp, bp, mo
+
+    def forward(self, pts, kpts, des_r, is_aligned_to_global_z, z_axis=None, is_aug=False, perm=None, debug=False, aug_angles=None):
+        """pts [1,N,3], kpts [1,K,3] CUDA f32; des_r python float or 1-element CUDA tensor.
+        ``perm`` (optional int32 [N]) replaces the host draw of the reference (patch_embedder.py:96).
+        ``is_aug``: SO(2) augmentation of the normalised patches and rand_axis (patch_embedder.py:54-67), one z-rotation per
+        patch; the angles are drawn from NumPy's global RNG after the permutation, like the reference, unless ``aug_angles``
+        ([K] fp32) are given.  ``aug_rotation`` is then the [K,3,3] rotations (None without augmentation)."""
+        if z_axis is not None:
+            raise NotImplementedError("an externally supplied z_axis is a training-time option outside the forward built here")
+        prep, patches, idx, delta, R, rand_axis, aug_R = self._front(pts, kpts, des_r, is_aligned_to_global_z, is_aug, perm, aug_angles,
+                                                                     want_idx=debug)
         res = ops.spt_pnt(delta, prep["voxels"], prep["rot"], self.delta / self.rad_n, self.voxel_sample, prep["w_pnt"],
                           prep["b_pnt"], self.azi_n, debug=debug)
         feat = res[0] if debug else res                                  # [K,4,V,4] channel-blocked
-        K = kpts.shape[0]
+        K = delta.shape[0]
         x, _ = self.conv_net(feat)                                       # [K,8,140,4] channel-blocked
         desc, equi = ops.pool_desc(x, prep["w1"], prep["b1"], prep["w2"], prep["b2"], channels_last=True)
         out = {"desc": desc, "equi": equi, "rand_axis": rand_axis, "R": R, "patches": delta, "aug_rotation": aug_R}
@@ -161,34 +183,12 @@ class MiniSpinNet(nn.Module):
         float64 moments of its de-rotated 3-vectors (it is linear: mean = W E[x] + b, var = diag(W Cov(x) W^T)); the pool
         layer's from its 1x1 convolutions over K x 140 positions.  ``stats``: optional list receiving (batch mean, batch
         variance) of every BatchNorm in module order (pnt_layer, conv_net, pool_layer), float64.  Returns ``forward``'s dict."""
-        pts = pts[0].contiguous()
-        kpts = kpts[0].contiguous()
-        dev = pts.device
-        N = pts.shape[0]
-        if perm is None:
-            perm = np.random.choice(N, N, replace=False)
-        if not isinstance(perm, torch.Tensor):
-            perm = torch.from_numpy(np.ascontiguousarray(perm, dtype=np.int32)).to(dev, non_blocking=True)
-        prep = self.prepared(dev)
-        pts4 = ops.permute_cloud(pts, perm)
-        patches, _ = ops.select_patches(pts4, kpts, des_r, self.patch_sample)
-        delta, R, rand_axis = ops.lrf(patches, des_r, bool(is_aligned_to_global_z))
-        aug_R = None
-        if is_aug:
-            if aug_angles is None:
-                aug_angles = (np.random.random([kpts.shape[0], 1]) * 2 * np.pi)[:, 0].astype(np.float32)
-            ang = torch.as_tensor(np.ascontiguousarray(aug_angles, dtype=np.float32)).to(dev, non_blocking=True)
-            aug_R = ops.so2_augment(delta, rand_axis, ang)
+        prep, _, _, delta, R, rand_axis, aug_R = self._front(pts, kpts, des_r, is_aligned_to_global_z, is_aug, perm, aug_angles)
+        dev = delta.device
         args = (delta, prep["voxels"], prep["rot"], self.delta / self.rad_n, self.voxel_sample)
         _, _, inv = ops.spt_pnt(*args, prep["w_pnt"], prep["b_pnt"], self.azi_n, debug=True)   # the samples the point layer sees
-        # point layer: batch statistics of the linear 3 -> 16 map from the moments of its inputs
+        mean, var, _, _, _ = self._pnt_batch_stats(inv, stats)
         conv, bn = self.pnt_layer[0], self.pnt_layer[1]
-        R_n = inv.numel() // 3
-        mean, var = pnt_stats_from_moments(ops.moments3(inv) / R_n, conv.weight.detach().double().view(16, 3),
-                                           conv.bias.detach().double())
-        pn.bn_batch_stats(torch.stack([mean * R_n, (var + mean * mean) * R_n]), R_n, bn)
-        if stats is not None:
-            stats.append((mean, var))
         Wt, b = pn.fold_conv_bn(conv.weight, conv.bias, mean, var, bn.weight, bn.bias, bn.eps)
         feat = ops.spt_pnt(*args, Wt[0].t().contiguous().to(dev), b.to(dev), self.azi_n)
         x = self.conv_net.forward_train(feat, stats)                      # [K,8,140,4]
@@ -218,18 +218,7 @@ class MiniSpinNet(nn.Module):
         """MiniSpinNet.forward of the Desc training stage (patch_embedder.py:44-90 under model.train(), no augmentation): the
         patches, frames and SPT of ``forward``, then ``train_desc``.  ``desc`` and ``equi`` carry a grad_fn into the
         parameters that require grad.  Returns ``forward``'s dict."""
-        pts = pts[0].contiguous()
-        kpts = kpts[0].contiguous()
-        dev = pts.device
-        N = pts.shape[0]
-        if perm is None:
-            perm = np.random.choice(N, N, replace=False)
-        if not isinstance(perm, torch.Tensor):
-            perm = torch.from_numpy(np.ascontiguousarray(perm, dtype=np.int32)).to(dev, non_blocking=True)
-        prep = self.prepared(dev)
-        pts4 = ops.permute_cloud(pts, perm)
-        patches, _ = ops.select_patches(pts4, kpts, des_r, self.patch_sample)
-        delta, R, rand_axis = ops.lrf(patches, des_r, bool(is_aligned_to_global_z))
+        prep, _, _, delta, R, rand_axis, _ = self._front(pts, kpts, des_r, is_aligned_to_global_z, False, perm, None)
         _, _, inv = ops.spt_pnt(delta, prep["voxels"], prep["rot"], self.delta / self.rad_n, self.voxel_sample, prep["w_pnt"],
                                 prep["b_pnt"], self.azi_n, debug=True)
         desc, equi = self.train_desc(inv, stats)
@@ -247,16 +236,9 @@ class MiniSpinNet(nn.Module):
     def _desc_forward_train(self, inv, stats):
         F64 = torch.float64
         dev = inv.device
-        K, V, nv = inv.shape[0], inv.shape[1], inv.shape[2]
-        # point layer: batch statistics of the linear 3 -> 16 map from the float64 moments of its inputs
-        conv, bn = self.pnt_layer[0], self.pnt_layer[1]
-        R_n = K * V * nv
-        mo = ops.moments3(inv)
-        Wp = conv.weight.detach().double().view(16, 3).contiguous()
-        bp = conv.bias.detach().double().contiguous()
-        mean, var = pnt_stats_from_moments(mo / R_n, Wp, bp)
-        pn.bn_batch_stats(torch.stack([mean * R_n, (var + mean * mean) * R_n]), R_n, bn)
-        stats.append((mean, var))
+        K = inv.shape[0]
+        mean, var, Wp, bp, mo = self._pnt_batch_stats(inv, stats)
+        bn = self.pnt_layer[1]
         scale, shift = pn.bn_scale_shift(mean, var, bn, F64)
         feat, arg = ops.pnt_forward(inv, Wp, bp, scale, shift)
         pnt = dict(inv=inv, arg=arg, W=Wp, b=bp, mean=mean.contiguous(), rstd=(1.0 / torch.sqrt(var + bn.eps)).contiguous(),
@@ -274,9 +256,9 @@ class MiniSpinNet(nn.Module):
             if bi is not None:
                 m, v = pn.bn_batch_stats(ops.channel_sums(z), N, net.ops[bi])
                 sc, sh = pn.bn_scale_shift(m, v, net.ops[bi], F64)
-                rec.update(scale=sc, shift=sh)
                 stats.append((m, v))
                 cur = ops.bn_apply(z, sc, sh, True)
+                rec.update(mean=m, scale=sc, y=cur)
             else:
                 cur = z
             layers.append(rec)
@@ -284,7 +266,7 @@ class MiniSpinNet(nn.Module):
         # pool layer: two 1x1 convolutions with affine batch-statistics BatchNorm and ReLU -> attention w; pooling
         c1, b1n, c2, b2n = self.pool_layer[0], self.pool_layer[1], self.pool_layer[3], self.pool_layer[4]
         W1 = c1.weight.detach().double().view(16, 32).t().contiguous()                    # [32, 16]
-        z1 = ops.conv1x1_f64(x, W1, c1.bias.detach().double().contiguous())
+        z1 = ops.conv1x1(x, W1, c1.bias.detach().double().contiguous())
         m1, v1 = pn.bn_batch_stats(ops.channel_sums(z1), N, b1n)
         sc1, sh1 = pn.bn_scale_shift(m1, v1, b1n, F64)
         h = ops.bn_apply(z1, sc1, sh1, True)
@@ -292,7 +274,7 @@ class MiniSpinNet(nn.Module):
         W2[:, 0] = c2.weight.detach().double().view(16)
         b2 = torch.zeros(4, dtype=F64, device=dev)
         b2[0] = c2.bias.detach().double()[0]
-        z2 = ops.conv1x1_f64(h, W2, b2)
+        z2 = ops.conv1x1(h, W2, b2)
         m2, v2 = pn.bn_batch_stats(ops.channel_sums(z2)[:, :1], N, b2n)
         sc2, sh2 = pn.bn_scale_shift(m2, v2, b2n, F64)
 
@@ -315,22 +297,21 @@ class MiniSpinNet(nn.Module):
         g = {}
         P = saved["pool"]
         dx, dw = ops.pool_backward(P["x"], P["w"], P["f"], ddesc, dequi)
-        dz2, s2 = ops.bn_affine_backward(dw, P["z2"], P["w"], *P["bn2"])        # masked by the forward's ReLU output
+        dz2, s2 = ops.bn_backward(dw, P["z2"], P["w"], *P["bn2"])        # masked by the forward's ReLU output
         g["pool_layer.4.weight"], g["pool_layer.4.bias"] = s2[1, :1], s2[0, :1]
         g["pool_layer.3.weight"] = ops.cross_sums(P["h"], dz2)[:, :1].t()
         g["pool_layer.3.bias"] = ops.channel_sums(dz2)[0, :1]
-        dh = ops.conv1x1_f64(dz2, P["W2"].t().contiguous())
-        dz1, s1 = ops.bn_affine_backward(dh, P["z1"], P["h"], *P["bn1"])
+        dh = ops.conv1x1(dz2, P["W2"].t().contiguous())
+        dz1, s1 = ops.bn_backward(dh, P["z1"], P["h"], *P["bn1"])
         g["pool_layer.1.weight"], g["pool_layer.1.bias"] = s1[1], s1[0]
         g["pool_layer.0.weight"] = ops.cross_sums(P["x"], dz1).t()
         g["pool_layer.0.bias"] = ops.channel_sums(dz1)[0]
-        dy = ops.conv1x1_f64(dz1, P["W1"].t().contiguous(), out=dx)
+        dy = ops.conv1x1(dz1, P["W1"].t().contiguous(), out=dx)
         net = self.conv_net
         for i in reversed(range(len(net.layers))):
             rec = saved["layers"][i]
-            if "scale" in rec:                        # ReLU mask + batch-statistics BatchNorm backward
-                s = ops.channel_sums(dy, rec["z"], rec["scale"], rec["shift"]) / (K * 140)
-                dz = ops.bn_backward(dy, rec["z"], rec["scale"], rec["shift"], s[0].contiguous(), s[1].contiguous())
+            if "scale" in rec:                        # ReLU mask + batch-statistics BatchNorm backward (affine=False)
+                dz, _ = ops.bn_backward(dy, rec["z"], rec["y"], rec["mean"], rec["scale"], torch.ones_like(rec["scale"]))
             else:
                 dz = dy
             ci = net.layers[i][0]

@@ -168,8 +168,9 @@ class _ConvStack(nn.Module):
         N = n * OD * OH * OW
         mean, var = bn_batch_stats(ops.channel_sums(z), N, bn)
         scale, shift = bn_scale_shift(mean, var, bn, z.dtype)
-        rec.update(scale=scale, shift=shift, N=N, batch_mean=mean, batch_var=var)
-        return ops.bn_apply(z, scale, shift, relu), rec
+        y = ops.bn_apply(z, scale, shift, relu)
+        rec.update(scale=scale, y=y, batch_mean=mean, batch_var=var)
+        return y, rec
 
 
 class Cylindrical_Net(_ConvStack):
@@ -345,9 +346,8 @@ class CostNet(_ConvStack):
             rec = saved["layers"][i]
             conv = self.ops[self.layers[i][0]]
             dy = dy.view(rec["z"].shape)
-            if "scale" in rec:                            # ReLU mask + batch-statistics BatchNorm backward
-                s = ops.channel_sums(dy, rec["z"], rec["scale"], rec["shift"]) / rec["N"]
-                dz = ops.bn_backward(dy, rec["z"], rec["scale"], rec["shift"], s[0].contiguous(), s[1].contiguous())
+            if "scale" in rec:                            # ReLU mask + batch-statistics BatchNorm backward (affine=False)
+                dz, _ = ops.bn_backward(dy, rec["z"], rec["y"], rec["batch_mean"], rec["scale"], torch.ones_like(rec["scale"]))
             else:
                 dz = dy
             db = ops.channel_sums(dz)[0]

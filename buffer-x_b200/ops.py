@@ -33,9 +33,9 @@ SYMBOLS = [
     "bx_ball_query_batched", "bx_gather_channels", "bx_knn1", "bx_svd3", "bx_icp_workspace_bytes", "bx_icp",
     "bx_fps_large", "bx_fps_large_workspace_bytes", "bx_fps_large_n", "bx_fps_large_size_class", "bx_radius_estimate_n_sub",
     "bx_ts_splits", "bx_ts_channel_sums", "bx_ts_channel_sums_f64", "bx_ts_moments3", "bx_ts_bn_apply", "bx_ts_bn_apply_f64",
-    "bx_ts_bn_backward", "bx_ts_conv1x1", "bx_ts_costvol", "bx_ts_softargmax", "bx_ts_conv_forward", "bx_ts_conv_backward",
-    "bx_td_cyl_forward", "bx_td_cyl_dgrad", "bx_td_cyl_wgrad", "bx_td_pnt_forward", "bx_td_pnt_backward", "bx_td_conv1x1",
-    "bx_td_cross_sums", "bx_td_bn_affine_backward", "bx_td_pool_forward", "bx_td_pool_backward", "bx_td_equi_match_backward",
+    "bx_ts_bn_backward", "bx_ts_conv1x1", "bx_ts_conv1x1_f64", "bx_ts_costvol", "bx_ts_softargmax", "bx_ts_conv_forward",
+    "bx_ts_conv_backward", "bx_td_cyl_forward", "bx_td_cyl_dgrad", "bx_td_cyl_wgrad", "bx_td_pnt_forward", "bx_td_pnt_backward",
+    "bx_td_cross_sums", "bx_td_pool_forward", "bx_td_pool_backward", "bx_td_equi_match_backward",
 ]
 
 GEOM_CYL3D, GEOM_CYL2D, GEOM_VALID3D, GEOM_COSTAB = 0, 1, 2, 4
@@ -132,13 +132,14 @@ def load_library():
     lib.bx_icp_workspace_bytes.restype = c_int64
     lib.bx_icp.argtypes = [P, c_int, P, c_int, c_double, P, c_double, c_double, c_int, P, P, P, P]
     lib.bx_ts_channel_sums.argtypes = [P, c_int, c_int, c_int, P, P, P]
-    lib.bx_ts_channel_sums_f64.argtypes = [P, P, P, P, c_int, c_int, c_int, P, P, P]
+    lib.bx_ts_channel_sums_f64.argtypes = [P, c_int, c_int, c_int, P, P, P]
     lib.bx_ts_bn_apply_f64.argtypes = [P, P, P, c_int, c_int, c_int, c_int, P, P]
     lib.bx_ts_conv_forward.argtypes = [P, P, P] + [c_int] * 9 + [P, P]
     lib.bx_ts_moments3.argtypes = [P, c_int64, P, P, P]
     lib.bx_ts_bn_apply.argtypes = [P, P, P, c_int, c_int, c_int, c_int, P, P]
-    lib.bx_ts_bn_backward.argtypes = [P, P, P, P, P, P, c_int, c_int, c_int, P, P]
-    lib.bx_ts_conv1x1.argtypes = [P, P, P, c_int, c_int, c_int, c_int, P, P]
+    lib.bx_ts_bn_backward.argtypes = [P] * 6 + [c_int, c_int, c_int, P, P, P, P]
+    lib.bx_ts_conv1x1.argtypes = [P, P, P, c_int, c_int, c_int, c_int, c_int, P, P]
+    lib.bx_ts_conv1x1_f64.argtypes = [P, P, P, c_int, c_int, c_int, c_int, c_int, P, P]
     lib.bx_ts_costvol.argtypes = [P, P, c_int, P, P]
     lib.bx_ts_softargmax.argtypes = [P, c_int, c_int, P, P, P, P]
     lib.bx_ts_conv_backward.argtypes = [P, P, P] + [c_int] * 9 + [P, P, P, P]
@@ -147,9 +148,7 @@ def load_library():
     lib.bx_td_cyl_wgrad.argtypes = [P, P, c_int, c_int, c_int, c_int, P, P, P]
     lib.bx_td_pnt_forward.argtypes = [P, P, P, P, P, c_int, c_int, c_int, P, P, P]
     lib.bx_td_pnt_backward.argtypes = [P] * 11 + [c_int, c_int, c_int, P, P, P]
-    lib.bx_td_conv1x1.argtypes = [P, P, P, c_int, c_int, c_int, c_int, c_int, P, P]
     lib.bx_td_cross_sums.argtypes = [P, P, c_int, c_int, c_int, c_int, P, P, P]
-    lib.bx_td_bn_affine_backward.argtypes = [P] * 6 + [c_int, c_int, c_int, P, P, P, P]
     lib.bx_td_pool_forward.argtypes = [P, P, c_int, P, P, P, P]
     lib.bx_td_pool_backward.argtypes = [P, P, P, P, P, c_int, P, P, P]
     lib.bx_td_equi_match_backward.argtypes = [P, P, P, c_int, c_int, c_int, c_int, P, P, P]
@@ -1098,25 +1097,15 @@ def _ts_blocked(what, x, name="x"):
     return x.shape[0], x.shape[1], x.shape[2]
 
 
-def channel_sums(x, z=None, scale=None, shift=None):
-    """-> float64 [2, C] per channel of the blocked x [n, C/4, S, 4] (fp32 or float64): (sum x, sum x^2); with z, scale,
-    shift (float64 only) the BatchNorm backward sums (sum dz, sum dz x^), x^ = z scale + shift, dz = x where x^ > 0."""
+def channel_sums(x):
+    """-> float64 [2, C] per channel of the blocked x [n, C/4, S, 4] (fp32 or float64): (sum x, sum x^2)."""
     n, G, S = _ts_blocked("channel_sums", x)
     C = 4 * G
-    if z is not None or scale is not None or shift is not None:
-        _ts_shape("channel_sums", z, x.shape, "z")
-        _ts_shape("channel_sums", scale, (C,), "scale")
-        _ts_shape("channel_sums", shift, (C,), "shift")
     partial = torch.empty(_splits() * 2 * C, dtype=F64, device=x.device)
     out = torch.empty(2 * C, dtype=F64, device=x.device)
-    lib = load_library()
-    if x.dtype == F64:
-        _check(lib.bx_ts_channel_sums_f64(_dp(x, F64, "x"), _dp(z, F64, "z"), _dp(scale, F64, "scale"), _dp(shift, F64, "shift"), n, C, S,
-                                          _dp(partial), _dp(out), _stream()), "bx_ts_channel_sums_f64")
-    else:
-        if z is not None:
-            raise BufferXError("channel_sums: the BatchNorm backward sums (z, scale, shift given) take float64 x only")
-        _check(lib.bx_ts_channel_sums(_dp(x, F32, "x"), n, C, S, _dp(partial), _dp(out), _stream()), "bx_ts_channel_sums")
+    f64 = x.dtype == F64
+    fn = load_library().bx_ts_channel_sums_f64 if f64 else load_library().bx_ts_channel_sums
+    _check(fn(_dp(x, F64 if f64 else F32, "x"), n, C, S, _dp(partial), _dp(out), _stream()), "bx_ts_channel_sums")
     return out.view(2, C)
 
 
@@ -1147,29 +1136,44 @@ def bn_apply(z, scale, shift, relu, out=None):
     return y
 
 
-def bn_backward(dy, z, scale, shift, m1, m2, out=None):
-    """float64 batch-statistics BatchNorm backward through the ReLU (see bx_ts_bn_backward)."""
+def bn_backward(dy, z, y, mean, rstd, gamma):
+    """Batch-statistics BatchNorm + ReLU backward, float64 blocked: -> (dz like z, sums [2, C] = (sum dz', sum dz' x^)
+    = (dbeta, dgamma)), dz' = dy [y > 0], x^ = (z - mean) rstd.  y is the forward's ReLU output (bn_apply's), so the
+    mask is the forward's bit for bit.  A BatchNorm with affine=False passes gamma = 1 and rstd = its scale."""
     n, G, S = _ts_blocked("bn_backward", z, "z")
     _ts_shape("bn_backward", dy, z.shape, "dy")
-    for name, t in (("scale", scale), ("shift", shift), ("m1", m1), ("m2", m2)):
+    _ts_shape("bn_backward", y, z.shape, "y")
+    for name, t in (("mean", mean), ("rstd", rstd), ("gamma", gamma)):
         _ts_shape("bn_backward", t, (4 * G,), name)
-    if out is not None:
-        _ts_shape("bn_backward", out, z.shape, "out")
-    dx = torch.empty_like(z) if out is None else out
-    _check(load_library().bx_ts_bn_backward(_dp(dy, F64, "dy"), _dp(z, F64, "z"), _dp(scale, F64, "scale"), _dp(shift, F64, "shift"),
-                                            _dp(m1, F64, "m1"), _dp(m2, F64, "m2"), n, 4 * G, S, _dp(dx, F64, "dx"), _stream()), "bx_ts_bn_backward")
-    return dx
+    C = 4 * G
+    partial = torch.empty(_splits() * 2 * C, dtype=F64, device=z.device)
+    sums = torch.empty(2 * C, dtype=F64, device=z.device)
+    dx = torch.empty_like(z)
+    _check(load_library().bx_ts_bn_backward(_dp(dy, F64, "dy"), _dp(z, F64, "z"), _dp(y, F64, "y"), _dp(mean, F64, "mean"),
+                                            _dp(rstd, F64, "rstd"), _dp(gamma, F64, "gamma"), n, C, S, _dp(partial), _dp(sums),
+                                            _dp(dx), _stream()), "bx_ts_bn_backward")
+    return dx, sums.view(2, C)
 
 
-def conv1x1(x, w, b):
-    """blocked x [n, Cin/4, S, 4], w [Cin, Cout4], b [Cout4] (Cout4 a multiple of 4, <= 16) -> blocked [n, Cout4/4, S, 4]."""
+def conv1x1(x, w, b=None, out=None):
+    """1x1 convolution of a blocked image, fp32 or float64 (w, b, out of x's dtype): x [n, Cin/4, S, 4], w [Cin, Cout],
+    b [Cout] or None -> [n, Cout/4, S, 4]; with ``out`` the result is added to it.  Cin, Cout <= 32, multiples of 4."""
     n, G, S = _ts_blocked("conv1x1", x)
     if not isinstance(w, torch.Tensor) or w.dim() != 2 or w.shape[0] != 4 * G:
-        raise BufferXError(f"conv1x1: w must be [{4 * G}, Cout4], got {tuple(w.shape) if isinstance(w, torch.Tensor) else w}")
-    Cout4 = w.shape[1]
-    _ts_shape("conv1x1", b, (Cout4,), "b")
-    out = torch.empty((n, Cout4 // 4, S, 4), dtype=F32, device=x.device)
-    _check(load_library().bx_ts_conv1x1(_dp(x, F32, "x"), _dp(w, F32, "w"), _dp(b, F32, "b"), n, 4 * G, Cout4, S, _dp(out), _stream()),
+        raise BufferXError(f"conv1x1: w must be [{4 * G}, Cout], got {tuple(w.shape) if isinstance(w, torch.Tensor) else w}")
+    Cout = w.shape[1]
+    if Cout % 4 or not 4 <= Cout <= 32 or 4 * G > 32:
+        raise BufferXError(f"conv1x1: {4 * G} -> {Cout} channels: both must be multiples of 4, at most 32")
+    if b is not None:
+        _ts_shape("conv1x1", b, (Cout,), "b")
+    acc = out is not None
+    if acc:
+        _ts_shape("conv1x1", out, (n, Cout // 4, S, 4), "out")
+    else:
+        out = torch.empty((n, Cout // 4, S, 4), dtype=x.dtype, device=x.device)
+    dt = F64 if x.dtype == F64 else F32
+    fn = load_library().bx_ts_conv1x1_f64 if dt == F64 else load_library().bx_ts_conv1x1
+    _check(fn(_dp(x, dt, "x"), _dp(w, dt, "w"), _dp(b, dt, "b"), n, 4 * G, Cout, S, int(acc), _dp(out, dt, "out"), _stream()),
            "bx_ts_conv1x1")
     return out
 
@@ -1336,27 +1340,6 @@ def pnt_backward(inv, arg, dfeat, W, b, mean, rstd, gamma, scale, shift, mo9):
     return out
 
 
-def conv1x1_f64(x, w, b=None, out=None):
-    """float64 1x1 convolution of a blocked image: x [n, Cin/4, S, 4], w [Cin, Cout], b [Cout] or None -> [n, Cout/4, S, 4];
-    with ``out`` the result is added to it.  Cin, Cout <= 32, multiples of 4."""
-    n, G, S = _ts_blocked("conv1x1_f64", x)
-    if not isinstance(w, torch.Tensor) or w.dim() != 2 or w.shape[0] != 4 * G:
-        raise BufferXError(f"conv1x1_f64: w must be [{4 * G}, Cout], got {tuple(w.shape) if isinstance(w, torch.Tensor) else w}")
-    Cout = w.shape[1]
-    if Cout % 4 or not 4 <= Cout <= 32 or 4 * G > 32:
-        raise BufferXError(f"conv1x1_f64: {4 * G} -> {Cout} channels: both must be multiples of 4, at most 32")
-    if b is not None:
-        _ts_shape("conv1x1_f64", b, (Cout,), "b")
-    acc = out is not None
-    if acc:
-        _ts_shape("conv1x1_f64", out, (n, Cout // 4, S, 4), "out")
-    else:
-        out = torch.empty((n, Cout // 4, S, 4), dtype=F64, device=x.device)
-    _check(load_library().bx_td_conv1x1(_dp(x, F64, "x"), _dp(w, F64, "w"), _dp(b, F64, "b"), n, 4 * G, Cout, S, int(acc), _dp(out, F64, "out"),
-                                        _stream()), "bx_td_conv1x1")
-    return out
-
-
 def cross_sums(X, D):
     """X [n, Ca/4, S, 4], D [n, Cb/4, S, 4] float64 -> [Ca, Cb] = sum over samples and positions of X[a] D[b]."""
     n, Ga, S = _ts_blocked("cross_sums", X, "X")
@@ -1368,25 +1351,6 @@ def cross_sums(X, D):
     _check(load_library().bx_td_cross_sums(_dp(X, F64, "X"), _dp(D, F64, "D"), n, Ca, Cb, S, _dp(partial), _dp(out), _stream()),
            "bx_td_cross_sums")
     return out
-
-
-def bn_affine_backward(dy, z, y, mean, rstd, gamma):
-    """Affine batch-statistics BatchNorm + ReLU backward, float64 blocked: -> (dz like z, sums [2, C] = (sum dz', sum dz' x^)
-    = (dbeta, dgamma)), dz' = dy [y > 0], x^ = (z - mean) rstd.  y is the forward's ReLU output (bn_apply's), so the
-    mask is the forward's bit for bit."""
-    n, G, S = _ts_blocked("bn_affine_backward", z, "z")
-    _ts_shape("bn_affine_backward", dy, z.shape, "dy")
-    _ts_shape("bn_affine_backward", y, z.shape, "y")
-    for name, t in (("mean", mean), ("rstd", rstd), ("gamma", gamma)):
-        _ts_shape("bn_affine_backward", t, (4 * G,), name)
-    C = 4 * G
-    partial = torch.empty(_splits() * 2 * C, dtype=F64, device=z.device)
-    sums = torch.empty(2 * C, dtype=F64, device=z.device)
-    dx = torch.empty_like(z)
-    _check(load_library().bx_td_bn_affine_backward(_dp(dy, F64, "dy"), _dp(z, F64, "z"), _dp(y, F64, "y"), _dp(mean, F64, "mean"),
-                                                   _dp(rstd, F64, "rstd"), _dp(gamma, F64, "gamma"), n, C, S, _dp(partial), _dp(sums),
-                                                   _dp(dx), _stream()), "bx_td_bn_affine_backward")
-    return dx, sums.view(2, C)
 
 
 def pool_forward(x, w):

@@ -455,17 +455,18 @@ int bx_so2_gt(const float *s_rand_axis, const float *s_R, const float *t_R, cons
  * Activations are channel-blocked [n][C/4][S][4]: fp32 for the frozen descriptor network, float64 for CostNet (forward and
  * backward).  Every reduction over samples x positions writes BX_TS_SPLITS per-block partials (workspace `partial`) that
  * one thread per output then adds in split order in float64: no atomics, bit-identical across runs.
- * bx_ts_channel_sums(_f64): out [2C] float64.  Without z: sum x and sum x^2 per channel (the batch statistics of the
- *   BatchNorm layers in training mode, models/patchnet.py:28,31 and patch_embedder.py:26-39).  With z, scale, shift [C]
- *   (_f64 only): the sums of the BatchNorm backward, sum dz and sum dz x^, where x^ = z scale + shift and dz = x [x^ > 0]
- *   (x = dL/dy of the ReLU).  partial [BX_TS_SPLITS * 2C] float64.
+ * bx_ts_channel_sums(_f64): out [2C] float64 = sum x and sum x^2 per channel (the batch statistics of the BatchNorm
+ *   layers in training mode, models/patchnet.py:28,31 and patch_embedder.py:26-39).  partial [BX_TS_SPLITS * 2C] float64.
  * bx_ts_moments3: the 3 first and 6 second moments (xx, xy, xz, yy, yz, zz) of R fp32 3-vectors, out9 float64, partial
  *   [BX_TS_SPLITS * 9]: the batch statistics of the linear 3 -> 16 point layer follow from them (patch_embedder.py:26-30).
  * bx_ts_bn_apply(_f64): y = z scale + shift per channel (ReLU if relu); y may alias z.
- * bx_ts_bn_backward: float64 dx = (dz - m1 - x^ m2) scale with x^, dz as above and m1 = mean dz, m2 = mean dz x^
- *   (affine = False: scale = 1/sqrt(var + eps)); dx may alias dy.
- * bx_ts_conv1x1: out [n][Cout4/4][S][4] = b + w^T x for w [Cin][Cout4] (the pool layer's 1x1 convolutions,
- *   patch_embedder.py:32-39); Cin <= 32, Cout4 <= 16.
+ * bx_ts_bn_backward: batch-statistics BatchNorm + ReLU backward, float64 (CostNet's and Cylindrical_Net's BatchNorms
+ *   with affine = False, patchnet.py:28,31, pass gamma = 1; the pool layer's pool_layer.{1,4}): x^ = (z - mean) rstd,
+ *   dz = dy [y > 0] with y the forward's ReLU output (bn_apply's, so the mask is the forward's bit for bit); sums [2C] =
+ *   (sum dz, sum dz x^) (= dbeta, dgamma), dx = gamma rstd (dz - m1 - x^ m2) with m1, m2 the sums over n*S.  partial
+ *   [BX_TS_SPLITS * 2C].
+ * bx_ts_conv1x1(_f64): out (+= if accumulate) b + w^T x, fp32 or float64, for w [Cin][Cout], b [Cout] or NULL (the pool
+ *   layer's 1x1 convolutions, patch_embedder.py:32-39, and their data gradients); Cin, Cout <= 32, multiples of 4.
  * bx_ts_costvol: the cost volume of CostVolume.forward (models/BUFFERX.py:52-64) on elevation rows 1..5 of the fp32 maps
  *   equi_s, equi_t [M,32,7,20]: cv float64 [M][8][20*5*20][4], cv[c][n][k][l] = s[c][k+1][(l-n) mod 20] - t[c][k+1][l].
  * bx_ts_softargmax: float64 ind [M] = sum_k softmax(logits)_k k (BUFFERX.py:66-68); with g = dL/dind [M] instead
@@ -477,14 +478,16 @@ int bx_so2_gt(const float *s_rand_axis, const float *s_R, const float *t_R, cons
 #define BX_TS_SPLITS 64
 int bx_ts_splits(void);
 int bx_ts_channel_sums(const float *x, int n, int C, int S, double *partial, double *out, void *stream);
-int bx_ts_channel_sums_f64(const double *x, const double *z, const double *scale, const double *shift, int n, int C, int S,
-                           double *partial, double *out, void *stream);
+int bx_ts_channel_sums_f64(const double *x, int n, int C, int S, double *partial, double *out, void *stream);
 int bx_ts_moments3(const float *v3, long long R, double *partial, double *out9, void *stream);
 int bx_ts_bn_apply(const float *z, const float *scale, const float *shift, int n, int C, int S, int relu, float *y, void *stream);
 int bx_ts_bn_apply_f64(const double *z, const double *scale, const double *shift, int n, int C, int S, int relu, double *y, void *stream);
-int bx_ts_bn_backward(const double *dy, const double *z, const double *scale, const double *shift, const double *m1, const double *m2,
-                      int n, int C, int S, double *dx, void *stream);
-int bx_ts_conv1x1(const float *x, const float *w, const float *b, int n, int Cin, int Cout4, int S, float *out, void *stream);
+int bx_ts_bn_backward(const double *dy, const double *z, const double *y, const double *mean, const double *rstd, const double *gamma,
+                      int n, int C, int S, double *partial, double *sums, double *dx, void *stream);
+int bx_ts_conv1x1(const float *x, const float *w, const float *b, int n, int Cin, int Cout, int S, int accumulate, float *out,
+                  void *stream);
+int bx_ts_conv1x1_f64(const double *x, const double *w, const double *b, int n, int Cin, int Cout, int S, int accumulate, double *out,
+                      void *stream);
 int bx_ts_costvol(const float *equi_s, const float *equi_t, int M, double *cv, void *stream);
 int bx_ts_softargmax(const double *logits, int M, int L, const double *g, double *ind, double *dlogits, void *stream);
 int bx_ts_conv_forward(const double *x, const double *w, const double *b, int n, int Cin, int Cout, int D, int H, int W, int kd, int kh,
@@ -513,13 +516,8 @@ int bx_ts_conv_backward(const double *x, const double *dy, const double *w, int 
  *   sum dz x^ and sum dz inv; the dense sums over every sample follow from mo9 (bx_ts_moments3 of inv).  mean, rstd, gamma
  *   [16] are the batch statistics and BatchNorm weight, scale / shift as in the forward.  out [16][6] = dW[c][0..2], db[c],
  *   dgamma[c], dbeta[c]; partial [BX_TS_SPLITS * 80].
- * bx_td_conv1x1: out (+= if accumulate) b + w^T x for w [Cin][Cout], b [Cout] or NULL (the pool layer's 1x1 convolutions,
- *   patch_embedder.py:32-39, and their data gradients); Cin, Cout <= 32, multiples of 4.
  * bx_td_cross_sums: out [Ca][Cb] = sum over (s, p) of X[s][a][p] D[s][b][p] (a 1x1 convolution's weight gradient);
  *   partial [BX_TS_SPLITS * Ca*Cb].
- * bx_td_bn_affine_backward: affine batch-statistics BatchNorm + ReLU backward (pool_layer.{1,4}): x^ = (z - mean) rstd,
- *   dz = dy [y > 0] with y the forward's ReLU output (bn_apply's, so the mask is the forward's bit for bit); sums [2C] = (sum dz, sum dz x^) (= dbeta, dgamma), dx = gamma rstd (dz - m1 - x^ m2) with
- *   m1, m2 the sums over n*S.  partial [BX_TS_SPLITS * 2C].
  * bx_td_pool_forward / bx_td_pool_backward: attention pooling and the L2 normalisations (patch_embedder.py:86-90):
  *   x [K][8][140][4], w the attention [K][1][140][4] (channel 0) -> f [K][32] float64, desc [K][32] and equi [K][32][140]
  *   fp32 (v / max(|v|, 1e-12)); the backward from ddesc, dequi (fp32) gives dx like x and dw like w.
@@ -533,11 +531,7 @@ int bx_td_pnt_forward(const float *inv, const double *W, const double *b, const 
 int bx_td_pnt_backward(const float *inv, const unsigned char *arg, const double *dfeat, const double *W, const double *b, const double *mean,
                        const double *rstd, const double *gamma, const double *scale, const double *shift, const double *mo9, int K, int V,
                        int nv, double *partial, double *out, void *stream);
-int bx_td_conv1x1(const double *x, const double *w, const double *b, int n, int Cin, int Cout, int S, int accumulate, double *out,
-                  void *stream);
 int bx_td_cross_sums(const double *X, const double *D, int n, int Ca, int Cb, int S, double *partial, double *out, void *stream);
-int bx_td_bn_affine_backward(const double *dy, const double *z, const double *y, const double *mean, const double *rstd,
-                             const double *gamma, int n, int C, int S, double *partial, double *sums, double *dx, void *stream);
 int bx_td_pool_forward(const double *x, const double *w, int K, double *f, float *desc, float *equi, void *stream);
 int bx_td_pool_backward(const double *x, const double *w, const double *f, const float *ddesc, const float *dequi, int K, double *dx,
                         double *dw, void *stream);

@@ -1,5 +1,5 @@
 """Edge inputs for the Desc training step's kernels (csrc/bx_train_desc.cu, one wrapper each in ops.py) and the float64
-checks they are held to, shared by tests/test_train_desc_kernels_fp64_*.py.
+checks they are held to, shared by tests/test_train_desc_kernels_fp64_*.py and tests/test_train_step_fp64_gpu.py.
 
 TEST INFRASTRUCTURE ONLY.  As in oracle/train_step_cases.py (whose gamma, ratio and layout helpers are used here): the
 ``check_*`` functions take the inputs and what an implementation returned (a kernel, or a float64 restatement of it on
@@ -12,16 +12,17 @@ terms, or ``dot2`` (products split exactly by Dekker's two-product, accumulated 
 within u |s| + gamma_n^2 sum |a b| of the exact dot product, Ogita, Rump and Oishi 2005), so a reference adds one
 rounding (+1 in k) to the kernel's k.  Reduction depths follow the kernels' order:
 
-* conv1x1_f64 (one thread per (sample, position), accumulator = bias, then Cin FMAs in channel order):
+* conv1x1, float64 (one thread per (sample, position), accumulator = bias, then Cin FMAs in channel order):
   gamma_{Cin+1} (|W|^T |x| + |b|); with ``out=`` the result is one more rounding of out + acc: gamma_{Cin+2} (... + |out|).
   A zero weight column with a zero bias writes exactly 0.
 * cross_sums (grid Ca/4 Cb/4 x 64 splits of 256 threads): split s takes the contiguous rows [s per, (s + 1) per),
   per = ceil(R / 64), R = n S; thread t its rows t, t + 256, ... by FMA, so ceil(per / 256) roundings; 8 levels of the
   block tree; 64 in-order split additions: d = ceil(ceil(R/64) / 256) + 72, bound gamma_{d+1} |X|^T |D|.
-* bn_affine_backward (grid C/4 x 64 splits): split s takes samples s, s + 64, ...; a thread the positions p, p + 256, ...
+* bn_backward (grid C/4 x 64 splits): split s takes samples s, s + 64, ...; a thread the positions p, p + 256, ...
   of them: d = ceil(n/64) ceil(S/256) + 72; sum dz x^ has the product's rounding more.  x^ = (z - mean) rstd is two
   roundings computed identically here.  The ReLU mask is the forward's: y > 0 for the output y of bn_apply.  dx =
   gamma rstd (dz - m1 - x^ m2) on the kernel's own m1, m2 (its sums / N): 2 gamma_3 (|dz| + |m1| + |x^ m2|) |gamma rstd|.
+  The pool layer's affine BatchNorms and, with gamma = 1, the affine = False ones of CostNet and Cylindrical_Net.
 * point layer: derived at check_pnt_forward / check_pnt_backward.
 * pool layer: f = sum_p x w / 140 by a serial FMA chain (140 roundings, the division one more); the normalisations and
   their backward are at most 40 roundings deep on any term: 2 gamma_40 of the same expression on absolute values, the
@@ -94,7 +95,7 @@ def fsum_rows(a):
     return np.array([math.fsum(r) for r in np.asarray(a, np.float64).tolist()], np.float64)
 
 
-# ------------------------------------------------------------------------------------------------ conv1x1_f64
+# ------------------------------------------------------------------------------------------------ conv1x1 (float64)
 def conv1x1_case(n, Cin, Cout, S, seed=0, live=None, live_in=None):
     """x [n, Cin, S], w [Cin, Cout], b [Cout], out0 [n, Cout, S] (nonzero, for ``out=``); ``live``: only the first
     ``live`` output channels have weights and bias (the attention's one channel padded to four, 16 -> 4); ``live_in``:
@@ -130,7 +131,7 @@ def check_conv1x1(x, w, b, got, out0=None):
     if out0 is not None:
         zero = zero & (out0 == 0).all(axis=(0, 2))
     assert (got[:, zero] == 0).all(), "a zero-padded output channel is not exactly 0"
-    return dict(conv1x1_f64=ratio(np.abs(got - ref), bound, "conv1x1_f64"))
+    return dict(conv1x1_f64=ratio(np.abs(got - ref), bound, "conv1x1 float64"))
 
 
 # ------------------------------------------------------------------------------------------------ cross_sums
@@ -165,7 +166,7 @@ def check_cross_sums(X, D, got):
     return dict(cross_sums=ratio(np.abs(got - ref), gamma(cross_depth(n * S) + 1) * ab, "cross_sums"))
 
 
-# ------------------------------------------------------------------------------------------------ bn_affine_backward
+# ------------------------------------------------------------------------------------------------ bn_backward
 def fwd_relu(z, scale, shift):
     """the forward's output bn_apply(z, scale, shift, relu): max(RN(z scale + shift), 0) (one fused multiply-add)."""
     from .train_step_cases import xhat
@@ -218,7 +219,7 @@ def bna_depth(n, S):
 
 
 def mask_from_dx(dy, z, mean, rstd, gam, sums, dx):
-    """The ReLU mask a bn_affine_backward applied, read back from its dx (channels with gamma rstd != 0): the kernel's dz =
+    """The ReLU mask a bn_backward applied, read back from its dx (channels with gamma rstd != 0): the kernel's dz =
     dx / (gamma rstd) + m1 + x^ m2 is dy (kept) or 0 (masked), and |dy| >= 0.5 tells them apart."""
     n, C, S = z.shape
     N = n * S
@@ -230,7 +231,7 @@ def mask_from_dx(dy, z, mean, rstd, gam, sums, dx):
 
 
 def check_bn_affine_backward(dy, z, y, mean, rstd, gam, dx, sums):
-    """dx, sums [2, C] of bn_affine_backward against the forward output y's mask."""
+    """dx, sums [2, C] of bn_backward against the forward output y's mask."""
     n, C, S = z.shape
     N = n * S
     dx, sums = np.asarray(dx, np.float64), np.asarray(sums, np.float64)

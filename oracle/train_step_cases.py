@@ -13,17 +13,16 @@ over float64 terms: the correctly rounded exact sum.  The square or product of t
 * channel_sums (grid C/4 x 64 splits of 256 threads): split s takes samples s, s + 64, ...; a thread adds the
   positions p, p + 256, ... of those samples, so one per-thread sum has ceil(n/64) ceil(S/256) terms; then 8 levels of
   the in-block tree and 64 in-order split additions: d = ceil(n/64) ceil(S/256) + 8 + 64.  With float64 inputs the
-  products x^2 and dz x^ are rounded (or fused) in the kernel and rounded in the reference's terms: d + 1.
+  product x^2 is rounded (or fused) in the kernel and rounded in the reference's terms: d + 1.
 * moments3 (64 blocks x 256 threads, grid-strided): ceil(R / 16384) terms per thread, + 8 + 64, each of the 9 slots
   against its own fsum (products exact).
 * bn_apply: y = fma(z, scale, shift), one rounding of the exact z scale + shift (bx_train_step.cu is built with FMA
   contraction).  fp32: |y - e| <= u32 |e|, e the exact value (z scale is exact in float64, e = RN64(z scale + shift) within
   u64 |e|): bound (u32 + 2 u64) |e|.  float64: the reference is RN(exact) (two-product + fsum) and the kernel one
   rounding of the same value: |y - ref| <= 2 u |ref| (1 + 2u).  With ReLU a value whose exact result is <= 0 is 0.
-* ReLU mask: x^ = fma(z, scale, shift) in the forward (bn_apply), in channel_sums mode 1 and in bn_backward; all three
-  must agree bit for bit with the exact sign of x^ (the cases make z scale exact: power-of-two scales).
-* bn_backward: dx = (dz - m1 - x^ m2) scale, three roundings in the kernel and three in the float64 reference on the
-  same x^ and (m1, m2): |dx - ref| <= 2 gamma_3 (|dz| + |m1| + |x^ m2|) |scale|.
+* ReLU mask: the forward's (bn_apply) is the sign of fma(z, scale, shift) bit for bit (the cases make z scale exact:
+  power-of-two scales); the backward (bn_backward, held to oracle/train_desc_cases.check_bn_affine_backward with
+  gamma = 1) reads it from the forward's output.
 * conv1x1 (fp32 FMA chain, bias first): gamma32_{Cin+1} (|W|^T |x| + |b|), plus the float64 reference's own
   gamma64_{Cin+1} of the same.
 * costvol: float64(s) - float64(t) is one IEEE subtraction on both sides: equal bits.
@@ -167,20 +166,22 @@ def check_channel_sums(x, got):
 
 
 def mask_case(n, C, S, seed=0):
-    """The BatchNorm backward's edge inputs, channel-first float64 -> (dy, z, scale [C], shift [C]).  Channel c % 4:
+    """The edge inputs of a BatchNorm with affine = False, channel-first float64 -> (dy, z, scale [C], shift [C], mean [C]):
+    the forward is x^ = fma(z, scale, shift) with scale = rstd and shift = -RN(mean scale), as patchnet.bn_scale_shift
+    forms them.  Channel c % 4 (mean z0):
     0 -- power-of-two scale, shift = -z0 scale (exact), about a third of the elements at z0 (x^ exactly 0) and at z0 +-1 ulp;
-    1 -- as 0 but every z < z0 (a dead channel: dz = 0, m1 = m2 = 0); 2 -- constant z with the scale of var = 0,
-    1 / sqrt(1e-5), and shift = -RN(z scale) (x^ the product's rounding error); 3 -- a generic channel."""
+    1 -- as 0 but every z < z0 (a dead channel: dz = 0, m1 = m2 = 0); 2 -- constant z = z0 with the scale of var = 0,
+    1 / sqrt(1e-5) (the forward's x^ the product's rounding error, (z - mean) rstd exactly 0); 3 -- a generic channel.
+    |dy| in [0.5, 1.5]: a mask flip moves dx by at least 0.5 |scale|."""
     rng = np.random.default_rng(seed)
-    dy = rng.normal(size=(n, C, S))
+    dy = rng.uniform(0.5, 1.5, (n, C, S)) * rng.choice([-1.0, 1.0], (n, C, S))
     z = np.empty((n, C, S))
-    scale, shift = np.empty(C), np.empty(C)
+    scale, mean = np.empty(C), np.empty(C)
     for c in range(C):
         k = c % 4
-        z0 = rng.uniform(-3, 3)
+        z0 = mean[c] = rng.uniform(-3, 3)
         if k in (0, 1):
             scale[c] = 2.0 ** int(rng.integers(-3, 4))
-            shift[c] = -z0 * scale[c]
             v = z0 + rng.uniform(-2, 2, (n, S)) if k == 0 else z0 - rng.uniform(1e-3, 2, (n, S))
             if k == 0:
                 pick = rng.integers(0, 6, (n, S))
@@ -188,31 +189,16 @@ def mask_case(n, C, S, seed=0):
             z[:, c] = v
         elif k == 2:
             scale[c] = 1.0 / math.sqrt(1e-5)
-            shift[c] = -(z0 * scale[c])
             z[:, c] = z0
         else:
             scale[c] = rng.uniform(0.2, 3)
-            shift[c] = rng.uniform(-1, 1)
-            z[:, c] = rng.normal(size=(n, S))
-    return dy, z, scale, shift
+            z[:, c] = z0 + rng.normal(size=(n, S))
+    return dy, z, scale, -(mean * scale), mean
 
 
 def xhat(z, scale, shift):
     """x^ = RN(z scale + shift), channel-first [n, C, S] (the kernels' fused multiply-add)."""
     return fma64(z, scale[None, :, None], shift[None, :, None])
-
-
-def check_bn_sums(dy, z, scale, shift, got, xh=None):
-    """channel_sums mode 1: got [2, C] = (sum dz, sum dz x^), dz = dy where x^ > 0 (``xh``: xhat of the inputs, if known)."""
-    n, C, S = z.shape
-    xh = xhat(z, scale, shift) if xh is None else xh
-    dz = np.where(xh > 0, dy, 0.0)
-    t0 = dz.transpose(1, 0, 2).reshape(C, -1)
-    t1 = (dz * xh).transpose(1, 0, 2).reshape(C, -1)
-    g = gamma(sums_depth(n, S, True))
-    got = np.asarray(got, np.float64)
-    return dict(bsum_dz=ratio(np.abs(got[0] - fsum_rows(t0)), g * np.abs(t0).sum(1), "sum dz"),
-                bsum_dzxh=ratio(np.abs(got[1] - fsum_rows(t1)), g * np.abs(t1).sum(1), "sum dz x^"))
 
 
 def check_mask(z, scale, shift, mask, xh=None):
@@ -221,19 +207,6 @@ def check_mask(z, scale, shift, mask, xh=None):
     bad = int((np.asarray(mask, bool) != ref).sum())
     assert bad == 0, f"ReLU mask differs from x^ > 0 at {bad} elements"
     return dict(mask_elems=float(0))
-
-
-def check_bn_backward(dy, z, scale, shift, m1, m2, got, xh=None):
-    """dx (channel-first) against (dz - m1 - x^ m2) scale in float64 on the exact x^; dead channels exactly 0."""
-    xh = xhat(z, scale, shift) if xh is None else xh
-    dz = np.where(xh > 0, dy, 0.0)
-    sc, a1, a2 = scale[None, :, None], m1[None, :, None], m2[None, :, None]
-    ref = ((dz - a1) - xh * a2) * sc
-    bound = 2 * gamma(3) * (np.abs(dz) + np.abs(a1) + np.abs(xh * a2)) * np.abs(sc)
-    got = np.asarray(got, np.float64)
-    dead = ~(xh > 0).any(axis=(0, 2))
-    assert (got[:, dead] == 0).all(), "a dead channel's dx is not exactly 0"
-    return dict(bn_bwd=ratio(np.abs(got - ref), bound, "bn_backward dx"))
 
 
 # ------------------------------------------------------------------------------------------------ bn_apply

@@ -206,7 +206,7 @@ def test_equi_match_backward(dev, B):
     assert (gt.double() - tr.grad).abs().max() <= 1e-6 * float(tr.grad.abs().max())
 
 
-def test_wrappers_refuse_misshaped_inputs(dev):
+def test_desc_wrappers_refuse_misshaped_inputs(dev):
     ops = _ops()
     x = torch.zeros((2, 4, 420, 4), dtype=torch.float64, device=dev)
     Wt = torch.zeros((27, 16, 64), dtype=torch.float64, device=dev)
@@ -230,4 +230,4 @@ def test_wrappers_refuse_misshaped_inputs(dev):
     with pytest.raises(ops.BufferXError):
         ops.equi_match_backward(torch.zeros((2, 32, 7, 20), device=dev), torch.zeros((2, 32, 7, 20), device=dev), torch.zeros((2, 19), device=dev))
     with pytest.raises(ops.BufferXError):
-        ops.conv1x1_f64(torch.zeros((2, 8, 140, 4), dtype=torch.float64, device=dev), torch.zeros((32, 36), dtype=torch.float64, device=dev))
+        ops.conv1x1(torch.zeros((2, 8, 140, 4), dtype=torch.float64, device=dev), torch.zeros((32, 36), dtype=torch.float64, device=dev))

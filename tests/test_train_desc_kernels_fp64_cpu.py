@@ -7,6 +7,7 @@ import numpy as np
 import pytest
 
 from oracle import train_desc_cases as D
+from oracle import train_step_cases as TS
 from oracle.train_step_cases import fma64
 
 
@@ -39,12 +40,16 @@ def emu_bn_affine_backward(dy, z, y, mean, rstd, gam, beta, mutation=None):
         keep = gam[None, :, None] * xh + beta[None, :, None] > 0
     elif mutation == "unfolded_mask_fma":              # the same, as nvcc contracts it: fma(gamma, x^, beta) > 0
         keep = fma64(gam[None, :, None], xh, beta[None, :, None]) > 0
+    elif mutation == "mask_ge":                        # >= for >: also keeps the forward's exact zeros before the ReLU
+        G = gam * rstd
+        keep = fma64(z, G[None, :, None], (beta - mean * G)[None, :, None]) >= 0
     else:
         keep = y > 0
     dz = np.where(keep, dy, 0.0)
     s0, s1 = dz.sum(axis=(0, 2)), (dz * xh).sum(axis=(0, 2))
     N = n * S
-    dx = (gam * rstd)[None, :, None] * ((dz - (s0 / N)[None, :, None]) - xh * (s1 / N)[None, :, None])
+    m2 = 0.0 if mutation == "no_xh_m2" else (s1 / N)[None, :, None]
+    dx = (gam * rstd)[None, :, None] * ((dz - (s0 / N)[None, :, None]) - xh * m2)
     return dx, np.stack([s0, s1])
 
 
@@ -199,6 +204,25 @@ def test_bn_affine_backward_check_rejects_the_unfolded_mask(C, mutation):
             with pytest.raises(AssertionError, match="ReLU mask"):
                 D.check_bn_affine_backward(dy, z, y, mean, rstd, gam, dx, sums)
     assert flips > 0
+
+
+@pytest.mark.parametrize("mutation", [None, "mask_ge", "no_xh_m2"], ids=["restatement", "mask_ge", "no_xh_m2"])
+def test_bn_backward_check_at_gamma_1(mutation):
+    """gamma = 1, the affine = False BatchNorms of CostNet and Cylindrical_Net (rstd = scale, y = bn_apply's
+    fma(z, scale, shift) with ReLU), on train_step_cases.mask_case: x^ exactly 0 and +-1 ulp, dead and constant channels.
+    The check accepts the restatement and, on every shape, rejects a mask that also keeps the forward's exact zeros and a
+    dx without x^ m2."""
+    for n, S in ((1, 257), (64, 5), (65, 3)):
+        dy, z, sc, sh, mean = TS.mask_case(n, 16, S, seed=n)
+        y = np.maximum(TS.xhat(z, sc, sh), 0.0)
+        TS.check_mask(z, sc, sh, y > 0)
+        gam, beta = np.ones(16), np.zeros(16)
+        got = emu_bn_affine_backward(dy, z, y, mean, sc, gam, beta, mutation)
+        if mutation is None:
+            TS.report(f"bn_backward at gamma = 1, n={n} S={S}", D.check_bn_affine_backward(dy, z, y, mean, sc, gam, *got))
+        else:
+            with pytest.raises(AssertionError):
+                D.check_bn_affine_backward(dy, z, y, mean, sc, gam, *got)
 
 
 @pytest.mark.parametrize("offset", [0.0, 1e3])

@@ -38,10 +38,10 @@ def _unblk(t):
     return from_blocked(t.cpu().numpy())
 
 
-# ------------------------------------------------------------------------------------------------ conv1x1_f64
+# ------------------------------------------------------------------------------------------------ conv1x1 (float64)
 @pytest.mark.parametrize("n", [1, 2, 65])
 @pytest.mark.parametrize("shape", D.CONV1X1_SHAPES)
-def test_conv1x1_f64(dev, shape, n):
+def test_conv1x1_float64(dev, shape, n):
     ops = _ops()
     Cin, Cout = shape
     res = {}
@@ -49,10 +49,10 @@ def test_conv1x1_f64(dev, shape, n):
         x, w, b, out0 = D.conv1x1_case(n, Cin, Cout, S, seed=Cin + Cout + S + n, live=1 if shape == (16, 4) else None,
                                        live_in=1 if shape == (4, 16) else None)
         xb, wg, bg = _blk(x, dev), _g(w, dev), _g(b, dev)
-        merge(res, D.check_conv1x1(x, w, b, _unblk(ops.conv1x1_f64(xb, wg, bg))))
-        merge(res, D.check_conv1x1(x, w, None, _unblk(ops.conv1x1_f64(xb, wg))))
+        merge(res, D.check_conv1x1(x, w, b, _unblk(ops.conv1x1(xb, wg, bg))))
+        merge(res, D.check_conv1x1(x, w, None, _unblk(ops.conv1x1(xb, wg))))
         ob = _blk(out0, dev)
-        r = ops.conv1x1_f64(xb, wg, bg, out=ob)
+        r = ops.conv1x1(xb, wg, bg, out=ob)
         assert r.data_ptr() == ob.data_ptr()
         merge(res, D.check_conv1x1(x, w, b, _unblk(ob), out0=out0))
     report(f"conv1x1_f64 {Cin}->{Cout} n={n}", res)
@@ -74,10 +74,10 @@ def test_cross_sums(dev, nS, C):
     report(f"cross_sums {C} n={n} S={S}", res)
 
 
-# ------------------------------------------------------------------------------------------------ bn_affine_backward
+# ------------------------------------------------------------------------------------------------ bn_backward
 @pytest.mark.parametrize("n", D.BNA_N)
 @pytest.mark.parametrize("C", [16, 4])
-def test_bn_affine_backward_mask_is_the_forwards(dev, C, n):
+def test_bn_backward_mask_is_the_forwards(dev, C, n):
     """The pool layer's BatchNorm + ReLU backward: the forward is ops.bn_apply on the folded (scale, shift), as
     MiniSpinNet.train_desc runs it; z within 8 ulp of each boundary channel's root.  C = 4 is the attention's BN(1)
     padded to four channels with all-zero parameters."""
@@ -88,7 +88,7 @@ def test_bn_affine_backward_mask_is_the_forwards(dev, C, n):
     yb = ops.bn_apply(zb, _g(scale, dev), _g(shift, dev), True)
     y = _unblk(yb)
     assert np.array_equal(y, D.fwd_relu(z, scale, shift)), "bn_apply is not one fused multiply-add"
-    dx, sums = ops.bn_affine_backward(_blk(dy, dev), zb, yb, *(_g(t, dev) for t in (mean, rstd, gam)))
+    dx, sums = ops.bn_backward(_blk(dy, dev), zb, yb, *(_g(t, dev) for t in (mean, rstd, gam)))
     res = D.check_bn_affine_backward(dy, z, y, mean, rstd, gam, _unblk(dx), sums.cpu().numpy())
     report(f"bn_affine_backward C={C} n={n}", res)
 

@@ -12,16 +12,11 @@ from oracle import train_step_cases as C
 
 
 # ------------------------------------------------------------------------------------------------ restatements
-def emu_channel_sums(x, z=None, scale=None, shift=None, mutation=None):
+def emu_channel_sums(x, mutation=None):
     """channel-first float64 [n, C, S] -> [2, C]: per split (samples s = split mod 64) the partial sums, added in split order."""
     n, Cc, S = x.shape
-    x = x.astype(np.float64)
-    if z is not None:
-        xh = C.xhat(z, scale, shift)
-        keep = xh >= 0 if mutation == "mask_ge" else xh > 0
-        a, b = np.where(keep, x, 0.0), np.where(keep, x, 0.0) * xh
-    else:
-        a, b = x, x * x
+    a = x.astype(np.float64)
+    b = a * a
     out = np.zeros((2, Cc))
     for split in range(C.SPLITS):
         if mutation == "drop_split63" and split == 63:
@@ -38,15 +33,6 @@ def emu_moments3(v, mutation=None):
     if mutation == "swap_xy_xz":
         out[[4, 5]] = out[[5, 4]]
     return out
-
-
-def emu_bn_backward(dy, z, scale, shift, m1, m2, mutation=None):
-    xh = C.xhat(z, scale, shift)
-    dz = np.where(xh > 0, dy, 0.0)
-    sc, a1, a2 = scale[None, :, None], m1[None, :, None], m2[None, :, None]
-    if mutation == "no_xh_m2":
-        return (dz - a1) * sc
-    return ((dz - a1) - xh * a2) * sc
 
 
 def emu_softargmax(lg, g=None, mutation=None):
@@ -145,20 +131,6 @@ def check_sums(mutation=None):
     return acc
 
 
-def check_bn(mutation=None):
-    acc = {}
-    for n, S in ((1, 257), (64, 5), (65, 3)):
-        dy, z, sc, sh = C.mask_case(n, 16, S, seed=n)
-        s = emu_channel_sums(dy, z, sc, sh, mutation=mutation)
-        C.merge(acc, C.check_bn_sums(dy, z, sc, sh, s))
-        xh = C.xhat(z, sc, sh)
-        keep = xh >= 0 if mutation == "mask_ge" else xh > 0
-        C.merge(acc, C.check_mask(z, sc, sh, keep))
-        N = n * S
-        C.merge(acc, C.check_bn_backward(dy, z, sc, sh, s[0] / N, s[1] / N, emu_bn_backward(dy, z, sc, sh, s[0] / N, s[1] / N, mutation)))
-    return acc
-
-
 def check_moments(mutation=None):
     acc = {}
     for R in (1, 255, 16385):
@@ -228,7 +200,7 @@ def check_pnt(mutation=None):
 
 
 # ------------------------------------------------------------------------------------------------ tests
-@pytest.mark.parametrize("check", [check_sums, check_bn, check_moments, check_sam, check_cv, check_conv, check_running, check_pnt],
+@pytest.mark.parametrize("check", [check_sums, check_moments, check_sam, check_cv, check_conv, check_running, check_pnt],
                          ids=lambda f: f.__name__)
 def test_restatement_passes(check):
     C.report(check.__name__, check())
@@ -236,8 +208,6 @@ def test_restatement_passes(check):
 
 MUTATIONS = [
     ("drop_split63", check_sums),
-    ("mask_ge", check_bn),
-    ("no_xh_m2", check_bn),
     ("no_minus_ind", check_sam),
     ("l_plus_nn", check_cv),
     ("rows_0_4", check_cv),

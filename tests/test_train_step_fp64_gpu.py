@@ -7,6 +7,7 @@ import numpy as np
 import pytest
 import torch
 
+from oracle import train_desc_cases as D
 from oracle import train_step_cases as C
 
 pytestmark = pytest.mark.gpu
@@ -47,29 +48,26 @@ def test_channel_sums(bx):
     C.report("channel_sums (fp32 + f64)", acc)
 
 
-def test_bn_mask_sums_and_backward(bx):
+def test_bn_backward_at_gamma_1_on_mask_edges(bx):
+    """The BatchNorm + ReLU backward with gamma = 1 (the affine = False layers of CostNet and Cylindrical_Net: rstd = scale)
+    held to check_bn_affine_backward on mask_case's edge inputs; the forward is bn_apply_f64 with ReLU, and the backward
+    takes its output y as the mask."""
     acc = {}
     for n, S, Cc in _sum_shapes():
-        dy, z, sc, sh = C.mask_case(n, Cc, S, seed=n + S)
+        dy, z, sc, sh, mean = C.mask_case(n, Cc, S, seed=n + S)
         xh = C.xhat(z, sc, sh)
         dyb, zb = _cu(C.to_blocked(dy)), _cu(C.to_blocked(z))
-        scb, shb = _cu(sc), _cu(sh)
-        # the forward's mask (bn_apply_f64 with ReLU) and the backward's (bn_backward with dy = 1, m1 = m2 = 0)
-        fwd = C.from_blocked(_np(bx.ops.bn_apply(zb, scb, shb, True))) > 0
-        C.check_mask(z, sc, sh, fwd, xh)
-        zero = torch.zeros(Cc, dtype=torch.float64, device="cuda")
-        bwd = C.from_blocked(_np(bx.ops.bn_backward(torch.ones_like(zb), zb, scb, shb, zero, zero))) != 0
-        C.check_mask(z, sc, sh, bwd, xh)
-        cnt = _np(bx.ops.channel_sums(torch.ones_like(zb), zb, scb, shb))[0]
-        assert np.array_equal(cnt, fwd.sum(axis=(0, 2)).astype(np.float64)), "channel_sums mode 1 counts another mask"
-        s = bx.ops.channel_sums(dyb, zb, scb, shb)
-        C.merge(acc, C.check_bn_sums(dy, z, sc, sh, _np(s), xh))
-        assert torch.equal(s, bx.ops.channel_sums(dyb, zb, scb, shb))
-        m = s / (n * S)
-        dx = bx.ops.bn_backward(dyb, zb, scb, shb, m[0].contiguous(), m[1].contiguous())
-        mm = _np(m)
-        C.merge(acc, C.check_bn_backward(dy, z, sc, sh, mm[0], mm[1], C.from_blocked(_np(dx)), xh))
-    C.report("bn mask / channel_sums mode 1 / bn_backward", acc)
+        scb, meanb, gam = _cu(sc), _cu(mean), torch.ones(Cc, dtype=torch.float64, device="cuda")
+        yb = bx.ops.bn_apply(zb, scb, _cu(sh), True)
+        y = C.from_blocked(_np(yb))
+        C.check_mask(z, sc, sh, y > 0, xh)
+        _, cnt = bx.ops.bn_backward(torch.ones_like(zb), zb, yb, meanb, scb, gam)
+        assert np.array_equal(_np(cnt)[0], (y > 0).sum(axis=(0, 2)).astype(np.float64)), "bn_backward's sums count another mask"
+        dx, s = bx.ops.bn_backward(dyb, zb, yb, meanb, scb, gam)
+        C.merge(acc, D.check_bn_affine_backward(dy, z, y, mean, sc, np.ones(Cc), C.from_blocked(_np(dx)), _np(s)))
+        dx2, s2 = bx.ops.bn_backward(dyb, zb, yb, meanb, scb, gam)
+        assert torch.equal(s, s2) and torch.equal(dx, dx2), "two calls differ"
+    C.report("bn mask / bn_backward at gamma = 1", acc)
 
 
 def test_bn_apply(bx):
@@ -225,7 +223,7 @@ def test_conv_forward_and_backward(bx):
 
 
 # ------------------------------------------------------------------------------------------------ refusals
-def test_refusals(bx):
+def test_wrapper_refusals(bx):
     ops, E = bx.ops, bx.ops.BufferXError
     f64 = dict(dtype=torch.float64, device="cuda")
     x = torch.zeros((1, 8, 4 * 1 * 4, 4), **f64)
@@ -252,20 +250,17 @@ def test_refusals(bx):
             ops.costvol(torch.zeros(s, **f32), torch.zeros(t, **f32))
     z = torch.zeros((2, 3, 5, 4), **f64)
     c12, c8 = torch.zeros(12, **f64), torch.zeros(8, **f64)
-    with pytest.raises(E):
-        ops.channel_sums(z, z, c8, c12)
-    with pytest.raises(E):
-        ops.channel_sums(z, torch.zeros((2, 3, 4, 4), **f64), c12, c12)
+    z4 = torch.zeros((2, 3, 4, 4), **f64)
     with pytest.raises(E):
         ops.channel_sums(torch.zeros((2, 3, 5), **f64))
-    with pytest.raises(E):                                 # the backward sums take float64 only
-        ops.channel_sums(torch.zeros((2, 3, 5, 4), dtype=torch.float32, device="cuda"), z, c12, c12)
-    with pytest.raises(E):                                 # z of another dtype than x
-        ops.channel_sums(z, z.float(), c12, c12)
-    with pytest.raises(E):
-        ops.bn_backward(z, z, c12, c12, c12, c8)
-    with pytest.raises(E):
-        ops.bn_backward(torch.zeros((2, 3, 4, 4), **f64), z, c12, c12, c12, c12)
+    for args in ((z, z, z4, c12, c12, c12), (z, z, z, c8, c12, c12), (z, z, z, c12, c8, c12), (z, z, z, c12, c12, c8),
+                 (z4, z, z, c12, c12, c12)):              # y, mean, rstd, gamma, dy of another shape
+        with pytest.raises(E):
+            ops.bn_backward(*args)
+    with pytest.raises(E):                                 # the backward takes float64 only
+        ops.bn_backward(z.float(), z.float(), z.float(), c12.float(), c12.float(), c12.float())
+    with pytest.raises(E):                                 # z of another dtype than dy
+        ops.bn_backward(z, z.float(), z, c12, c12, c12)
     with pytest.raises(E):
         ops.bn_apply(z, c8, c12, True)
     with pytest.raises(E):
@@ -274,6 +269,10 @@ def test_refusals(bx):
         ops.moments3(torch.zeros((5, 2), **f32))
     with pytest.raises(E):
         ops.conv1x1(torch.zeros((1, 2, 3, 4), **f32), torch.zeros((4, 4), **f32), torch.zeros(4, **f32))
+    with pytest.raises(E):                                 # Cout above 32
+        ops.conv1x1(torch.zeros((1, 2, 3, 4), **f32), torch.zeros((8, 36), **f32), torch.zeros(36, **f32))
+    with pytest.raises(E):                                 # w of another dtype than x
+        ops.conv1x1(torch.zeros((1, 2, 3, 4), **f32), torch.zeros((8, 4), **f64))
 
 
 # ------------------------------------------------------------------------------------------------ CostNet, module level
