@@ -6,7 +6,7 @@ Package layout (only what the path needs):
     models/    host-side mirror of the reference's models/BUFFERX.py API (BufferX, MiniSpinNet, ...)
     config/    make_cfg mirror (reference config/ semantics)
     synth.py   seeded synthetic pairs shaped like the reference's datasets
-    driver.py  one-process-per-GPU pair sharding + one all-gather of result records
+    driver.py  one-process-per-GPU pair sharding + one all-gather of result records; sharded training
 
 The directory name contains a hyphen (fixed by the task), so the importable name is ``bufferx_b200``
 (see the shim ``bufferx_b200.py`` at the repository root); both names map to the same module objects.

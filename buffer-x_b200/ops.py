@@ -35,7 +35,7 @@ SYMBOLS = [
     "bx_ts_splits", "bx_ts_channel_sums", "bx_ts_channel_sums_f64", "bx_ts_moments3", "bx_ts_bn_apply", "bx_ts_bn_apply_f64",
     "bx_ts_bn_backward", "bx_ts_conv1x1", "bx_ts_conv1x1_f64", "bx_ts_costvol", "bx_ts_softargmax", "bx_ts_conv_forward",
     "bx_ts_conv_backward", "bx_td_cyl_forward", "bx_td_cyl_dgrad", "bx_td_cyl_wgrad", "bx_td_pnt_forward", "bx_td_pnt_backward",
-    "bx_td_cross_sums", "bx_td_pool_forward", "bx_td_pool_backward", "bx_td_equi_match_backward",
+    "bx_td_cross_sums", "bx_td_pool_forward", "bx_td_pool_backward", "bx_td_equi_match_backward", "bx_dp_mean",
 ]
 
 GEOM_CYL3D, GEOM_CYL2D, GEOM_VALID3D, GEOM_COSTAB = 0, 1, 2, 4
@@ -152,6 +152,7 @@ def load_library():
     lib.bx_td_pool_forward.argtypes = [P, P, c_int, P, P, P, P]
     lib.bx_td_pool_backward.argtypes = [P, P, P, P, P, c_int, P, P, P]
     lib.bx_td_equi_match_backward.argtypes = [P, P, P, c_int, c_int, c_int, c_int, P, P, P]
+    lib.bx_dp_mean.argtypes = [P, c_int, ctypes.c_longlong, P, P, P]
     _lib = lib
     return lib
 
@@ -1394,3 +1395,21 @@ def equi_match_backward(d1, d2, dcor):
     _check(load_library().bx_td_equi_match_backward(_dp(d1, F32, "d1"), _dp(d2, F32, "d2"), _dp(dcor, F32, "dcor"), B, C, K, L, _dp(g1),
                                                     _dp(g2), _stream()), "bx_td_equi_match_backward")
     return g1, g2
+
+
+# --------------------------------------------------------------------------- #
+def dp_mean(gathered: torch.Tensor):
+    """The cross-rank mean of one sharded training step (driver.train_sharded): ``gathered`` [W, n + 1] fp32 CUDA holds
+    one record per rank, n values then the rank's contribution flag.  Returns (out [n] fp32, count [1] int32 on the
+    device): out[i] = fl32((sum over the rows with a non-zero flag, in ascending row order, of (double) gathered[r, i]) /
+    count); out is left unwritten (torch.empty) when count is 0."""
+    if not isinstance(gathered, torch.Tensor) or gathered.dim() != 2 or gathered.shape[0] < 1 or gathered.shape[1] < 1:
+        raise BufferXError(f"dp_mean: gathered must be a [W >= 1, n + 1 >= 1] tensor, got "
+                           f"{tuple(gathered.shape) if isinstance(gathered, torch.Tensor) else type(gathered).__name__}")
+    W, n = gathered.shape[0], gathered.shape[1] - 1
+    ptr = _dp(gathered, F32, "gathered")
+    out = torch.empty(n, dtype=F32, device=gathered.device)
+    count = torch.empty(1, dtype=I32, device=gathered.device)
+    # an empty tensor's data_ptr() may be NULL, which the C-ABI refuses: with n = 0 nothing is written through `out`
+    _check(load_library().bx_dp_mean(ptr, W, n, _dp(out) if n else _dp(count), _dp(count), _stream()), "bx_dp_mean")
+    return out, count

@@ -538,6 +538,15 @@ int bx_td_pool_backward(const double *x, const double *w, const double *f, const
 int bx_td_equi_match_backward(const float *s, const float *t, const float *dcor, int B, int C, int E, int L, float *ds, float *dt,
                               void *stream);
 
+/* ---- sharded training: the cross-rank mean of one step (driver.train_sharded, DESIGN.md §8) -------------------------
+ * gathered [W][n + 1] fp32 (row-major, device) holds one record per rank: n values (the trainable parameters' gradients,
+ * then the BatchNorm buffers) followed by the rank's contribution flag.  With count = the number of rows whose flag is not
+ * 0, out[i] = fl32((sum over those rows r, ascending, of (double) gathered[r][i]) / count) for i < n: the float64 sum starts
+ * from the first contributing row (one contributor is the identity, bit for bit) and is neither reordered nor contracted;
+ * NaN and inf propagate.  *count (device int32) is always written; out is not written when count = 0.  Every rank that
+ * runs this on the same gathered matrix gets the same bits.  Refuses NULL pointers, W < 1 and n < 0 before any launch. */
+int bx_dp_mean(const float *gathered, int W, long long n, float *out, int32_t *count, void *stream);
+
 /* ---- loader-side ground truth: point-to-point ICP ---------------------------------------------------
  * Replaces open3d.pipelines.registration.registration_icp(source, target, r, init, TransformationEstimationPointToPoint(),
  * ICPConvergenceCriteria(...)) (Open3D 0.18), which the KITTI loader runs on the CPU to refine every pair's ground-truth
