@@ -21,7 +21,7 @@ OBJ = os.path.join(HERE, "_obj")
 
 EXACT = ["bx_api.cu", "bx_fps.cu", "bx_fps_large.cu", "bx_radius.cu", "bx_patches.cu", "bx_spt.cu", "bx_match.cu", "bx_ransac.cu", "bx_neighbors.cu",
          "bx_bootstrap.cu", "bx_train.cu", "bx_group.cu", "bx_svd.cu", "bx_icp.cu", "bx_dp.cu"]
-FAST = ["bx_conv.cu", "bx_conv_tc.cu", "bx_conv_sd.cu", "bx_train_step.cu", "bx_train_desc.cu"]
+FAST = ["bx_conv.cu", "bx_conv_tc.cu", "bx_conv_sd.cu", "bx_conv_ps.cu", "bx_train_step.cu", "bx_train_desc.cu"]
 ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 COMMON = ["-O3", "-lineinfo", "-std=c++17", "-Xcompiler", "-fPIC,-fvisibility=hidden", "--expt-relaxed-constexpr"]
 

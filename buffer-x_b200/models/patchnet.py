@@ -31,6 +31,9 @@ USE_TF32_DESC = os.environ.get("BX_CONV", "sd").lower() == "tc"
 # they have been scheduled), so the static stride stays the default; that was measured on the B200 and has not been
 # re-measured on the H100.  The path is kept and tested.
 DYNAMIC_TILES = os.environ.get("BX_SD_DYNAMIC", "0") == "1"
+# BX_DESC_CONV=sd: the descriptor stack's presplit-input layers on conv_sd_kernel (128-row tiles, all 176 raster rows of a
+# sample computed) instead of the per-sample kernel (bx_conv_ps.cu, the default), for A/B runs.  Both write the same bytes.
+DESC_CONV_SD = os.environ.get("BX_DESC_CONV", "ps").lower() == "sd"
 
 
 def fold_conv_bn(conv_w, conv_b, bn_mean=None, bn_var=None, bn_w=None, bn_b=None, eps=1e-5):
@@ -209,8 +212,12 @@ class Cylindrical_Net(_ConvStack):
             out = torch.empty((K, l["cout"] // 4, 140, 4), dtype=torch.float32, device=dev)
             if use_sd:       # layer-to-layer activations in the presplit padded fp16 format; fp32 in at the first, fp32 out at the last layer
                 out = out if i == len(L) - 1 else ops.conv_sd_buffer(K, l["cout"], dev)
-                ops.conv_layer_sd(ops.GEOM_CYL3D if i == 0 else ops.GEOM_CYL2D, cur, l["w_sd"], l["b"], out, K, l["cin"], l["cout"], l["relu"], flag,
-                                  d_n=d_n, tile_ctr=None if ctrs is None else ctrs[2 * i:2 * i + 2])
+                # presplit input and output: the per-sample kernel.  conv_sd_kernel keeps an fp32 first-layer input (its loader
+                # warps) and the fp32-output last layer, whose two-chunk mainloop is too short to pay for the per-sample epilogue
+                # (DESIGN.md section 5: 3.5 % slower on the per-sample kernel)
+                conv = ops.conv_layer_ps if cur.dtype == torch.float16 and out.dtype == torch.float16 and not DESC_CONV_SD else ops.conv_layer_sd
+                conv(ops.GEOM_CYL3D if i == 0 else ops.GEOM_CYL2D, cur, l["w_sd"], l["b"], out, K, l["cin"], l["cout"], l["relu"], flag,
+                     d_n=d_n, tile_ctr=None if ctrs is None else ctrs[2 * i:2 * i + 2])
                 cur = out
                 continue
             if i == 0:

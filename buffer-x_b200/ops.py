@@ -24,7 +24,7 @@ SYMBOLS = [
     "bx_pool_desc", "bx_mutual_nn",
     "bx_hypotheses", "bx_consensus", "bx_ransac_workspace_bytes", "bx_ransac", "bx_refine", "bx_conv_tc_set_segment_stages",
     "bx_radius_neighbors", "bx_grid_subsample", "bx_costvol_ab", "bx_concat_matches",
-    "bx_pca_analysis", "bx_project_range", "bx_voxel_down_sample", "bx_conv_layer_sd", "bx_conv_sd_rows", "bx_spt_pnt_sd", "bx_fps_set_sync_mode", "bx_conv_layer_sd_costab", "bx_lrf_batched", "bx_select_patches_batched", "bx_fps_ex", "bx_select_patches_grid", "bx_select_patches_grid_workspace_bytes", "bx_select_patches_grid_batched",
+    "bx_pca_analysis", "bx_project_range", "bx_voxel_down_sample", "bx_conv_layer_sd", "bx_conv_layer_ps", "bx_conv_sd_rows", "bx_spt_pnt_sd", "bx_fps_set_sync_mode", "bx_conv_layer_sd_costab", "bx_lrf_batched", "bx_select_patches_batched", "bx_fps_ex", "bx_select_patches_grid", "bx_select_patches_grid_workspace_bytes", "bx_select_patches_grid_batched",
     "bx_gt_matches", "bx_so2_augment", "bx_equi_match", "bx_so2_gt",
     "bx_select_patches_batched_n", "bx_select_patches_grid_batched_n", "bx_lrf_batched_n", "bx_spt_pnt_sd_n", "bx_pool_desc_n",
     "bx_mutual_nn_n", "bx_early_exit_gate",
@@ -102,6 +102,7 @@ def load_library():
     lib.bx_conv_layer_tc.argtypes = [c_int, P, P, P, P, c_int, P] + [c_int] * 9 + [P, P, P]
     lib.bx_conv_tc_ntile.argtypes = [c_int]
     lib.bx_conv_layer_sd.argtypes = [c_int, P, c_int, P, P, P, c_int, c_int, P, c_int, c_int, c_int, c_int, c_int, P, P, P]
+    lib.bx_conv_layer_ps.argtypes = [c_int, P, c_int, P, P, P, c_int, c_int, P, c_int, c_int, c_int, c_int, c_int, P, P, P]
     lib.bx_conv_sd_rows.argtypes = [c_int, c_int]
     lib.bx_conv_layer_sd_costab.argtypes = [P, P, P, P, P, c_int, c_int, P, c_int, P, P]
     lib.bx_fps_set_sync_mode.argtypes = [c_int]
@@ -680,6 +681,22 @@ def conv_layer_sd(geom, x, w_sd, bias, out, n, Cin, Cout, relu, flag=None, d_n=N
     _check(load_library().bx_conv_layer_sd(geom, _dp(x, None, "x"), int(in_sd), _dp(w_sd, torch.float16, "w_sd"), _dp(bias, F32, "bias"),
                                            _dp(out, None, "out"), int(out_sd), int(n), _dp(d_n, I32, "d_n"), Cin, Cout, int(D), int(W), int(bool(relu)),
                                            _dp(flag, I32, "flag"), _dp(tile_ctr, I32, "tile_ctr"), _stream()), "bx_conv_layer_sd")
+    if ev:
+        ev[1].record()
+    return out
+
+
+def conv_layer_ps(geom, x, w_sd, bias, out, n, Cin, Cout, relu, flag=None, d_n=None, D=0, W=0, tile_ctr=None):
+    """A descriptor-stack layer (GEOM_CYL3D / GEOM_CYL2D) on the per-sample kernel (bx_conv_layer_ps): the arguments and the
+    bytes written are those of ``conv_layer_sd``; x must be the presplit fp16 image [Cin/16, 4, rows, 8]."""
+    ev = None
+    if profiler is not None:
+        ev = profiler.span("conv_desc", 2.0 * n * 140 * Cout * Cin * (27 if geom == GEOM_CYL3D else 9))
+        ev[0].record()
+    _check(load_library().bx_conv_layer_ps(geom, _dp(x, None, "x"), int(x.dtype == torch.float16), _dp(w_sd, torch.float16, "w_sd"),
+                                           _dp(bias, F32, "bias"), _dp(out, None, "out"), int(out.dtype == torch.float16), int(n),
+                                           _dp(d_n, I32, "d_n"), Cin, Cout, int(D), int(W), int(bool(relu)), _dp(flag, I32, "flag"),
+                                           _dp(tile_ctr, I32, "tile_ctr"), _stream()), "bx_conv_layer_ps")
     if ev:
         ev[1].record()
     return out

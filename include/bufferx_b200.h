@@ -279,6 +279,13 @@ int bx_conv_layer_sd(int geom, const void *in, int in_presplit, const void *w_sd
                      int n, const int32_t *d_n, int Cin, int Cout, int D, int W, int relu, int32_t *d_flag, int32_t *d_tile_ctr,
                      void *stream);
 long long bx_conv_sd_rows(int n, int rows_per_sample);
+/* The descriptor-stack layers (geom = BX_GEOM_CYL3D / BX_GEOM_CYL2D, presplit input) on the per-sample kernel
+ * (bx_conv_ps.cu): same arguments, weight image and bytes written as bx_conv_layer_sd, bit-identical values.  A sample's
+ * 152 live raster rows are one wgmma operand, so the 24 dead rows (y = 7) of every sample are never computed.  D, W unused;
+ * d_tile_ctr schedules units of one sample (Cout > 64) or two (Cout <= 64). */
+int bx_conv_layer_ps(int geom, const void *in, int in_presplit, const void *w_sd, const float *bias, void *out, int out_presplit,
+                     int n, const int32_t *d_n, int Cin, int Cout, int D, int W, int relu, int32_t *d_flag, int32_t *d_tile_ctr,
+                     void *stream);
 /* The second CostNet layer (32 -> 64, k = 3x3x3 over relu(A - B) regenerated from the factor maps of bx_costvol_ab) as a
  * 96 -> 64, k = (3,1,3) convolution over the 18 x 18 (n, l) raster on the same kernel.  fa [n,8,60,4], fb [n,8,54,4] fp32;
  * w_sd: ops.conv_sd_weights_costab; out: fp32 [n,16,256,4] or presplit over the 16 x 16 raster (rows = bx_conv_sd_rows(n, 256)). */
