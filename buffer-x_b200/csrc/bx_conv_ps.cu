@@ -31,8 +31,8 @@
 //   epilogue    the next layer's presplit image (ReLU, fp16 hi / lo, the wrap columns, the zero row of sample s + 1 and of
 //               sample 0), or fp32 channel-blocked for the last layer -- the bytes conv_sd_kernel writes.  A finished sample
 //               goes through a shared-memory staging buffer 32 rows at a time.
-//   scheduling  persistent CTAs, one per SM, static stride or the dynamic unit counter (d_tile_ctr); the device sample count
-//               d_n bounds the units.  Weights resident when the whole image fits next to two A chunks per warpgroup
+//   scheduling  persistent CTAs, one per SM, each taking every gridDim.x-th unit; the device sample count d_n bounds the
+//               units.  Weights resident when the whole image fits next to two A chunks per warpgroup
 //               stream, else streamed in stages of three taps, as in conv_sd_kernel.
 #include <cuda_fp16.h>
 
@@ -51,7 +51,6 @@ constexpr int PS_CHUNK = 4 * PS_KBYTES;          // [split(hi,lo)][kcore(2)]
 constexpr int PS_NC = 8;                         // MMA warps: two warpgroups
 constexpr int PS_WGT_WARP = PS_NC + 3;           // weight thread: last warp of the producer warpgroup
 constexpr int PS_MAXNA = 12, PS_MAXNBS = 24;     // A chunk slots; weight stages
-constexpr int PS_TRING = 32;                     // published units of dynamic scheduling
 constexpr int PS_SR = 32;                        // rows per staging round of a finished sample
 constexpr int PS_SMEM = 227 * 1024 - 2048;       // dynamic shared memory of one CTA (the rest: barriers, bias)
 
@@ -63,7 +62,6 @@ struct ConvPsParams {
     __half *out_sd;            // presplit padded output [Cout/16][4][rows_out][8 x fp16] (OUT_SD = 1)
     int *flag;
     const int *d_n;            // optional device-side sample count (<= n)
-    int *tile_ctr;             // dynamic scheduling: [0] next unit, [1] CTAs that have finished; NULL = static stride
     long long rows_in, rows_out;
     int n, Cout, nchunks, relu, NA, nbs, resident;
 };
@@ -171,10 +169,9 @@ __global__ void __launch_bounds__(PsCfg<NT>::THREADS, 1) conv_ps_kernel(const Co
     using C = PsCfg<NT>;
     constexpr int SPU = C::SPU, CH = C::CH, NACC = C::NACC, NRUN = C::NRUN;
     constexpr int BAR_AFULL = 0, BAR_AEMPTY = PS_MAXNA, BAR_BFULL = 2 * PS_MAXNA, BAR_BEMPTY = BAR_BFULL + PS_MAXNBS;
-    constexpr int BAR_UNIT = BAR_BEMPTY + PS_MAXNBS, NBARS = BAR_UNIT + PS_TRING;
+    constexpr int NBARS = BAR_BEMPTY + PS_MAXNBS;
     extern __shared__ __align__(128) unsigned char smem[];
     __shared__ __align__(8) unsigned long long bars[NBARS];
-    __shared__ int unit_ring[PS_TRING];
     __shared__ __align__(16) float bias_s[128];
 
     const int tid = threadIdx.x, lane = tid & 31;
@@ -182,7 +179,7 @@ __global__ void __launch_bounds__(PsCfg<NT>::THREADS, 1) conv_ps_kernel(const Co
     const int NA = p.NA, NBS = p.nbs, nchunks = p.nchunks;
     const bool resident = p.resident != 0;
     const int n_samples = p.d_n ? min(*p.d_n, p.n) : p.n;
-    const int n_units = (n_samples + SPU - 1) / SPU;
+    const int n_units = (n_samples + SPU - 1) / SPU;          // CTA b takes units b, b + gridDim.x, ...
     // shared memory: A ring | weight ring | staging buffer of a finished sample
     float *const stage = reinterpret_cast<float *>(smem + (size_t)NA * PS_CHUNK + (size_t)NBS * C::B_STAGE);
 
@@ -195,7 +192,6 @@ __global__ void __launch_bounds__(PsCfg<NT>::THREADS, 1) conv_ps_kernel(const Co
             mbar_init(smem_u32(&bars[BAR_BFULL + s]), 1);
             mbar_init(smem_u32(&bars[BAR_BEMPTY + s]), PS_NC);
         }
-        for (int s = 0; s < PS_TRING; ++s) mbar_init(smem_u32(&bars[BAR_UNIT + s]), 1);
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
     if (threadIdx.x < 128) bias_s[threadIdx.x] = (int)threadIdx.x < p.Cout ? __ldg(p.bias + threadIdx.x) : 0.0f;
@@ -204,15 +200,6 @@ __global__ void __launch_bounds__(PsCfg<NT>::THREADS, 1) conv_ps_kernel(const Co
     uint32_t b_base = a_base + (uint32_t)NA * PS_CHUNK;
     uint32_t bar_base = smem_u32(&bars[0]);
     asm volatile("" : "+r"(a_base), "+r"(b_base), "+r"(bar_base));
-
-    // Unit sequence of this CTA: static stride, or (p.tile_ctr) drawn by the A producer from a global counter and published
-    // in a shared-memory ring that the other roles read (-1 = no more units).
-    const bool dyn = p.tile_ctr != nullptr;
-    auto unit_of = [&](uint32_t k) -> int {
-        if (!dyn) { const long long u = (long long)blockIdx.x + (long long)k * gridDim.x; return u < n_units ? (int)u : -1; }
-        mbar_wait(bar_base + 8u * (BAR_UNIT + (k & (PS_TRING - 1))), (k / PS_TRING) & 1u);
-        return unit_ring[k & (PS_TRING - 1)];
-    };
 
     if (warp < PS_NC) {
         // =========================== MMA warpgroups: wgmma, chunk folds, sample stores ===================================
@@ -234,7 +221,7 @@ __global__ void __launch_bounds__(PsCfg<NT>::THREADS, 1) conv_ps_kernel(const Co
         auto jb = [](int i) { return NT == 32 ? i >> 1 : i >> 2; };
         auto ch = [&](int i) { return NT == 32 ? 8 * wq + (lane >> 2) : 16 * wq + (lane >> 2) + 8 * ((i & 3) >> 1); };
         auto col = [&](int i) { return 8 * jb(i) + 2 * (lane & 3) + (i & 1); };
-        uint32_t slot = 0, a_par = 0, q = 0, k = 0;
+        uint32_t slot = 0, a_par = 0, q = 0;
         float run[NRUN], acc[NACC];
         // the wgmmas of one N pass of a chunk (27 for Cout >= 64, 18 for Cout <= 32), then one wait and the fold.  Pass h
         // covers sample rows h * NB0 .. h * NB0 + NB - 1: B descriptors h * NB0 rows on, running sums run[h * NB0 / 2 ...]
@@ -295,7 +282,7 @@ __global__ void __launch_bounds__(PsCfg<NT>::THREADS, 1) conv_ps_kernel(const Co
         };
         float *const st = stage + (size_t)wg * PS_SR * CH;                   // this warpgroup's [CH / 4][32 rows][4]
         const float4 *st4 = reinterpret_cast<const float4 *>(st);
-        for (int u = unit_of(0); u >= 0; u = unit_of(++k)) {
+        for (int u = blockIdx.x; u < n_units; u += gridDim.x) {
 #pragma unroll
             for (int i = 0; i < NRUN; ++i) run[i] = bias_s[co_wg + ch(i)];
             for (int c = 0; c < nchunks; ++c) chunk(c);
@@ -339,17 +326,7 @@ __global__ void __launch_bounds__(PsCfg<NT>::THREADS, 1) conv_ps_kernel(const Co
             if (lane == 0) {
                 const uint32_t nslots = (uint32_t)NA / SPU;
                 uint32_t slot = 0, par = 0, round = 0;
-                for (uint32_t k = 0;; ++k) {
-                    int u;
-                    if (dyn) {
-                        u = atomicAdd(p.tile_ctr, 1);
-                        if (u >= n_units) u = -1;
-                        unit_ring[k & (PS_TRING - 1)] = u;
-                        mbar_arrive(bar_base + 8u * (BAR_UNIT + (k & (PS_TRING - 1))));
-                    } else {
-                        u = unit_of(k);
-                    }
-                    if (u < 0) break;
+                for (int u = blockIdx.x; u < n_units; u += gridDim.x) {
                     for (int c = 0; c < nchunks; ++c) {
 #pragma unroll
                         for (uint32_t g = 0; g < (uint32_t)SPU; ++g) {
@@ -373,8 +350,7 @@ __global__ void __launch_bounds__(PsCfg<NT>::THREADS, 1) conv_ps_kernel(const Co
             if (lane == 0) {
                 const int n_st = nchunks * 3;
                 uint32_t q = 0;
-                for (uint32_t k = 0; unit_of(k) >= 0; ++k) {
-                    if (resident && k >= 1) break;                      // resident weights: loaded for the first unit only
+                for (int u = blockIdx.x; u < n_units; u += gridDim.x) {
                     for (int s = 0; s < n_st; ++s, ++q) {
                         const uint32_t sb = q % (uint32_t)NBS, use = q / (uint32_t)NBS;
                         if (use > 0) mbar_wait(bar_base + 8u * (BAR_BEMPTY + sb), (use - 1) & 1u);
@@ -382,15 +358,11 @@ __global__ void __launch_bounds__(PsCfg<NT>::THREADS, 1) conv_ps_kernel(const Co
                         bulk_g2s(b_base + sb * (uint32_t)C::B_STAGE, reinterpret_cast<const unsigned char *>(p.w) + (size_t)s * C::B_STAGE,
                                  (uint32_t)C::B_STAGE, bar_base + 8u * (BAR_BFULL + sb));
                     }
+                    if (resident) break;                                // resident weights: loaded for the first unit only
                 }
             }
             __syncwarp();
         }
-    }
-    __syncthreads();
-    if (dyn && tid == 0) {      // the last CTA to finish rewinds the counters for the next launch that uses them
-        __threadfence();
-        if (atomicAdd(p.tile_ctr + 1, 1) == (int)gridDim.x - 1) { p.tile_ctr[0] = 0; p.tile_ctr[1] = 0; __threadfence(); }
     }
 }
 
@@ -430,7 +402,7 @@ int dispatch_ps(const ConvPsParams &p, int out_sd, cudaStream_t st) {
 }  // namespace
 
 BX_API int bx_conv_layer_ps(int geom, const void *in, int in_presplit, const void *w_sd, const float *bias, void *out, int out_presplit,
-                            int n, const int32_t *d_n, int Cin, int Cout, int D, int W, int relu, int32_t *d_flag, int32_t *d_tile_ctr, void *stream) {
+                            int n, const int32_t *d_n, int Cin, int Cout, int D, int W, int relu, int32_t *d_flag, void *stream) {
     (void)D; (void)W;
     BX_REQUIRE(in && w_sd && bias && out, "bx_conv_layer_ps: null pointer");
     BX_REQUIRE(geom == BX_GEOM_CYL3D || geom == BX_GEOM_CYL2D, "bx_conv_layer_ps: geometry must be CYL3D or CYL2D (the descriptor stack)");
@@ -444,7 +416,7 @@ BX_API int bx_conv_layer_ps(int geom, const void *in, int in_presplit, const voi
     BX_REQUIRE((long long)n * PS_SROWS + 4 * 128 < 0x7fffffffLL, "bx_conv_layer_ps: too many samples (raster rows must stay below 2^31)");
     ConvPsParams p = {};
     p.in_sd = reinterpret_cast<const __half *>(in);
-    p.w = reinterpret_cast<const __half *>(w_sd); p.bias = bias; p.flag = d_flag; p.d_n = d_n; p.tile_ctr = d_tile_ctr;
+    p.w = reinterpret_cast<const __half *>(w_sd); p.bias = bias; p.flag = d_flag; p.d_n = d_n;
     p.out = out_presplit ? nullptr : reinterpret_cast<float *>(out);
     p.out_sd = out_presplit ? reinterpret_cast<__half *>(out) : nullptr;
     p.n = n; p.Cout = Cout; p.relu = relu;

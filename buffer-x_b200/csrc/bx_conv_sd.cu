@@ -73,7 +73,6 @@ constexpr int SD_NL = 3;                         // loader warps (fp32 input)
 constexpr int SD_NC = 8;                         // MMA warps: two warpgroups of 64 tile rows
 constexpr int SD_WGT_WARP = SD_NC + 3;           // weight thread: last warp of the producer warpgroup
 constexpr int SD_MAXNA = 12, SD_MAXNBS = 24;     // A chunk slots; weight stages (resident: every stage of up to 8 chunks)
-constexpr int SD_TRING = 32;                     // published tile indices of dynamic scheduling
 constexpr int SD_SMEM = 227 * 1024 - 2048;       // dynamic shared memory of one CTA (the rest: barriers, bias)
 
 struct ConvSdParams {
@@ -91,7 +90,6 @@ struct ConvSdParams {
     long long rows_in, rows_out;
     int nbs;                   // weight ring length in stages of three taps (resident: == nchunks * 3, every stage is loaded once)
     int resident;              // the whole weight image stays in shared memory: no re-streaming per tile
-    int *tile_ctr;             // dynamic tile scheduling (presplit-input kernels): [0] next tile, [1] CTAs that have finished; NULL = static stride
 };
 
 template <int NT, int IN_SD> struct SdCfg {
@@ -201,10 +199,9 @@ __global__ void __launch_bounds__(SdCfg<NT, IN_SD>::THREADS, 1) conv_sd_kernel(c
     using C = SdCfg<NT, IN_SD>;
     constexpr int NB = C::NB, NH = C::NH, SB = C::SB, WGT_WARP = SD_WGT_WARP;
     constexpr int BAR_AFULL = 0, BAR_AEMPTY = SD_MAXNA, BAR_BFULL = 2 * SD_MAXNA, BAR_BEMPTY = BAR_BFULL + SD_MAXNBS;
-    constexpr int BAR_TILE = BAR_BEMPTY + SD_MAXNBS, NBARS = BAR_TILE + SD_TRING;
+    constexpr int NBARS = BAR_BEMPTY + SD_MAXNBS;
     extern __shared__ __align__(128) unsigned char smem[];
     __shared__ __align__(8) unsigned long long bars[NBARS];
-    __shared__ int tile_ring[SD_TRING];
     __shared__ __align__(16) float bias_s[128];        // the running sums of a tile start from the bias
 
     const int tid = threadIdx.x, lane = tid & 31;
@@ -213,7 +210,7 @@ __global__ void __launch_bounds__(SdCfg<NT, IN_SD>::THREADS, 1) conv_sd_kernel(c
     const bool resident = p.resident != 0;
     const int n_samples = p.d_n ? min(*p.d_n, p.n) : p.n;
     const int n_tiles = (int)(((long long)n_samples * p.rs + SD_BM - 1) / SD_BM);   // <= the host's bound the grid was sized for
-    const int n_units = (n_tiles + C::TPU - 1) / C::TPU;
+    const int n_units = (n_tiles + C::TPU - 1) / C::TPU;      // units of C::TPU tiles; CTA b takes units b, b + gridDim.x, ...
     // shared memory: A ring | weight ring | staging buffer of a finished tile (C::STAGE_BYTES)
     float *const stage = reinterpret_cast<float *>(smem + (size_t)NA * SD_CHUNK + (size_t)NBS * C::B_STAGE);
 
@@ -226,7 +223,6 @@ __global__ void __launch_bounds__(SdCfg<NT, IN_SD>::THREADS, 1) conv_sd_kernel(c
             mbar_init(smem_u32(&bars[BAR_BFULL + s]), 1);
             mbar_init(smem_u32(&bars[BAR_BEMPTY + s]), SD_NC);
         }
-        for (int s = 0; s < SD_TRING; ++s) mbar_init(smem_u32(&bars[BAR_TILE + s]), 1);
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
     if (threadIdx.x < 128) bias_s[threadIdx.x] = (int)threadIdx.x < p.Cout ? __ldg(p.bias + threadIdx.x) : 0.0f;
@@ -235,18 +231,6 @@ __global__ void __launch_bounds__(SdCfg<NT, IN_SD>::THREADS, 1) conv_sd_kernel(c
     uint32_t b_base = a_base + (uint32_t)NA * SD_CHUNK;
     uint32_t bar_base = smem_u32(&bars[0]);
     asm volatile("" : "+r"(a_base), "+r"(b_base), "+r"(bar_base));
-
-    // Unit sequence of this CTA (a unit is C::TPU tiles).  Static: blockIdx.x, + gridDim.x, ...  Dynamic (presplit input,
-    // p.tile_ctr): the A producer draws the next unit from a global counter and publishes it in a shared-memory ring; every
-    // other role reads the k-th entry (-1 = no more units).  With several pairs in flight a convolution often starts with some
-    // SMs still held by another stream's kernels; with the static stride the CTAs that start late still own their share of
-    // the tiles and the whole launch waits for them.
-    const bool dyn = IN_SD && p.tile_ctr != nullptr;
-    auto tile_of = [&](uint32_t k) -> int {
-        if (!dyn) { const long long t = (long long)blockIdx.x + (long long)k * gridDim.x; return t < n_units ? (int)t : -1; }
-        mbar_wait(bar_base + 8u * (BAR_TILE + (k & (SD_TRING - 1))), (k / SD_TRING) & 1u);
-        return tile_ring[k & (SD_TRING - 1)];
-    };
 
     // Each role branch starts with its warpgroup's setmaxnreg (one instruction for all threads of a warpgroup): the MMA
     // warpgroups take the registers the producer warpgroup gives up.
@@ -260,7 +244,7 @@ __global__ void __launch_bounds__(SdCfg<NT, IN_SD>::THREADS, 1) conv_sd_kernel(c
         // weight image [kcore][split][WR][16 B]: K-adjacent core matrices one kcore (2 WR rows) apart, taps 64 WR rows apart
         constexpr uint32_t B_LBO = ((uint32_t)(2 * C::WR * 16) >> 4) << 16, B_TAP16 = (64u * C::WR) >> 4;
         const uint32_t Wrow = (uint32_t)p.W;                             // tap (g, tt) reads rows R + g * W + tt
-        uint32_t slot = 0, a_par = 0, q = 0, k = 0;
+        uint32_t slot = 0, a_par = 0, q = 0;
         if constexpr (C::CM) {
             // ---- channels-as-M: warpgroup wg owns tile 2u + wg; weights = A operand (64 channel rows), activations = B (128 rows)
             // Fragment of thread (warp w = warp & 3, lane): acc[4j + e] is M row 16 w + lane / 4 + 8 (e / 2), tile row
@@ -320,7 +304,7 @@ __global__ void __launch_bounds__(SdCfg<NT, IN_SD>::THREADS, 1) conv_sd_kernel(c
             };
             float *const st = stage + (size_t)wg * 64 * NT;                  // this warpgroup's [NT / 4][64 rows][4]
             const float4 *st4 = reinterpret_cast<const float4 *>(st);
-            for (int u = tile_of(0); u >= 0; u = tile_of(++k)) {
+            for (int u = blockIdx.x; u < n_units; u += gridDim.x) {
 #pragma unroll
                 for (int i = 0; i < NT; ++i) run[i] = bias_s[ch(i)];
                 // Two chunks per iteration, the second one guarded: the code of a chunk appears twice, so a Cout <= 32 kernel
@@ -356,7 +340,7 @@ __global__ void __launch_bounds__(SdCfg<NT, IN_SD>::THREADS, 1) conv_sd_kernel(c
             const uint32_t a0 = ((a_base + (uint32_t)wg * 64u * 16u) >> 4) | A_LBO;   // this warpgroup's 64 rows
             const uint32_t b0 = (b_base >> 4) | B_LBO;
             float run[NT / 2], acc[NB];      // acc = [main NB / 2 | cross NB / 2]: disjoint blocks, each written by whole wgmmas
-            for (int t = tile_of(0); t >= 0; t = tile_of(++k)) {
+            for (int t = blockIdx.x; t < n_units; t += gridDim.x) {
 #pragma unroll
                 for (int i = 0; i < NT / 2; ++i) run[i] = bias_s[(i / (NB / 2)) * NB + 8 * ((i % (NB / 2)) >> 2) + cq + (i & 1)];
                 for (int c = 0; c < nchunks; ++c) {
@@ -437,17 +421,7 @@ __global__ void __launch_bounds__(SdCfg<NT, IN_SD>::THREADS, 1) conv_sd_kernel(c
                     constexpr uint32_t TPU = C::TPU;
                     const uint32_t nslots = (uint32_t)NA / TPU;
                     uint32_t slot = 0, par = 0, round = 0;
-                    for (uint32_t k = 0;; ++k) {
-                        int u;
-                        if (dyn) {           // draw the next unit and publish it to the other roles
-                            u = atomicAdd(p.tile_ctr, 1);
-                            if (u >= n_units) u = -1;
-                            tile_ring[k & (SD_TRING - 1)] = u;
-                            mbar_arrive(bar_base + 8u * (BAR_TILE + (k & (SD_TRING - 1))));
-                        } else {
-                            u = tile_of(k);
-                        }
-                        if (u < 0) break;
+                    for (int u = blockIdx.x; u < n_units; u += gridDim.x) {
                         for (int c = 0; c < nchunks; ++c) {
 #pragma unroll
                             for (uint32_t g = 0; g < TPU; ++g) {
@@ -581,8 +555,7 @@ __global__ void __launch_bounds__(SdCfg<NT, IN_SD>::THREADS, 1) conv_sd_kernel(c
             if (lane == 0) {
                 const int n_st = nchunks * 3;
                 uint32_t q = 0;
-                for (uint32_t k = 0; tile_of(k) >= 0; ++k) {
-                    if (resident && k >= 1) break;                      // resident weights: loaded by the first tile, never again
+                for (int u = blockIdx.x; u < n_units; u += gridDim.x) {
                     for (int s = 0; s < n_st; ++s, ++q) {
                         const uint32_t sb = q % (uint32_t)NBS, use = q / (uint32_t)NBS;
                         if (use > 0) mbar_wait(bar_base + 8u * (BAR_BEMPTY + sb), (use - 1) & 1u);
@@ -590,15 +563,11 @@ __global__ void __launch_bounds__(SdCfg<NT, IN_SD>::THREADS, 1) conv_sd_kernel(c
                         bulk_g2s(b_base + sb * (uint32_t)C::B_STAGE, reinterpret_cast<const unsigned char *>(p.w) + (size_t)s * C::B_STAGE,
                                  (uint32_t)C::B_STAGE, bar_base + 8u * (BAR_BFULL + sb));
                     }
+                    if (resident) break;                                // resident weights: loaded by the first unit, never again
                 }
             }
             __syncwarp();
         }
-    }
-    __syncthreads();
-    if (dyn && tid == 0) {      // the last CTA to finish rewinds the counters for the next launch that uses them
-        __threadfence();
-        if (atomicAdd(p.tile_ctr + 1, 1) == (int)gridDim.x - 1) { p.tile_ctr[0] = 0; p.tile_ctr[1] = 0; __threadfence(); }
     }
 }
 
@@ -647,7 +616,7 @@ BX_API long long bx_conv_sd_rows(int n, int rows_per_sample) {
 }
 
 BX_API int bx_conv_layer_sd(int geom, const void *in, int in_presplit, const void *w_sd, const float *bias, void *out, int out_presplit,
-                            int n, const int32_t *d_n, int Cin, int Cout, int D, int W, int relu, int32_t *d_flag, int32_t *d_tile_ctr, void *stream) {
+                            int n, const int32_t *d_n, int Cin, int Cout, int D, int W, int relu, int32_t *d_flag, void *stream) {
     BX_REQUIRE(in && w_sd && bias && out, "bx_conv_layer_sd: null pointer");
     BX_REQUIRE(geom == BX_GEOM_CYL3D || geom == BX_GEOM_CYL2D || geom == BX_GEOM_VALID3D, "bx_conv_layer_sd: geometry must be CYL3D, CYL2D or VALID3D (k = 3x1x3)");
     BX_REQUIRE(n >= 0 && Cin >= 16 && Cin % 16 == 0 && Cout >= 4 && Cout % 4 == 0 && Cout <= 128, "bx_conv_layer_sd: bad channels Cin=%d Cout=%d", Cin, Cout);
@@ -658,7 +627,7 @@ BX_API int bx_conv_layer_sd(int geom, const void *in, int in_presplit, const voi
                "bx_conv_layer_sd: activations, weights and bias must be 16-byte aligned");
     if (n == 0) return BX_OK;
     ConvSdParams p = {};
-    p.w = reinterpret_cast<const __half *>(w_sd); p.bias = bias; p.flag = d_flag; p.d_n = d_n; p.tile_ctr = d_tile_ctr;
+    p.w = reinterpret_cast<const __half *>(w_sd); p.bias = bias; p.flag = d_flag; p.d_n = d_n;
     p.in = in_presplit ? nullptr : reinterpret_cast<const float *>(in);
     p.in_sd = in_presplit ? reinterpret_cast<const __half *>(in) : nullptr;
     p.out = out_presplit ? nullptr : reinterpret_cast<float *>(out);

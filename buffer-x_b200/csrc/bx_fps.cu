@@ -46,23 +46,11 @@ __device__ __forceinline__ Cand warp_best(const Cand c) {
     return r;
 }
 
-// ---- cluster exchange without cluster.sync: remote stores + remote mbarrier arrive (release.cluster), local wait
-//      (acquire.cluster).  A cluster.sync per FPS iteration is a full cluster barrier and flushes L1; this costs one
-//      DSMEM round.
 __device__ __forceinline__ uint32_t fps_smem_u32(const void *p) { return (uint32_t)__cvta_generic_to_shared(p); }
 __device__ __forceinline__ uint32_t fps_mapa(uint32_t saddr, uint32_t cta) {
     uint32_t r;
     asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(r) : "r"(saddr), "r"(cta));
     return r;
-}
-__device__ __forceinline__ void fps_st_cluster_v4(uint32_t a, uint4 v) {
-    asm volatile("st.shared::cluster.v4.u32 [%0], {%1, %2, %3, %4};" ::"r"(a), "r"(v.x), "r"(v.y), "r"(v.z), "r"(v.w) : "memory");
-}
-__device__ __forceinline__ void fps_st_cluster_f32(uint32_t a, float v) {
-    asm volatile("st.shared::cluster.f32 [%0], %1;" ::"r"(a), "f"(v) : "memory");
-}
-__device__ __forceinline__ void fps_arrive_cluster(uint32_t rbar) {
-    asm volatile("mbarrier.arrive.release.cluster.shared::cluster.b64 _, [%0];" ::"r"(rbar) : "memory");
 }
 // One-way exchange: st.async writes 16 bytes into the peer's shared memory AND completes that many transaction bytes on the
 // peer's mbarrier when they have landed -- no separate release-arrive that has to wait for the stores (one DSMEM trip
@@ -92,7 +80,7 @@ __device__ __forceinline__ void fps_wait_cluster(uint32_t bar, uint32_t parity) 
 template <int THREADS, int PPT>
 __global__ void __launch_bounds__(THREADS, 1)
 fps_cluster_kernel(const float *__restrict__ xyz_all, const FpsOffsets offsets, int npoint,
-                   int *__restrict__ idx_out, float *__restrict__ kpts_out, int sync_mode, const int *__restrict__ d_counts) {
+                   int *__restrict__ idx_out, float *__restrict__ kpts_out, const int *__restrict__ d_counts) {
     constexpr int NW = THREADS / 32;
     cg::cluster_group cluster = cg::this_cluster();
     const int CL = (int)cluster.num_blocks();
@@ -116,11 +104,8 @@ fps_cluster_kernel(const float *__restrict__ xyz_all, const FpsOffsets offsets, 
 
     __shared__ uint4 w_a[2][32];
     __shared__ float w_z[2][32];
-    __shared__ uint4 c_a[2][16];
-    __shared__ float c_z[2][16];
-    __shared__ uint4 x_a[2][16][2];                      // st.async exchange: two 16-byte halves per (parity, sender)
-    __shared__ __align__(8) unsigned long long cbar[2];   // one exchange barrier per parity, CL arrivals each
-    __shared__ __align__(8) unsigned long long xbar[2];   // st.async exchange: 1 arrival (own expect_tx) + 32 * CL bytes per phase
+    __shared__ uint4 x_a[2][16][2];                      // cluster exchange: two 16-byte halves per (parity, sender)
+    __shared__ __align__(8) unsigned long long xbar[2];   // one per parity: 1 arrival (own expect_tx) + 32 * CL bytes per phase
 
     float px[PPT], py[PPT], pz[PPT], tmp[PPT];
     const int stride = CL * THREADS;
@@ -146,8 +131,6 @@ fps_cluster_kernel(const float *__restrict__ xyz_all, const FpsOffsets offsets, 
         if (kp) { kp[0] = p0x; kp[1] = p0y; kp[2] = p0z; }
     }
     if (tid == 0) {
-        asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(fps_smem_u32(&cbar[0])), "r"(CL) : "memory");
-        asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(fps_smem_u32(&cbar[1])), "r"(CL) : "memory");
         asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(fps_smem_u32(&xbar[0])), "r"(1) : "memory");
         asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(fps_smem_u32(&xbar[1])), "r"(1) : "memory");
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
@@ -185,49 +168,29 @@ fps_cluster_kernel(const float *__restrict__ xyz_all, const FpsOffsets offsets, 
             const uint4 a = w_a[par][lane];
             c.hi = a.x; c.lo = a.y; c.x = __uint_as_float(a.z); c.y = __uint_as_float(a.w); c.z = w_z[par][lane];
         }
-        Cand cb = warp_best(c);
-        if (CL > 1 && sync_mode == 0) {
-            // production: every CTA posts its candidate into every peer's slot with st.async (data + transaction bytes in one
-            // DSMEM trip); a CTA's barrier phase completes when its own expect_tx arrival and all 32 * CL bytes are in.
-            if (warp == 0) {
-                if (lane == 0) fps_expect_tx(fps_smem_u32(&xbar[par]), 32u * (uint32_t)CL);
-                if (lane < CL) {
-                    const uint32_t dst = fps_mapa(fps_smem_u32(&x_a[par][rank][0]), (uint32_t)lane);
-                    const uint32_t rb = fps_mapa(fps_smem_u32(&xbar[par]), (uint32_t)lane);
-                    fps_st_async_v4(dst, make_uint4(cb.hi, cb.lo, __float_as_uint(cb.x), __float_as_uint(cb.y)), rb);
-                    fps_st_async_v4(dst + 16u, make_uint4(__float_as_uint(cb.z), 0u, 0u, 0u), rb);
-                }
-            }
-            fps_wait_cluster(fps_smem_u32(&xbar[par]), (uint32_t)(((j >> 1) - (par ? 0 : 1)) & 1));
-            Cand g;
-            g.hi = 0u; g.lo = 0u; g.x = p0x; g.y = p0y; g.z = p0z;
+        const Cand cc = warp_best(c);          // this CTA's candidate
+        // every CTA posts its candidate into every peer's slot with st.async (data + transaction bytes in one DSMEM trip); a
+        // CTA's barrier phase completes when its own expect_tx arrival and all 32 * CL bytes are in.  Buffers and barriers
+        // are double-buffered by parity: a peer can only be one iteration ahead (its next wait needs our next post), so
+        // slot [par] is not rewritten before everybody has read it.
+        if (warp == 0) {
+            if (lane == 0) fps_expect_tx(fps_smem_u32(&xbar[par]), 32u * (uint32_t)CL);
             if (lane < CL) {
-                const uint4 a = x_a[par][lane][0];
-                g.hi = a.x; g.lo = a.y; g.x = __uint_as_float(a.z); g.y = __uint_as_float(a.w);
-                g.z = __uint_as_float(x_a[par][lane][1].x);
+                const uint32_t dst = fps_mapa(fps_smem_u32(&x_a[par][rank][0]), (uint32_t)lane);
+                const uint32_t rb = fps_mapa(fps_smem_u32(&xbar[par]), (uint32_t)lane);
+                fps_st_async_v4(dst, make_uint4(cc.hi, cc.lo, __float_as_uint(cc.x), __float_as_uint(cc.y)), rb);
+                fps_st_async_v4(dst + 16u, make_uint4(__float_as_uint(cc.z), 0u, 0u, 0u), rb);
             }
-            cb = warp_best(g);
-        } else if (CL > 1) {
-            if (warp == 0 && lane < CL) {   // lane = destination CTA: candidate into its slot [rank], then arrive on its barrier
-                fps_st_cluster_v4(fps_mapa(fps_smem_u32(&c_a[par][rank]), (uint32_t)lane),
-                                  make_uint4(cb.hi, cb.lo, __float_as_uint(cb.x), __float_as_uint(cb.y)));
-                fps_st_cluster_f32(fps_mapa(fps_smem_u32(&c_z[par][rank]), (uint32_t)lane), cb.z);
-                if (sync_mode != 1) fps_arrive_cluster(fps_mapa(fps_smem_u32(&cbar[par]), (uint32_t)lane));
-            }
-            // Buffers and barriers are double-buffered by parity: a peer can only be one iteration ahead (its next
-            // wait needs our next arrive), so slot [par] is not rewritten before everybody has read it.
-            // sync_mode (BX_FPS_SYNC=1, verification only): the same exchange ordered by a plain cluster.sync() -- the form
-            // compute-sanitizer's racecheck models; results are bit-identical (tests/test_gpu_parity.py).
-            if (sync_mode == 1) cluster.sync();
-            else fps_wait_cluster(fps_smem_u32(&cbar[par]), (uint32_t)(((j >> 1) - (par ? 0 : 1)) & 1));
-            Cand g;
-            g.hi = 0u; g.lo = 0u; g.x = p0x; g.y = p0y; g.z = p0z;
-            if (lane < CL) {
-                const uint4 a = c_a[par][lane];
-                g.hi = a.x; g.lo = a.y; g.x = __uint_as_float(a.z); g.y = __uint_as_float(a.w); g.z = c_z[par][lane];
-            }
-            cb = warp_best(g);
         }
+        fps_wait_cluster(fps_smem_u32(&xbar[par]), (uint32_t)(((j >> 1) - (par ? 0 : 1)) & 1));
+        Cand g;
+        g.hi = 0u; g.lo = 0u; g.x = p0x; g.y = p0y; g.z = p0z;
+        if (lane < CL) {
+            const uint4 a = x_a[par][lane][0];
+            g.hi = a.x; g.lo = a.y; g.x = __uint_as_float(a.z); g.y = __uint_as_float(a.w);
+            g.z = __uint_as_float(x_a[par][lane][1].x);
+        }
+        const Cand cb = warp_best(g);          // the cluster's winner
         ox = cb.x; oy = cb.y; oz = cb.z;
         if (rank == 0 && tid == 0) {
             int k = 0;
@@ -243,8 +206,6 @@ fps_cluster_kernel(const float *__restrict__ xyz_all, const FpsOffsets offsets, 
     }
     cluster.sync();  // nobody exits while a peer may still write into its shared memory
 }
-
-int g_fps_sync_override = -1;
 
 template <int THREADS, int PPT>
 int launch_fps(const float *xyz, const FpsOffsets off, int B, int CL, int npoint, int *idx, float *kpts, const int *d_counts,
@@ -263,10 +224,7 @@ int launch_fps(const float *xyz, const FpsOffsets off, int B, int CL, int npoint
     at[0].val.clusterDim.z = 1;
     cfg.attrs = at;
     cfg.numAttrs = 1;
-    static int sync_mode = -1;     // BX_FPS_SYNC: 0 = st.async exchange (production), 1 = cluster.sync() (racecheck-clean reference form),
-    if (sync_mode < 0) { const char *e = getenv("BX_FPS_SYNC"); sync_mode = e ? atoi(e) : 0; }   // 2 = remote stores + mbarrier arrive / acquire wait (round 1)
-    if (g_fps_sync_override >= 0) sync_mode = g_fps_sync_override;
-    BX_CUDA(cudaLaunchKernelEx(&cfg, kern, xyz, off, npoint, idx, kpts, sync_mode, d_counts));
+    BX_CUDA(cudaLaunchKernelEx(&cfg, kern, xyz, off, npoint, idx, kpts, d_counts));
     ++g_bx_launches;
     return BX_OK;
 }
@@ -274,26 +232,14 @@ int launch_fps(const float *xyz, const FpsOffsets off, int B, int CL, int npoint
 
 // Launch configuration of a cloud of n points (the largest cloud of the call): register tier = (threads, points per thread,
 // CTAs per cloud).  Also returns, in *hi, the largest n that gets the same configuration -- the cloud's size class.
-enum FpsTier { T256x2, T256x4, T1024x4c, T1024x6c, T1024x10c, T1024x12c, T1024x1c16, T1024x2c16, T1024x2, T1024x3, T1024x4,
-               T1024x8, T1024x8c16, T512x32, T512x64 };
+enum FpsTier { T256x2, T256x4, T1024x2, T1024x3, T1024x4, T1024x8, T1024x8c16, T512x32, T512x64 };
 
-FpsTier fps_tier(int n, int max_cluster, int *hi) {
+FpsTier fps_tier(int n, int *hi) {
     if (n <= 4096) { *hi = 4096; return T256x2; }
     if (n <= 8192) { *hi = 8192; return T256x4; }
     // larger clouds: 1024 threads per CTA and few points per thread -- the per-iteration register scan is a dependent
     // chain per thread, so its latency scales with the points per thread, while the reductions / cluster exchange
     // do not depend on the thread count
-    if (max_cluster > 0 && n <= 49152) {
-        const int cl = max_cluster >= 4 ? 4 : 2;
-        const int per_cta = (n + cl - 1) / cl;          // points per CTA of 1024 threads
-        if (per_cta <= 4096) { *hi = min(4096 * cl, 49152); return T1024x4c; }
-        if (per_cta <= 6144) { *hi = min(6144 * cl, 49152); return T1024x6c; }
-        if (per_cta <= 10240) { *hi = min(10240 * cl, 49152); return T1024x10c; }
-        if (per_cta <= 12288) { *hi = min(12288 * cl, 49152); return T1024x12c; }
-    }
-    { static int cl16 = -1; if (cl16 < 0) { const char *e = getenv("BX_FPS_CL16"); cl16 = e ? atoi(e) : 0; }     // experiment: 16-CTA clusters, fewer points per thread
-      if (cl16 && n <= 16384) { *hi = 16384; return T1024x1c16; }
-      if (cl16 && n <= 32768) { *hi = 32768; return T1024x2c16; } }
     if (n <= 16384) { *hi = 16384; return T1024x2; }
     if (n <= 24576) { *hi = 24576; return T1024x3; }
     if (n <= 32768) { *hi = 32768; return T1024x4; }
@@ -308,33 +254,14 @@ FpsTier fps_tier(int n, int max_cluster, int *hi) {
 
 }  // namespace
 
-// Exchange switch: 0 = st.async + transaction-count mbarrier (production), 1 = plain stores ordered by cluster.sync() (the form
-// compute-sanitizer racecheck models), 2 = remote stores + remote mbarrier arrive / acquire wait (round 1's production);
-// same results in all three.  -1 = follow the BX_FPS_SYNC environment variable.  Returns the previous value.
-BX_API int bx_fps_set_sync_mode(int mode) {
-    const int old = g_fps_sync_override;
-    g_fps_sync_override = mode;
-    return old;
-}
-
 BX_API int bx_fps(const float *xyz, const int32_t *h_offsets, int B, int npoint, int32_t *idx, float *kpts,
                   void *stream) {
-    return bx_fps_n(xyz, h_offsets, B, npoint, idx, kpts, 0, nullptr, stream);
-}
-
-// max_cluster > 0: THROUGHPUT form -- at most that many CTAs per cloud (2 or 4), more points per thread.  An iteration is a
-// latency chain (reductions + cluster exchange) whatever the cluster size, so the default form spreads a cloud over 8 SMs
-// only to shorten the register scan; when several pairs are in flight the 16 SMs of a pair's two clouds are taken from the
-// other pairs' convolutions for the whole sampling.  Two CTAs per cloud hold 10 points per thread: a longer chain on a
-// quarter of the SMs.  Same indices in every form (the tie rank does not depend on the layout).
-BX_API int bx_fps_ex(const float *xyz, const int32_t *h_offsets, int B, int npoint, int32_t *idx, float *kpts, int max_cluster,
-                     void *stream) {
-    return bx_fps_n(xyz, h_offsets, B, npoint, idx, kpts, max_cluster, nullptr, stream);
+    return bx_fps_n(xyz, h_offsets, B, npoint, idx, kpts, nullptr, stream);
 }
 
 // d_counts (optional, device, B ints): cloud b holds min(max(d_counts[b], 1), h_offsets[b+1] - h_offsets[b]) points at
 // h_offsets[b]; the launch is sized by the capacities, so one captured launch serves every count up to them.
-BX_API int bx_fps_n(const float *xyz, const int32_t *h_offsets, int B, int npoint, int32_t *idx, float *kpts, int max_cluster,
+BX_API int bx_fps_n(const float *xyz, const int32_t *h_offsets, int B, int npoint, int32_t *idx, float *kpts,
                     const int32_t *d_counts, void *stream) {
     BX_REQUIRE(xyz && h_offsets && idx, "bx_fps: null pointer");
     BX_REQUIRE(B >= 1 && B <= kMaxClouds, "bx_fps: B=%d out of range [1,%d]", B, kMaxClouds);
@@ -352,15 +279,9 @@ BX_API int bx_fps_n(const float *xyz, const int32_t *h_offsets, int B, int npoin
     for (int b = 0; b <= kMaxClouds; ++b) d_off.v[b] = h_offsets[b <= B ? b : B];
     const int *dc = d_counts;
     int hi;
-    switch (fps_tier(maxN, max_cluster, &hi)) {
+    switch (fps_tier(maxN, &hi)) {
         case T256x2: return launch_fps<256, 2>(xyz, d_off, B, 8, npoint, idx, kpts, dc, st);
         case T256x4: return launch_fps<256, 4>(xyz, d_off, B, 8, npoint, idx, kpts, dc, st);
-        case T1024x4c: return launch_fps<1024, 4>(xyz, d_off, B, max_cluster >= 4 ? 4 : 2, npoint, idx, kpts, dc, st);
-        case T1024x6c: return launch_fps<1024, 6>(xyz, d_off, B, max_cluster >= 4 ? 4 : 2, npoint, idx, kpts, dc, st);
-        case T1024x10c: return launch_fps<1024, 10>(xyz, d_off, B, max_cluster >= 4 ? 4 : 2, npoint, idx, kpts, dc, st);
-        case T1024x12c: return launch_fps<1024, 12>(xyz, d_off, B, max_cluster >= 4 ? 4 : 2, npoint, idx, kpts, dc, st);
-        case T1024x1c16: return launch_fps<1024, 1>(xyz, d_off, B, 16, npoint, idx, kpts, dc, st);
-        case T1024x2c16: return launch_fps<1024, 2>(xyz, d_off, B, 16, npoint, idx, kpts, dc, st);
         case T1024x2: return launch_fps<1024, 2>(xyz, d_off, B, 8, npoint, idx, kpts, dc, st);
         case T1024x3: return launch_fps<1024, 3>(xyz, d_off, B, 8, npoint, idx, kpts, dc, st);
         case T1024x4: return launch_fps<1024, 4>(xyz, d_off, B, 8, npoint, idx, kpts, dc, st);
@@ -373,10 +294,10 @@ BX_API int bx_fps_n(const float *xyz, const int32_t *h_offsets, int B, int npoin
 
 // Size class of a cloud of n points: the largest point count whose launch gets the same configuration as n (n <= 0: 0;
 // n > 524288: -1, no launch exists).  Capacity buffers of this size keep the kernel on n's register tier.
-BX_API int bx_fps_size_class(int n, int max_cluster) {
+BX_API int bx_fps_size_class(int n) {
     if (n <= 0) return 0;
     if (n > 524288) return -1;
     int hi;
-    fps_tier(n, max_cluster, &hi);
+    fps_tier(n, &hi);
     return hi;
 }

@@ -246,8 +246,8 @@ BX_API int bx_fps_large_n(const float *xyz, int cap, const int32_t *d_n, int npo
     return launch<true>("bx_fps_large_n", xyz, cap, d_n, npoint, idx, kpts, workspace, stream);
 }
 
-BX_API int bx_fps_large_size_class(int n, int max_cluster) {
-    if (n <= 524288) return bx_fps_size_class(n, max_cluster);
+BX_API int bx_fps_large_size_class(int n) {
+    if (n <= 524288) return bx_fps_size_class(n);
     if (n > kMaxN) return -1;
     for (const int g : kClassCtas)
         if (n <= g * kPerCta) return g * kPerCta;

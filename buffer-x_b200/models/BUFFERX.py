@@ -26,8 +26,6 @@ Throughput API on top of the reference surface (CUDA streams + graphs instead of
     With ``cfg.match.enable_early_exit`` the scale-0 RANSAC result gates the later scales on the device
     (``_enqueue_device_exit``), so early-exit pairs are captured and replayed too.
 """
-import os
-
 import numpy as np
 import torch
 import torch.nn as nn
@@ -256,7 +254,6 @@ class BufferX(nn.Module):
         self._slots_per_shape = 2
         self._size_classes = False
         self._large_classes = False
-        self._fps_cluster = 0        # > 0: throughput form of the FPS kernel (ops.fps max_cluster), chosen by enable_cuda_graphs
         self._rr = {}
 
     def get_parameter(self):
@@ -335,12 +332,6 @@ class BufferX(nn.Module):
         self._slots_per_shape = int(slots_per_shape)
         self._size_classes = bool(size_classes)
         self._large_classes = bool(large_classes)
-        # three or more pairs in flight: the key-point sampling of a pair runs beside the other pairs' convolutions; bx_fps_ex offers
-        # a 2- / 4-CTA-per-cloud form (fewer SMs, longer)
-        # (what the other streams lose is governed by how LONG the sampling holds its SMs, not by how many, so the default stays
-        # the latency form; this choice was measured on the B200 and has not been re-measured on the H100; BX_FPS_CLUSTER=2|4
-        # selects the throughput form for experiments)
-        self._fps_cluster = int(os.environ.get("BX_FPS_CLUSTER", "0")) if (flag and self._slots_per_shape >= 3) else 0
         self._slots.clear()
         self._rr.clear()
         return self
@@ -366,10 +357,10 @@ class BufferX(nn.Module):
         """(slot key, capacities, counted) of a pair.  The early-exit threshold is baked into a captured gate launch: a
         graph is never replayed under another setting."""
         if self._size_classes and self._large_classes:
-            Cs, Ct = ops.fps_large_size_class(Ns, self._fps_cluster), ops.fps_large_size_class(Nt, self._fps_cluster)
+            Cs, Ct = ops.fps_large_size_class(Ns), ops.fps_large_size_class(Nt)
             return (Cs, Ct, bool(aligned)) + self._exit_key(), Cs, Ct, True
         if self._size_classes and max(Ns, Nt) <= self.MAX_CLASS_POINTS:
-            Cs, Ct = ops.fps_size_class(Ns, self._fps_cluster), ops.fps_size_class(Nt, self._fps_cluster)
+            Cs, Ct = ops.fps_size_class(Ns), ops.fps_size_class(Nt)
             return (Cs, Ct, bool(aligned)) + self._exit_key(), Cs, Ct, True
         return (Ns, Nt, bool(aligned)) + self._exit_key(), Ns, Nt, False
 
@@ -464,10 +455,10 @@ class BufferX(nn.Module):
             xyz = torch.cat([src, tgt], dim=0)
         nfps = max(Kr, K)
         if max(Ns, Nt) <= ops.FPS_MAX_POINTS:
-            fidx, fk = ops.fps(xyz, [0, Ns, Ns + Nt], nfps, max_cluster=self._fps_cluster, d_counts=counts)
+            fidx, fk = ops.fps(xyz, [0, Ns, Ns + Nt], nfps, d_counts=counts)
         else:   # beyond one cluster's registers: that cloud on the grid-wide kernel (a capacity above it holds such a cloud)
             per = [ops.fps_large(c, nfps, d_count=None if counts is None else counts[j:j + 1]) if c.shape[0] > ops.FPS_MAX_POINTS
-                   else ops.fps(c, [0, c.shape[0]], nfps, max_cluster=self._fps_cluster, d_counts=None if counts is None else counts[j:j + 1])
+                   else ops.fps(c, [0, c.shape[0]], nfps, d_counts=None if counts is None else counts[j:j + 1])
                    for j, c in enumerate((src, tgt))]
             fidx = torch.stack([i.reshape(nfps) for i, _ in per])
             fk = torch.stack([k.reshape(nfps, 3) for _, k in per])

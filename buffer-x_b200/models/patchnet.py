@@ -15,25 +15,12 @@ does in training mode.  CostNet's forward sits behind one autograd Function whos
 BatchNorm backward, float64) gives the gradients of every ``ops.*`` weight and bias.
 """
 import itertools
-import os
 
 import torch
 import torch.nn as nn
 from torch.autograd.function import once_differentiable
 
 from bufferx_b200 import ops
-
-# BX_CONV=tc: the descriptor stack on the TF32 kernel (bx_conv_tc.cu) instead of the shifted-descriptor fp16-split
-# kernel (bx_conv_sd.cu, the default).  The TF32 kernel is also the automatic fall-back when an activation leaves fp16 range.
-USE_TF32_DESC = os.environ.get("BX_CONV", "sd").lower() == "tc"
-# BX_SD_DYNAMIC=1: the persistent conv kernels draw their tiles from a device-side counter (bx_conv_layer_sd d_tile_ctr) instead
-# of the static stride.  It brought no gain with six pairs in flight (a launch whose CTAs start late still cannot finish before
-# they have been scheduled), so the static stride stays the default; that was measured on the B200 and has not been
-# re-measured on the H100.  The path is kept and tested.
-DYNAMIC_TILES = os.environ.get("BX_SD_DYNAMIC", "0") == "1"
-# BX_DESC_CONV=sd: the descriptor stack's presplit-input layers on conv_sd_kernel (128-row tiles, all 176 raster rows of a
-# sample computed) instead of the per-sample kernel (bx_conv_ps.cu, the default), for A/B runs.  Both write the same bytes.
-DESC_CONV_SD = os.environ.get("BX_DESC_CONV", "ps").lower() == "sd"
 
 
 def fold_conv_bn(conv_w, conv_b, bn_mean=None, bn_var=None, bn_w=None, bn_b=None, eps=1e-5):
@@ -186,7 +173,7 @@ class Cylindrical_Net(_ConvStack):
         super().__init__(spec)
         self.out_dim = dim
         self.sd_kernel_sizes = ((1, 3, 3), (3, 3, 3))
-        self.force_tf32 = USE_TF32_DESC      # set (sticky) by BufferX when the fp16-range flag fired once
+        self.force_tf32 = False      # run on the TF32 kernel (bx_conv_tc.cu); set (sticky) by BufferX when the fp16-range flag fired once
         self._flag = None
 
     def overflow_flag(self, dev):
@@ -206,8 +193,6 @@ class Cylindrical_Net(_ConvStack):
         use_sd = not self.force_tf32
         assert use_sd or not presplit_in
         flag = self.overflow_flag(dev) if use_sd else None
-        # dynamic tile scheduling of the persistent conv kernels: one zeroed counter pair per layer (and per call = per stream)
-        ctrs = torch.zeros(2 * len(L), dtype=torch.int32, device=dev) if (use_sd and DYNAMIC_TILES) else None
         for i, l in enumerate(L):
             out = torch.empty((K, l["cout"] // 4, 140, 4), dtype=torch.float32, device=dev)
             if use_sd:       # layer-to-layer activations in the presplit padded fp16 format; fp32 in at the first, fp32 out at the last layer
@@ -215,9 +200,9 @@ class Cylindrical_Net(_ConvStack):
                 # presplit input and output: the per-sample kernel.  conv_sd_kernel keeps an fp32 first-layer input (its loader
                 # warps) and the fp32-output last layer, whose two-chunk mainloop is too short to pay for the per-sample epilogue
                 # (DESIGN.md section 5: 3.5 % slower on the per-sample kernel)
-                conv = ops.conv_layer_ps if cur.dtype == torch.float16 and out.dtype == torch.float16 and not DESC_CONV_SD else ops.conv_layer_sd
+                conv = ops.conv_layer_ps if cur.dtype == torch.float16 and out.dtype == torch.float16 else ops.conv_layer_sd
                 conv(ops.GEOM_CYL3D if i == 0 else ops.GEOM_CYL2D, cur, l["w_sd"], l["b"], out, K, l["cin"], l["cout"], l["relu"], flag,
-                     d_n=d_n, tile_ctr=None if ctrs is None else ctrs[2 * i:2 * i + 2])
+                     d_n=d_n)
                 cur = out
                 continue
             if i == 0:
@@ -267,7 +252,7 @@ class CostNet(_ConvStack):
         super().__init__(spec)
         self.out_dim = dim
         self.sd_kernel_sizes = ((3, 1, 3),)
-        self.force_tf32 = USE_TF32_DESC
+        self.force_tf32 = False
         self.flag_source = None          # set by BufferX: the descriptor stack's overflow_flag (one sticky flag per model)
 
     def forward_matches(self, equi_s, equi_t, s_mids, t_mids, d_M, maxM):
@@ -280,7 +265,6 @@ class CostNet(_ConvStack):
         cur = None
         use_sd = not self.force_tf32
         flag = self.flag_source(dev) if (use_sd and self.flag_source is not None) else None
-        ctrs = torch.zeros(2 * len(L), dtype=torch.int32, device=dev) if (use_sd and DYNAMIC_TILES) else None
         for i, l in enumerate(L):
             kd, kh, kw = l["k"]
             OD, OH, OW = D - kd + 1, H - kh + 1, W - kw + 1
@@ -289,8 +273,7 @@ class CostNet(_ConvStack):
                 nxt_sd = nxt is not None and nxt.get("w_sd") is not None
                 out = (ops.conv_sd_buffer(maxM, l["cout"], dev, OD * OW) if nxt_sd
                        else torch.empty((maxM, l["cout"] // 4, OD * OW, 4), dtype=torch.float32, device=dev))
-                ops.conv_layer_sd(ops.GEOM_VALID3D, cur, l["w_sd"], l["b"], out, maxM, l["cin"], l["cout"], l["relu"], flag, d_n=d_M, D=D, W=W,
-                                  tile_ctr=None if ctrs is None else ctrs[2 * i:2 * i + 2])
+                ops.conv_layer_sd(ops.GEOM_VALID3D, cur, l["w_sd"], l["b"], out, maxM, l["cin"], l["cout"], l["relu"], flag, d_n=d_M, D=D, W=W)
                 cur, D, H, W = out, OD, OH, OW
                 continue
             if i == 0:

@@ -24,7 +24,7 @@ SYMBOLS = [
     "bx_pool_desc", "bx_mutual_nn",
     "bx_hypotheses", "bx_consensus", "bx_ransac_workspace_bytes", "bx_ransac", "bx_refine", "bx_conv_tc_set_segment_stages",
     "bx_radius_neighbors", "bx_grid_subsample", "bx_costvol_ab", "bx_concat_matches",
-    "bx_pca_analysis", "bx_project_range", "bx_voxel_down_sample", "bx_conv_layer_sd", "bx_conv_layer_ps", "bx_conv_sd_rows", "bx_spt_pnt_sd", "bx_fps_set_sync_mode", "bx_conv_layer_sd_costab", "bx_lrf_batched", "bx_select_patches_batched", "bx_fps_ex", "bx_select_patches_grid", "bx_select_patches_grid_workspace_bytes", "bx_select_patches_grid_batched",
+    "bx_pca_analysis", "bx_project_range", "bx_voxel_down_sample", "bx_conv_layer_sd", "bx_conv_layer_ps", "bx_conv_sd_rows", "bx_spt_pnt_sd", "bx_conv_layer_sd_costab", "bx_lrf_batched", "bx_select_patches_batched", "bx_select_patches_grid", "bx_select_patches_grid_workspace_bytes", "bx_select_patches_grid_batched",
     "bx_gt_matches", "bx_so2_augment", "bx_equi_match", "bx_so2_gt",
     "bx_select_patches_batched_n", "bx_select_patches_grid_batched_n", "bx_lrf_batched_n", "bx_spt_pnt_sd_n", "bx_pool_desc_n",
     "bx_mutual_nn_n", "bx_early_exit_gate",
@@ -67,14 +67,13 @@ def load_library():
     lib.bx_ransac_workspace_bytes.argtypes = [c_int]
     P = c_void_p
     lib.bx_fps.argtypes = [P, P, c_int, c_int, P, P, P]
-    lib.bx_fps_ex.argtypes = [P, P, c_int, c_int, P, P, c_int, P]
-    lib.bx_fps_n.argtypes = [P, P, c_int, c_int, P, P, c_int, P, P]
-    lib.bx_fps_size_class.argtypes = [c_int, c_int]
+    lib.bx_fps_n.argtypes = [P, P, c_int, c_int, P, P, P, P]
+    lib.bx_fps_size_class.argtypes = [c_int]
     lib.bx_fps_large.argtypes = [P, c_int, c_int, P, P, P, P]
     lib.bx_fps_large_workspace_bytes.argtypes = [c_int]
     lib.bx_fps_large_workspace_bytes.restype = c_int64
     lib.bx_fps_large_n.argtypes = [P, c_int, P, c_int, P, P, P, P]
-    lib.bx_fps_large_size_class.argtypes = [c_int, c_int]
+    lib.bx_fps_large_size_class.argtypes = [c_int]
     lib.bx_radius_estimate_n_sub.argtypes = [P, P, c_int, P, P, c_int, c_int, P, P, P, c_int, c_double, P, P, P, P, P]
     lib.bx_radius_estimate_n.argtypes = [P, P, c_int, P, P, c_int, c_int, P, P, c_int, c_double, P, P, P, P, P]
     lib.bx_permute_cloud_n.argtypes = [P, P, c_int, P, P, P]
@@ -101,11 +100,10 @@ def load_library():
     lib.bx_spt_pnt.argtypes = [P, c_int, c_int, P, c_int, c_int, P, c_float, c_int, P, P, P, P, P, P]
     lib.bx_conv_layer_tc.argtypes = [c_int, P, P, P, P, c_int, P] + [c_int] * 9 + [P, P, P]
     lib.bx_conv_tc_ntile.argtypes = [c_int]
-    lib.bx_conv_layer_sd.argtypes = [c_int, P, c_int, P, P, P, c_int, c_int, P, c_int, c_int, c_int, c_int, c_int, P, P, P]
-    lib.bx_conv_layer_ps.argtypes = [c_int, P, c_int, P, P, P, c_int, c_int, P, c_int, c_int, c_int, c_int, c_int, P, P, P]
+    lib.bx_conv_layer_sd.argtypes = [c_int, P, c_int, P, P, P, c_int, c_int, P, c_int, c_int, c_int, c_int, c_int, P, P]
+    lib.bx_conv_layer_ps.argtypes = [c_int, P, c_int, P, P, P, c_int, c_int, P, c_int, c_int, c_int, c_int, c_int, P, P]
     lib.bx_conv_sd_rows.argtypes = [c_int, c_int]
     lib.bx_conv_layer_sd_costab.argtypes = [P, P, P, P, P, c_int, c_int, P, c_int, P, P]
-    lib.bx_fps_set_sync_mode.argtypes = [c_int]
     lib.bx_spt_pnt_sd.argtypes = [P, c_int, c_int, P, c_int, c_int, P, c_float, c_int, P, P, P, c_int64, P, P]
     lib.bx_spt_pnt_sd_n.argtypes = [P, c_int, c_int, P, c_int, c_int, P, c_float, c_int, P, P, P, c_int64, P, P, P]
     lib.bx_conv_sd_rows.restype = c_int64
@@ -237,22 +235,19 @@ class _Span:
         return False
 
 
-def fps(xyz: torch.Tensor, offsets, npoint: int, want_kpts=True, max_cluster=0, d_counts=None):
+def fps(xyz: torch.Tensor, offsets, npoint: int, want_kpts=True, d_counts=None):
     """xyz [sumN,3] f32 cuda; offsets: host sequence of B+1 ints.  Returns idx [B,npoint] i32, kpts [B,npoint,3].
-    max_cluster 2 / 4: throughput form (fewer SMs per cloud, same indices).  d_counts: optional [B] int32 CUDA tensor of
-    point counts; the offsets then give each cloud's capacity and cloud b is its first min(d_counts[b], capacity) points."""
+    d_counts: optional [B] int32 CUDA tensor of point counts; the offsets then give each cloud's capacity and cloud b is its
+    first min(d_counts[b], capacity) points."""
     lib = load_library()
     off = np.ascontiguousarray(offsets, dtype=np.int32)
     B = len(off) - 1
     idx = torch.empty((B, npoint), dtype=I32, device=xyz.device)
     kp = torch.empty((B, npoint, 3), dtype=F32, device=xyz.device) if want_kpts else None
+    assert d_counts is None or d_counts.numel() >= B
     with _Span("fps"):
-        if d_counts is None:
-            _check(lib.bx_fps_ex(_dp(xyz, F32, "xyz"), off.ctypes.data_as(c_void_p), B, npoint, _dp(idx), _dp(kp), int(max_cluster), _stream()), "bx_fps")
-        else:
-            assert d_counts.numel() >= B
-            _check(lib.bx_fps_n(_dp(xyz, F32, "xyz"), off.ctypes.data_as(c_void_p), B, npoint, _dp(idx), _dp(kp), int(max_cluster),
-                                _dp(d_counts, I32, "d_counts"), _stream()), "bx_fps_n")
+        _check(lib.bx_fps_n(_dp(xyz, F32, "xyz"), off.ctypes.data_as(c_void_p), B, npoint, _dp(idx), _dp(kp),
+                            _dp(d_counts, I32, "d_counts"), _stream()), "bx_fps_n")
     return idx, kp
 
 
@@ -283,16 +278,16 @@ def fps_large(xyz: torch.Tensor, npoint: int, want_kpts=True, d_count=None):
     return idx, kp
 
 
-def fps_size_class(n: int, max_cluster=0) -> int:
+def fps_size_class(n: int) -> int:
     """The largest point count that gets the same FPS launch configuration as an n-point cloud (-1 above the FPS limit)."""
-    return int(load_library().bx_fps_size_class(int(n), int(max_cluster)))
+    return int(load_library().bx_fps_size_class(int(n)))
 
 
-def fps_large_size_class(n: int, max_cluster=0) -> int:
-    """Capacity of an n-point cloud's size class up to FPS_LARGE_MAX_POINTS: fps_size_class(n, max_cluster) up to
+def fps_large_size_class(n: int) -> int:
+    """Capacity of an n-point cloud's size class up to FPS_LARGE_MAX_POINTS: fps_size_class(n) up to
     FPS_MAX_POINTS; above, multiples of 18432 points (bx_fps_large_n's CTAs) each at most 1.25x the smallest cloud of its
     class, then FPS_LARGE_MAX_POINTS.  -1 above FPS_LARGE_MAX_POINTS."""
-    return int(load_library().bx_fps_large_size_class(int(n), int(max_cluster)))
+    return int(load_library().bx_fps_large_size_class(int(n)))
 
 
 _round_tables = {}
@@ -402,7 +397,7 @@ def select_patches(pts4: torch.Tensor, kpts: torch.Tensor, radius, P: int, want_
 # clouds of at least this many points gather their patches through the spatial hash grid (bx_select_patches_grid) instead of the
 # streaming scan: a ball then holds so small a part of the cloud that reading the cloud front to back costs more than binning it.
 # The threshold was chosen on the B200 and has not been re-measured on the H100.
-GRID_MIN_POINTS = int(os.environ.get("BX_PATCHES_GRID_MIN", "12000"))
+GRID_MIN_POINTS = 12000
 
 
 def select_patches_grid(pts4: torch.Tensor, kpts: torch.Tensor, radius: torch.Tensor, P: int, want_idx=False, patches=None):
@@ -666,10 +661,9 @@ def conv_sd_buffer(n: int, C: int, device, rows_per_sample: int = 176):
     return torch.empty((C // 16, 4, conv_sd_rows(n, rows_per_sample), 8), dtype=torch.float16, device=device)
 
 
-def conv_layer_sd(geom, x, w_sd, bias, out, n, Cin, Cout, relu, flag=None, d_n=None, D=0, W=0, tile_ctr=None):
+def conv_layer_sd(geom, x, w_sd, bias, out, n, Cin, Cout, relu, flag=None, d_n=None, D=0, W=0):
     """x: fp32 channel-blocked [n, Cin/4, S_in, 4] or presplit fp16 [Cin/16, 4, rows, 8]; out likewise (dtype decides);
-    ``flag``: int32[1] fp16-range flag (sticky); ``d_n``: device-side sample count; D, W: input raster of GEOM_VALID3D;
-    ``tile_ctr``: int32[2] zeroed device counters -> dynamic tile scheduling (one pair per launch in flight)."""
+    ``flag``: int32[1] fp16-range flag (sticky); ``d_n``: device-side sample count; D, W: input raster of GEOM_VALID3D."""
     ev = None
     if profiler is not None:
         if geom == GEOM_VALID3D:
@@ -680,13 +674,13 @@ def conv_layer_sd(geom, x, w_sd, bias, out, n, Cin, Cout, relu, flag=None, d_n=N
     in_sd, out_sd = x.dtype == torch.float16, out.dtype == torch.float16
     _check(load_library().bx_conv_layer_sd(geom, _dp(x, None, "x"), int(in_sd), _dp(w_sd, torch.float16, "w_sd"), _dp(bias, F32, "bias"),
                                            _dp(out, None, "out"), int(out_sd), int(n), _dp(d_n, I32, "d_n"), Cin, Cout, int(D), int(W), int(bool(relu)),
-                                           _dp(flag, I32, "flag"), _dp(tile_ctr, I32, "tile_ctr"), _stream()), "bx_conv_layer_sd")
+                                           _dp(flag, I32, "flag"), _stream()), "bx_conv_layer_sd")
     if ev:
         ev[1].record()
     return out
 
 
-def conv_layer_ps(geom, x, w_sd, bias, out, n, Cin, Cout, relu, flag=None, d_n=None, D=0, W=0, tile_ctr=None):
+def conv_layer_ps(geom, x, w_sd, bias, out, n, Cin, Cout, relu, flag=None, d_n=None, D=0, W=0):
     """A descriptor-stack layer (GEOM_CYL3D / GEOM_CYL2D) on the per-sample kernel (bx_conv_layer_ps): the arguments and the
     bytes written are those of ``conv_layer_sd``; x must be the presplit fp16 image [Cin/16, 4, rows, 8]."""
     ev = None
@@ -696,7 +690,7 @@ def conv_layer_ps(geom, x, w_sd, bias, out, n, Cin, Cout, relu, flag=None, d_n=N
     _check(load_library().bx_conv_layer_ps(geom, _dp(x, None, "x"), int(x.dtype == torch.float16), _dp(w_sd, torch.float16, "w_sd"),
                                            _dp(bias, F32, "bias"), _dp(out, None, "out"), int(out.dtype == torch.float16), int(n),
                                            _dp(d_n, I32, "d_n"), Cin, Cout, int(D), int(W), int(bool(relu)), _dp(flag, I32, "flag"),
-                                           _dp(tile_ctr, I32, "tile_ctr"), _stream()), "bx_conv_layer_ps")
+                                           _stream()), "bx_conv_layer_ps")
     if ev:
         ev[1].record()
     return out

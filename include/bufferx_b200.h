@@ -51,25 +51,17 @@ unsigned long long bx_launch_count(void); /* kernels launched by this library si
  * idx: [B,npoint] int32 (index inside the cloud); kpts: [B,npoint,3] (may be NULL).
  * Limit: N <= 131072 per cloud. */
 int bx_fps(const float *xyz, const int32_t *h_offsets, int B, int npoint, int32_t *idx, float *kpts, void *stream);
-/* The same with at most max_cluster (2 or 4) CTAs per cloud: fewer SMs, ~1.4x the latency -- for callers that keep several
- * pairs in flight (0 = bx_fps).  Identical indices. */
-int bx_fps_ex(const float *xyz, const int32_t *h_offsets, int B, int npoint, int32_t *idx, float *kpts, int max_cluster,
-              void *stream);
 /* With device-side point counts (size-class buffers: one captured launch serves every cloud up to a capacity).  h_offsets
  * give each cloud's first point and its CAPACITY (h_offsets[b+1] - h_offsets[b]); cloud b holds its first
  * n_b = min(max(d_counts[b], 1), capacity) points, and points beyond n_b are never read.  The launch configuration and
- * the grid follow the capacities; indices and key-points are those of bx_fps_ex on the n_b-point clouds (the tie rule's
- * block size bs is derived from n_b).  d_counts NULL = bx_fps_ex. */
-int bx_fps_n(const float *xyz, const int32_t *h_offsets, int B, int npoint, int32_t *idx, float *kpts, int max_cluster,
+ * the grid follow the capacities; indices and key-points are those of bx_fps on the n_b-point clouds (the tie rule's
+ * block size bs is derived from n_b).  d_counts NULL = bx_fps. */
+int bx_fps_n(const float *xyz, const int32_t *h_offsets, int B, int npoint, int32_t *idx, float *kpts,
              const int32_t *d_counts, void *stream);
 /* Size class of an n-point cloud: the largest point count that gets the same FPS launch configuration (register tier,
- * CTAs per cloud) as n under this max_cluster -- the capacity whose buffers keep the kernel on n's tier.  0 for n <= 0,
- * -1 above the 524288-point limit. */
-int bx_fps_size_class(int n, int max_cluster);
-/* Switch for the FPS cluster exchange: 0 = st.async + transaction-count mbarrier (production), 1 = cluster.sync() per iteration
- * (racecheck-clean reference form), 2 = remote stores + remote mbarrier arrive / acquire wait (round 1), -1 = BX_FPS_SYNC
- * environment variable.  Same results in every mode.  Returns the old value. */
-int bx_fps_set_sync_mode(int mode);
+ * CTAs per cloud) as n -- the capacity whose buffers keep the kernel on n's tier.  0 for n <= 0, -1 above the
+ * 524288-point limit. */
+int bx_fps_size_class(int n);
 /* One cloud of any size up to 1638400 points (models/BUFFERX.py:286-290 on the first-downsampled clouds of dense sensors,
  * which bx_fps refuses above 524288 points): xyz [n,3], idx [npoint] int32, kpts [npoint,3] (may be NULL).  Same result
  * contract as bx_fps, so any n gives bx_fps's indices.  The cloud is spread over ceil(n / 18432) SMs of one cooperative
@@ -84,10 +76,10 @@ long long bx_fps_large_workspace_bytes(int n);
  * bx_fps_large on the n-point cloud.  workspace: bx_fps_large_workspace_bytes(cap) bytes. */
 int bx_fps_large_n(const float *xyz, int cap, const int32_t *d_n, int npoint, int32_t *idx, float *kpts, void *workspace,
                    void *stream);
-/* Size class of an n-point cloud up to 1638400 points: bx_fps_size_class(n, max_cluster) up to 524288 points; above, the
+/* Size class of an n-point cloud up to 1638400 points: bx_fps_size_class(n) up to 524288 points; above, the
  * capacities 18432 * {35, 43, 53, 66, 82} and 1638400 (bx_fps_large_n's grid), each at most 1.25x the smallest cloud of its
  * class.  0 for n <= 0, -1 above 1638400. */
-int bx_fps_large_size_class(int n, int max_cluster);
+int bx_fps_large_size_class(int n);
 
 /* ---- a2: density-aware radius estimation ----------------------------------------------------
  * Replaces density_aware_radius_estimation + squared_cdist (models/BUFFERX.py:610-696) without
@@ -269,23 +261,16 @@ int bx_spt_pnt_sd_n(const float *delta, int K, int P, const float *voxels, int V
  * w_sd: fp16 hi/lo weight image [chunk][tap][kcore][split][NT][8] (ops.conv_sd_weights; NT = bx_conv_tc_ntile(Cout)); for
  * Cout <= 32 it is [chunk][tap][kcore][P | Q][64][8] (hi / lo and zero / hi of 8 channels per 16-row group, see bx_conv_sd.cu);
  * bias fp32 [Cout].  An activation with |x| >= 65000 cannot be split into fp16 operands -> *d_flag |= 1 (d_flag may be
- * NULL) and the caller re-runs the stack with bx_conv_layer_tc.
- * d_tile_ctr (optional, device, int32[2], zero before its first use): dynamic tile scheduling for presplit-input layers --
- * the persistent CTAs draw units of work (one 128-row tile, or two for Cout <= 64) from the counter instead of a fixed
- * stride, so a launch that starts while other
- * streams still hold some SMs is not held up by its late CTAs; the kernel rewinds the counter when it finishes.  One
- * counter pair per launch in flight (the callers keep one per layer and stream). */
+ * NULL) and the caller re-runs the stack with bx_conv_layer_tc. */
 int bx_conv_layer_sd(int geom, const void *in, int in_presplit, const void *w_sd, const float *bias, void *out, int out_presplit,
-                     int n, const int32_t *d_n, int Cin, int Cout, int D, int W, int relu, int32_t *d_flag, int32_t *d_tile_ctr,
-                     void *stream);
+                     int n, const int32_t *d_n, int Cin, int Cout, int D, int W, int relu, int32_t *d_flag, void *stream);
 long long bx_conv_sd_rows(int n, int rows_per_sample);
 /* The descriptor-stack layers (geom = BX_GEOM_CYL3D / BX_GEOM_CYL2D, presplit input) on the per-sample kernel
  * (bx_conv_ps.cu): same arguments, weight image and bytes written as bx_conv_layer_sd, bit-identical values.  A sample's
- * 152 live raster rows are one wgmma operand, so the 24 dead rows (y = 7) of every sample are never computed.  D, W unused;
- * d_tile_ctr schedules units of one sample (Cout > 64) or two (Cout <= 64). */
+ * 152 live raster rows are one wgmma operand, so the 24 dead rows (y = 7) of every sample are never computed.  D, W
+ * unused. */
 int bx_conv_layer_ps(int geom, const void *in, int in_presplit, const void *w_sd, const float *bias, void *out, int out_presplit,
-                     int n, const int32_t *d_n, int Cin, int Cout, int D, int W, int relu, int32_t *d_flag, int32_t *d_tile_ctr,
-                     void *stream);
+                     int n, const int32_t *d_n, int Cin, int Cout, int D, int W, int relu, int32_t *d_flag, void *stream);
 /* The second CostNet layer (32 -> 64, k = 3x3x3 over relu(A - B) regenerated from the factor maps of bx_costvol_ab) as a
  * 96 -> 64, k = (3,1,3) convolution over the 18 x 18 (n, l) raster on the same kernel.  fa [n,8,60,4], fb [n,8,54,4] fp32;
  * w_sd: ops.conv_sd_weights_costab; out: fp32 [n,16,256,4] or presplit over the 16 x 16 raster (rows = bx_conv_sd_rows(n, 256)). */

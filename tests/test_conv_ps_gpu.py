@@ -1,7 +1,7 @@
 """The per-sample descriptor-stack convolution (csrc/bx_conv_ps.cu, ops.conv_layer_ps) against conv_sd_kernel
 (ops.conv_layer_sd) on the same input: every output byte -- values, wrap columns, zero rows, and the rows neither kernel
 writes -- must be identical.  Covers every Cylindrical_Net layer shape at the production batch, sample counts at the edges of
-the unit schedule, a device sample count below the capacity, dynamic scheduling and the fp16-range flag."""
+the unit schedule, a device sample count below the capacity and the fp16-range flag."""
 import pytest
 import torch
 
@@ -44,7 +44,7 @@ def _bits(t):
     return t.view(torch.int16) if t.dtype == torch.float16 else t.view(torch.int32)
 
 
-def _both(dev, n, layer, seed, d_n=None, scale=1.0, flag=False, tile_ctr=False):
+def _both(dev, n, layer, seed, d_n=None, scale=1.0, flag=False):
     from bufferx_b200 import ops
     geom, Cin, Cout, relu, presplit = layer
     G = ops.GEOM_CYL3D if geom == "3d" else ops.GEOM_CYL2D
@@ -53,16 +53,15 @@ def _both(dev, n, layer, seed, d_n=None, scale=1.0, flag=False, tile_ctr=False):
     for conv in (ops.conv_layer_sd, ops.conv_layer_ps):
         o = _out(dev, n, Cout, presplit)
         f = torch.zeros(1, dtype=torch.int32, device=dev) if flag else None
-        ctr = torch.zeros(2, dtype=torch.int32, device=dev) if tile_ctr else None
-        conv(G, x, w, b, o, n, Cin, Cout, relu, f, d_n=d_n, tile_ctr=ctr)
+        conv(G, x, w, b, o, n, Cin, Cout, relu, f, d_n=d_n)
         torch.cuda.synchronize()
-        res.append((o, f, ctr))
+        res.append((o, f))
     return res
 
 
 @pytest.mark.parametrize("layer", LAYERS, ids=[f"{g}-{ci}-{co}" for g, ci, co, _, _ in LAYERS])
 def test_conv_ps_bit_identical_production_batch(dev, layer):
-    (ref, _, _), (got, _, _) = _both(dev, 9000, layer, seed=1)
+    (ref, _), (got, _) = _both(dev, 9000, layer, seed=1)
     assert torch.equal(_bits(got), _bits(ref)), f"{layer}: {(_bits(got) != _bits(ref)).sum().item()} differing elements"
 
 
@@ -70,7 +69,7 @@ def test_conv_ps_bit_identical_production_batch(dev, layer):
 @pytest.mark.parametrize("li", [0, 2, 3, 6, 7])
 def test_conv_ps_bit_identical_edge_counts(dev, n, li):
     """1, 2, odd, and one less than a multiple of 132 (the H100's SM count = the grid of a large launch) samples."""
-    (ref, _, _), (got, _, _) = _both(dev, n, LAYERS[li], seed=10 + n)
+    (ref, _), (got, _) = _both(dev, n, LAYERS[li], seed=10 + n)
     assert torch.equal(_bits(got), _bits(ref))
 
 
@@ -78,34 +77,17 @@ def test_conv_ps_bit_identical_edge_counts(dev, n, li):
 def test_conv_ps_device_count_below_capacity(dev, li):
     """d_n = 217 of n = 300: both kernels compute and write the first 217 samples (and the zero row after them) only."""
     d_n = torch.tensor([217], dtype=torch.int32, device=dev)
-    (ref, _, _), (got, _, _) = _both(dev, 300, LAYERS[li], seed=5, d_n=d_n)
+    (ref, _), (got, _) = _both(dev, 300, LAYERS[li], seed=5, d_n=d_n)
     assert torch.equal(_bits(got), _bits(ref))
-
-
-@pytest.mark.parametrize("li", [2, 4, 6])
-def test_conv_ps_dynamic_units_same_bits(dev, li):
-    """The dynamic unit counter writes the same bytes as the static stride, and is rewound for the next launch."""
-    from bufferx_b200 import ops
-    geom, Cin, Cout, relu, presplit = LAYERS[li]
-    x, w, b = _case(dev, 1001, geom, Cin, Cout, 3)
-    ref = _out(dev, 1001, Cout, presplit)
-    ops.conv_layer_ps(ops.GEOM_CYL2D, x, w, b, ref, 1001, Cin, Cout, relu)
-    ctr = torch.zeros(2, dtype=torch.int32, device=dev)
-    for _ in range(2):
-        o = _out(dev, 1001, Cout, presplit)
-        ops.conv_layer_ps(ops.GEOM_CYL2D, x, w, b, o, 1001, Cin, Cout, relu, tile_ctr=ctr)
-        torch.cuda.synchronize()
-        assert torch.equal(_bits(o), _bits(ref))
-        assert ctr.tolist() == [0, 0]
 
 
 @pytest.mark.parametrize("li", [1, 3, 6])
 def test_conv_ps_fp16_range_flag(dev, li):
     """Activations past fp16 range raise the flag in both kernels (the caller then re-runs the stack on the TF32 kernel);
     in range, neither raises it."""
-    (_, f_ref, _), (_, f_got, _) = _both(dev, 64, LAYERS[li], seed=7, flag=True)
+    (_, f_ref), (_, f_got) = _both(dev, 64, LAYERS[li], seed=7, flag=True)
     assert f_ref.item() == 0 and f_got.item() == 0
-    (_, f_ref, _), (_, f_got, _) = _both(dev, 64, LAYERS[li], seed=7, scale=4.0e5, flag=True)
+    (_, f_ref), (_, f_got) = _both(dev, 64, LAYERS[li], seed=7, scale=4.0e5, flag=True)
     assert f_ref.item() == 1 and f_got.item() == 1
 
 
@@ -120,10 +102,9 @@ def test_conv_ps_refuses_fp32_input(dev):
 
 def test_cylindrical_net_runs_the_per_sample_kernel(dev, monkeypatch):
     """Cylindrical_Net.forward on a presplit input calls conv_layer_ps for every layer but the fp32-output last one, and its
-    result equals the BX_DESC_CONV=sd route (conv_sd_kernel) bit for bit."""
+    result equals the same stack run layer by layer on conv_sd_kernel (ops.conv_layer_sd) bit for bit."""
     import bufferx_b200 as bx
     from bufferx_b200 import ops
-    from bufferx_b200.models import patchnet as pn
     from bufferx_b200.synth import init_synthetic_weights, workload_cfg
     net = init_synthetic_weights(bx.BufferX(workload_cfg("C2"))).cuda().Desc.conv_net
     K = 517
@@ -133,7 +114,10 @@ def test_cylindrical_net_runs_the_per_sample_kernel(dev, monkeypatch):
     monkeypatch.setattr(ops, "conv_layer_ps", lambda *a, **k: (calls.append(1), real(*a, **k))[1])
     got, _ = net(x, K=K)
     assert len(calls) == len(net.layers) - 1
-    monkeypatch.setattr(pn, "DESC_CONV_SD", True)
-    ref, _ = net(x, K=K)
-    assert len(calls) == len(net.layers) - 1
+    L = net.folded()
+    ref = x
+    for i, l in enumerate(L):
+        out = ops.conv_sd_buffer(K, l["cout"], dev) if i < len(L) - 1 else torch.empty((K, l["cout"] // 4, 140, 4), device=dev)
+        ref = ops.conv_layer_sd(ops.GEOM_CYL3D if i == 0 else ops.GEOM_CYL2D, ref, l["w_sd"], l["b"], out, K, l["cin"], l["cout"],
+                                l["relu"])
     assert torch.equal(_bits(got), _bits(ref))

@@ -37,7 +37,7 @@ def _cyl_case(seed, n, Cin, Cout):
 @pytest.mark.parametrize("n,Cin,Cout", [(3, 64, 64), (5, 32, 32), (1, 16, 64), (9, 64, 20)])
 def test_conv_sd_odd_tile_count(dev, n, Cin, Cout):
     """n * 176 rows = an odd number of 128-row tiles (n = 1: two tiles): the last unit's second warpgroup has no tile of its own.
-    Static and dynamic scheduling write the same bits, and the rows of every sample are right."""
+    The rows of every sample are right."""
     from bufferx_b200 import ops
     assert ((n * 176 + 127) // 128) % 2 == (0 if n == 1 else 1)
     x, W, b, y = _cyl_case(100 + n, n, Cin, Cout)
@@ -45,12 +45,6 @@ def test_conv_sd_odd_tile_count(dev, n, Cin, Cout):
     o = torch.full((n, Cout // 4, 140, 4), float("nan"), device=dev)
     ops.conv_layer_sd(ops.GEOM_CYL2D, xs, w, bd, o, n, Cin, Cout, True)
     assert _rel(ops.from_blocked(o).view(n, Cout, 7, 20), y) < 2e-5
-    ctr = torch.zeros(2, dtype=torch.int32, device=dev)
-    for _ in range(2):
-        od = torch.full_like(o, float("nan"))
-        ops.conv_layer_sd(ops.GEOM_CYL2D, xs, w, bd, od, n, Cin, Cout, True, tile_ctr=ctr)
-        assert torch.equal(od.view(torch.int32), o.view(torch.int32))
-        assert ctr.tolist() == [0, 0]
 
 
 def test_conv_sd_cin128_cout64_streamed_weights(dev):

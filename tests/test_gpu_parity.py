@@ -35,11 +35,14 @@ def relerr(a, b):
 # ------------------------------------------------------------------------------------------------ a1
 @pytest.mark.parametrize("n,m,kind", [(300, 64, "dup"), (5000, 2000, "plain"), (20000, 2000, "plain"),
                                       (20000, 300, "dup"), (40000, 200, "plain"), (70000, 128, "plain"),
-                                      (120000, 96, "plain"), (200000, 24, "plain"), (300000, 12, "dup")])
+                                      (120000, 96, "plain"), (200000, 24, "plain"), (300000, 12, "dup"),
+                                      (20000, 1500, "normal"), (120000, 300, "normal"), (5000, 512, "normal")])
 def test_fps_bit_exact(dev, oracle, n, m, kind):
     from bufferx_b200 import ops
-    rng = np.random.default_rng(n + m)
-    xyz = rng.uniform(-3, 3, size=(n, 3)).astype(np.float32)
+    if kind == "normal":                    # long runs of iterations through the cluster exchange on gaussian clouds
+        xyz = np.random.default_rng(n).normal(size=(n, 3)).astype(np.float32)
+    else:
+        xyz = np.random.default_rng(n + m).uniform(-3, 3, size=(n, 3)).astype(np.float32)
     if kind == "dup":                       # exact ties + candidates the |p|^2 <= 1e-3 rule must skip
         xyz[n // 2:] = xyz[: n - n // 2]
         xyz[5] = [0.01, 0.02, 0.01]
@@ -51,42 +54,21 @@ def test_fps_bit_exact(dev, oracle, n, m, kind):
     assert (kp[0].cpu().numpy() == xyz[exp]).all()
 
 
-@pytest.mark.parametrize("n,m", [(20000, 1500), (120000, 300), (5000, 512)])
-def test_fps_mbarrier_exchange_equals_cluster_sync_exchange(dev, oracle, n, m):
-    """The production cluster exchange (remote st.shared::cluster + mbarrier.arrive.release.cluster, local acquire wait) and
-    the verification form (the same stores ordered by cluster.sync(), which racecheck models)
-    give the same indices -- and both equal the oracle."""
-    from bufferx_b200 import ops
-    lib = ops.load_library()
-    rng = np.random.default_rng(n)
-    xyz = rng.normal(size=(n, 3)).astype(np.float32)
-    d = cu(xyz, dev)
-    old = lib.bx_fps_set_sync_mode(1)
-    try:
-        a, _ = ops.fps(d, [0, n], m)                 # cluster.sync() exchange (racecheck-clean reference form)
-        lib.bx_fps_set_sync_mode(0)
-        b, _ = ops.fps(d, [0, n], m)                 # st.async + transaction-count mbarrier (production)
-        lib.bx_fps_set_sync_mode(2)
-        c, _ = ops.fps(d, [0, n], m)                 # remote stores + mbarrier arrive / acquire wait (round 1)
-    finally:
-        lib.bx_fps_set_sync_mode(old)
-    assert torch.equal(a, b) and torch.equal(a, c) and (a[0].cpu().numpy() == oracle.fps(xyz, m)).all()
-
-
 @pytest.mark.parametrize("n,m", [(20000, 700), (7000, 300), (40000, 200), (4097, 64)])
-@pytest.mark.parametrize("cl", [2, 4])
-def test_fps_throughput_form_same_indices(dev, oracle, n, m, cl):
-    """bx_fps_ex with 2 / 4 CTAs per cloud (the form BufferX uses with several pairs in flight): the indices of the default
-    8-CTA form and of the oracle, incl. exact ties (duplicated points)."""
+@pytest.mark.parametrize("seed", [2, 4])
+def test_fps_duplicated_points_two_clouds_one_launch(dev, oracle, n, m, seed):
+    """A cloud with exact duplicates (tie-breaking by rank) and its reverse in one launch: each gets the oracle's indices
+    and its own key-points."""
     from bufferx_b200 import ops
-    rng = np.random.default_rng(n + cl)
+    rng = np.random.default_rng(n + seed)
     xyz = rng.normal(size=(n, 3)).astype(np.float32)
     xyz[n // 2:n // 2 + 50] = xyz[:50]                                   # exact duplicates: tie-breaking by rank
-    d = cu(np.concatenate([xyz, xyz[::-1]]), dev)                        # two clouds in one launch
-    a, ka = ops.fps(d, [0, n, 2 * n], m)
-    b, kb = ops.fps(d, [0, n, 2 * n], m, max_cluster=cl)
-    assert torch.equal(a, b) and torch.equal(ka, kb)
-    assert (b[0].cpu().numpy() == oracle.fps(xyz, m)).all()
+    clouds = [xyz, np.ascontiguousarray(xyz[::-1])]
+    idx, kp = ops.fps(cu(np.concatenate(clouds), dev), [0, n, 2 * n], m)
+    for b, c in enumerate(clouds):
+        exp = oracle.fps(c, m)
+        assert (idx[b].cpu().numpy() == exp).all()
+        assert (kp[b].cpu().numpy() == c[exp]).all()
 
 
 def test_fps_two_clouds_one_launch(dev, oracle):
@@ -753,24 +735,6 @@ def test_conv_layer_kernels(dev, geom, Cin, Cout, dims, k, n, impl):
     got = out.cpu().numpy().reshape(ref.shape)
     err = np.abs(got - ref.numpy()).max() / np.abs(ref.numpy()).max()
     assert err < 2e-5, f"{impl} {geom} Cin={Cin} Cout={Cout}: rel err {err}"     # fp32-grade (fp16 / 3xTF32 split) vs torch fp32
-
-
-def test_conv_sd_dynamic_tiles_same_bits(dev):
-    """bx_conv_layer_sd with a device-side tile counter (dynamic scheduling of the persistent CTAs) writes exactly what the
-    static stride writes, launch after launch (the kernel rewinds the counter itself), incl. a device-side sample count."""
-    from bufferx_b200 import ops
-    torch.manual_seed(5)
-    n, Cin, Cout = 700, 64, 64
-    x = ops.sd_pack(torch.relu(torch.randn(n, Cin, 7, 20, device=dev)))
-    Wt = torch.randn(9, Cin, Cout, device=dev) * 0.05
-    w, b = ops.conv_sd_weights(Wt), torch.randn(Cout, device=dev) * 0.1
-    ref = ops.conv_layer_sd(ops.GEOM_CYL2D, x, w, b, ops.conv_sd_buffer(n, Cout, dev).zero_(), n, Cin, Cout, True, None)
-    ctr = torch.zeros(2, dtype=torch.int32, device=dev)
-    for _ in range(3):
-        out = ops.conv_layer_sd(ops.GEOM_CYL2D, x, w, b, ops.conv_sd_buffer(n, Cout, dev).zero_(), n, Cin, Cout, True, None, tile_ctr=ctr)
-        assert torch.equal(out.view(torch.int16), ref.view(torch.int16))
-        assert ctr.tolist() == [0, 0]
-
 
 
 @pytest.mark.parametrize("tap", list(range(9)))

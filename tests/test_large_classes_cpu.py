@@ -58,10 +58,9 @@ def test_ladder_is_monotone_and_idempotent(ops):
         prev = c
 
 
-@pytest.mark.parametrize("max_cluster", [0, 2, 4])
-def test_ladder_equals_fps_size_class_up_to_the_cluster_limit(ops, max_cluster):
+def test_ladder_equals_fps_size_class_up_to_the_cluster_limit(ops):
     for n in [0, 1, 4096, 4097, 9000, 30000, 49152, 60000, 131073, 200000, 200001, 262145, 524288]:
-        assert ops.fps_large_size_class(n, max_cluster) == ops.fps_size_class(n, max_cluster)
+        assert ops.fps_large_size_class(n) == ops.fps_size_class(n)
 
 
 def _model(**kw):

@@ -2,7 +2,7 @@
 BufferX under enable_cuda_graphs(..., size_classes=True).  Host-side only: no kernel runs."""
 import pytest
 
-# the default launch table of bx_fps_ex (max_cluster 0): the largest point count of every register tier
+# the launch table of bx_fps: the largest point count of every register tier
 BOUNDARIES = [4096, 8192, 16384, 24576, 32768, 65536, 131072, 262144, 524288]
 
 
@@ -28,20 +28,6 @@ def test_size_class_is_monotone_and_idempotent(ops):
         c = ops.fps_size_class(n)
         assert c >= n and ops.fps_size_class(c) == c and c >= prev
         prev = c
-
-
-@pytest.mark.parametrize("max_cluster", [2, 4])
-def test_size_class_throughput_form(ops, max_cluster):
-    """The 2- / 4-CTA form has its own tiers up to 49152 points; a class never crosses a change of launch configuration."""
-    per_cta = [4096, 6144, 10240, 12288]
-    cl = max_cluster
-    expect = [4096, 8192] + [min(p * cl, 49152) for p in per_cta if p * cl > 8192]
-    if cl == 2:
-        expect += [32768, 65536]          # 24577..49152 points fall back to the latency form's tiers
-    for b in expect:
-        assert ops.fps_size_class(b, max_cluster) == b
-        assert ops.fps_size_class(b - 1, max_cluster) == b
-    assert ops.fps_size_class(50000, max_cluster) == 65536
 
 
 def _model(**kw):

@@ -1,19 +1,26 @@
 """GPU experiment: the descriptor conv stack alone (Cylindrical_Net on K patches), per-layer CUDA-event times.
-    python tools/conv_bench.py [K] [reps]           # prints per-layer ms and TFLOP/s (fp32-equivalent)
-Under ncu:  ncu --set full -k regex:conv_tc --launch-skip 16 -c 8 python tools/conv_bench.py 1500 3"""
-import os, sys
+    python tools/conv_bench.py [K] [reps] [--tf32]  # prints per-layer ms and TFLOP/s (fp32-equivalent)
+--tf32 sets the stack's force_tf32, its fall-back to the TF32 tensor-core kernel, instead of the shifted-descriptor
+fp16-split kernel.
+Under ncu:  ncu --set full -k regex:conv_tc --launch-skip 16 -c 8 python tools/conv_bench.py 1500 3 --tf32"""
+import argparse, os, sys
 import torch
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import bufferx_b200 as bx
 from bufferx_b200 import ops
 from bufferx_b200.synth import init_synthetic_weights, workload_cfg
 
-MODE = os.environ.get("BX_CONV", "sd").lower()          # sd (shifted-descriptor fp16-split kernel) | tc (TF32 tensor-core kernel)
-K = int(sys.argv[1]) if len(sys.argv) > 1 else 1500
-reps = int(sys.argv[2]) if len(sys.argv) > 2 else 10
+ap = argparse.ArgumentParser()
+ap.add_argument("K", type=int, nargs="?", default=1500)
+ap.add_argument("reps", type=int, nargs="?", default=10)
+ap.add_argument("--tf32", action="store_true", help="run the stack on the TF32 tensor-core kernel (force_tf32)")
+args = ap.parse_args()
+K, reps = args.K, args.reps
 cfg = workload_cfg("C2")
 model = init_synthetic_weights(bx.BufferX(cfg)).cuda()
 net = model.Desc.conv_net
+net.force_tf32 = args.tf32
+MODE = "tc" if net.force_tf32 else "sd"
 L = net.folded()
 dev = torch.device("cuda")
 torch.manual_seed(0)
@@ -26,7 +33,6 @@ if MODE == "sd":     # layer-to-layer activations in the presplit padded fp16 fo
 else:
     bufs = [torch.empty((K, l["cout"] // 4, 140, 4), device=dev) for l in L]
 times = [[] for _ in L]
-ctrs = torch.zeros(2 * len(L), dtype=torch.int32, device=dev)
 for r in range(reps + 2):
     flush.zero_()
     cur = x
@@ -34,7 +40,7 @@ for r in range(reps + 2):
         a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
         a.record()
         if MODE == "sd":
-            ops.conv_layer_sd(ops.GEOM_CYL3D if i == 0 else ops.GEOM_CYL2D, cur, l["w_sd"], l["b"], bufs[i], K, l["cin"], l["cout"], l["relu"], None, tile_ctr=(ctrs[2 * i:2 * i + 2] if os.environ.get("BX_SD_DYNAMIC", "0") == "1" else None))
+            ops.conv_layer_sd(ops.GEOM_CYL3D if i == 0 else ops.GEOM_CYL2D, cur, l["w_sd"], l["b"], bufs[i], K, l["cin"], l["cout"], l["relu"], None)
         elif i == 0:
             ops.conv_layer_tc(ops.GEOM_CYL3D, cur, l["w_tc"], l["b"], bufs[i], K, l["cin"], l["cout"], 3, 7, 20, 3, 3, 3, l["relu"])
         else:
